@@ -2,14 +2,14 @@
 """bench.py — denoise-steps/s of STDiT3-XL/2 (bf16) on a 64x32x32 latent, BASELINE.json's metric.
 
 One "step" = one denoiser forward on one synthetic latent [1,4,64,32,32] with T5 embeddings
-[1,1,300,4096] (36.13 algorithmic TFLOP, BASELINE.md §3 config 2) through the osb200 sm_100a path.
+[1,1,300,4096] (36.13 algorithmic TFLOP, BASELINE.md §3 config 2) through the osb200 sm_90a (H100) path.
 
     python bench.py --gpus N --steps K --warmup W          # our arm (N>1 under torchrun)
     python bench.py --impl reference ...                   # the reference's CPU arithmetic (oracle port)
 
-JSON line keys follow the driver's contract: `value` is device-resident throughput, `e2e` is the same
+JSON line keys: `value` is device-resident throughput, `e2e` is the same
 metric through the public model API with pinned-host inputs copied in and the result copied out
-inside the timed region, `roofline` is the dominant kernel family (tcgen05 GEMM) measured live with
+inside the timed region, `roofline` is the dominant kernel family (wgmma GEMM) measured live with
 CUDA events on the launching stream, `cpu_baseline` is the oracle timed on the host cores.
 """
 from __future__ import annotations
@@ -46,11 +46,12 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(burst=d.get("bf16_tflops"), sustained=d.get("bf16_tflops_sustained"), hbm=d.get("hbm_gbs"), src="measured")
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (dense bf16, HBM3 at 700 W): an upper bound, not a measured rate
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -267,16 +268,22 @@ def host_inputs(seed):
                 height=torch.tensor([256.0]), width=torch.tensor([256.0]))
 
 
+VAE_VIDEO = (33, 720, 1280)   # untiled 720p: 33 frames fit the 80 GB of one H100 (65 frames need more)
+
+
 def vae_leg():
-    """Second half of BASELINE.json's metric: causal 3D VAE encode / decode fps on a synthetic 65x720x1280 video
-    (configs[2]), untiled, bf16, one B200; per-family device times from the same CUDA-event hook as the roofline."""
+    """Second half of BASELINE.json's metric: causal 3D VAE encode / decode fps on a synthetic 33x720x1280 video
+    (configs[2] at half its frame count), untiled, bf16, one GPU; per-family device times from the same CUDA-event hook
+    as the roofline."""
     import osb200
     from tests.vae_bench import DEC_TF, ENC_TF, run
 
     del_model = torch.cuda.empty_cache
     del_model()
     try:
-        res = run(65, 720, 1280, iters=2)
+        T, H, W = VAE_VIDEO
+        res = run(T, H, W, iters=2)
+        scale = (T * H * W) / (65 * 720 * 1280)   # ENC_TF / DEC_TF are the algorithmic FLOPs at 65x720x1280
         osb200.start_profile()
         from opensora.registry import MODELS, build_module
 
@@ -284,7 +291,7 @@ def vae_leg():
         with torch.device("cuda"):
             m = build_module(dict(type="hunyuan_vae"), MODELS, device_map="cuda").eval()
         with torch.no_grad():
-            z = torch.randn(1, 16, 17, 90, 160, device="cuda").to(torch.bfloat16)
+            z = torch.randn(1, 16, *res["latent"], device="cuda").to(torch.bfloat16)
             m.decode(z)
             osb200.stop_profile()
             osb200.start_profile()
@@ -298,11 +305,14 @@ def vae_leg():
         conv_ms = fam.get("conv3d", [0, 1.0])[1]
         pk = peaks()
         res["conv_roofline"] = {"bound": "tensor", "kernel": "gemm_bf16_kernel<conv> (all conv3d launches of one decode)",
-                                "achieved": DEC_TF / (conv_ms * 1e-3), "peak": pk["sustained"], "unit": "TFLOP/s",
-                                "frac": DEC_TF / (conv_ms * 1e-3) / pk["sustained"],
-                                "note": "algorithmic conv FLOPs (1017.9 TF, SURVEY.md 8d) / summed conv3d device time"}
-        res["config"] = {"workload": "hunyuan causal 3D VAE, video 1x3x65x720x1280 <-> latent 1x16x17x90x160, untiled, bf16",
-                         "algorithmic_conv_tflop": {"encode": ENC_TF, "decode": DEC_TF},
+                                "achieved": DEC_TF * scale / (conv_ms * 1e-3), "peak": pk["sustained"], "unit": "TFLOP/s",
+                                "frac": DEC_TF * scale / (conv_ms * 1e-3) / pk["sustained"],
+                                "note": "approximate: algorithmic conv FLOPs of 65x720x1280 (1017.9 TF, SURVEY.md 8d) scaled by "
+                                        "the voxel count (the latent frame count, 9 against 17, does not scale like the video's) / "
+                                        "summed conv3d device time"}
+        res["config"] = {"workload": "hunyuan causal 3D VAE, video 1x3x%dx%dx%d <-> latent 1x16x%dx%dx%d, untiled, bf16"
+                                     % (T, H, W, *res["latent"]),
+                         "algorithmic_conv_tflop": {"encode": ENC_TF * scale, "decode": DEC_TF * scale},
                          "mid_block_attention": "torch SDPA per frame prefix (library kernel; osb200 D=512 kernel pending)"}
         res["e2e"] = _vae_e2e(m, z, tuple(res["out_shape"]))
         res["tiled"] = _vae_tiled(m, z)
@@ -474,6 +484,15 @@ def mmdit_leg(timeout_s: float = 180.0):
         return {"error": repr(e)[:300]}
 
 
+def dump_outputs(dirname: str, arrays: dict) -> None:
+    """Write each tensor as dirname/<name>.npy in float32 (the denoiser output of one step is 2 MB)."""
+    import numpy as np
+
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -492,6 +511,9 @@ def main():
     ap.add_argument("--leg", default=None, choices=["mmdit"], help="run ONE auxiliary leg in this process and print its JSON")
     ap.add_argument("--no-mmdit", action="store_true", help="skip the MMDiT 256px leg (a child process of the N = 1 run)")
     ap.add_argument("--no-vae", action="store_true", help="skip the VAE leg (encode/decode fps of BASELINE.json's metric)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32), so "
+                         "that two builds can be compared output for output on identical seeded inputs")
     ap.add_argument("--profile-step", action="store_true",
                     help="after warm-up, bracket ONE step with cudaProfilerStart/Stop and exit (for `ncu --profile-from-start off`: "
                          "the launch list of exactly one step; prints no bench line)")
@@ -601,6 +623,8 @@ def main():
     if replay is not None:   # a replay re-issues the captured kernels without passing through the C ABI counter
         launches = graph_launches * args.steps
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:   # before anything else replays the graph into the same output buffer
+        dump_outputs(args.dump_outputs, {"denoise_out": out_holder["o"]})
     for _ in range(2):
         step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
@@ -678,7 +702,7 @@ def main():
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak" if args.parallel == "dp" else "strong",   # the --parallel mode the N > 1 runs of this line use (default sp: total work fixed)
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic (seeded N(0,1) latents / T5 embeddings, random-init weights)",
         "config": {"workload": WORKLOAD, "parallelism": mode + str(world), "cuda_graph": bool(args.graph),
-                   "l2": "weights 2.2 GB + activations stream through every step (>> 126 MB L2): inputs larger than L2",
+                   "l2": "weights 2.2 GB + activations stream through every step (>> 50 MB L2): inputs larger than L2",
                    "algorithmic_tflop_per_step": FLOP_PER_STEP / 1e12},
         "clocks": clk, "gpu_launches": launches,
         "e2e": {"value": e2e, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": host_out.numel() * 4,

@@ -1,5 +1,5 @@
 /*
- * osb200 — C ABI of the B200-native (sm_100a) hot path for Open-Sora's denoiser blocks and
+ * osb200 — C ABI of the H100-native (sm_90a) hot path for Open-Sora's denoiser blocks and
  * causal 3D VAE.  This header is the drop-in boundary: plain pointers and sizes, no torch
  * types, no exceptions.  Each entry point cites the reference call site (path:line under the
  * reference checkout hpcaitech/Open-Sora @ 7ad6a96) whose arithmetic it replaces.
@@ -35,7 +35,7 @@ typedef enum osb_status {
 
 /* Bind to `device`, resolve cuTensorMapEncodeTiled through the runtime, opt kernels into
  * large dynamic shared memory.  Must be called once per process and device before any op.
- * Fails with OSB_ERR_UNSUPPORTED on anything that is not compute capability 10.x. */
+ * Fails with OSB_ERR_UNSUPPORTED on anything that is not compute capability 9.0. */
 int osb_init(int device);
 int osb_version(void);
 const char* osb_last_error(void);
@@ -56,7 +56,7 @@ int osb_ln_modulate(const void* x, const float* shift, const float* scale, void*
                     int64_t rows, int C, int64_t group_rows, const int32_t* mod_index,
                     int64_t mod_stride, float eps, void* stream);
 
-/* ---- bf16 GEMM on tcgen05 with fused epilogues -------------------------------------------- */
+/* ---- bf16 GEMM on wgmma with fused epilogues ---------------------------------------------- */
 typedef enum osb_epilogue {
   OSB_EPI_BIAS = 0,           /* D = A W^T + bias                                              */
   OSB_EPI_BIAS_GELU_TANH = 1, /* D = gelu_tanh(A W^T + bias)      layers.py:277-281 (MLP[0:2]) */
@@ -77,14 +77,14 @@ typedef struct osb_gemm_args {
   int64_t group_rows;  /* g = row / group_rows                                                   */
   int64_t gate_stride;
   int32_t epilogue;    /* osb_epilogue                                                           */
-  int32_t cta_group;   /* 0 = library default, 1 = single-CTA MMA, 2 = CTA-pair MMA (cta_group::2) */
+  int32_t cta_group;   /* 0, 1 or 2; kept for ABI compatibility: sm_90a has no CTA-pair MMA, all run one CTA per tile */
   int32_t block_n;     /* 0 = library default, else 64/128/192/256                               */
   int32_t reserved;
 } osb_gemm_args;
 
 /* Replaces every nn.Linear on the block path: layers.py:209,212-214 (qkv / q,k,v proj),
  * :247,251 (attn out proj + gated residual), :277-281 (MLP), :314-333 (linear1/linear2), :401.
- * fp32 accumulation in TMEM; epilogue math in fp32; single rounding to bf16 on store.
+ * fp32 accumulation in registers; epilogue math in fp32; single rounding to bf16 on store.
  * Requires K % 8 == 0, N % 8 == 0. */
 int osb_gemm_bf16(const osb_gemm_args* args, void* stream);
 
@@ -98,7 +98,7 @@ typedef struct osb_attn_short_args {
   int64_t num_seqs, seqs_per_batch;
   int64_t q_batch_stride, q_seq_stride, q_tok_stride;
   int64_t k_batch_stride, k_seq_stride, k_tok_stride;
-  int32_t Lq, Lk;                 /* tokens per sequence; Lk (x sequences packed per tile) <= 320 */
+  int32_t Lq, Lk;                 /* tokens per sequence (Lq < 128: 128 / Lq sequences share a query tile) */
   const int32_t* kv_lens;         /* optional [num_seqs]: valid keys per sequence (<= Lk)       */
   int32_t num_heads, head_dim;    /* head_dim: 72 (STDiT3-XL) or 64                              */
   const void* q_norm_w;           /* bf16 [D] RMSNorm weight for q, or NULL = no QK-norm         */
@@ -110,8 +110,8 @@ typedef struct osb_attn_short_args {
   const void* q_norm_w2;          /* optional second RMSNorm weight pair used by tokens >= norm_split: the     */
   const void* k_norm_w2;          /*   joint txt|img sequence of MMDiT has per-stream QKNorm (layers.py:222,238) */
   int32_t norm_split;
-  int32_t reserved;               /* implementation switch: 0 auto, 1 resident-key kernel, 2 flash (P via smem), 3 flash (P in TMEM),
-                                     4 two-slot ping-pong kernel (resident key sets <= 320 keys, head_dim <= 72; other shapes fall back to auto) */
+  int32_t reserved;               /* implementation switch, kept for ABI compatibility: every value runs the one
+                                     flash-attention kernel of sm_90a */
   int32_t rope_half;              /* 1: rope tables are applied with the rotate-half pairing (i, i + D/2) of HF /   */
   int32_t reserved2;              /*    Liger RoPE (math.py:27); 0: interleaved pairs (2i, 2i+1) (math.py:60-65)     */
 } osb_attn_short_args;
@@ -123,7 +123,7 @@ typedef struct osb_attn_short_args {
 int osb_attn_short(const osb_attn_short_args* args, void* stream);
 
 /* ---- head tiles: projection GEMM -> attention without a layout pass ------------------------------------ */
-/* A head tile is the HBM image of one tcgen05 operand tile: tile_rows <= 128 token rows of ONE head, head_dim
+/* A head tile is the HBM image of one attention operand tile: tile_rows <= 128 token rows of ONE head, head_dim
  * padded to a multiple of 16, 64-column chunks in the 128-byte-swizzle layout followed by the head-dim tail in the
  * no-swizzle core-matrix layout (open-sora_b200/csrc/tiles.cuh).  The projection GEMM writes q / k / v straight into
  * this form (bias + per-head RMSNorm + RoPE fused in its epilogue) and the attention kernel loads whole tiles with
@@ -148,9 +148,8 @@ typedef struct osb_head_tiles_args {
   int32_t nkinds;           /* column group kidx is of kind kidx % nkinds                                            */
   uint32_t norm_mask;       /* bit k: kind k gets per-head RMSNorm with norm_w[k]        (layers.py:102-135)         */
   uint32_t rope_mask;       /* bit k: kind k gets interleaved-pair RoPE by position      (math.py:60-65)             */
-  int32_t reserved;         /* bit 0: force the general per-row-store epilogue (default: when a CTA's rows coincide with
-                               one tile - contiguous sequences of whole 128-row tiles, or the temporal view loaded through
-                               a strided TMA box - the tile image is staged in shared memory and bulk-stored)           */
+  int32_t reserved;         /* kept for ABI compatibility (bit 0 selected a store path that sm_90a does not have): the
+                               epilogue stores every head row straight into its tile                                  */
   const void* norm_w[4];    /* bf16 [head_dim] per kind or NULL                                                      */
   float norm_eps;
   int32_t reserved2;
@@ -188,8 +187,8 @@ typedef struct osb_attn_tiles_args {
   const struct osb_scatter* out_scatter; /* optional: route output rows to peer buffers (sequence parallel), else NULL   */
 } osb_attn_tiles_args;
 
-/* out = softmax(q k^T * scale) v per (sequence, head) over head tiles: persistent CTAs, bulk-copy loads, two
- * query tiles in flight per CTA (open-sora_b200/csrc/attn_tiles_sm100.cu).  Replaces mmdit/math.py:22-36. */
+/* out = softmax(q k^T * scale) v per (sequence, head) over head tiles: one CTA per (query tile, head), bulk-copy loads
+ * with the next key tile in flight (open-sora_b200/csrc/attn_sm90.cu).  Replaces mmdit/math.py:22-36. */
 int osb_attn_tiles(const osb_attn_tiles_args* args, void* stream);
 
 /* ---- sequence-parallel exchange over peer memory (NVLink / NVSwitch; SURVEY.md §8b, §8e) ------------------------- */
@@ -249,9 +248,9 @@ typedef struct osb_conv3d_args {
   int32_t block_n;      /* 0 = library default                                                                 */
 } osb_conv3d_args;
 
-/* y = conv3d(x_pad) + bias (+ residual), fp32 accumulation in TMEM, one rounding to bf16.  Every k-block is a
+/* y = conv3d(x_pad) + bias (+ residual), fp32 accumulation in registers, one rounding to bf16.  Every k-block is a
  * 5-D TMA box load of the padded NDHWC input at the tap offset (strided boxes for stride-2 convolutions), fed to
- * the same tcgen05 main loop and epilogue as osb_gemm_bf16.
+ * the same wgmma main loop and epilogue as osb_gemm_bf16.
  * Replaces: opensora/models/hunyuan_vae/unet_causal_3d_blocks.py:94-96 (CausalConv3d.forward: F.pad replicate +
  * ChannelChunkConv3d) and opensora/models/vae/utils.py:172-190 (the cuDNN conv3d it dispatches to). */
 int osb_conv3d_ndhwc(const osb_conv3d_args* args, void* stream);

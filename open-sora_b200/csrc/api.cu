@@ -155,15 +155,14 @@ int make_row_scatter(RowScatter* dst, const osb_scatter* src, int64_t rows, cons
   return OSB_OK;
 }
 
-int gemm_init();   // gemm_sm100.cu
-int attn_init();   // attn_short_sm100.cu
-int attn_tiles_init();   // attn_tiles_sm100.cu
+int gemm_init();   // gemm_sm90.cu
+int attn_init();   // attn_sm90.cu
 
 }  // namespace osb
 
 extern "C" {
 
-int osb_version(void) { return 100; }
+int osb_version(void) { return 200; }
 const char* osb_last_error(void) { return osb::g_err; }
 int64_t osb_launch_count(void) { return osb::g_launches.load(); }
 
@@ -182,8 +181,8 @@ int osb_init(int device) {
   OSB_CHECK_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   OSB_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("osb200 is built for sm_100a only; device %d is sm_%d%d", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("osb200 is built for sm_90a only; device %d is sm_%d%d", device, prop.major,
               prop.minor);
     return OSB_ERR_UNSUPPORTED;
   }
@@ -200,8 +199,6 @@ int osb_init(int device) {
   int rc = gemm_init();
   if (rc) return rc;
   rc = attn_init();
-  if (rc) return rc;
-  rc = attn_tiles_init();
   if (rc) return rc;
   g_init = true;
   return OSB_OK;

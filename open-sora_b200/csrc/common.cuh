@@ -1,5 +1,5 @@
-// Shared device/host helpers for the osb200 sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX
-// wrappers, error plumbing for the C ABI.  Hand-written for Blackwell (sm_100a) only.
+// Shared device/host helpers for the osb200 sm_90a kernels: mbarrier, TMA, wgmma and mma.sync PTX
+// wrappers, error plumbing for the C ABI.  Hand-written for Hopper (sm_90a).
 #pragma once
 
 #include <cuda.h>
@@ -125,16 +125,6 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) 
       "r"(cta)
       : "memory");
 }
-// relaxed variant: no release fence, i.e. the arrive does not wait for this thread's earlier global stores to become
-// visible.  For hand-offs whose payload is tensor memory (ordered by tcgen05.wait + tcgen05.fence::before_thread_sync),
-// where the release of an epilogue's scattered global stores would otherwise sit on the tensor pipe's critical path.
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(bar),
-      "r"(cta)
-      : "memory");
-}
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -164,6 +154,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
              blockIdx.x, threadIdx.x, bar, parity);
       __trap();
     }
+  }
+}
+// the same bounded wait with no call on its timeout path: inside a wgmma region a function call (printf) makes ptxas
+// serialise every wgmma.mma_async of the kernel (C7510), so wgmma consumers wait with this one
+__device__ __forceinline__ void mbar_wait_notrace(uint32_t bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > OSB_SPIN_LIMIT) __trap();
   }
 }
 // acquire at cluster scope (used when the arrivals come from the peer CTA)
@@ -200,7 +198,7 @@ __device__ __forceinline__ void cluster_sync_all() {
 
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------------
 // Every osb200 kernel is launched with cudaLaunchAttributeProgrammaticStreamSerialization (osb::launch_config):
-// its prologue (barrier init, TMEM allocation, descriptor prefetch) may overlap the tail of the previous kernel in
+// its prologue (barrier init, descriptor prefetch) may overlap the tail of the previous kernel in
 // the stream; pdl_wait() must precede the first access to memory the previous kernel may have written, and
 // pdl_launch_dependents() lets the next kernel's CTAs start filling SMs this kernel has already vacated.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -225,17 +223,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint32_t bar, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// CTA-pair variant: data lands in this CTA's smem, complete_tx is signalled on the barrier at
-// `bar` (a shared::cluster address, normally the leader CTA's barrier)
-__device__ __forceinline__ void tma_load_2d_cg2(const CUtensorMap* m, uint32_t bar_cluster,
-                                                uint32_t dst, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-
 // 5D tile loads (NDHWC activations of the causal-conv VAE: coordinates c, w, h, t, n)
 __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint32_t bar, uint32_t dst, int32_t c0,
                                             int32_t c1, int32_t c2, int32_t c3, int32_t c4) {
@@ -245,163 +232,47 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint32_t bar, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_5d_cg2(const CUtensorMap* m, uint32_t bar_cluster, uint32_t dst,
-                                                int32_t c0, int32_t c1, int32_t c2, int32_t c3, int32_t c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
+// ---- wgmma (warpgroup MMA) ----------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- tcgen05 / TMEM ----------------------------------------------------------------------
-template <int kCta>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  if constexpr (kCta == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int kCta>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCta == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-  }
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 bf16 (128 B),
-// 8-row swizzle atoms 1024 B apart (cute::UMMA::SmemDescriptor, version 1, LayoutType 2).
+// shared-memory matrix descriptor (sm_90), K-major operand, 128-byte swizzle, rows of 64 bf16 (128 B),
+// 8-row swizzle atoms 1024 B apart.  The tile base must be 1024-byte aligned; +32 B along K = +2.
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);        // start address  [0,14)
-  d |= static_cast<uint64_t>(0) << 16;                            // LBO (unused for swizzled K-major)
+  d |= static_cast<uint64_t>(1) << 16;                            // LBO (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                    // SBO = 1024 B   [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                            // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                            // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                            // SWIZZLE_128B
   return d;
 }
 
-// kind::f16 instruction descriptor: A,B = bf16 (K-major), D = fp32, shape M x N x 16
-__host__ __device__ constexpr uint32_t make_idesc_bf16_f32(uint32_t M, uint32_t N) {
-  return (1u << 4)      // D format  : f32
-         | (1u << 7)    // A format  : bf16
-         | (1u << 10)   // B format  : bf16
-         | (0u << 15)   // A K-major
-         | (0u << 16)   // B K-major
-         | ((N >> 3) << 17) | ((M >> 4) << 24);
+// ---- mma.sync / ldmatrix (register-operand tensor core path of the attention kernels) -----------------
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr));
 }
-
-template <int kCta>
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kCta == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr));
 }
-
-// tcgen05.commit: arrive on `bar` when all previously issued MMAs of this thread have completed.
-// kCta==2: multicast the arrive to the barrier at the same offset in both CTAs of the pair.
-template <int kCta>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (kCta == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-  } else {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-        "[%0], %1;" ::"r"(bar),
-        "h"(static_cast<uint16_t>(3))
-        : "memory");
-  }
-}
-
-// TMEM -> registers: 32 lanes (this warp's quarter) x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
+// D[16 x 8] += A[16 x 16] * B[16 x 8], bf16 operands, fp32 accumulator
+__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM: 32 lanes (this warp's quarter) x 16 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: A operand read from tensor memory (bf16 pairs packed per 32-bit column)
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // ---- output row routing to peer buffers (osb_scatter) ----------------------------------------------------------

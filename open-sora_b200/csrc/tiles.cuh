@@ -1,16 +1,16 @@
-// Head tiles: the on-HBM image of a tcgen05 operand tile for one attention head.
+// Head tiles: the on-HBM image of a shared-memory attention operand tile for one attention head.
 //
-// A head tile holds TR <= 128 token rows (TR % 8 == 0) of ONE head, already in the shared-memory layout the tensor
-// core reads, so the attention kernel moves it with a single 1-D bulk copy (cp.async.bulk) and never touches the
-// data:
+// A head tile holds TR <= 128 token rows (TR % 8 == 0) of ONE head, already in the shared-memory layout the attention
+// kernel reads (bank-conflict-free ldmatrix rows of 16 bytes), so the kernel moves it with a single 1-D bulk copy
+// (cp.async.bulk) and never transforms the data:
 //   bytes [0, MAIN * TR * 128)    MAIN = D / 64 chunks of [TR rows x 64 columns] bf16, 128-byte swizzle
 //                                 (row r, 16-byte unit u at (r/8)*1024 + (r%8)*128 + ((u ^ r%8) * 16))
 //   bytes [.., + TR * 32)         head-dim tail (D % 64 != 0: columns 64*MAIN .. +15, zero padded) in the
 //                                 no-swizzle core-matrix layout (8 rows x 16 B; K-adjacent matrices 128 B apart,
 //                                 8-row groups 256 B apart)
-// The same bytes serve as the K-major A/B operand of S = Q K^T and as the MN-major B operand of O = P V.
-// Producers: the head-tile epilogue of gemm_bf16_kernel (bias + per-head RMSNorm + RoPE fused, gemm_sm100.cu).
-// Consumer: attn_tiles_kernel (attn_tiles_sm100.cu).
+// The same bytes serve as the operand of S = Q K^T (ldmatrix) and of O = P V (ldmatrix.trans).
+// Producers: the head-tile epilogue of gemm_bf16_kernel (bias + per-head RMSNorm + RoPE fused, gemm_sm90.cu) and the
+// staging step of attn_short_kernel.  Consumers: attn_tiles_kernel / attn_short_kernel (attn_sm90.cu).
 #pragma once
 
 #include "common.cuh"
@@ -79,36 +79,13 @@ __device__ __forceinline__ uint32_t sw128_off(int r, int u) {
 __device__ __forceinline__ uint32_t tail_off(int r, int u) {
   return (uint32_t)((r >> 3) * 256 + u * 128 + (r & 7) * 16);
 }
-__device__ __forceinline__ uint64_t make_noswz_kmajor_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(128 >> 4) << 16;  // LBO: next core matrix along K
-  d |= static_cast<uint64_t>(256 >> 4) << 32;  // SBO: next 8-row group
-  d |= static_cast<uint64_t>(1) << 46;         // descriptor version (sm_100)
-  return d;                                    // layout type 0 = SWIZZLE_NONE
+// byte offset of the 16-byte unit holding columns [8u, 8u + 8) of row `r` in a tile whose 64-column chunks are
+// `chunk_bytes` apart (= rows * 128) and that has MAIN such chunks before the tail
+template <int MAIN>
+__device__ __forceinline__ uint32_t tile_unit_off(int r, int u, uint32_t chunk_bytes) {
+  return u < MAIN * 8 ? (uint32_t)(u >> 3) * chunk_bytes + sw128_off(r, u & 7)
+                      : (uint32_t)MAIN * chunk_bytes + tail_off(r, u - MAIN * 8);
 }
-__device__ __forceinline__ uint64_t make_sw128_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;  // LBO: next 64-wide block along N
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // SBO: next group of 8 K-rows
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;                          // SWIZZLE_128B
-  return d;
-}
-__device__ __forceinline__ uint64_t make_noswz_mnmajor_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(256 >> 4) << 16;  // LBO: next group of 8 K-rows
-  d |= static_cast<uint64_t>(128 >> 4) << 32;  // SBO: next 8-wide unit along N
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
-// kind::f16 instruction descriptor with an MN-major B operand (bit 16)
-__host__ __device__ constexpr uint32_t make_idesc_bf16_f32_bmn(uint32_t M, uint32_t N) {
-  return make_idesc_bf16_f32(M, N) | (1u << 16);
-}
-
 // 1-D bulk copy global -> this CTA's shared memory, completion (bytes) on an mbarrier.  size % 16 == 0.
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile(

@@ -1,4 +1,4 @@
-"""Peer-memory exchange for sequence parallelism: the B200-native replacement of the reference's autograd all_to_all
+"""Peer-memory exchange for sequence parallelism: the osb200 replacement of the reference's autograd all_to_all
 (`opensora/acceleration/communications.py:8-18,57-63`) on the STDiT3 path.
 
 The reference packs, calls `dist.all_to_all`, and unpacks around every temporal attention.  Here the kernels that

@@ -1,10 +1,10 @@
 """`AutoencoderKLCausal3D` / `CausalVAE3D_HUNYUAN` with the reference's public surface
 (`opensora/models/hunyuan_vae/autoencoder_kl_causal_3d.py:59-146,269-358,554-638`): registry key
 `"hunyuan_vae"`, `encode / decode / forward / get_latent_size`, `scale_factor`, `shift_factor`, `z_channels`,
-compression ratios, tiling toggles, identical state-dict keys — arithmetic on libosb200 (sm_100a).
+compression ratios, tiling toggles, identical state-dict keys — arithmetic on libosb200 (sm_90a).
 
-Untiled (`:298-304`, `:318-335`) is the fast path on B200 (a 65x720x1280 decode peaks at 87 GB of the 180 GB and
-avoids the ~1.65x tile-overlap recompute).  The reference's tiled / blended modes (`:384-552`) are reproduced with the
+Untiled (`:298-304`, `:318-335`) is the fast path wherever the activations fit (it avoids the ~1.65x tile-overlap
+recompute); on one 80 GB H100 that holds for 720p videos of about 33 frames, longer ones need tiling.  The reference's tiled / blended modes (`:384-552`) are reproduced with the
 same tile grid, overlap, in-place blending order and cropping, because their numerics differ from untiled by
 construction (per-tile GroupNorm statistics and causal start) and a caller that enables tiling must get the
 reference's result; every tile runs through the same osb200 encoder / decoder."""

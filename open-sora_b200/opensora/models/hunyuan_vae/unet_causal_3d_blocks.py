@@ -6,7 +6,7 @@ Same class names, constructor meaning and state-dict keys as the reference's
 `DownEncoderBlockCausal3D`, `UpDecoderBlockCausal3D`).  The nn.Modules hold parameters only; `forward` takes and
 returns **NDHWC bf16** tensors and runs on libosb200: GroupNorm statistics (`osb_group_stats`), one fused
 GN-apply + SiLU + nearest-upsample + replicate-pad pass (`osb_vae_prep`) and the implicit-GEMM convolution
-(`osb_conv3d_ndhwc`, tcgen05, residual add fused in the epilogue).  1x1x1 convolutions are plain GEMMs.
+(`osb_conv3d_ndhwc`, wgmma, residual add fused in the epilogue).  1x1x1 convolutions are plain GEMMs.
 No CPU / eager fallback."""
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 block-`processor` plug-in hook as the reference's `opensora/models/mmdit/layers.py`
 (`DoubleStreamBlock.set_processor / forward = self.processor(self, img, txt, vec, pe)` :295-306,
 `SingleStreamBlock` :378-388).  The nn.Modules hold parameters; the two processor classes below ARE the drop-in:
-they read the block's own parameters and run every FLOP on libosb200 (sm_100a):
+they read the block's own parameters and run every FLOP on libosb200 (sm_90a):
 
   LN(no affine)+modulate -> `osb_ln_modulate`; every Linear -> `osb_gemm_bf16` (bias / GELU-tanh / gate*x+residual
   epilogues); QK-RMSNorm + RoPE + joint txt|img softmax attention -> `osb_attn_short` (per-stream norm weights via

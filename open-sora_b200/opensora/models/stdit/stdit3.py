@@ -1,12 +1,12 @@
-"""STDiT3 (Open-Sora v1.2 denoiser) on the B200-native osb200 kernels.
+"""STDiT3 (Open-Sora v1.2 denoiser) on the H100-native osb200 kernels.
 
 Same class / module path / registry keys / state-dict keys as upstream
 `opensora/models/stdit/stdit3.py` (witnessed in the reference tree only by `gradio/app.py:119-137`
 and docs/report_0{1,2,3}.md — see SURVEY.md §8(a-S), Appendix A), so `STDiT3.from_pretrained(...)`,
 `build_module({"type": "STDiT3-XL/2", ...}, MODELS)` and `model(x, timestep, y, mask=..., fps=...,
 height=..., width=...)` keep working.  The nn.Modules below only HOLD parameters; every FLOP of the
-forward runs in libosb200.so (tcgen05 GEMMs with fused bias/GELU/gate+residual epilogues, the
-short-KV tcgen05 attention with fused QK-RMSNorm + RoPE, the LN+modulate row kernel).  There is no
+forward runs in libosb200.so (wgmma GEMMs with fused bias/GELU/gate+residual epilogues, the
+flash attention with fused QK-RMSNorm + RoPE, the LN+modulate row kernel).  There is no
 CPU or eager fallback: calling forward on a non-CUDA / non-bf16 model raises.
 
 Per block (SURVEY.md §8a-S `STDiT3Block.forward`), 10 launches:

@@ -10,7 +10,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("OSB200_LIB", os.path.join(_HERE, "libosb200.so"))  # override: instrumented debug builds
+LIB_PATH = os.environ.get("OSB200_LIB", os.path.join(_HERE, "libosb200.so"))  # override: another build of the library
 
 # every symbol include/osb200.h declares (tests check the library exports all of them)
 EXPORTS = (
@@ -35,7 +35,6 @@ EXPORTS = (
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
-ATTN_IMPL = int(os.environ.get("OSB_ATTN_IMPL", "0"))  # experiment switch for osb_attn_short's implementation
 
 
 class OsbError(RuntimeError):
@@ -45,7 +44,7 @@ class OsbError(RuntimeError):
 def _load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise OsbError(
-            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "osb200 has no CPU or PyTorch fallback."
         )
     lib = C.CDLL(LIB_PATH)
@@ -200,7 +199,7 @@ def init(device: int | None = None) -> None:
     import torch
 
     if not torch.cuda.is_available():
-        raise OsbError("osb200 needs a CUDA device (sm_100a); there is no CPU path")
+        raise OsbError("osb200 needs a CUDA device (sm_90a); there is no CPU path")
     if device is None:
         device = torch.cuda.current_device()
     if device in _initialised_devices:
@@ -364,7 +363,7 @@ def attn_short(q, k, v, out, *, num_seqs: int, seqs_per_batch: int, q_strides, k
     a.k_norm_w2 = k_norm_w2.data_ptr() if k_norm_w2 is not None else None
     a.norm_split = norm_split
     a.rope_half = int(rope_half)
-    a.reserved = impl if impl else ATTN_IMPL  # 0 = library default; 1 resident keys, 2 flash (P via smem), 3 flash (P in TMEM), 4 ping-pong
+    a.reserved = impl   # implementation switch of the C ABI; every value runs the one sm_90a kernel
     with _Timed("attn_short", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):  # QK^T + PV FLOPs
         _check(_lib.osb_attn_short(C.byref(a), _stream()), "osb_attn_short")
     return out

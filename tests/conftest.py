@@ -10,7 +10,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a); run with -m gpu")
 
 
 import pytest

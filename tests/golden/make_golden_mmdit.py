@@ -8,12 +8,12 @@ The fixtures pin oracle/mmdit_oracle.py and the pieces oracle/stdit3_oracle.py s
 import os
 import sys
 
-import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 from oracle import ref_loader  # noqa: E402
+from tests.util import save_golden, seeded_init  # noqa: E402
 
 
 def ids_for(B, Lt, T, H, W):
@@ -40,19 +40,11 @@ def main():
     pe_liger = layers.LigerEmbedND(D, 10000, axes)(ids)
     out.update(img=img, txt=txt, vec=vec, ids=ids, pe_flux=pe_flux, pe_liger_cos=pe_liger[0], pe_liger_sin=pe_liger[1])
 
-    def randomize(m):
-        with torch.no_grad():
-            for n, p in m.named_parameters():
-                if n.endswith("scale"):
-                    p.copy_(1 + 0.2 * torch.randn_like(p))
-                elif p.dim() == 1:
-                    p.copy_(0.1 * torch.randn_like(p))
-
     with torch.no_grad():
         # --- small pieces -------------------------------------------------------------------------
         x = torch.randn(B, Hh, Li, D)
         rn = layers.RMSNorm(D)
-        randomize(rn)
+        seeded_init(rn, "rms")
         out.update(rms_x=x, rms_scale=rn.scale.detach(), rms_y=rn(x))
         out.update(rms_y_bf16=rn(x.bfloat16()).float())
         q, k = torch.randn(B, Hh, Lt + Li, D), torch.randn(B, Hh, Lt + Li, D)
@@ -66,17 +58,17 @@ def main():
         for fused in (True, False):
             tag = "fused" if fused else "split"
             blk = layers.DoubleStreamBlock(C, Hh, 4.0, qkv_bias=True, fused_qkv=fused)
-            randomize(blk)
+            seeded_init(blk, f"double_{tag}")
             oi, ot = blk(img, txt, vec, pe_flux)
             out.update({f"double_{tag}.{n}": p.detach() for n, p in blk.state_dict().items()})
             out.update({f"double_{tag}_out_img": oi, f"double_{tag}_out_txt": ot})
             sb = layers.SingleStreamBlock(C, Hh, 4.0, fused_qkv=fused)
-            randomize(sb)
+            seeded_init(sb, f"single_{tag}")
             xcat = torch.cat((txt, img), 1)
             out.update({f"single_{tag}.{n}": p.detach() for n, p in sb.state_dict().items()})
             out.update({f"single_{tag}_out": sb(xcat, vec, pe_flux)})
         ll = layers.LastLayer(C, 1, 16)
-        randomize(ll)
+        seeded_init(ll, "last")
         out.update({f"last.{n}": p.detach() for n, p in ll.state_dict().items()})
         out.update(last_out=ll(img, vec))
         # --- tiny full model (prepare_block_inputs + blocks + final layer), executed by the reference ---------
@@ -85,9 +77,7 @@ def main():
                    depth_single_blocks=1, axes_dim=axes, theta=10000, qkv_bias=True, guidance_embed=True, cond_embed=True,
                    fused_qkv=True)
         fm = model_m.Flux(device_map="cpu", torch_dtype=torch.float32, **cfg)
-        randomize(fm)
-        nn_init = torch.nn.init.normal_
-        nn_init(fm.cond_in.weight, std=0.05)
+        seeded_init(fm, "model")
         m_img, m_cond = torch.randn(B, Li, 8), torch.randn(B, Li, 12)
         m_txt, m_y = torch.randn(B, Lt, 20), torch.randn(B, 12)
         m_t, m_g = torch.tensor([0.3, 0.8]), torch.tensor([4.0, 7.5])
@@ -95,10 +85,9 @@ def main():
         m_out = fm(img=m_img, img_ids=img_ids, txt=m_txt, txt_ids=txt_ids, timesteps=m_t, y_vec=m_y, cond=m_cond, guidance=m_g)
         out.update({f"model.{n}": p.detach() for n, p in fm.state_dict().items()})
         out.update(model_img=m_img, model_cond=m_cond, model_txt=m_txt, model_y=m_y, model_t=m_t, model_g=m_g, model_out=m_out)
-    arrs = {k: v.detach().float().numpy().astype(np.float32) for k, v in out.items()}
     path = os.path.join(HERE, "mmdit_blocks.npz")
-    np.savez_compressed(path, **arrs)
-    print("wrote", path, os.path.getsize(path) // 1024, "KiB,", len(arrs), "arrays")
+    save_golden(path, out)
+    print("wrote", path, os.path.getsize(path) // 1024, "KiB,", len(out), "arrays")
 
 
 if __name__ == "__main__":

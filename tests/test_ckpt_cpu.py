@@ -7,6 +7,8 @@ import os
 
 import pytest
 import torch
+
+from tests.util import load_golden
 import torch.nn as nn
 from safetensors.torch import save_file
 
@@ -85,7 +87,7 @@ def test_model_factories_load_reference_keyed_checkpoints(tmp_path):
     from opensora.registry import MODELS, build_module
     from tests.test_mmdit_gpu import CFG
 
-    G = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(os.path.dirname(__file__), "golden", "vae_blocks.npz")).items()}
+    G = load_golden("vae_blocks.npz")
     kw = dict(type="hunyuan_vae", block_out_channels=(16, 32, 32, 32), layers_per_block=1, norm_num_groups=4, latent_channels=4)
     src = build_module(dict(kw), MODELS, device_map="cpu")
     src.encoder.load_state_dict({k[4:]: v for k, v in G.items() if k.startswith("enc.")})

@@ -1,6 +1,9 @@
 """Host-side logic of the MMDiT drop-in (`opensora/models/mmdit/{layers,model}.py`: processors, both QKV layouts, both RoPE
 layouts, modulation plumbing, the conditioning residual) on the CPU, through the stand-in of the binding, against the
 oracle that tests/test_oracle_cpu.py pins to the executed reference source."""
+import os
+
+import numpy as np
 import pytest
 import torch
 
@@ -77,22 +80,16 @@ def test_processor_hook_is_the_plugin_point(fake_osb):
     assert len(seen) == CFG["depth"] and out.shape == (1, 16, 64) and torch.isfinite(out.float()).all()
 
 
-@pytest.mark.parametrize("fused", [True, False])
-def test_processors_run_on_the_reference_own_blocks(fake_osb, fused):
-    """INTEGRATION.md 2: the processors are installed with `set_processor` on block objects built from the REFERENCE's
-    own source (`/root/reference/opensora/models/mmdit/layers.py`, executed by path) - classes that have only the
-    reference's attributes - and must reproduce what those blocks compute with their stock processors."""
-    from oracle import ref_loader
+TOKEN_STRIDE = 3   # tests/golden/ref_classes.npz keeps every third token of the reference outputs (float16)
 
-    if not ref_loader.available():
-        pytest.skip("reference checkout not present (GPU box)")
-    R, Rmath, _ = ref_loader.load_mmdit()
-    from opensora.models.mmdit.layers import DoubleStreamBlockProcessor, SingleStreamBlockProcessor
 
+def mmdit_block_case(L, fused):
+    """Seeded DoubleStreamBlock / SingleStreamBlock (C = 256, 2 heads) built from the layers module `L` (the reference's
+    mmdit/layers.py executed by path, or the in-tree mirror, which draws identical parameters) and their inputs."""
     torch.manual_seed(5)
     C, H, B, Lt, Li = 256, 2, 2, 24, 48
-    dbl = R.DoubleStreamBlock(C, H, mlp_ratio=4.0, qkv_bias=True, fused_qkv=fused).eval()
-    sgl = R.SingleStreamBlock(C, H, mlp_ratio=4.0, fused_qkv=fused).eval()
+    dbl = L.DoubleStreamBlock(C, H, mlp_ratio=4.0, qkv_bias=True, fused_qkv=fused).eval()
+    sgl = L.SingleStreamBlock(C, H, mlp_ratio=4.0, fused_qkv=fused).eval()
     with torch.no_grad():
         for blk in (dbl, sgl):
             for n, p in blk.named_parameters():
@@ -101,14 +98,29 @@ def test_processors_run_on_the_reference_own_blocks(fake_osb, fused):
     ids[:, Lt:, 0] = torch.arange(Li) // 16
     ids[:, Lt:, 1] = (torch.arange(Li) // 4) % 4
     ids[:, Lt:, 2] = torch.arange(Li) % 4
-    pe = R.EmbedND(dim=C // H, theta=10000, axes_dim=[16, 56, 56])(ids)
+    pe = L.EmbedND(dim=C // H, theta=10000, axes_dim=[16, 56, 56])(ids)
     bf = torch.bfloat16
     img, txt, vec = torch.randn(B, Li, C).to(bf), torch.randn(B, Lt, C).to(bf), torch.randn(B, C).to(bf)
+    return dbl, sgl, pe, img, txt, vec
+
+
+@pytest.mark.parametrize("fused", [True, False])
+def test_processors_run_on_the_reference_own_blocks(fake_osb, fused):
+    """INTEGRATION.md 2: the processors, installed with `set_processor` on blocks that carry only the reference's
+    attributes, must reproduce what the reference's own blocks (mmdit/layers.py, stock processors, fp32) compute on the
+    same seeded parameters and inputs (tests/golden/ref_classes.npz, made by tests/golden/make_golden_ref_classes.py,
+    which also checks that the in-tree blocks draw exactly the reference's parameters)."""
+    from opensora.models.mmdit import layers
+    from opensora.models.mmdit.layers import DoubleStreamBlockProcessor, SingleStreamBlockProcessor
+
+    G = np.load(os.path.join(os.path.dirname(__file__), "golden", "ref_classes.npz"))
+    tag = "fused" if fused else "split"
+    ref_i, ref_t, ref_x = (torch.from_numpy(G[f"mmdit_{tag}_{k}"]).float() for k in ("img", "txt", "single"))
+    rn = float(G[f"mmdit_{tag}_bf16_floor"])   # the reference's own bf16 path against its fp32 output
+    dbl, sgl, pe, img, txt, vec = mmdit_block_case(layers, fused)
+    bf = torch.bfloat16
     with torch.no_grad():
-        ref_i, ref_t = dbl(img.float(), txt.float(), vec.float(), pe)                  # stock processor, fp32
-        ref_x = sgl(torch.cat((txt, img), 1).float(), vec.float(), pe)
         dbl_b, sgl_b = dbl.to(bf), sgl.to(bf)
-        noise_i, _ = dbl_b(img, txt, vec, pe)                                          # the reference's own bf16 path
         dbl_b.set_processor(DoubleStreamBlockProcessor())
         sgl_b.set_processor(SingleStreamBlockProcessor())
         out_i, out_t = dbl_b(img, txt, vec, pe)
@@ -117,9 +129,9 @@ def test_processors_run_on_the_reference_own_blocks(fake_osb, fused):
         if not fused:
             sgl_b.q_proj.weight.mul_(1.0)
             sgl_b(torch.cat((txt, img), 1), vec, pe)
-    rn = rel_l2(noise_i.float(), ref_i)
     for got, ref in ((out_i, ref_i), (out_t, ref_t), (out_x, ref_x)):
-        r = rel_l2(got.float(), ref)
+        got = got[:, ::TOKEN_STRIDE].float()
+        r = rel_l2(got, ref)
         assert got.shape == ref.shape and r < max(2.0 * rn, 6e-3), (r, rn)
     names = [c[0] for c in fake_osb.calls]
     assert names.count("attn_short") == (2 if fused else 3) and "ln_modulate" in names

@@ -8,13 +8,13 @@ import numpy as np
 import pytest
 import torch
 
-from tests.util import rel_l2
+from tests.util import load_golden, rel_l2
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def _golden(name):
-    return {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", name)).items()}
+    return load_golden(name)
 
 
 def _model(G, **kw):
@@ -94,31 +94,35 @@ def test_causal_conv_is_causal_and_latent_size_api(fake_osb):
     assert list(z.shape) == [1, 4] + m.get_latent_size([9, 32, 32]) and rec.shape == v.shape and torch.equal(z, z2)
 
 
-def test_posterior_distribution_matches_the_reference_class():
-    """`DiagonalGaussianDistribution` (sample with a seeded generator, kl with and without a second distribution, nll, mode,
-    the deterministic switch, token-shaped parameters) against the reference's own class executed by path."""
-    from oracle import ref_loader
-
-    if not ref_loader.available():
-        pytest.skip("reference checkout not present (GPU box)")
-    _, Rvae = ref_loader.load_hunyuan_vae()
-    from opensora.models.hunyuan_vae.vae import DiagonalGaussianDistribution as Ours
-
+def posterior_inputs():
+    """Seeded (parameters, second parameters) pairs: 5-D latent, 4-D image and token-shaped distributions."""
     g = torch.Generator().manual_seed(5)
+    out = []
     for shape in ((2, 8, 3, 4, 5), (2, 8, 6, 7), (2, 9, 8)):
         par = torch.randn(*shape, generator=g) * 3.0
         par2 = torch.randn(*shape, generator=g)
-        a, b = Ours(par), Rvae.DiagonalGaussianDistribution(par)
-        a2, b2 = Ours(par2), Rvae.DiagonalGaussianDistribution(par2)
-        assert torch.equal(a.mode(), b.mode()) and torch.equal(a.std, b.std) and torch.equal(a.logvar, b.logvar)
+        out.append((par, par2))
+    return out
+
+
+def test_posterior_distribution_matches_the_reference_class():
+    """`DiagonalGaussianDistribution` (sample with a seeded generator, kl with and without a second distribution, nll, mode,
+    the deterministic switch, token-shaped parameters) against what the reference's own class computes on the same inputs
+    (tests/golden/ref_classes.npz, made by tests/golden/make_golden_ref_classes.py)."""
+    from opensora.models.hunyuan_vae.vae import DiagonalGaussianDistribution as Ours
+
+    G = np.load(os.path.join(os.path.dirname(__file__), "golden", "ref_classes.npz"))
+    for i, (par, par2) in enumerate(posterior_inputs()):
+        ref = lambda k: torch.from_numpy(G[f"posterior{i}_{k}"])  # noqa: E731
+        a, a2 = Ours(par), Ours(par2)
+        assert torch.equal(a.mode(), ref("mode")) and torch.equal(a.std, ref("std")) and torch.equal(a.logvar, ref("logvar"))
         sa = a.sample(torch.Generator().manual_seed(11))
-        sb = b.sample(torch.Generator().manual_seed(11))
-        assert torch.equal(sa, sb) and sa.shape == a.mean.shape
-        torch.testing.assert_close(a.kl(), b.kl(), rtol=1e-6, atol=1e-6)
-        torch.testing.assert_close(a.kl(a2), b.kl(b2), rtol=1e-6, atol=1e-6)
+        assert torch.equal(sa, ref("sample")) and sa.shape == a.mean.shape
+        torch.testing.assert_close(a.kl(), ref("kl"), rtol=1e-6, atol=1e-6)
+        torch.testing.assert_close(a.kl(a2), ref("kl2"), rtol=1e-6, atol=1e-6)
         if par.ndim >= 4:
             dims = list(range(1, par.ndim))
-            torch.testing.assert_close(a.nll(sa, dims), b.nll(sb, dims), rtol=1e-6, atol=1e-5)
+            torch.testing.assert_close(a.nll(sa, dims), ref("nll"), rtol=1e-6, atol=1e-5)
         d = Ours(par, deterministic=True)
         assert torch.equal(d.sample(), d.mean) and float(d.kl()) == 0.0 and float(d.nll(sa)) == 0.0
     with pytest.raises(NotImplementedError):

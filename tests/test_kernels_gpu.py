@@ -67,13 +67,33 @@ GEMM_SHAPES = [
 ]
 
 
+def _gemm(osb, *args, cta_group, **kw):
+    """cta_group is accepted for ABI compatibility and selects nothing on sm_90a: any value must give the bits of the
+    default."""
+    out = osb.gemm(*args, cta_group=cta_group, **kw)
+    if cta_group:
+        assert torch.equal(out, osb.gemm(*args, cta_group=0, **kw)), f"cta_group={cta_group} changed the result"
+    return out
+
+
+def _attn_short(osb, q, k, v, out, **kw):
+    """The implementation switch (osb_attn_short_args.reserved) selects nothing on sm_90a: any value must give the bits
+    of the default (rows the call does not write are carried over by the clone)."""
+    osb.attn_short(q, k, v, out, **kw)
+    if kw.get("impl", 0):
+        alt = out.clone()
+        osb.attn_short(q, k, v, alt, **{**kw, "impl": 0})
+        assert torch.equal(alt, out), f"impl={kw['impl']} changed the result"
+    return out
+
+
 @pytest.mark.parametrize("cta", [1, 2])
 @pytest.mark.parametrize("M,N,K", GEMM_SHAPES)
 def test_gemm_bias(osb, M, N, K, cta):
     a = _randn(M, K, seed=3)
     w = _randn(N, K, scale=K ** -0.5, seed=4)
     b = _randn(N, seed=5)
-    out = osb.gemm(a, w, b, cta_group=cta)
+    out = _gemm(osb, a, w, b, cta_group=cta)
     ref = a.float() @ w.float().t() + b.float()
     r, _ = report(f"gemm bias {M}x{N}x{K} cta{cta}", out, ref)
     assert r < BF16_ONE_ROUNDING_REL_L2
@@ -85,7 +105,7 @@ def test_gemm_block_n(osb, bn, cta):
     M, N, K = 777, 1152, 1152
     a = _randn(M, K, seed=6)
     w = _randn(N, K, scale=K ** -0.5, seed=7)
-    out = osb.gemm(a, w, None, cta_group=cta, block_n=bn)
+    out = _gemm(osb, a, w, None, cta_group=cta, block_n=bn)
     ref = a.float() @ w.float().t()
     r, _ = report(f"gemm bn{bn} cta{cta}", out, ref)
     assert r < BF16_ONE_ROUNDING_REL_L2
@@ -97,7 +117,7 @@ def test_gemm_gelu(osb, cta):
     a = _randn(M, K, seed=8)
     w = _randn(N, K, scale=K ** -0.5, seed=9)
     b = _randn(N, seed=10)
-    out = osb.gemm(a, w, b, epilogue=osb.EPI_BIAS_GELU_TANH, cta_group=cta)
+    out = _gemm(osb, a, w, b, epilogue=osb.EPI_BIAS_GELU_TANH, cta_group=cta)
     ref = torch.nn.functional.gelu(a.float() @ w.float().t() + b.float(), approximate="tanh")
     r, _ = report(f"gemm gelu cta{cta}", out, ref)
     assert r < BF16_ONE_ROUNDING_REL_L2
@@ -112,7 +132,7 @@ def test_gemm_gate_residual(osb, cta, use_gate):
     b = _randn(N, seed=13)
     res = _randn(M, N, seed=14)
     gate = torch.randn(M // group, N, device="cuda") if use_gate else None
-    out = osb.gemm(a, w, b, epilogue=osb.EPI_BIAS_GATE_RES, residual=res, gate=gate, group_rows=group, cta_group=cta)
+    out = _gemm(osb, a, w, b, epilogue=osb.EPI_BIAS_GATE_RES, residual=res, gate=gate, group_rows=group, cta_group=cta)
     lin = a.float() @ w.float().t() + b.float()
     if use_gate:
         lin = lin * gate[torch.arange(M, device="cuda") // group]
@@ -137,14 +157,14 @@ def test_gemm_inplace_residual_and_strided_a(osb):
 
 
 def test_gemm_large_persistent(osb):
-    # many tiles per CTA: exercises the smem ring wrap, both TMEM accumulator stages and phases
+    # many k-blocks per tile: exercises the smem ring wrap and both mbarrier phases
     M, N, K = 16384, 1152, 1152
     a = _randn(M, K, seed=18)
     w = _randn(N, K, scale=K ** -0.5, seed=19)
     b = _randn(N, seed=20)
     ref = a.float() @ w.float().t() + b.float()
     for cta in (1, 2):
-        out = osb.gemm(a, w, b, cta_group=cta)
+        out = _gemm(osb, a, w, b, cta_group=cta)
         r, _ = report(f"gemm large cta{cta}", out, ref)
         assert r < BF16_ONE_ROUNDING_REL_L2
 
@@ -179,7 +199,7 @@ def _rope_tables(L, D):
     return ang.cos().contiguous(), ang.sin().contiguous()
 
 
-IMPLS = [1, 2, 3, 4]  # resident keys, flash with P through smem, flash with P in TMEM, two-slot ping-pong
+IMPLS = [1, 2, 3, 4]  # values of the implementation switch (osb_attn_short_args.reserved): see _attn_short
 
 
 @pytest.mark.parametrize("impl", IMPLS)
@@ -199,14 +219,14 @@ def test_attn_self(osb, D, H, mode, impl):
     q2, k2, v2 = qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:]
     if mode == "spatial":
         strides = (N, S, 1)
-        osb.attn_short(q2, k2, v2, out, num_seqs=B * T, seqs_per_batch=T, q_strides=strides, k_strides=strides,
+        _attn_short(osb, q2, k2, v2, out, num_seqs=B * T, seqs_per_batch=T, q_strides=strides, k_strides=strides,
                        Lq=S, Lk=S, num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, impl=impl)
         x = qkv.float().view(B * T, S, 3, H, D).permute(2, 0, 3, 1, 4)
         ref = _attn_ref(x[0], x[1], x[2], qw, kw, None, None, D ** -0.5)       # [B*T, H, S, D]
         ref = ref.permute(0, 2, 1, 3).reshape(B * N, C)
     else:
         strides = (N, 1, S)
-        osb.attn_short(q2, k2, v2, out, num_seqs=B * S, seqs_per_batch=S, q_strides=strides, k_strides=strides,
+        _attn_short(osb, q2, k2, v2, out, num_seqs=B * S, seqs_per_batch=S, q_strides=strides, k_strides=strides,
                        Lq=T, Lk=T, num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, rope_cos=cos, rope_sin=sin, impl=impl)
         x = qkv.float().view(B, T, S, 3, H, D).permute(3, 0, 2, 4, 1, 5).reshape(3, B * S, H, T, D)
         ref = _attn_ref(x[0], x[1], x[2], qw, kw, cos, sin, D ** -0.5)          # [B*S, H, T, D]
@@ -224,7 +244,7 @@ def test_attn_cross(osb, Ly, impl):
     kv = _randn(B * Ly, 2 * C, seed=25)
     lens = torch.tensor([Ly, max(1, Ly // 3)], device="cuda", dtype=torch.int32)
     out = torch.zeros(B * N, C, dtype=torch.bfloat16, device="cuda")
-    osb.attn_short(q, kv[:, :C], kv[:, C:], out, num_seqs=B, seqs_per_batch=1, q_strides=(N, 0, 1),
+    _attn_short(osb, q, kv[:, :C], kv[:, C:], out, num_seqs=B, seqs_per_batch=1, q_strides=(N, 0, 1),
                    k_strides=(Ly, 0, 1), Lq=N, Lk=Ly, num_heads=H, head_dim=D, kv_lens=lens, impl=impl)
     qf = q.float().view(B, N, H, D).permute(0, 2, 1, 3)
     kvf = kv.float().view(B, Ly, 2, H, D).permute(2, 0, 3, 1, 4)
@@ -238,7 +258,7 @@ def test_attn_cross(osb, Ly, impl):
 @pytest.mark.parametrize("T,S", [(4, 24), (3, 40), (5, 7)])
 def test_attn_packed_ragged(osb, T, S, impl):
     """Short sequences packed G per 128-row tile where G*L < 128 and rows of one warp belong to different sequences
-    (XS parity shapes: S=24 -> G=5): block-diagonal masking must not make warp-collective TMEM accesses diverge."""
+    (XS parity shapes: S=24 -> G=5): block-diagonal masking must not make warp-collective loads or shuffles diverge."""
     B, H, D = 2, 4, 72
     C, N = H * D, T * S
     qkv = _randn(B * N, 3 * C, seed=41)
@@ -248,14 +268,14 @@ def test_attn_packed_ragged(osb, T, S, impl):
         out = torch.zeros(B * N, C, dtype=torch.bfloat16, device="cuda")
         if mode == "spatial":
             st = (N, S, 1)
-            osb.attn_short(q2, k2, v2, out, num_seqs=B * T, seqs_per_batch=T, q_strides=st, k_strides=st, Lq=S, Lk=S,
+            _attn_short(osb, q2, k2, v2, out, num_seqs=B * T, seqs_per_batch=T, q_strides=st, k_strides=st, Lq=S, Lk=S,
                            num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, impl=impl)
             x = qkv.float().view(B * T, S, 3, H, D).permute(2, 0, 3, 1, 4)
             ref = _attn_ref(x[0], x[1], x[2], qw, kw, None, None, D ** -0.5).permute(0, 2, 1, 3).reshape(B * N, C)
         else:
             cos, sin = _rope_tables(T, D)
             st = (N, 1, S)
-            osb.attn_short(q2, k2, v2, out, num_seqs=B * S, seqs_per_batch=S, q_strides=st, k_strides=st, Lq=T, Lk=T,
+            _attn_short(osb, q2, k2, v2, out, num_seqs=B * S, seqs_per_batch=S, q_strides=st, k_strides=st, Lq=T, Lk=T,
                            num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, rope_cos=cos, rope_sin=sin, impl=impl)
             x = qkv.float().view(B, T, S, 3, H, D).permute(3, 0, 2, 4, 1, 5).reshape(3, B * S, H, T, D)
             ref = _attn_ref(x[0], x[1], x[2], qw, kw, cos, sin, D ** -0.5)
@@ -279,7 +299,7 @@ def test_attn_pingpong_many_sets(osb, mode, big_logits):
         kv = _randn(B * Ly, 2 * C, seed=32)
         lens = torch.tensor([260, 300], device="cuda", dtype=torch.int32)
         out = torch.zeros(B * N, C, dtype=torch.bfloat16, device="cuda")
-        osb.attn_short(q, kv[:, :C], kv[:, C:], out, num_seqs=B, seqs_per_batch=1, q_strides=(N, 0, 1),
+        _attn_short(osb, q, kv[:, :C], kv[:, C:], out, num_seqs=B, seqs_per_batch=1, q_strides=(N, 0, 1),
                        k_strides=(Ly, 0, 1), Lq=N, Lk=Ly, num_heads=H, head_dim=D, kv_lens=lens, impl=4)
         qf = q.float().view(B, N, H, D).permute(0, 2, 1, 3)
         kvf = kv.float().view(B, Ly, 2, H, D).permute(2, 0, 3, 1, 4)
@@ -293,14 +313,14 @@ def test_attn_pingpong_many_sets(osb, mode, big_logits):
         q2, k2, v2 = qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:]
         if mode == "spatial":
             st = (N, S, 1)
-            osb.attn_short(q2, k2, v2, out, num_seqs=B * T, seqs_per_batch=T, q_strides=st, k_strides=st, Lq=S, Lk=S,
+            _attn_short(osb, q2, k2, v2, out, num_seqs=B * T, seqs_per_batch=T, q_strides=st, k_strides=st, Lq=S, Lk=S,
                            num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, impl=4)
             x = qkv.float().view(B * T, S, 3, H, D).permute(2, 0, 3, 1, 4)
             ref = _attn_ref(x[0], x[1], x[2], qw, kw, None, None, D ** -0.5).permute(0, 2, 1, 3).reshape(B * N, C)
         else:
             cos, sin = _rope_tables(T, D)
             st = (N, 1, S)
-            osb.attn_short(q2, k2, v2, out, num_seqs=B * S, seqs_per_batch=S, q_strides=st, k_strides=st, Lq=T, Lk=T,
+            _attn_short(osb, q2, k2, v2, out, num_seqs=B * S, seqs_per_batch=S, q_strides=st, k_strides=st, Lq=T, Lk=T,
                            num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, rope_cos=cos, rope_sin=sin, impl=4)
             x = qkv.float().view(B, T, S, 3, H, D).permute(3, 0, 2, 4, 1, 5).reshape(3, B * S, H, T, D)
             ref = _attn_ref(x[0], x[1], x[2], qw, kw, cos, sin, D ** -0.5)
@@ -321,7 +341,7 @@ def test_attn_long_sequence(osb, D, impl):
     cos, sin = _rope_tables(L, D)
     out = torch.zeros(nseq * L, C, dtype=torch.bfloat16, device="cuda")
     split = 100
-    osb.attn_short(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out, num_seqs=nseq, seqs_per_batch=1, q_strides=(L, 0, 1),
+    _attn_short(osb, qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out, num_seqs=nseq, seqs_per_batch=1, q_strides=(L, 0, 1),
                    k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H, head_dim=D, q_norm_w=qw, k_norm_w=kw, q_norm_w2=qw2,
                    k_norm_w2=kw2, norm_split=split, rope_cos=cos, rope_sin=sin, impl=impl)
     x = qkv.float().view(nseq, L, 3, H, D).permute(2, 0, 3, 1, 4)
@@ -344,7 +364,7 @@ def test_attn_ragged_tail(osb):
     for (nseq, L) in [(5, 48), (3, 200)]:
         qkv = _randn(nseq * L, 3 * C, seed=26)
         out = torch.zeros(nseq * L, C, dtype=torch.bfloat16, device="cuda")
-        osb.attn_short(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out, num_seqs=nseq, seqs_per_batch=nseq,
+        _attn_short(osb, qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out, num_seqs=nseq, seqs_per_batch=nseq,
                        q_strides=(0, L, 1), k_strides=(0, L, 1), Lq=L, Lk=L, num_heads=H, head_dim=D)
         x = qkv.float().view(nseq, L, 3, H, D).permute(2, 0, 3, 1, 4)
         ref = _attn_ref(x[0], x[1], x[2], None, None, None, None, D ** -0.5).permute(0, 2, 1, 3).reshape(nseq * L, C)

@@ -13,11 +13,13 @@ import numpy as np
 import pytest
 import torch
 
+from tests.util import load_golden
+
 from oracle import mmdit_oracle as M
 from oracle import stdit3_oracle as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-G = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", "mmdit_blocks.npz")).items()}
+G = load_golden("mmdit_blocks.npz")
 C, H, AXES = 64, 2, [8, 12, 12]
 TOL = dict(rtol=2e-5, atol=2e-5)
 
@@ -167,7 +169,7 @@ def test_bench_auxiliary_legs_fail_soft():
 # ---- causal 3D VAE oracle pinned by reference-executed goldens --------------------------------------
 from oracle import vae_oracle as V  # noqa: E402
 
-GV = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", "vae_blocks.npz")).items()}
+GV = load_golden("vae_blocks.npz")
 VTOL = dict(rtol=1e-4, atol=1e-4)
 
 
@@ -224,7 +226,7 @@ def test_mmdit_full_model_matches_reference():
 @pytest.mark.parametrize("tag,sp,tp", [("none", False, False), ("spatial", True, False), ("temporal", False, True), ("both", True, True)])
 def test_tiled_autoencoder_matches_reference(tag, sp, tp):
     """autoencoder_kl_causal_3d.py:269-358,384-552 executed by the reference (tests/golden/make_golden_vae_tiled.py)."""
-    GT = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", "vae_tiled.npz")).items()}
+    GT = load_golden("vae_tiled.npz")
     down, up = V.stage_plan(4, 4, 8)
     We, Wd = _wv("enc"), _wv("dec")
     enc_fn = lambda x: V.causal_conv3d(V.encoder(We, x, groups=4, strides=down), GT["quant_w"], GT["quant_b"])  # noqa: E731

@@ -5,7 +5,7 @@ Tolerance (north_star: 'within 1e-3 rel of the reference', made meaningful for b
 hard part 2): the product rounds the residual stream and every GEMM output to bf16 exactly where the
 reference's own bf16 path does, so its error vs the fp32 oracle must not exceed the error of the
 oracle itself run in bf16 (the reference-precision noise floor, measured in the same test) by more
-than 1.1x (measured ratios 0.77 - 0.97, profiles/r02_parity_report.txt), and must stay below an absolute
+than 1.1x, and must stay below an absolute
 1.5e-2 (depth 2) / 3e-2 (depth 28) rel-L2."""
 import pytest
 import torch
@@ -41,7 +41,6 @@ def test_xs_parity(B, T, H, W):
     rn = rel_l2(noise, ref)
     print(f"[parity] oracle-in-bf16 noise floor rel_l2={rn:.3e}")
     assert out.shape == ref.shape
-    # measured 7.4e-3 / 7.6e-3 against the oracle's own bf16 error 9.6e-3 / 9.4e-3 (profiles/r02_parity_report.txt)
     assert r < 1.5e-2 and r < 1.1 * rn
 
 

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.util import report
+from tests.util import load_golden, report
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -140,7 +140,7 @@ def test_encoder_decoder_against_reference_goldens(osb):
     reproduce it within bf16 tolerance."""
     from opensora.registry import MODELS, build_module
 
-    G = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", "vae_blocks.npz")).items()}
+    G = load_golden("vae_blocks.npz")
     m = build_module(dict(type="hunyuan_vae", block_out_channels=(16, 32, 32, 32), layers_per_block=1, norm_num_groups=4,
                           latent_channels=4), MODELS, device_map="cpu")
     m.encoder.load_state_dict({k[4:]: v for k, v in G.items() if k.startswith("enc.")})
@@ -204,8 +204,8 @@ def test_tiled_modes_against_reference_goldens(osb, tag, sp, tp):
     from oracle import vae_oracle as V
     from tests.util import rel_l2
 
-    G = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", "vae_blocks.npz")).items()}
-    GT = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, "golden", "vae_tiled.npz")).items()}
+    G = load_golden("vae_blocks.npz")
+    GT = load_golden("vae_tiled.npz")
     m = build_module(dict(type="hunyuan_vae", block_out_channels=(16, 32, 32, 32), layers_per_block=1, norm_num_groups=4,
                           latent_channels=4, sample_size=32, sample_tsize=8, use_spatial_tiling=sp, use_temporal_tiling=tp),
                      MODELS, device_map="cpu")
@@ -232,5 +232,4 @@ def test_tiled_modes_against_reference_goldens(osb, tag, sp, tp):
     ry, _ = report(f"tiled decode [{tag}]", y, GT[f"y_{tag}"].cuda())
     print(f"[parity] reference-in-bf16 noise floor: encode {zf:.3e} decode {yf:.3e}")
     assert z.shape == GT[f"z_{tag}"].shape and y.shape == GT[f"y_{tag}"].shape
-    # measured: encode 0.71 - 0.96 of the reference-in-bf16 floor, decode 0.66 - 0.78 (profiles/r02_parity_report.txt)
     assert rz < 1.1 * zf and ry < yf

@@ -1,5 +1,5 @@
-"""VAE leg of BASELINE.json's metric: encode / decode fps of the causal 3D VAE on a synthetic 65x720x1280 video
-(configs[2]), untiled, bf16, 1 B200.  Also usable at reduced sizes: python tests/vae_bench.py T H W [iters]."""
+"""VAE leg of BASELINE.json's metric: encode / decode fps of the causal 3D VAE on a synthetic video (bench.py runs
+33x720x1280: untiled, bf16, one H100).  Usable at any size: python tests/vae_bench.py T H W [iters]."""
 import json
 import os
 import sys
