@@ -290,6 +290,24 @@ int osb_vae_prep(const osb_vae_prep_args* args, void* stream);
 int osb_cfg_euler(const void* cond, const void* uncond, const void* uncond2, const void* x, void* out, int64_t n,
                   float g_txt, float g_img, const void* g_img_map, int64_t map_period, float dt, void* stream);
 
+/* Frame-masked step of image / video conditioning (Open-Sora v1.2 RFLOW.sample, mask branch; parity unpinned): the end
+ * of sampling step i fused with the start of step i + 1, in one pass over x.  N = num_timesteps; per frame (b, f) with
+ * m = frame_mask[b, f] * N (1 = generate, 0 = keep the reference, in between = edit ratio):
+ *   update:  m >= t_cur[b]  -> x' = x + dt * (uncond + guidance * (cond - uncond)),  dt = (t_cur[b] - t_next[b]) * (1/N)
+ *            (the fp32 expression of osb_cfg_euler's two-branch mode, and dt as torch computes (t_cur - t_next) / N on
+ *            the GPU: an all-ones mask gives the bits of osb_cfg_euler called with that dt);
+ *            otherwise x' = x, bit for bit.  update == 0 (prologue, launched once before the first model call): x' = x.
+ *   re-noise (noise != NULL): prev = update ? (m >= t_cur[b]) : (frame_mask[b, f] == 1);
+ *            m >= t_next[b] && !prev -> out = (1 - a) * x' + a * noise, a = t_next[b] * (1/N);  otherwise out = x'.
+ * cond, uncond, x, noise, out: bf16 [B, C, T, H*W] contiguous, 16-byte aligned; out may alias x.  cond / uncond may be
+ * NULL when update == 0; noise may be NULL when update != 0.  frame_mask: fp32 [B, T]; t_cur, t_next: DEVICE fp32 [B]
+ * (per-sample schedules in one launch, no host synchronisation: the call is graph-capturable and a replay reads the
+ * current contents).  fp32 math, one rounding per element.  Any H*W (16-byte vectors when H*W % 8 == 0).
+ * Replaces the torch add_noise / where / CFG / Euler ops of each step of v1.2 schedulers/rf/__init__.py::RFLOW.sample. */
+int osb_rf_masked_step(const void* cond, const void* uncond, const void* x, const void* noise, void* out,
+                       const float* frame_mask, const float* t_cur, const float* t_next, int32_t B, int32_t C, int32_t T,
+                       int64_t HW, float guidance, int32_t num_timesteps, int32_t update, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

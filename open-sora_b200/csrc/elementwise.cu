@@ -220,6 +220,13 @@ extern "C" int osb_comm_barrier(const osb_comm_barrier_args* a, void* stream) {
 // Replaces opensora/utils/sampling.py:204-222 (I2VDenoiser.denoise update).  HBM bound: 5 tensors x 2 B/element.
 // ------------------------------------------------------------------------------------------------------------
 namespace osb {
+// The combine + Euler arithmetic of one element, shared by osb_cfg_euler and osb_rf_masked_step so that the two produce
+// bit-identical latents for the same inputs (the same fp32 expression, contracted the same way).
+__device__ __forceinline__ float cfg_euler_elem(float c, float u, float u2, float gi, float g_txt, float x, float dt) {
+  const float p = u2 + gi * (u - u2) + g_txt * (c - u);
+  return x + dt * p;
+}
+
 __global__ void __launch_bounds__(256)
 cfg_euler_kernel(const uint4* __restrict__ c, const uint4* __restrict__ u, const uint4* __restrict__ u2,
                  const uint4* __restrict__ x, uint4* __restrict__ out, int64_t nvec, float g_txt, float g_img,
@@ -237,9 +244,8 @@ cfg_euler_kernel(const uint4* __restrict__ c, const uint4* __restrict__ u, const
       const float2 cf = unpack_bf16x2(cw[e]), uf = unpack_bf16x2(uw[e]), vf = unpack_bf16x2(vw[e]), xf = unpack_bf16x2(xw[e]);
       float2 gi = make_float2(g_img, g_img);
       if (g_map) gi = unpack_bf16x2(gw[e]);
-      const float p0 = vf.x + gi.x * (uf.x - vf.x) + g_txt * (cf.x - uf.x);
-      const float p1 = vf.y + gi.y * (uf.y - vf.y) + g_txt * (cf.y - uf.y);
-      ow[e] = pack_bf16x2(xf.x + dt * p0, xf.y + dt * p1);
+      ow[e] = pack_bf16x2(cfg_euler_elem(cf.x, uf.x, vf.x, gi.x, g_txt, xf.x, dt),
+                          cfg_euler_elem(cf.y, uf.y, vf.y, gi.y, g_txt, xf.y, dt));
     }
     out[i] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
   }
@@ -264,6 +270,132 @@ extern "C" int osb_cfg_euler(const void* cond, const void* uncond, const void* u
       static_cast<const uint4*>(cond), static_cast<const uint4*>(uncond), static_cast<const uint4*>(uncond2),
       static_cast<const uint4*>(x), static_cast<uint4*>(out), nvec, g_txt, g_img, static_cast<const uint4*>(g_img_map),
       g_img_map ? map_period / 8 : 1, dt);
+  OSB_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return OSB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// osb_rf_masked_step: the frame-masked rectified-flow step of image / video conditioning (Open-Sora v1.2 RFLOW.sample,
+// mask branch) in ONE pass over the latent: the end of step i (combine + Euler update of the frames being generated)
+// fused with the start of step i + 1 (re-noising of the frames whose edit ratio the schedule has just reached).
+// Per frame (b, f), with m = frame_mask[b, f] * N:
+//   upd     = update && m >= t_cur[b]                     z' = upd ? z + dt * (vu + g (vc - vu)) : z   (dt = (t_cur - t_next) * (1/N))
+//   prev    = update ? upd : frame_mask[b, f] == 1
+//   renoise = noise && m >= t_next[b] && !prev            out = renoise ? (1 - a) z' + a noise : z'    (a = t_next * (1/N))
+// A frame is never both updated and re-noised in one pass, so every output element is rounded once.  Frames left alone
+// are copied bit for bit (in place: not written at all).  HBM bound: up to 5 tensors x 2 B/element.
+// ------------------------------------------------------------------------------------------------------------
+namespace osb {
+struct MaskedFrame {
+  bool upd, renoise;
+  float dt, a;
+};
+
+__device__ __forceinline__ MaskedFrame masked_frame(int64_t row, int T, int64_t CT, const float* __restrict__ fm,
+                                                    const float* __restrict__ tc, const float* __restrict__ tn, float N,
+                                                    bool update, bool has_noise) {
+  const int64_t b = row / CT;
+  const float mv = __ldg(fm + b * T + row % T);
+  const float m = mv * N;
+  const float t0 = __ldg(tc + b), t1 = __ldg(tn + b);
+  MaskedFrame r;
+  r.upd = update && m >= t0;
+  const bool prev = update ? r.upd : mv == 1.0f;
+  r.renoise = has_noise && m >= t1 && !prev;
+  r.dt = (t0 - t1) * (1.0f / N);   // torch's (t_cur - t_next) / N on the GPU: the t2v loop's dt, to the bit
+  r.a = t1 * (1.0f / N);
+  return r;
+}
+
+__device__ __forceinline__ float renoise_elem(float x, float n, float a) { return (1.0f - a) * x + a * n; }
+
+// kVec: 8 elements (one uint4) per unit, H*W % 8 == 0 so a unit never straddles two frames; else one element per unit
+template <bool kVec>
+__global__ void __launch_bounds__(256)
+rf_masked_step_kernel(const __nv_bfloat16* __restrict__ c, const __nv_bfloat16* __restrict__ u, const __nv_bfloat16* x,
+                      const __nv_bfloat16* __restrict__ noise, __nv_bfloat16* out, const float* __restrict__ fm,
+                      const float* __restrict__ tc, const float* __restrict__ tn, int64_t units, int64_t units_per_row,
+                      int T, int64_t CT, float g, float N, int update) {
+  pdl_wait();
+  const bool in_place = out == x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < units; i += (int64_t)gridDim.x * blockDim.x) {
+    const MaskedFrame f = masked_frame(i / units_per_row, T, CT, fm, tc, tn, N, update != 0, noise != nullptr);
+    if (in_place && !f.upd && !f.renoise) continue;
+    if constexpr (kVec) {
+      const uint4 xv = reinterpret_cast<const uint4*>(x)[i];
+      uint4 ov = xv;
+      const uint32_t xw[4] = {xv.x, xv.y, xv.z, xv.w};
+      uint32_t ow[4];
+      if (f.upd) {
+        const uint4 cv = reinterpret_cast<const uint4*>(c)[i], uv = reinterpret_cast<const uint4*>(u)[i];
+        const uint32_t cw[4] = {cv.x, cv.y, cv.z, cv.w}, uw[4] = {uv.x, uv.y, uv.z, uv.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 cf = unpack_bf16x2(cw[e]), uf = unpack_bf16x2(uw[e]), xf = unpack_bf16x2(xw[e]);
+          ow[e] = pack_bf16x2(cfg_euler_elem(cf.x, uf.x, uf.x, 1.0f, g, xf.x, f.dt),
+                              cfg_euler_elem(cf.y, uf.y, uf.y, 1.0f, g, xf.y, f.dt));
+        }
+        ov = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      } else if (f.renoise) {
+        const uint4 nv = reinterpret_cast<const uint4*>(noise)[i];
+        const uint32_t nw[4] = {nv.x, nv.y, nv.z, nv.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 nf = unpack_bf16x2(nw[e]), xf = unpack_bf16x2(xw[e]);
+          ow[e] = pack_bf16x2(renoise_elem(xf.x, nf.x, f.a), renoise_elem(xf.y, nf.y, f.a));
+        }
+        ov = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      }
+      reinterpret_cast<uint4*>(out)[i] = ov;
+    } else {
+      __nv_bfloat16 o = x[i];
+      if (f.upd) {
+        const float uf = __bfloat162float(u[i]);
+        o = __float2bfloat16_rn(cfg_euler_elem(__bfloat162float(c[i]), uf, uf, 1.0f, g, __bfloat162float(o), f.dt));
+      } else if (f.renoise) {
+        o = __float2bfloat16_rn(renoise_elem(__bfloat162float(o), __bfloat162float(noise[i]), f.a));
+      }
+      out[i] = o;
+    }
+  }
+}
+}  // namespace osb
+
+extern "C" int osb_rf_masked_step(const void* cond, const void* uncond, const void* x, const void* noise, void* out,
+                                  const float* frame_mask, const float* t_cur, const float* t_next, int32_t B, int32_t C,
+                                  int32_t T, int64_t HW, float guidance, int32_t num_timesteps, int32_t update, void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(x && out && frame_mask && t_cur && t_next, "osb_rf_masked_step: null tensor");
+  OSB_REQUIRE(!update || (cond && uncond), "osb_rf_masked_step: the update needs cond and uncond");
+  OSB_REQUIRE(update || noise, "osb_rf_masked_step: without the update there must be noise to add");
+  OSB_REQUIRE(B > 0 && C > 0 && T > 0 && HW > 0, "osb_rf_masked_step: B, C, T, H*W must be positive");
+  OSB_REQUIRE(num_timesteps > 0, "osb_rf_masked_step: num_timesteps must be positive");
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(cond) | reinterpret_cast<uintptr_t>(uncond) | reinterpret_cast<uintptr_t>(x) |
+                reinterpret_cast<uintptr_t>(noise) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+              "osb_rf_masked_step: bf16 tensors must be 16-byte aligned");
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(frame_mask) | reinterpret_cast<uintptr_t>(t_cur) |
+                reinterpret_cast<uintptr_t>(t_next)) & 3) == 0,
+              "osb_rf_masked_step: fp32 tensors must be 4-byte aligned");
+  const bool vec = HW % 8 == 0;
+  const int64_t CT = (int64_t)C * T;
+  const int64_t units_per_row = vec ? HW / 8 : HW;
+  const int64_t units = (int64_t)B * CT * units_per_row;
+  int64_t blocks = (units + 255) / 256;
+  if (blocks > (int64_t)sm_count() * 16) blocks = (int64_t)sm_count() * 16;
+  const auto* cb = static_cast<const __nv_bfloat16*>(cond);
+  const auto* ub = static_cast<const __nv_bfloat16*>(uncond);
+  const auto* xb = static_cast<const __nv_bfloat16*>(x);
+  const auto* nb = static_cast<const __nv_bfloat16*>(noise);
+  auto* ob = static_cast<__nv_bfloat16*>(out);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (vec)
+    rf_masked_step_kernel<true><<<(unsigned)blocks, 256, 0, s>>>(cb, ub, xb, nb, ob, frame_mask, t_cur, t_next, units,
+                                                                 units_per_row, T, CT, guidance, (float)num_timesteps, update);
+  else
+    rf_masked_step_kernel<false><<<(unsigned)blocks, 256, 0, s>>>(cb, ub, xb, nb, ob, frame_mask, t_cur, t_next, units,
+                                                                  units_per_row, T, CT, guidance, (float)num_timesteps, update);
   OSB_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return OSB_OK;

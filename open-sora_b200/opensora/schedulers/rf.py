@@ -5,8 +5,16 @@ MMDiT sampler, mirrored in `opensora/utils/sampling.py`); this is the restatemen
 
 Per step: the latent is doubled (conditional | null-caption branch, "CFG batch 2"), the model predicts a velocity (its first
 `out_channels / 2` channels when `pred_sigma`), `v = v_u + s (v_c - v_u)`, `z += v * (t_i - t_{i+1}) / 1000`.  The combine +
-Euler update is ONE `osb_cfg_euler` launch (two-branch mode).  Text-to-video only: the v1.2 image / video conditioning (`mask`:
-per-frame re-noising schedule) is not restated."""
+Euler update is ONE `osb_cfg_euler` launch (two-branch mode).
+
+Image / video conditioning (v1.2 `mask` argument, here `frame_mask` [B, T]: 1 = generate, 0 = keep the reference written into
+`z`, in between = edit ratio; built by `opensora.utils.inference_utils.apply_mask_strategy`), also restated and **parity
+unpinned** (self-consistent with `tests/rf_conditioning_ref.py::rflow_sample_masked`).  Frame f of sample b takes part in step i
+when `frame_mask * 1000 >= t_i` (the model gets that as `x_mask`, so kept frames are modulated with timestep 0); other frames
+keep their values bit for bit.  A frame with edit ratio e stays the reference while t > e * 1000 and is re-noised once, at
+the first t_i <= e * 1000, to (1 - t_i/1000) z + (t_i/1000) noise (SDEdit).  One noise tensor is drawn per step, as upstream's
+`randn_like`.  Each step's update and the next step's re-noise are ONE `osb_rf_masked_step` launch (plus one re-noise-only
+launch before the first step); the schedule stays on the device, so the loop never synchronises with the host."""
 from __future__ import annotations
 
 import torch
@@ -44,10 +52,13 @@ class RFLOW:
         return ts
 
     def sample(self, model, z: torch.Tensor, y: torch.Tensor, y_null: torch.Tensor, mask=None, additional_args: dict | None = None,
-               guidance_scale: float | None = None, progress: bool = False) -> torch.Tensor:
+               guidance_scale: float | None = None, progress: bool = False, frame_mask: torch.Tensor | None = None,
+               generator: torch.Generator | None = None) -> torch.Tensor:
         """z [B, C, T, H, W] noise (bf16 on the model's device), y [B, 1, L, D] caption embeddings, y_null the null caption
         (`model.y_embedder.y_embedding` broadcast, as upstream's `text_encoder.null`), mask [B, L] caption mask.  Extra model
-        inputs (fps, height, width, num_frames) ride in `additional_args`.  Returns the denoised latent."""
+        inputs (fps, height, width, num_frames) ride in `additional_args`.  Returns the denoised latent.
+        frame_mask [B, T] (upstream's `mask`): conditioned sampling, see the module docstring; the reference latents must
+        already be in `z`.  `generator` draws its per-step noise (default: torch's global generator for z's device)."""
         import osb200
 
         s = self.cfg_scale if guidance_scale is None else guidance_scale
@@ -60,6 +71,8 @@ class RFLOW:
             args["mask"] = torch.cat((mask, mask), 0)   # upstream passes the caption mask unchanged to both branches
         ts = self.schedule(B, z.device, additional_args)
         z = z.contiguous()
+        if frame_mask is not None:
+            return self._sample_masked(osb200, model, z, args, ts, frame_mask, float(s), generator)
         for i, t in enumerate(ts):
             pred = model(torch.cat((z, z), 0), torch.cat((t, t), 0), **args)
             pred = pred.chunk(2, dim=1)[0]                                   # drop the sigma half (pred_sigma)
@@ -71,4 +84,26 @@ class RFLOW:
                                for b in range(B)], 0)
             else:
                 z = osb200.cfg_euler(vc, vu, None, z, g_txt=float(s), dt=float(dt[0]))
+        return z
+
+    def _sample_masked(self, osb200, model, z, args, ts, frame_mask, s, generator):
+        N = self.num_timesteps
+        fm = frame_mask.to(device=z.device, dtype=torch.float32).contiguous()
+        sched = torch.stack(ts + [torch.zeros_like(ts[0])]).contiguous()      # [steps + 1, B] on the device, t_n = 0
+
+        def randn():
+            return torch.randn(z.shape, generator=generator, device=z.device, dtype=z.dtype)
+
+        # step 0's re-noise (frames with 0 < edit ratio whose t_0 is already reached); then each launch ends step i and
+        # starts step i + 1 with the noise step i + 1 draws
+        z = osb200.rf_masked_step(None, None, z, fm, sched[0], sched[0], guidance=s, noise=randn(), update=False,
+                                  num_timesteps=N)
+        for i in range(len(ts)):
+            t = sched[i]
+            args["x_mask"] = (fm * N >= t[:, None]).repeat(2, 1)
+            pred = model(torch.cat((z, z), 0), torch.cat((t, t), 0), **args)
+            pred = pred.chunk(2, dim=1)[0]
+            vc, vu = (p.to(z.dtype).contiguous() for p in pred.chunk(2, dim=0))
+            noise = randn() if i + 1 < len(ts) else None
+            osb200.rf_masked_step(vc, vu, z, fm, sched[i], sched[i + 1], guidance=s, noise=noise, num_timesteps=N, out=z)
         return z

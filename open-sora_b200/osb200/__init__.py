@@ -32,6 +32,7 @@ EXPORTS = (
     "osb_tmap_cache_stats",
     "osb_ln_modulate_scatter",
     "osb_comm_barrier",
+    "osb_rf_masked_step",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -79,6 +80,9 @@ def _load() -> C.CDLL:
         C.c_void_p, C.c_void_p,
     ]
     lib.osb_comm_barrier.argtypes = [C.c_void_p, C.c_void_p]
+    lib.osb_rf_masked_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float, C.c_int32,
+                                       C.c_int32, C.c_void_p]
     return lib
 
 
@@ -623,4 +627,36 @@ def cfg_euler(cond, uncond, uncond2, x, *, g_txt: float, g_img: float = 1.0, g_i
         _check(_lib.osb_cfg_euler(_ptr(cond), _ptr(uncond), _ptr(uncond2), _ptr(x), _ptr(out), n, g_txt, g_img,
                                   _ptr(g_img_map), g_img_map.numel() if g_img_map is not None else 0, dt, _stream()),
                "osb_cfg_euler")
+    return out
+
+
+def rf_masked_step(vc, vu, z, frame_mask, t_cur, t_next, *, guidance: float, noise=None, update: bool = True,
+                   num_timesteps: int = 1000, out=None):
+    """The frame-masked rectified-flow step (osb_rf_masked_step): z bf16 [B, C, T, H, W]; frame_mask fp32 [B, T] (1 =
+    generate, 0 = keep, in between = edit ratio); t_cur / t_next fp32 [B] on the device.  Frames with frame_mask * N >=
+    t_cur get z + (t_cur - t_next) / N * (vu + guidance (vc - vu)), the rest keep z bit for bit; with `noise`, frames that
+    reach t_next for the first time are then re-noised to (1 - t_next/N) z + (t_next/N) noise.  update=False is the
+    prologue before the first model call (re-noise only, vc / vu unused; "first time" = frame_mask != 1).  out may be z."""
+    import torch
+
+    for t, n in ((vc, "vc"), (vu, "vu"), (z, "z"), (noise, "noise"), (out, "out")):
+        _need(t, torch.bfloat16, n)
+        if t is not None and (t.shape != z.shape or not t.is_contiguous()):
+            raise OsbError(f"{n} must be a contiguous tensor of the latent's shape {tuple(z.shape)}")
+    for t, n in ((frame_mask, "frame_mask"), (t_cur, "t_cur"), (t_next, "t_next")):
+        _need(t, torch.float32, n)
+        if not t.is_contiguous():
+            raise OsbError(f"{n} must be contiguous")
+    if z.dim() != 5:
+        raise OsbError("z must be [B, C, T, H, W]")
+    B, Cc, T, H, W = z.shape
+    if frame_mask.shape != (B, T) or t_cur.shape != (B,) or t_next.shape != (B,):
+        raise OsbError(f"frame_mask must be [B, T] = [{B}, {T}] and t_cur / t_next [B]")
+    if out is None:
+        out = torch.empty_like(z)
+    n = z.numel()
+    with _Timed("rf_masked_step", 2.0 * n * (2 + 2 * int(update) + int(noise is not None))):  # dense bytes: all frames
+        _check(_lib.osb_rf_masked_step(_ptr(vc), _ptr(vu), _ptr(z), _ptr(noise), _ptr(out), _ptr(frame_mask), _ptr(t_cur),
+                                       _ptr(t_next), B, Cc, T, H * W, guidance, num_timesteps, int(update), _stream()),
+               "osb_rf_masked_step")
     return out
