@@ -88,6 +88,22 @@ typedef struct osb_gemm_args {
  * Requires K % 8 == 0, N % 8 == 0. */
 int osb_gemm_bf16(const osb_gemm_args* args, void* stream);
 
+/* ---- LoRA: unmerged low-rank update in the same accumulator ------------------------------------------------------ */
+typedef struct osb_lora_args {
+  const void* U;  /* bf16 [M, r], row stride ldu: x · A^T (the down projection)          */
+  const void* B;  /* bf16 [N, r], row stride ldb: scaling · lora_B                       */
+  int64_t ldu, ldb;
+  int32_t r;      /* multiple of 8 (the host zero-pads smaller ranks)                    */
+  int32_t reserved;
+} osb_lora_args;
+
+/* D = epilogue(A W^T + U B^T + bias): osb_gemm_bf16 whose K loop is followed by ceil(r / 64) k-blocks of U and B
+ * through the same wgmma pipeline, so the base product and the adapter's update share one fp32 accumulator and one
+ * rounding to bf16 (merging the update into bf16 weights would round most of a small update away).  Every epilogue,
+ * block_n and alignment rule of osb_gemm_bf16 applies.  The down projection U = x A^T is osb_gemm_bf16 with N = r.
+ * Replaces the unmerged peft LoRA layer the reference wraps the denoiser with (opensora/utils/sampling.py:542-545). */
+int osb_gemm_lora(const osb_gemm_args* gemm, const osb_lora_args* lora, void* stream);
+
 /* ---- attention with short key sets (whole key set resident in one CTA) -------------------- */
 typedef struct osb_attn_short_args {
   const void* q; const void* k; const void* v; /* bf16; element (row, h*D + d) at ptr + row*ld + h*D + d */

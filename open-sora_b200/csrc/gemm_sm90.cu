@@ -8,10 +8,13 @@
 // One wgmma group stays in flight while the next stage is waited for; a stage is handed back to the producer as soon
 // as the group that read it has retired.
 //
-// The same main loop serves three front ends (template kMode):
+// The same main loop serves four front ends (template kMode):
 //   kPlain      nn.Linear with fused bias / GELU(tanh) / gate * x + residual epilogues;
 //   kConv       causal 3D convolution as implicit GEMM: every k-block is ONE 5-D TMA box of the padded NDHWC input;
-//   kHeadTiles  q / k / v projection whose epilogue writes per-head operand tiles (tiles.cuh) with RMSNorm + RoPE.
+//   kHeadTiles  q / k / v projection whose epilogue writes per-head operand tiles (tiles.cuh) with RMSNorm + RoPE;
+//   kLora       kPlain plus an unmerged low-rank update: after the K loop the producer streams ceil(r / 64) more
+//               k-blocks, U = x A^T [M, r] in the A slot and s B [N, r] in the W slot, through the same stage ring, so
+//               A W^T + U (s B)^T lands in one fp32 accumulator before the unchanged epilogue.
 //
 // Replaces every nn.Linear on the denoiser block path of the reference
 // (opensora/models/mmdit/layers.py:209-214,247-252,277-281,314-334,401) and the fused epilogues
@@ -29,7 +32,7 @@ constexpr int kBlockK = 64;
 constexpr int kNumThreads = 384;            // producer warpgroup + two consumer warpgroups
 constexpr int kStageBudget = 200 * 1024;    // operand ring (one CTA per SM; 227 KB is the per-block limit)
 
-enum { kPlain = 0, kConv = 1, kHeadTiles = 2 };
+enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3 };
 
 struct GemmEpilogueParams {
   const __nv_bfloat16* bias;
@@ -89,7 +92,9 @@ struct GemmCfg {
 template <int BLOCK_N, int kMode>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                 const GemmEpilogueParams p, const ConvGeom cg, const HeadTileParams ht) {
+                 const GemmEpilogueParams p, const ConvGeom cg, const HeadTileParams ht,
+                 const __grid_constant__ CUtensorMap tmap_u, const __grid_constant__ CUtensorMap tmap_lb,
+                 const int32_t lora_k_blocks) {   // kLora only: U / s B maps and ceil(r / 64)
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::STAGES;
 
@@ -106,6 +111,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int64_t num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int64_t m_blk = blockIdx.x / num_n_blocks, n_blk = blockIdx.x % num_n_blocks;
   const int64_t num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
+  const int64_t total_k_blocks = kMode == kLora ? num_k_blocks + lora_k_blocks : num_k_blocks;
   // conv: m_blk -> (batch, t-tile, h-tile, w-tile); the box origin in OUTPUT coordinates
   int n_i = 0, t0 = 0, h0 = 0, w0 = 0;
   if constexpr (kMode == kConv) {
@@ -121,6 +127,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w);
+    if constexpr (kMode == kLora) {
+      tma_prefetch_desc(&tmap_u);
+      tma_prefetch_desc(&tmap_lb);
+    }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
@@ -154,6 +164,15 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         tma_load_2d(&tmap_w, full_bar(stage), smem_b(stage), k0, w_row);
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
+      if constexpr (kMode == kLora) {   // the rank tail beyond r is zero filled in both U and s B
+        for (int32_t lk = 0; lk < lora_k_blocks; ++lk) {
+          mbar_wait_notrace(empty_bar(stage), phase ^ 1);
+          mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+          tma_load_2d(&tmap_u, full_bar(stage), smem_a(stage), lk * kBlockK, a_row);
+          tma_load_2d(&tmap_lb, full_bar(stage), smem_b(stage), lk * kBlockK, w_row);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
       pdl_launch_dependents();  // all loads issued: dependents may start filling SMs as they are vacated
     }
     return;
@@ -167,7 +186,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   {
     int stage = 0, prev = 0;
     uint32_t phase = 0;
-    for (int64_t kb = 0; kb < num_k_blocks; ++kb) {
+    for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
       mbar_wait_notrace(full_bar(stage), phase);
       const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
       const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
@@ -299,7 +318,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
       if (!row_ok) continue;
       const float* gate_row = nullptr;
-      if (kMode == kPlain && p.epilogue == OSB_EPI_BIAS_GATE_RES && p.gate != nullptr) {
+      if ((kMode == kPlain || kMode == kLora) && p.epilogue == OSB_EPI_BIAS_GATE_RES && p.gate != nullptr) {
         int64_t gi = (uint32_t)row / group_rows32;
         if (p.mod_index) gi = p.mod_index[gi];
         gate_row = p.gate + gi * p.gate_stride;
@@ -342,11 +361,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // ------------------------------------------------------------------------------------------
 template <int BLOCK_N, int kMode>
 static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tw, const GemmEpilogueParams& p, const ConvGeom& cg,
-                         const HeadTileParams& ht, int64_t tiles, cudaStream_t stream) {
+                         const HeadTileParams& ht, int64_t tiles, cudaStream_t stream, const CUtensorMap* tu = nullptr,
+                         const CUtensorMap* tlb = nullptr, int32_t lora_k_blocks = 0) {
   if (tiles >= (1ll << 31)) { set_error("osb gemm: too many output tiles (%lld)", (long long)tiles); return OSB_ERR_UNSUPPORTED; }
   cudaLaunchAttribute attr[2];
   cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)tiles), dim3(kNumThreads), GemmCfg<BLOCK_N>::SMEM_BYTES, stream, attr);
-  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<BLOCK_N, kMode>, ta, tw, p, cg, ht));
+  // the LoRA maps are read by kLora only; every other mode gets the main maps as placeholders
+  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<BLOCK_N, kMode>, ta, tw, p, cg, ht, tu ? *tu : ta,
+                                    tlb ? *tlb : tw, lora_k_blocks));
   count_launch();
   return OSB_OK;
 }
@@ -370,7 +392,7 @@ static int launch_gemm_ht(const osb_gemm_args& a, const HeadTileParams& ht, cuda
 }
 
 template <int BLOCK_N>
-static int launch_gemm(const osb_gemm_args& a, bool has_res, cudaStream_t stream) {
+static int launch_gemm(const osb_gemm_args& a, bool has_res, cudaStream_t stream, const osb_lora_args* lora = nullptr) {
   CUtensorMap ta, tw;
   int rc = make_tmap_2d_bf16(&ta, a.A, a.M, a.K, a.lda, kBlockM, kBlockK);
   if (rc) return rc;
@@ -391,7 +413,11 @@ static int launch_gemm(const osb_gemm_args& a, bool has_res, cudaStream_t stream
   const int64_t tiles = ((a.M + kBlockM - 1) / kBlockM) * ((a.N + BLOCK_N - 1) / BLOCK_N);
   ConvGeom cg = {};
   HeadTileParams ht = {};
-  return launch_kernel<BLOCK_N, kPlain>(ta, tw, p, cg, ht, tiles, stream);
+  if (lora == nullptr) return launch_kernel<BLOCK_N, kPlain>(ta, tw, p, cg, ht, tiles, stream);
+  CUtensorMap tu, tlb;
+  if ((rc = make_tmap_2d_bf16(&tu, lora->U, a.M, lora->r, lora->ldu, kBlockM, kBlockK))) return rc;
+  if ((rc = make_tmap_2d_bf16(&tlb, lora->B, a.N, lora->r, lora->ldb, BLOCK_N, kBlockK))) return rc;
+  return launch_kernel<BLOCK_N, kLora>(ta, tw, p, cg, ht, tiles, stream, &tu, &tlb, (lora->r + kBlockK - 1) / kBlockK);
 }
 
 template <int BLOCK_N, int kMode>
@@ -414,6 +440,10 @@ int gemm_init() {
   if ((rc = init_one<128, kConv>())) return rc;
   if ((rc = init_one<192, kConv>())) return rc;
   if ((rc = init_one<256, kConv>())) return rc;
+  if ((rc = init_one<64, kLora>())) return rc;
+  if ((rc = init_one<128, kLora>())) return rc;
+  if ((rc = init_one<192, kLora>())) return rc;
+  if ((rc = init_one<256, kLora>())) return rc;
   return OSB_OK;
 }
 
@@ -469,38 +499,60 @@ static int launch_conv(const osb_conv3d_args& a, const ConvGeom& cg, const uint3
 
 }  // namespace osb
 
-extern "C" int osb_gemm_bf16(const osb_gemm_args* args, void* stream) {
-  using namespace osb;
+namespace osb {
+
+// Argument checks and tile-width dispatch shared by osb_gemm_bf16 and osb_gemm_lora (`fn` names the entry point in errors).
+static int gemm_dispatch(const char* fn, const osb_gemm_args* args, const osb_lora_args* lora, void* stream) {
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
-  OSB_REQUIRE(args != nullptr, "osb_gemm_bf16: null args");
+  OSB_REQUIRE(args != nullptr, "%s: null args", fn);
   const osb_gemm_args& a = *args;
-  OSB_REQUIRE(a.A && a.W && a.D, "osb_gemm_bf16: null operand");
-  OSB_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "osb_gemm_bf16: empty problem (M %lld N %lld K %lld)",
+  OSB_REQUIRE(a.A && a.W && a.D, "%s: null operand", fn);
+  OSB_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "%s: empty problem (M %lld N %lld K %lld)", fn,
               (long long)a.M, (long long)a.N, (long long)a.K);
-  OSB_REQUIRE(a.K % 8 == 0 && a.N % 8 == 0, "osb_gemm_bf16: K and N must be multiples of 8 (K %lld N %lld)",
+  OSB_REQUIRE(a.K % 8 == 0 && a.N % 8 == 0, "%s: K and N must be multiples of 8 (K %lld N %lld)", fn,
               (long long)a.K, (long long)a.N);
   OSB_REQUIRE(a.ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(a.D) & 15) == 0,
-              "osb_gemm_bf16: D must be 16-byte aligned with ldd %% 8 == 0");
+              "%s: D must be 16-byte aligned with ldd %% 8 == 0", fn);
   OSB_REQUIRE(a.epilogue >= OSB_EPI_BIAS && a.epilogue <= OSB_EPI_BIAS_GATE_RES,
-              "osb_gemm_bf16: unknown epilogue %d", a.epilogue);
+              "%s: unknown epilogue %d", fn, a.epilogue);
   if (a.epilogue == OSB_EPI_BIAS_GATE_RES) {
     OSB_REQUIRE(a.R == nullptr || (a.ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(a.R) & 15) == 0),
-                "osb_gemm_bf16: R must be 16-byte aligned with ldr %% 8 == 0");
+                "%s: R must be 16-byte aligned with ldr %% 8 == 0", fn);
     OSB_REQUIRE(a.gate == nullptr || (a.gate_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(a.gate) & 15) == 0),
-                "osb_gemm_bf16: gate must be 16-byte aligned with gate_stride %% 4 == 0");
+                "%s: gate must be 16-byte aligned with gate_stride %% 4 == 0", fn);
   }
   OSB_REQUIRE(a.bias == nullptr || (reinterpret_cast<uintptr_t>(a.bias) & 15) == 0,
-              "osb_gemm_bf16: bias must be 16-byte aligned");
-  OSB_REQUIRE(a.cta_group >= 0 && a.cta_group <= 2, "osb_gemm_bf16: cta_group must be 0, 1 or 2");
+              "%s: bias must be 16-byte aligned", fn);
+  OSB_REQUIRE(a.cta_group >= 0 && a.cta_group <= 2, "%s: cta_group must be 0, 1 or 2", fn);
+  if (lora != nullptr) {
+    const osb_lora_args& l = *lora;
+    OSB_REQUIRE(l.U && l.B, "%s: null U or B", fn);
+    OSB_REQUIRE(l.r > 0 && l.r % 8 == 0, "%s: rank r must be a positive multiple of 8 (zero-pad A and B), got %d", fn, l.r);
+    OSB_REQUIRE(l.ldu >= l.r && l.ldb >= l.r && l.ldu % 8 == 0 && l.ldb % 8 == 0 &&
+                ((reinterpret_cast<uintptr_t>(l.U) | reinterpret_cast<uintptr_t>(l.B)) & 15) == 0,
+                "%s: U and B must be 16-byte aligned with ldu, ldb >= r and multiples of 8 (r %d ldu %lld ldb %lld)", fn,
+                l.r, (long long)l.ldu, (long long)l.ldb);
+  }
   const bool has_res = (a.epilogue == OSB_EPI_BIAS_GATE_RES) && a.R != nullptr;
   const int bn = a.block_n ? a.block_n : pick_block_n(a.M, a.N);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (bn == 64) return launch_gemm<64>(a, has_res, s);
-  if (bn == 128) return launch_gemm<128>(a, has_res, s);
-  if (bn == 192) return launch_gemm<192>(a, has_res, s);
-  if (bn == 256) return launch_gemm<256>(a, has_res, s);
-  set_error("osb_gemm_bf16: unsupported block_n %d", bn);
+  if (bn == 64) return launch_gemm<64>(a, has_res, s, lora);
+  if (bn == 128) return launch_gemm<128>(a, has_res, s, lora);
+  if (bn == 192) return launch_gemm<192>(a, has_res, s, lora);
+  if (bn == 256) return launch_gemm<256>(a, has_res, s, lora);
+  set_error("%s: unsupported block_n %d", fn, bn);
   return OSB_ERR_UNSUPPORTED;
+}
+
+}  // namespace osb
+
+extern "C" int osb_gemm_bf16(const osb_gemm_args* args, void* stream) {
+  return osb::gemm_dispatch("osb_gemm_bf16", args, nullptr, stream);
+}
+
+extern "C" int osb_gemm_lora(const osb_gemm_args* gemm, const osb_lora_args* lora, void* stream) {
+  if (lora == nullptr) { osb::set_error("osb_gemm_lora: null lora args"); return OSB_ERR_INVALID; }
+  return osb::gemm_dispatch("osb_gemm_lora", gemm, lora, stream);
 }
 
 extern "C" int osb_conv3d_ndhwc(const osb_conv3d_args* args, void* stream) {

@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 
 from opensora.registry import MODELS
+from opensora.utils.lora import refuse_adapters
 
 from .vae import DecoderCausal3D, DiagonalGaussianDistribution, EncoderCausal3D
 
@@ -254,6 +255,7 @@ class AutoencoderKLCausal3D(nn.Module):
     # ---- public API (:269-358, :554-622) -------------------------------------------------------------------
     def encode(self, x, sample_posterior=True, return_posterior=False, generator=None):
         self._check()
+        refuse_adapters(self, "AutoencoderKLCausal3D")   # no LoRA path: never silently run the base model
         assert x.dim() == 5, "The input tensor should have 5 dimensions."
         x = x.to(self.quant_conv.weight.device, torch.bfloat16)
         if self.use_temporal_tiling and x.shape[2] > self.tile_sample_min_tsize:
@@ -275,6 +277,7 @@ class AutoencoderKLCausal3D(nn.Module):
 
     def decode(self, z):
         self._check()
+        refuse_adapters(self, "AutoencoderKLCausal3D")   # no LoRA path: never silently run the base model
         z = z.to(self.quant_conv.weight.device, torch.bfloat16) / self.scale_factor + self.shift_factor
         if self.use_slicing and z.shape[0] > 1:
             return torch.cat([self._decode(zs) for zs in z.split(1)])

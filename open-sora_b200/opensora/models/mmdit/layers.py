@@ -10,7 +10,12 @@ they read the block's own parameters and run every FLOP on libosb200 (sm_90a):
   GELU GEMM wrote side by side (no torch.cat materialisation, SURVEY.md §2.2 K9).
 
 Any joint sequence length (the flash attention variant streams key blocks), both RoPE layouts (`EmbedND`
-interleaved pairs and `LigerEmbedND` rotate-half) and both QKV checkpoint layouts (`fused_qkv` True / False)."""
+interleaved pairs and `LigerEmbedND` rotate-half) and both QKV checkpoint layouts (`fused_qkv` True / False).
+
+LoRA (opensora/utils/lora.py): every Linear is read through `linear_parts` / `lora_pack`, which also return the active
+adapter's (A, scaling * B), if any.  Linears that read one input share one down GEMM U = x A_cat^T; each output weight
+then runs `osb_gemm_lora` (x W^T + U B^T in one accumulator).  Without an adapter the launches are those of the plain
+model."""
 from __future__ import annotations
 
 import math
@@ -18,6 +23,8 @@ from dataclasses import dataclass
 
 import torch
 from torch import Tensor, nn
+
+from opensora.utils.lora import adapter_of, lora_pack
 
 from .math import liger_rope, rope, rope_tables
 
@@ -68,8 +75,26 @@ def timestep_embedding(t: Tensor, dim, max_period=10000, time_factor: float = 10
     return emb
 
 
+def linear_parts(lin: nn.Module, k_pad: int = 0):
+    """(weight, bias, lora) of a Linear the forward sends to osb200: lora is None, or (A [r, K + k_pad], scaling * B)
+    of its adapter (lora_pack)."""
+    if adapter_of(lin) is None:
+        return lin.weight, lin.bias, None
+    A, (B,) = lora_pack([[(lin, 0, lin.out_features)]], k_pad)
+    return lin.weight, lin.bias, (A, B)
+
+
+def _gemm(osb, x2d: Tensor, w: Tensor, b, lora, u: Tensor | None = None, **kw) -> Tensor:
+    """osb.gemm, or with lora = (A, B) the fused base + update GEMM; `u` = x2d A^T when a shared down GEMM made it."""
+    if lora is None or lora[1] is None:
+        return osb.gemm(x2d, w, b, **kw)
+    if u is None:
+        u = osb.gemm(x2d, lora[0])
+    return osb.gemm_lora(x2d, w, b, u, lora[1], **kw)
+
+
 def _linear(x2d: Tensor, lin: nn.Linear, **kw) -> Tensor:
-    return _osb().gemm(x2d, lin.weight, lin.bias, **kw)
+    return _gemm(_osb(), x2d, *linear_parts(lin), **kw)
 
 
 class MLPEmbedder(nn.Module):
@@ -237,6 +262,15 @@ class _ProcessorBase:
             torch.cat(ws, 0).contiguous(), None if bs[0] is None else torch.cat(bs, 0).contiguous()))
 
     @staticmethod
+    def _qkv_lora(sa: nn.Module):
+        """Adapters of the q|k|v projection in the row order of `_qkv`: (A_cat, B_cat) or None."""
+        if getattr(sa, "fused_qkv", hasattr(sa, "qkv")):
+            return linear_parts(sa.qkv)[2]
+        C = sa.q_proj.out_features
+        p = lora_pack([[(sa.q_proj, 0, C), (sa.k_proj, 0, C), (sa.v_proj, 0, C)]])
+        return None if p is None else (p[0], p[1][0])
+
+    @staticmethod
     def _modulation(osb, mod: nn.Module, vec: Tensor):
         """layers.py:186-192 on osb200: lin(silu(vec)) -> fp32 [B, C] row views (row stride multiplier*C) the kernels take
         as shift / scale / gate.  When the model has already projected `vec` through EVERY block's modulation layer in one
@@ -246,7 +280,7 @@ class _ProcessorBase:
             lo, hi = grouped[1][id(mod.lin)]
             out = grouped[0][:, lo:hi]
         else:
-            out = osb.gemm(torch.nn.functional.silu(vec).contiguous(), mod.lin.weight, mod.lin.bias).float()
+            out = _gemm(osb, torch.nn.functional.silu(vec).contiguous(), *linear_parts(mod.lin)).float()
         mult = getattr(mod, "multiplier", None) or (mod.lin.out_features // mod.lin.in_features)
         c = out.chunk(mult, dim=-1)
         return ModulationOut(*c[:3]), (ModulationOut(*c[3:6]) if mult >= 6 else None)
@@ -268,15 +302,21 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
         qkv = torch.empty(B * L, 3 * C, dtype=img.dtype, device=img.device)
         wi, bi = self._qkv(attn, attn.img_attn, "img_qkv")
         wt, bt = self._qkv(attn, attn.txt_attn, "txt_qkv")
+        li, lt = self._qkv_lora(attn.img_attn), self._qkv_lora(attn.txt_attn)
+        ui = ut = None   # adapters: one down projection over all rows of a stream, sliced per sample below
         if Li:
             xi = osb.ln_modulate(img2, im1.shift, im1.scale, group_rows=Li)
+            ui = None if li is None else osb.gemm(xi, li[0])
         if Lt:
             xt = osb.ln_modulate(txt2, tm1.shift, tm1.scale, group_rows=Lt)
+            ut = None if lt is None else osb.gemm(xt, lt[0])
         for b in range(B):
             if Lt:
-                osb.gemm(xt[b * Lt:(b + 1) * Lt], wt, bt, out=qkv[b * L:b * L + Lt])
+                _gemm(osb, xt[b * Lt:(b + 1) * Lt], wt, bt, lt, None if ut is None else ut[b * Lt:(b + 1) * Lt],
+                      out=qkv[b * L:b * L + Lt])
             if Li:
-                osb.gemm(xi[b * Li:(b + 1) * Li], wi, bi, out=qkv[b * L + Lt:(b + 1) * L])
+                _gemm(osb, xi[b * Li:(b + 1) * Li], wi, bi, li, None if ui is None else ui[b * Li:(b + 1) * Li],
+                      out=qkv[b * L + Lt:(b + 1) * L])
         cos, sin, half = _rope(pe)
         kw = dict(q_norm_w=attn.txt_attn.norm.query_norm.scale, k_norm_w=attn.txt_attn.norm.key_norm.scale,
                   q_norm_w2=attn.img_attn.norm.query_norm.scale, k_norm_w2=attn.img_attn.norm.key_norm.scale,
@@ -285,23 +325,29 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
         split_full = getattr(vec, "_osb_txt_len", Lt)
         ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img.dtype, img.device)
         img_o, txt_o = torch.empty_like(img2), torch.empty_like(txt2)
+        # both output projections read `ao`: one down projection for their adapters
+        pi, pt = attn.img_attn.proj, attn.txt_attn.proj
+        lp = lora_pack([[(pi, 0, pi.out_features)], [(pt, 0, pt.out_features)]])
+        up = None if lp is None else osb.gemm(ao, lp[0])
+        lpi, lpt = (None, None) if lp is None else ((lp[0], lp[1][0]), (lp[0], lp[1][1]))
         for b in range(B):  # x + gate * proj(attn)   (layers.py:247, 251)
             if Li:
-                osb.gemm(ao[b * L + Lt:(b + 1) * L], attn.img_attn.proj.weight, attn.img_attn.proj.bias,
-                         epilogue=osb.EPI_BIAS_GATE_RES, residual=img2[b * Li:(b + 1) * Li], gate=im1.gate[b:b + 1],
-                         out=img_o[b * Li:(b + 1) * Li])
+                _gemm(osb, ao[b * L + Lt:(b + 1) * L], pi.weight, pi.bias, lpi,
+                      None if up is None else up[b * L + Lt:(b + 1) * L],
+                      epilogue=osb.EPI_BIAS_GATE_RES, residual=img2[b * Li:(b + 1) * Li], gate=im1.gate[b:b + 1],
+                      out=img_o[b * Li:(b + 1) * Li])
             if Lt:
-                osb.gemm(ao[b * L:b * L + Lt], attn.txt_attn.proj.weight, attn.txt_attn.proj.bias,
-                         epilogue=osb.EPI_BIAS_GATE_RES, residual=txt2[b * Lt:(b + 1) * Lt], gate=tm1.gate[b:b + 1],
-                         out=txt_o[b * Lt:(b + 1) * Lt])
+                _gemm(osb, ao[b * L:b * L + Lt], pt.weight, pt.bias, lpt, None if up is None else up[b * L:b * L + Lt],
+                      epilogue=osb.EPI_BIAS_GATE_RES, residual=txt2[b * Lt:(b + 1) * Lt], gate=tm1.gate[b:b + 1],
+                      out=txt_o[b * Lt:(b + 1) * Lt])
         # x + gate * MLP((1 + scale) * LN(x) + shift)   (layers.py:248, 252)
         for x_o, mod, mlp, n in ((img_o, im2, attn.img_mlp, Li), (txt_o, tm2, attn.txt_mlp, Lt)):
             if n == 0:
                 continue
             xm = osb.ln_modulate(x_o, mod.shift, mod.scale, group_rows=n)
-            hid = osb.gemm(xm, mlp[0].weight, mlp[0].bias, epilogue=osb.EPI_BIAS_GELU_TANH)
-            osb.gemm(hid, mlp[2].weight, mlp[2].bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=x_o, gate=mod.gate,
-                     group_rows=n, out=x_o)
+            hid = _gemm(osb, xm, *linear_parts(mlp[0]), epilogue=osb.EPI_BIAS_GELU_TANH)
+            _gemm(osb, hid, *linear_parts(mlp[2]), epilogue=osb.EPI_BIAS_GATE_RES, residual=x_o, gate=mod.gate,
+                  group_rows=n, out=x_o)
         return img_o.view(B, Li, C), txt_o.view(B, Lt, C)
 
 
@@ -349,6 +395,18 @@ class SingleStreamBlockProcessor(_ProcessorBase):
             torch.cat([blk.q_proj.bias, blk.k_proj.bias, blk.v_mlp.bias[:C]], 0).contiguous()))
         return wq, bq, blk.v_mlp.weight[C:], blk.v_mlp.bias[C:]
 
+    @staticmethod
+    def _split_lora(blk: nn.Module, M4: int):
+        """Adapters of the qkv and mlp parts of `_split_weights`, which read the same input: (A_cat, B_qkv, B_mlp) with
+        one A_cat for both, or None."""
+        C = blk.linear2.out_features
+        if getattr(blk, "fused_qkv", hasattr(blk, "linear1")):
+            groups = [[(blk.linear1, 0, 3 * C)], [(blk.linear1, 3 * C, 3 * C + M4)]]
+        else:
+            groups = [[(blk.q_proj, 0, C), (blk.k_proj, 0, C), (blk.v_mlp, 0, C)], [(blk.v_mlp, C, C + M4)]]
+        p = lora_pack(groups)
+        return None if p is None else (p[0], p[1][0], p[1][1])
+
     def __call__(self, attn: nn.Module, x: Tensor, vec: Tensor, pe) -> Tensor:
         osb = _check(x)
         B, L, C = x.shape
@@ -358,15 +416,18 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         x2 = x.reshape(B * L, C).contiguous()
         xm = osb.ln_modulate(x2, mod.shift, mod.scale, group_rows=L)
         wq, bq, wm, bm = self._split_weights(attn)
-        qkv = osb.gemm(xm, wq, bq)                                               # [B*L, 3C]
+        lo = self._split_lora(attn, M4)
+        u = None if lo is None else osb.gemm(xm, lo[0])                          # shared down projection
+        lq, lm = (None, None) if lo is None else ((lo[0], lo[1]), (lo[0], lo[2]))
+        qkv = _gemm(osb, xm, wq, bq, lq, u)                                      # [B*L, 3C]
         cos, sin, half = _rope(pe)
         kw = dict(q_norm_w=attn.norm.query_norm.scale, k_norm_w=attn.norm.key_norm.scale, rope_cos=cos, rope_sin=sin,
                   rope_half=half)
         # [attn | gelu(mlp)] side by side: the attention output and the GELU GEMM write one [rows, C + 4C] buffer
         cat = _sp_attention(osb, qkv, C + M4, B, L, H, D, kw, 0, x.dtype, x.device)
-        osb.gemm(xm, wm, bm, epilogue=osb.EPI_BIAS_GELU_TANH, out=cat[:, C:])
-        out = osb.gemm(cat, attn.linear2.weight, attn.linear2.bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=x2,
-                       gate=mod.gate, group_rows=L)
+        _gemm(osb, xm, wm, bm, lm, u, epilogue=osb.EPI_BIAS_GELU_TANH, out=cat[:, C:])
+        out = _gemm(osb, cat, *linear_parts(attn.linear2), epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
+                    group_rows=L)
         return out.view(B, L, C)
 
 

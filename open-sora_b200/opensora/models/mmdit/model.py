@@ -10,8 +10,10 @@ from torch import Tensor, nn
 
 from opensora.registry import MODELS
 
-from .layers import (DoubleStreamBlock, EmbedND, LastLayer, LigerEmbedND, MLPEmbedder, SingleStreamBlock, _linear,
-                     timestep_embedding)
+from opensora.utils.lora import adapter_of, lora_pack
+
+from .layers import (DoubleStreamBlock, EmbedND, LastLayer, LigerEmbedND, MLPEmbedder, SingleStreamBlock, _gemm,
+                     linear_parts, timestep_embedding)
 
 
 @dataclass
@@ -79,12 +81,13 @@ class MMDiTModel(nn.Module):
         self._input_requires_grad = False
         self._cond_w = None
         self._mod_pack = None
+        self._mod_lora = None
         self._pe_cache = None
         self._sp_group = None
         self.register_load_state_dict_post_hook(lambda m, k: m._drop_caches())
 
     def _drop_caches(self):
-        self._cond_w = self._mod_pack = self._pe_cache = None
+        self._cond_w = self._mod_pack = self._mod_lora = self._pe_cache = None
 
     def _apply(self, fn, *a, **k):
         self._drop_caches()
@@ -97,16 +100,35 @@ class MMDiTModel(nn.Module):
         slice (a processor installed on a block this model does not own simply does its own projection)."""
         import osb200
 
-        if self._mod_pack is None:
-            lins = [m.lin for b in self.double_blocks for m in (b.img_mod, b.txt_mod)] + [b.modulation.lin for b in self.single_blocks]
+        lins = [m.lin for b in self.double_blocks for m in (b.img_mod, b.txt_mod)] + [b.modulation.lin for b in self.single_blocks]
+        adapted = [lin for lin in lins if adapter_of(lin) is not None]
+        key = tuple((id(l), l.weight.data_ptr(), l.weight._version) for l in lins)
+        if self._mod_pack is None or self._mod_pack[0] != key:
             cols, off = {}, 0
             for lin in lins:
                 cols[id(lin)] = (off, off + lin.out_features)
                 off += lin.out_features
-            self._mod_pack = (torch.cat([l.weight for l in lins], 0).contiguous(), torch.cat([l.bias for l in lins], 0).contiguous(), cols)
-        w, b, cols = self._mod_pack
-        out = osb200.gemm(torch.nn.functional.silu(vec).contiguous(), w, b).float()
-        vec._osb_grouped_modulation = (out, cols)
+            self._mod_pack = (key, torch.cat([l.weight for l in lins], 0).contiguous(),
+                              torch.cat([l.bias for l in lins], 0).contiguous(), cols)
+        _, w, b, cols = self._mod_pack
+        sv = torch.nn.functional.silu(vec).contiguous()
+        out = osb200.gemm(sv, w, b)
+        if adapted:
+            # The base projection keeps its one launch.  Each adapted layer's update is then added into its slice of the
+            # bf16 output (R = D, no gate): peft's own two roundings, without a block-diagonal B over every layer and
+            # without reading the modulation weights again.  One down projection serves all layers (same input).
+            parts = [lora_pack([[(lin, 0, lin.out_features)]]) for lin in adapted]   # per layer (A, [s B]), cached
+            ml = self._mod_lora
+            if ml is None or len(ml[0]) != len(parts) or any(a is not b for a, b in zip(ml[0], parts)):
+                self._mod_lora = ml = (parts, torch.cat([p[0] for p in parts], 0).contiguous())
+            u = osb200.gemm(sv, ml[1])
+            ro = 0
+            for lin, (A, (lb,)) in zip(adapted, parts):
+                lo, hi = cols[id(lin)]
+                osb200.gemm(u[:, ro:ro + A.shape[0]], lb, None, epilogue=osb200.EPI_BIAS_GATE_RES, residual=out[:, lo:hi],
+                            out=out[:, lo:hi])
+                ro += A.shape[0]
+        vec._osb_grouped_modulation = (out.float(), cols)
 
     def _pe(self, txt_ids: Tensor, img_ids: Tensor):
         """`pe_embedder(cat(txt_ids, img_ids))` is step-invariant (utils/sampling.py:437-447 builds the ids once per sample):
@@ -126,16 +148,16 @@ class MMDiTModel(nn.Module):
         """Linear over a [B, L, K] tensor; K is zero-padded to a multiple of 8 when needed (cond_in: K = 68)."""
         B, L, K = x.shape
         x2 = x.to(lin.weight.dtype).reshape(B * L, K)
-        w = lin.weight
-        if K % 8:
-            pad = -K % 8
+        pad = -K % 8
+        w, bias, lora = linear_parts(lin, k_pad=pad)   # the adapter's A is padded along K like the weight
+        if pad:
             x2 = torch.nn.functional.pad(x2, (0, pad))
             if self._cond_w is None or self._cond_w[0] is not lin:
                 self._cond_w = (lin, torch.nn.functional.pad(lin.weight, (0, pad)).contiguous())
             w = self._cond_w[1]
         import osb200
 
-        return osb200.gemm(x2.contiguous(), w, lin.bias, **kw).view(B, L, -1)
+        return _gemm(osb200, x2.contiguous(), w, bias, lora, **kw).view(B, L, -1)
 
     def prepare_block_inputs(self, img: Tensor, img_ids: Tensor, txt: Tensor, txt_ids: Tensor, timesteps: Tensor,
                              y_vec: Tensor, cond: Tensor = None, guidance: Tensor | None = None):

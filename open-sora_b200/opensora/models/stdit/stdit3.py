@@ -29,6 +29,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from opensora.registry import MODELS
+from opensora.utils.lora import refuse_adapters
 
 
 @dataclass
@@ -350,6 +351,7 @@ class STDiT3(nn.Module):
 
         w0 = self.x_embedder.proj.weight
         osb.require_cuda_bf16(w0, "STDiT3")
+        refuse_adapters(self, "STDiT3")   # its head-tile GEMMs have no LoRA path: never silently run the base model
         dev = w0.device
         bf = torch.bfloat16
         C, Hh, D = self.hidden_size, self.num_heads, self.head_dim

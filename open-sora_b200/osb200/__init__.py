@@ -33,6 +33,7 @@ EXPORTS = (
     "osb_ln_modulate_scatter",
     "osb_comm_barrier",
     "osb_rf_masked_step",
+    "osb_gemm_lora",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -60,6 +61,7 @@ def _load() -> C.CDLL:
         C.c_int64, C.c_float, C.c_void_p,
     ]
     lib.osb_gemm_bf16.argtypes = [C.c_void_p, C.c_void_p]
+    lib.osb_gemm_lora.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_conv3d_ndhwc.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_vae_prep.argtypes = [C.c_void_p, C.c_void_p]
@@ -139,6 +141,11 @@ class GemmArgs(C.Structure):
         ("group_rows", C.c_int64), ("gate_stride", C.c_int64),
         ("epilogue", C.c_int32), ("cta_group", C.c_int32), ("block_n", C.c_int32), ("reserved", C.c_int32),
     ]
+
+
+class LoraArgs(C.Structure):
+    _fields_ = [("U", C.c_void_p), ("B", C.c_void_p), ("ldu", C.c_int64), ("ldb", C.c_int64), ("r", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 class AttnShortArgs(C.Structure):
@@ -304,10 +311,7 @@ def ln_modulate(x, shift, scale, *, group_rows: int, mod_index=None, eps: float 
     return out
 
 
-def gemm(a, w, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None, group_rows: int = 0,
-         mod_index=None, out=None, cta_group: int = 0, block_n: int = 0):
-    """out = epilogue(a @ w.T + bias).  a bf16 [M,K] (row stride free), w bf16 [N,K], bias bf16 [N].
-    GATE_RES: out = residual + gate[g] * (a @ w.T + bias), gate fp32 [G, N] view, may be None."""
+def _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, cta_group, block_n):
     import torch
 
     _need(a, torch.bfloat16, "a"); _need(w, torch.bfloat16, "w"); _need(bias, torch.bfloat16, "bias")
@@ -330,8 +334,35 @@ def gemm(a, w, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None,
     args.group_rows = group_rows if group_rows > 0 else M
     args.gate_stride = gate.stride(0) if gate is not None else 0
     args.epilogue, args.cta_group, args.block_n = epilogue, cta_group, block_n
-    with _Timed("gemm", 2.0 * M * N * K):  # algorithmic FLOPs
+    return args, out
+
+
+def gemm(a, w, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None, group_rows: int = 0,
+         mod_index=None, out=None, cta_group: int = 0, block_n: int = 0):
+    """out = epilogue(a @ w.T + bias).  a bf16 [M,K] (row stride free), w bf16 [N,K], bias bf16 [N].
+    GATE_RES: out = residual + gate[g] * (a @ w.T + bias), gate fp32 [G, N] view, may be None."""
+    args, out = _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, cta_group, block_n)
+    with _Timed("gemm", 2.0 * args.M * args.N * args.K):  # algorithmic FLOPs
         _check(_lib.osb_gemm_bf16(C.byref(args), _stream()), "osb_gemm_bf16")
+    return out
+
+
+def gemm_lora(a, w, bias, u, b, *, epilogue: int = EPI_BIAS, residual=None, gate=None, group_rows: int = 0,
+              mod_index=None, out=None, block_n: int = 0):
+    """out = epilogue(a @ w.T + u @ b.T + bias) in one fp32 accumulator (osb_gemm_lora): `gemm` plus an unmerged LoRA
+    update.  u bf16 [M, r] = x @ lora_A.T (the down projection, row stride free), b bf16 [N, r] = scaling * lora_B; r is
+    a multiple of 8 (zero-pad A's rows and B's columns)."""
+    import torch
+
+    _need(u, torch.bfloat16, "u"); _need(b, torch.bfloat16, "b")
+    if u.dim() != 2 or b.dim() != 2 or u.shape[0] != a.shape[0] or b.shape[0] != w.shape[0] or u.shape[1] != b.shape[1]:
+        raise OsbError(f"gemm_lora: u must be [M, r] and b [N, r] for a {tuple(a.shape)} x {tuple(w.shape)} GEMM, got "
+                       f"{tuple(u.shape)} and {tuple(b.shape)}")
+    args, out = _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, 0, block_n)
+    la = LoraArgs()
+    la.U, la.B, la.ldu, la.ldb, la.r = u.data_ptr(), b.data_ptr(), u.stride(0), b.stride(0), u.shape[1]
+    with _Timed("gemm", 2.0 * args.M * args.N * (args.K + la.r)):
+        _check(_lib.osb_gemm_lora(C.byref(args), C.byref(la), _stream()), "osb_gemm_lora")
     return out
 
 
