@@ -196,6 +196,8 @@ typedef struct osb_attn_tiles_args {
   int32_t reserved;
   int64_t num_seqs;
   const int32_t* kv_lens;    /* optional [num_seqs]: valid keys per sequence (G == 1)                               */
+                             /* With a packed q map (G > 1) kv_lens is not read: every packed sequence sees its Lk keys.
+                                The Python binding refuses kv_lens with a packed map rather than ignore it.            */
   void* out;                 /* bf16, row of token = inverse of q_map, head h at columns [h*head_dim, (h+1)*head_dim) */
   int64_t out_ld;
   float softmax_scale;

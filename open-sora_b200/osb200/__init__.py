@@ -522,6 +522,8 @@ def attn_tiles(q: HeadTiles, kv: HeadTiles, out, *, q_kind: int = 0, k_kind: int
 
     _need(out, torch.bfloat16, "out"); _need(kv_lens, torch.int32, "kv_lens")
     assert (out is None) != (out_scatter is None), "exactly one of out / out_scatter"
+    if kv_lens is not None and q.map.G > 1:   # the kernel reads kv_lens for unpacked query maps only
+        raise OsbError("attn_tiles: kv_lens applies to unpacked query maps only (G == 1); packed sequences see all Lk keys")
     a = AttnTilesArgs()
     a.q_tiles, a.k_tiles, a.v_tiles = q.kind_ptr(q_kind), kv.kind_ptr(k_kind), kv.kind_ptr(v_kind)
     if out_map is not None:   # output rows in another order than the rows the tiles were written from (same tiling)

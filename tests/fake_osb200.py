@@ -26,9 +26,9 @@ class OsbError(RuntimeError):
     pass
 
 
-def _count(name, detail=None):
+def _count(name, detail=None, launches=1):
     global _launches
-    _launches += 1
+    _launches += launches
     calls.append((name, detail))
 
 
@@ -98,7 +98,9 @@ def ln_modulate(x, shift, scale, *, group_rows: int, mod_index=None, eps: float 
     _need(mod_index, torch.int32, "mod_index")
     assert x.dim() == 2 and x.is_contiguous()
     assert shift.dim() == 2 and scale.dim() == 2 and shift.stride(0) == scale.stride(0)
-    rows, _ = x.shape
+    rows, C = x.shape
+    if C % 8 or C > 8192:
+        raise OsbError(f"osb_ln_modulate failed (-1): C must be a multiple of 8 and <= 8192 (got {C})")
     xf = x.float()
     mu = xf.mean(-1, keepdim=True)
     var = (xf - mu).pow(2).mean(-1, keepdim=True)
@@ -170,7 +172,13 @@ def attn_short(q, k, v, out, *, num_seqs: int, seqs_per_batch: int, q_strides, k
     _need(rope_cos, torch.float32, "rope_cos"); _need(rope_sin, torch.float32, "rope_sin"); _need(kv_lens, torch.int32, "kv_lens")
     if (q_norm_w is None) != (k_norm_w is None) or (rope_cos is None) != (rope_sin is None):
         raise OsbError("osb_attn_short: norm weights / rope tables must come in pairs")
+    if (q_norm_w2 is None) != (k_norm_w2 is None) or (q_norm_w2 is not None and q_norm_w is None):
+        raise OsbError("osb_attn_short: the second norm weight pair needs the first")
     H, D = num_heads, head_dim
+    if D not in (64, 72, 128):
+        raise OsbError(f"osb_attn_short failed (-1): head_dim {D} not built (64, 72, 128)")
+    if rope_cos is not None and rope_half and D % 16:
+        raise OsbError("osb_attn_short failed (-1): rotate-half RoPE needs head_dim % 16 == 0")
     dev = q.device
     s = torch.arange(num_seqs, device=dev)
     b, j = s // seqs_per_batch, s % seqs_per_batch
@@ -216,10 +224,12 @@ def group_stats(x, groups: int, eps: float = 1e-6):
     _need(x, torch.bfloat16, "x")
     assert x.dim() == 5 and x.is_contiguous()
     nb, C = x.shape[0], x.shape[-1]
+    if groups <= 0 or C % groups or C % 8 or 256 % (C // 8) or groups > 1024:
+        raise OsbError(f"osb_group_stats failed (-1): C/8 must divide 256 and groups C (C = {C}, groups {groups})")
     xf = x.float().reshape(nb, -1, groups, C // groups)
     mean = xf.mean(dim=(1, 3))
     var = (xf - mean[:, None, :, None]).pow(2).mean(dim=(1, 3))
-    _count("group_stats", tuple(x.shape))
+    _count("group_stats", tuple(x.shape), launches=2)   # block partials + fp64 finalize
     return torch.stack((mean, torch.rsqrt(var + eps)), dim=-1)
 
 
@@ -230,6 +240,12 @@ def vae_prep(x, *, stats=None, gamma=None, beta=None, groups: int = 32, silu: bo
     assert x.dim() == 5 and x.is_contiguous()
     nb, T, H, W, C = x.shape
     cp = cp or C
+    if C % 8 or cp % 8 or cp < C:
+        raise OsbError(f"osb_vae_prep failed (-1): channels must be multiples of 8 (c {C} cp {cp})")
+    if any(f not in (1, 2) for f in up):
+        raise OsbError(f"osb_vae_prep failed (-1): upsample factors must be 1 or 2, got {tuple(up)}")
+    if stats is not None and (gamma is None or beta is None or groups <= 0 or C % groups):
+        raise OsbError("osb_vae_prep failed (-1): GroupNorm needs gamma, beta and a valid group count")
     y = x.float()
     if stats is not None:
         cg = C // groups
@@ -275,6 +291,10 @@ def conv3d(x_pad, w_packed, bias, *, out_thw, stride=(1, 1, 1), taps=(3, 3, 3), 
     nb, tp, hp, wp, cp = x_pad.shape
     kt, kh, kw = taps
     cout = w_packed.shape[0]
+    if any(s not in (1, 2) for s in stride):
+        raise OsbError(f"osb_conv3d_ndhwc failed (-1): strides must be 1 or 2, got {tuple(stride)}")
+    if any(k not in (1, 2, 3) for k in taps):
+        raise OsbError(f"osb_conv3d_ndhwc failed (-1): taps must be 1..3, got {tuple(taps)}")
     if cout % 8:
         raise OsbError(f"osb_conv3d_ndhwc: Cout must be a multiple of 8 (pad the weights), got {cout}")
     if narrow:
@@ -302,6 +322,9 @@ def conv3d(x_pad, w_packed, bias, *, out_thw, stride=(1, 1, 1), taps=(3, 3, 3), 
 def cfg_euler(cond, uncond, uncond2, x, *, g_txt: float, g_img: float = 1.0, g_img_map=None, dt: float, out=None):
     for t, n in ((cond, "cond"), (uncond, "uncond"), (uncond2, "uncond2"), (x, "x"), (g_img_map, "g_img_map")):
         _need(t, torch.bfloat16, n)
+    if x.numel() % 8 or (g_img_map is not None and (g_img_map.numel() % 8 or x.numel() % g_img_map.numel())):
+        raise OsbError("osb_cfg_euler failed (-1): element count and guidance map period must be multiples of 8, "
+                       "the period dividing the count")
     c, u = cond.float(), uncond.float()
     if uncond2 is None:
         pred = u + g_txt * (c - u)
@@ -320,28 +343,9 @@ def cfg_euler(cond, uncond, uncond2, x, *, g_txt: float, g_img: float = 1.0, g_i
 # ---- head tiles (include/osb200.h osb_gemm_head_tiles / osb_attn_tiles): the double keeps the tile buffer as a dense
 # [kinds, rows, heads*D] tensor - the byte layout of a tile is the kernels' business, the CONTRACT is which token row and
 # head a value belongs to, what was applied to it (bias, RMSNorm, RoPE by position) and which keys a query may see. ------
-class TileMap:
-    def __init__(self):
-        self.mode = self.L = self.S = self.T = self.G = self.tps = self.tile_rows = 0
-
-    def key(self):
-        return (self.mode, self.L, self.S, self.T, self.G, self.tps, self.tile_rows)
-
-
-def tile_map(mode: int, L: int, S: int = 0, T: int = 0, *, keys_only: bool = False, pack: bool = True) -> TileMap:
-    m = TileMap()
-    m.mode, m.L, m.S, m.T = mode, L, S, T
-    if L <= 64 and pack and not keys_only:
-        m.G, m.tps = 128 // L, 1
-        m.tile_rows = -(-(m.G * L) // 16) * 16
-    else:
-        m.G = 1
-        n = -(-L // 128)
-        # (keys-only tiles used to be balanced, 300 -> 3 x 112; a 112-row tile ends in the middle of a 32-column softmax
-        # chunk and sent a quarter of the chunks through the per-element masked path: full 128-row tiles + a short last one)
-        m.tile_rows = 128 if L > 128 else -(-(-(-L // n)) // 16) * 16
-        m.tps = -(-L // m.tile_rows)
-    return m
+# The tile map is host arithmetic of the binding itself (pure Python over a ctypes struct, no device needed): the double
+# uses it as is, so the two can never disagree on how a sequence is tiled.
+from osb200 import TileMap, tile_map  # noqa: E402,F401
 
 
 class HeadTiles:
@@ -372,6 +376,12 @@ def gemm_head_tiles(a, w, bias, tiles, *, nkinds, norm_w=(), rope=None, rope_kin
     assert M == tiles.rows and N % Cc == 0 and kind0 + N // Cc <= tiles.kinds and a.shape[1] == w.shape[1]
     if D not in (64, 72, 128) or H % 2:
         raise OsbError("osb_gemm_head_tiles failed (-1): head_dim / head count not built")
+    if K % 8:
+        raise OsbError(f"osb_gemm_head_tiles failed (-1): K must be a multiple of 8 (K {K})")
+    if not 1 <= nkinds <= 4:
+        raise OsbError(f"osb_gemm_head_tiles failed (-1): nkinds must be 1..4, got {nkinds}")
+    if any(nw is not None for nw in norm_w[nkinds:]):
+        raise OsbError("osb_gemm_head_tiles failed (-1): RMSNorm weight given for a kind >= nkinds")
     acc = a.float() @ w.float().t()
     if bias is not None:
         acc = acc + bias.float()
@@ -395,6 +405,8 @@ def attn_tiles(q, kv, out, *, q_kind=0, k_kind=1, v_kind=2, Lk, num_seqs, kv_len
                out_scatter=None, out_ld=None, out_map=None):
     H, D = q.heads, q.head_dim
     m = q.map
+    if kv_lens is not None and m.G > 1:
+        raise OsbError("attn_tiles: kv_lens applies to unpacked query maps only (G == 1); packed sequences see all Lk keys")
     scale = softmax_scale if softmax_scale is not None else D ** -0.5
     seq_q, pos_q = _seq_pos(m, q.rows, out.device)
     out_rows = None
@@ -419,7 +431,10 @@ def attn_tiles(q, kv, out, *, q_kind=0, k_kind=1, v_kind=2, Lk, num_seqs, kv_len
         qq = q.dense[q_kind][rq].float().view(-1, H, D).permute(1, 0, 2)
         kk = kv.dense[k_kind][rk].float().view(-1, H, D).permute(1, 0, 2)
         vv = kv.dense[v_kind][rk].float().view(-1, H, D).permute(1, 0, 2)
-        pr = torch.softmax(qq @ kk.transpose(-1, -2) * scale, dim=-1).to(torch.bfloat16).float()
-        out[ro] = (pr @ vv).permute(1, 0, 2).reshape(len(rq), H * D).to(torch.bfloat16)
+        sc = qq @ kk.transpose(-1, -2) * scale
+        p = torch.exp(sc - sc.amax(-1, keepdim=True))
+        # as the kernel: the UNnormalised P is rounded to bf16 for P V, the sum is taken over the unrounded P
+        o = (p.to(torch.bfloat16).float() @ vv) / p.sum(-1, keepdim=True)
+        out[ro] = o.permute(1, 0, 2).reshape(len(rq), H * D).to(torch.bfloat16)
     _count("attn_tiles", (num_seqs, m.L, Lk, H, D))
     return out

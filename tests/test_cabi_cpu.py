@@ -177,13 +177,27 @@ def test_tile_map_arithmetic():
     assert osb200._lib.osb_head_tiles_per_head(ctypes.byref(m), 2 * 16 * 12) == 3   # 24 sequences, 8 per tile
 
 
-def test_stand_in_tile_map_equals_the_binding():
-    """tests/fake_osb200.py restates `tile_map`; the host tests are only meaningful if both agree on every shape."""
+def test_stand_in_tile_map_is_the_binding():
+    """tests/fake_osb200.py uses the binding's own `tile_map` (host arithmetic, no device), so the host tests tile every
+    sequence exactly as the kernels do.  The arithmetic itself is checked against the rules of include/osb200.h for every
+    mode, L in 1..400, keys_only and pack."""
     import osb200
     from tests import fake_osb200
 
+    assert fake_osb200.tile_map is osb200.tile_map and fake_osb200.TileMap is osb200.TileMap
     for mode in (0, 1):
-        for L in (1, 7, 16, 17, 32, 48, 64, 65, 100, 128, 129, 200, 256, 300, 1200, 16384):
-            for kw in ({}, {"keys_only": True}, {"pack": False}):
+        for L in range(1, 401):
+            for kw in ({}, {"keys_only": True}, {"pack": False}, {"keys_only": True, "pack": False}):
                 S, T = (12, L) if mode == 1 else (0, 0)
-                assert fake_osb200.tile_map(mode, L, S, T, **kw).key() == osb200.tile_map(mode, L, S, T, **kw).key(), (mode, L, kw)
+                m = fake_osb200.tile_map(mode, L, S, T, **kw)
+                assert m.key()[:4] == (mode, L, S, T)
+                assert 16 <= m.tile_rows <= 128 and m.tile_rows % 16 == 0, (mode, L, kw, m.key())
+                if L <= 64 and kw.get("pack", True) and not kw.get("keys_only", False):
+                    assert m.G == 128 // L and m.tps == 1 and m.G * L <= m.tile_rows < m.G * L + 16, (mode, L, kw, m.key())
+                else:
+                    assert m.G == 1 and m.tps == -(-L // m.tile_rows) and (L > 128) == (m.tile_rows == 128 and m.tps > 1)
+                    assert m.tile_rows * (m.tps - 1) < L <= m.tile_rows * m.tps, (mode, L, kw, m.key())
+                rows = 3 * L * (S if mode == 1 else 1)
+                seqs = rows // L
+                want = -(-seqs // m.G) if m.G > 1 else seqs * m.tps
+                assert osb200._lib.osb_head_tiles_per_head(ctypes.byref(m), rows) == want
