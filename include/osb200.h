@@ -60,8 +60,11 @@ int osb_ln_modulate(const void* x, const float* shift, const float* scale, void*
 typedef enum osb_epilogue {
   OSB_EPI_BIAS = 0,           /* D = A W^T + bias                                              */
   OSB_EPI_BIAS_GELU_TANH = 1, /* D = gelu_tanh(A W^T + bias)      layers.py:277-281 (MLP[0:2]) */
-  OSB_EPI_BIAS_GATE_RES = 2   /* D = R + gate[g,:] * (A W^T + bias); gate==NULL -> plain add   */
+  OSB_EPI_BIAS_GATE_RES = 2,  /* D = R + gate[g,:] * (A W^T + bias); gate==NULL -> plain add   */
                               /*                      layers.py:247-252, 333-334               */
+  OSB_EPI_GATED_GELU = 3,     /* D[:, c] = gelu_tanh(P[:, 2c]) * P[:, 2c+1], P = A W^T + bias: W's rows interleave
+                                 T5's wi_0 (even) and wi_1 (odd), D has N/2 columns (T5DenseGatedActDense)      */
+  OSB_EPI_BIAS_QUICK_GELU = 4 /* D = x * sigmoid(1.702 x), x = A W^T + bias (CLIP mlp.fc1 + quick_gelu)          */
 } osb_epilogue;
 
 typedef struct osb_gemm_args {
@@ -137,6 +140,22 @@ typedef struct osb_attn_short_args {
  * (`attention`), layers.py:126-135 (QKNorm), and upstream STDiT3 Attention / MultiHeadCrossAttention
  * (SURVEY.md §8a-S, Appendix A). */
 int osb_attn_short(const osb_attn_short_args* args, void* stream);
+
+/* osb_attn_short with an additive fp32 bias by relative position: the score of query token i and key token j is
+ * q.k * softmax_scale + bias[h * bias_head_stride + j - i + Lq - 1] (bias: [heads][Lq + Lk - 1], or one shared vector
+ * with bias_head_stride = 0), added before the running maximum.  -inf entries mask keys; key blocks that are -inf for
+ * every query of a 128-row query tile are skipped, and a row never evaluates -inf - (-inf).  head_dim 64 only; kv_lens
+ * and packed short sequences as in osb_attn_short; QK-norm and RoPE arguments keep their meaning.
+ * Replaces the self-attention of HF T5Attention (relative_attention_bias, unscaled scores: softmax_scale = 1) and
+ * CLIPAttention (causal mask: bias 0 for j <= i, -inf for j > i) run by the reference's text_embedder
+ * (opensora/models/text/conditioner.py:10-53). */
+int osb_attn_short_bias(const osb_attn_short_args* args, const float* bias, int64_t bias_head_stride, void* stream);
+
+/* ---- RMSNorm with weight (T5LayerNorm) ----------------------------------------------------------------------------- */
+/* y[r,:] = bf16(w * bf16(x[r,:] * rsqrt(mean(x[r,:]^2) + eps))): fp32 mean of squares, the reference's two roundings
+ * (opensora/acceleration/shardformer/modeling/t5.py:14-27).  x, y: bf16 [rows, C] contiguous, w: bf16 [C].
+ * C % 8 == 0, C <= 4096 (T5-XXL's d_model), 16-byte aligned.  One warp per row, one HBM pass. */
+int osb_rms_norm(const void* x, const void* w, void* y, int64_t rows, int C, float eps, void* stream);
 
 /* ---- head tiles: projection GEMM -> attention without a layout pass ------------------------------------ */
 /* A head tile is the HBM image of one attention operand tile: tile_rows <= 128 token rows of ONE head, head_dim

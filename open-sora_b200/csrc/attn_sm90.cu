@@ -1,6 +1,6 @@
 // Attention on sm_90a: softmax(q k^T * scale) v per (sequence, head), non-causal, exact online softmax.
 //
-// Both entry points run the same flash-attention core.  One CTA (8 warps) owns 128 query rows of one head; every
+// All entry points run the same flash-attention core.  One CTA (8 warps) owns 128 query rows of one head; every
 // warp owns 16 rows and keeps its Q fragments, the running row maximum / sum and the fp32 O accumulator in
 // registers.  Key / value tiles sit in shared memory in the head-tile layout (tiles.cuh: 64-column chunks with the
 // 128-byte swizzle plus the head-dim tail), so the 16-byte rows that ldmatrix gathers are bank-conflict free for
@@ -13,6 +13,10 @@
 //                   on an mbarrier, with the next key tile in flight while the current one is consumed.
 //   osb_attn_short: q / k / v are token-layout rows (any strides); the CTA stages them into the same tile layout,
 //                   applying per-head RMSNorm and RoPE in fp32 on the way, so q / k / v are read exactly once.
+//   osb_attn_short_bias: the osb_attn_short kernel (template kBias) with an fp32 additive bias indexed by the relative
+//                   position, bias[h][j - i + Lq - 1], added to the scaled score before the running max (T5's relative
+//                   attention bias; a 0 / -inf vector is CLIP's causal mask).  Key blocks whose bias is -inf for every
+//                   query of the tile are skipped.
 //
 // Replaces: opensora/models/mmdit/math.py:22-36 (attention), layers.py:102-135 (QK RMSNorm) and the
 // upstream-v1.2 STDiT3 Attention / MultiHeadCrossAttention restated in SURVEY.md App. A.
@@ -55,9 +59,11 @@ __device__ __forceinline__ void flash_load_q(FlashState<D>& f, uint32_t sq, uint
 // One block of up to 64 keys: rows [krow0, krow0 + 16 n16) of the K / V tile images (chunk_bytes apart), whose key
 // slots are key0 + 0, 1, ...  Row i of this thread (i = 0: lane/4, 1: lane/4 + 8) may only see key slots in
 // [lo[i], hi[i]).  sc = softmax scale * log2(e).
-template <int D>
+// kBias: the score of key slot `key` in row i is s * bscale + bias[key + boff_i] (fp32) and sc = log2(e).
+template <int D, bool kBias = false>
 __device__ __forceinline__ void flash_block(FlashState<D>& f, uint32_t sk, uint32_t sv, uint32_t chunk_bytes, int krow0,
-                                            int n16, int key0, const int (&lo)[2], const int (&hi)[2], float sc) {
+                                            int n16, int key0, const int (&lo)[2], const int (&hi)[2], float sc,
+                                            const float* bias = nullptr, int boff0 = 0, int boff1 = 0, float bscale = 0.f) {
   using Cfg = HeadTileCfg<D>;
   constexpr int NB = kKeyBlock / 8;
   const int lane = threadIdx.x & 31;
@@ -86,6 +92,7 @@ __device__ __forceinline__ void flash_block(FlashState<D>& f, uint32_t sk, uint3
       const int i = e >> 1;
       const int key = key0 + 8 * j + 2 * (lane & 3) + (e & 1);
       if (j >= 2 * n16 || key < lo[i] || key >= hi[i]) s[j][e] = -INFINITY;
+      else if constexpr (kBias) s[j][e] = fmaf(s[j][e], bscale, __ldg(bias + key + (i ? boff1 : boff0)));
       mx[i] = fmaxf(mx[i], s[j][e]);
     }
   }
@@ -310,6 +317,9 @@ struct AttnParams {
   float scale_log2;      // softmax_scale * log2(e)
   int32_t G;             // sequences packed per 128-row query tile (1 when Lq >= 128)
   int32_t tiles_per_seq; // query tiles per sequence (G == 1)
+  const float* bias;     // kBias: fp32 [heads][Lq + Lk - 1], head h at bias + h * bias_hs
+  int64_t bias_hs;
+  float scale;           // kBias: softmax_scale (the bias is added to the scaled score)
 };
 
 __device__ __forceinline__ void unpack8(const uint4& t, float* x) {
@@ -398,7 +408,7 @@ __device__ __forceinline__ void stage_row(uint4 (&raw)[HeadTileCfg<D>::U], bool 
     *reinterpret_cast<uint4*>(tile + tile_unit_off<Cfg::MAIN>(row, u, chunk_bytes)) = u < U ? raw[u] : make_uint4(0, 0, 0, 0);
 }
 
-template <int D>
+template <int D, bool kBias>
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_short_kernel(const AttnParams p) {
   using Cfg = HeadTileCfg<D>;
   constexpr int U = Cfg::U;
@@ -446,6 +456,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_short_kernel(const AttnP
 
   // my two query rows: valid key slots [lo, hi) and output pointers
   int lo[2], hi[2];
+  int boff[2] = {0, 0};   // kBias: bias index of key slot `key` = key + boff (= key token - query token + Lq - 1)
   __nv_bfloat16* dst[2] = {nullptr, nullptr};
   int nkeys = 0;   // key slots any row of the CTA may see
 #pragma unroll
@@ -460,6 +471,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_short_kernel(const AttnP
       len = len < p.Lk ? (len < 0 ? 0 : len) : p.Lk;
       lo[i] = g * p.Lk;
       hi[i] = lo[i] + len;
+      if constexpr (kBias) boff[i] = p.Lq - 1 - tok - lo[i];
       dst[i] = p.out + row_of(seq, tok, p.q_bs, p.q_ss, p.q_ts) * p.out_ld + (int64_t)h * D;
     }
     nkeys = hi[i] > nkeys ? hi[i] : nkeys;
@@ -471,7 +483,20 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_short_kernel(const AttnP
   FlashState<D> f;
   flash_load_q<D>(f, smem_u32(sQ), 128u * 128u);
   const float sc = p.scale_log2;
+  const float* bh = nullptr;
+  if constexpr (kBias) bh = p.bias + (int64_t)h * p.bias_hs;
   for (int k0 = 0; k0 < nkeys; k0 += kKeyBlock) {
+    if constexpr (kBias) {
+      // Skip the block when the bias is -inf for every (query, key) pair of the tile: the pairs cover the relative
+      // positions [k0 - last query, block end - first query], at most 64 + 127 of them, one per thread.
+      if (p.G == 1) {
+        const int iq0 = qt * 128, iq1 = (iq0 + 128 < p.Lq ? iq0 + 128 : p.Lq) - 1;
+        const int kend = k0 + kKeyBlock < nkeys ? k0 + kKeyBlock : nkeys;
+        const int d0 = k0 - iq1 + p.Lq - 1, d1 = kend - 1 - iq0 + p.Lq - 1;
+        const bool live = d0 + tid <= d1 && __ldg(bh + d0 + tid) != -INFINITY;
+        if (!__syncthreads_or(live)) continue;
+      }
+    }
     // ---- stage keys / values [k0, k0 + 64): K with RMSNorm + RoPE, V as is ----
     for (int s = tid; s < kKeyBlock; s += kAttnThreads) {
       const int slot = k0 + s;
@@ -499,29 +524,34 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_short_kernel(const AttnP
     }
     __syncthreads();
     const int n = nkeys - k0 < kKeyBlock ? nkeys - k0 : kKeyBlock;
-    flash_block<D>(f, smem_u32(sK), smem_u32(sV), kKeyBlock * 128u, 0, (n + 15) >> 4, k0, lo, hi, sc);
+    if constexpr (kBias)
+      flash_block<D, true>(f, smem_u32(sK), smem_u32(sV), kKeyBlock * 128u, 0, (n + 15) >> 4, k0, lo, hi, sc, bh, boff[0],
+                           boff[1], p.scale);
+    else
+      flash_block<D>(f, smem_u32(sK), smem_u32(sV), kKeyBlock * 128u, 0, (n + 15) >> 4, k0, lo, hi, sc);
     __syncthreads();   // the next block overwrites sK / sV
   }
   pdl_launch_dependents();
   flash_store<D>(f, dst[0], dst[1]);
 }
 
-template <int D>
+template <int D, bool kBias = false>
 static int attn_short_launch(const AttnParams& p, int64_t units, int H, cudaStream_t stream) {
   using Cfg = HeadTileCfg<D>;
   const int smem = (128 + 2 * kKeyBlock) * Cfg::ROW_BYTES;
   cudaLaunchAttribute attr[2];
   cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)units, (unsigned)H), dim3(kAttnThreads), smem, stream, attr);
-  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_short_kernel<D>, p));
+  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_short_kernel<D, kBias>, p));
   count_launch();
   return OSB_OK;
 }
 
 int attn_init() {
   constexpr int kMax = 200 * 1024;   // largest carve-up: 128-row Q slot + two K/V stages of 128-row D = 128 tiles
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<72>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<72, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<72>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
@@ -585,7 +615,8 @@ extern "C" int osb_attn_tiles(const osb_attn_tiles_args* a, void* stream) {
   return attn_tiles_launch<128>(p, a->num_heads, s);
 }
 
-extern "C" int osb_attn_short(const osb_attn_short_args* a, void* stream) {
+// Argument checks and launch shared by osb_attn_short and osb_attn_short_bias (bias == nullptr: the plain kernel).
+static int attn_short_entry(const osb_attn_short_args* a, const float* bias, int64_t bias_head_stride, void* stream) {
   using namespace osb;
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
   OSB_REQUIRE(a != nullptr, "osb_attn_short: null args");
@@ -640,7 +671,23 @@ extern "C" int osb_attn_short(const osb_attn_short_args* a, void* stream) {
   OSB_REQUIRE((int64_t)p.G * a->Lk < (1ll << 31), "osb_attn_short: too many keys per query tile");
   OSB_REQUIRE(units <= 0x7fffffff && a->num_heads <= 65535, "osb_attn_short: grid too large");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  p.bias = bias;
+  p.bias_hs = bias_head_stride;
+  p.scale = a->softmax_scale;
+  if (bias != nullptr) {
+    OSB_REQUIRE(D == 64, "osb_attn_short_bias: head_dim %d not built (64)", D);
+    OSB_REQUIRE(bias_head_stride >= 0, "osb_attn_short_bias: negative bias_head_stride");
+    p.scale_log2 = 1.4426950408889634f;   // the scale is applied before the bias is added
+    return attn_short_launch<64, true>(p, units, a->num_heads, s);
+  }
   if (D == 64) return attn_short_launch<64>(p, units, a->num_heads, s);
   if (D == 72) return attn_short_launch<72>(p, units, a->num_heads, s);
   return attn_short_launch<128>(p, units, a->num_heads, s);
+}
+
+extern "C" int osb_attn_short(const osb_attn_short_args* a, void* stream) { return attn_short_entry(a, nullptr, 0, stream); }
+
+extern "C" int osb_attn_short_bias(const osb_attn_short_args* a, const float* bias, int64_t bias_head_stride, void* stream) {
+  if (bias == nullptr) { osb::set_error("osb_attn_short_bias: null bias"); return OSB_ERR_INVALID; }
+  return attn_short_entry(a, bias, bias_head_stride, stream);
 }

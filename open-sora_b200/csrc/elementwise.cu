@@ -100,8 +100,90 @@ ln_modulate_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict_
   }
 }
 
+// T5LayerNorm (RMSNorm with weight): y = bf16(w * bf16(x * rsqrt(mean(x^2) + eps))), fp32 mean of squares, the two
+// roundings of the reference (shardformer/modeling/t5.py:14-27, transformers T5LayerNorm).  One warp per row.
+template <int NCH>
+__global__ void __launch_bounds__(kLnWarpsPerBlock * 32)
+rms_norm_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ y,
+                int64_t rows, int C, float eps) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * kLnWarpsPerBlock + (threadIdx.x >> 5);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (row >= rows) return;
+  const int nchunks = C >> 3;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + row * C);
+  float v[NCH][8];
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+      uint4 t;
+      asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+                   : "=r"(t.x), "=r"(t.y), "=r"(t.z), "=r"(t.w) : "l"(xr + c));
+      const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = unpack_bf16x2(tw[e]);
+        v[i][2 * e] = f.x;
+        v[i][2 * e + 1] = f.y;
+        ss += f.x * f.x + f.y * f.y;
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  const float r = rsqrtf(ss / (float)C + eps);
+  uint4* yr = reinterpret_cast<uint4*>(y + row * C);
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+      const uint4 wt = __ldg(reinterpret_cast<const uint4*>(w) + c);
+      const uint32_t ww[4] = {wt.x, wt.y, wt.z, wt.w};
+      uint32_t o[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 wf = unpack_bf16x2(ww[e]);
+        const float a = __bfloat162float(__float2bfloat16_rn(v[i][2 * e] * r));
+        const float b = __bfloat162float(__float2bfloat16_rn(v[i][2 * e + 1] * r));
+        o[e] = pack_bf16x2(wf.x * a, wf.y * b);
+      }
+      yr[c] = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+  }
+}
 
 }  // namespace osb
+
+extern "C" int osb_rms_norm(const void* x, const void* w, void* y, int64_t rows, int C, float eps, void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(x && w && y, "osb_rms_norm: null tensor");
+  OSB_REQUIRE(rows > 0, "osb_rms_norm: rows must be positive");
+  OSB_REQUIRE(C > 0 && C % 8 == 0 && C <= 4096, "osb_rms_norm: C must be a multiple of 8 and <= 4096 (got %d)", C);
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(y)) & 15) == 0,
+              "osb_rms_norm: tensors must be 16-byte aligned");
+  const int nch = (C / 8 + 31) / 32;
+  const unsigned blocks = (unsigned)((rows + kLnWarpsPerBlock - 1) / kLnWarpsPerBlock);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const __nv_bfloat16* xb = static_cast<const __nv_bfloat16*>(x);
+  const __nv_bfloat16* wb = static_cast<const __nv_bfloat16*>(w);
+  __nv_bfloat16* yb = static_cast<__nv_bfloat16*>(y);
+#define OSB_RMS_CASE(N)                                                                                       \
+  if (nch <= N) {                                                                                             \
+    cudaLaunchAttribute attr[2];                                                                              \
+    cudaLaunchConfig_t cfg = launch_config(dim3(blocks), dim3(kLnWarpsPerBlock * 32), 0, s, attr);            \
+    OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, rms_norm_kernel<N>, xb, wb, yb, rows, C, eps));                    \
+    count_launch();                                                                                           \
+    return OSB_OK;                                                                                            \
+  }
+  OSB_RMS_CASE(1) OSB_RMS_CASE(2) OSB_RMS_CASE(4) OSB_RMS_CASE(8) OSB_RMS_CASE(16)
+#undef OSB_RMS_CASE
+  set_error("osb_rms_norm: unsupported C %d", C);
+  return OSB_ERR_UNSUPPORTED;
+}
 
 static int ln_modulate_launch(const void* x, const float* shift, const float* scale, void* y,
                               int64_t rows, int C, int64_t group_rows, const int32_t* mod_index,

@@ -8,13 +8,16 @@
 // One wgmma group stays in flight while the next stage is waited for; a stage is handed back to the producer as soon
 // as the group that read it has retired.
 //
-// The same main loop serves four front ends (template kMode):
+// The same main loop serves five front ends (template kMode):
 //   kPlain      nn.Linear with fused bias / GELU(tanh) / gate * x + residual epilogues;
 //   kConv       causal 3D convolution as implicit GEMM: every k-block is ONE 5-D TMA box of the padded NDHWC input;
 //   kHeadTiles  q / k / v projection whose epilogue writes per-head operand tiles (tiles.cuh) with RMSNorm + RoPE;
 //   kLora       kPlain plus an unmerged low-rank update: after the K loop the producer streams ceil(r / 64) more
 //               k-blocks, U = x A^T [M, r] in the A slot and s B [N, r] in the W slot, through the same stage ring, so
 //               A W^T + U (s B)^T lands in one fp32 accumulator before the unchanged epilogue.
+//   kText       nn.Linear with the text encoders' activations: T5's gated GELU gelu_tanh(x wi_0^T) * (x wi_1^T) over a
+//               weight whose rows interleave wi_0 and wi_1 (both halves of an output column sit in one thread's
+//               accumulator pair, the [M, 2 d_ff] product never leaves registers), and CLIP's bias + quick GELU.
 //
 // Replaces every nn.Linear on the denoiser block path of the reference
 // (opensora/models/mmdit/layers.py:209-214,247-252,277-281,314-334,401) and the fused epilogues
@@ -32,7 +35,7 @@ constexpr int kBlockK = 64;
 constexpr int kNumThreads = 384;            // producer warpgroup + two consumer warpgroups
 constexpr int kStageBudget = 200 * 1024;    // operand ring (one CTA per SM; 227 KB is the per-block limit)
 
-enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3 };
+enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4 };
 
 struct GemmEpilogueParams {
   const __nv_bfloat16* bias;
@@ -301,6 +304,32 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           *reinterpret_cast<uint32_t*>(dst + tile_unit_off<HT::MAIN>(r, HT::U, chunk_bytes) + c_frag * 2) = 0u;
       }
     }
+  } else if constexpr (kMode == kText) {
+    // ===================== epilogue: gated GELU / bias + quick GELU =====================
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
+      if (row >= p.M) continue;
+      __nv_bfloat16* drow = p.D + row * p.ldd;
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int64_t n = n_blk * BLOCK_N + 8 * j + c_frag;
+        if (n >= p.N) continue;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (p.bias) {
+          const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+          v0 += b.x;
+          v1 += b.y;
+        }
+        if (p.epilogue == OSB_EPI_GATED_GELU) {   // columns (n, n + 1) = (wi_0, wi_1) of output column n / 2
+          drow[n >> 1] = __float2bfloat16_rn(gelu_tanh(v0) * v1);
+        } else {                                  // x * sigmoid(1.702 x)
+          v0 = v0 / (1.0f + __expf(-1.702f * v0));
+          v1 = v1 / (1.0f + __expf(-1.702f * v1));
+          *reinterpret_cast<uint32_t*>(drow + n) = pack_bf16x2(v0, v1);
+        }
+      }
+    }
   } else {
     // ===================== epilogue: bias / GELU / gate + residual =====================
     const uint32_t group_rows32 = (uint32_t)(p.group_rows > 0xffffffffll ? 0xffffffffu : p.group_rows);
@@ -413,6 +442,7 @@ static int launch_gemm(const osb_gemm_args& a, bool has_res, cudaStream_t stream
   const int64_t tiles = ((a.M + kBlockM - 1) / kBlockM) * ((a.N + BLOCK_N - 1) / BLOCK_N);
   ConvGeom cg = {};
   HeadTileParams ht = {};
+  if (lora == nullptr && a.epilogue >= OSB_EPI_GATED_GELU) return launch_kernel<BLOCK_N, kText>(ta, tw, p, cg, ht, tiles, stream);
   if (lora == nullptr) return launch_kernel<BLOCK_N, kPlain>(ta, tw, p, cg, ht, tiles, stream);
   CUtensorMap tu, tlb;
   if ((rc = make_tmap_2d_bf16(&tu, lora->U, a.M, lora->r, lora->ldu, kBlockM, kBlockK))) return rc;
@@ -444,6 +474,10 @@ int gemm_init() {
   if ((rc = init_one<128, kLora>())) return rc;
   if ((rc = init_one<192, kLora>())) return rc;
   if ((rc = init_one<256, kLora>())) return rc;
+  if ((rc = init_one<64, kText>())) return rc;
+  if ((rc = init_one<128, kText>())) return rc;
+  if ((rc = init_one<192, kText>())) return rc;
+  if ((rc = init_one<256, kText>())) return rc;
   return OSB_OK;
 }
 
@@ -513,8 +547,10 @@ static int gemm_dispatch(const char* fn, const osb_gemm_args* args, const osb_lo
               (long long)a.K, (long long)a.N);
   OSB_REQUIRE(a.ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(a.D) & 15) == 0,
               "%s: D must be 16-byte aligned with ldd %% 8 == 0", fn);
-  OSB_REQUIRE(a.epilogue >= OSB_EPI_BIAS && a.epilogue <= OSB_EPI_BIAS_GATE_RES,
+  OSB_REQUIRE(a.epilogue >= OSB_EPI_BIAS && a.epilogue <= OSB_EPI_BIAS_QUICK_GELU,
               "%s: unknown epilogue %d", fn, a.epilogue);
+  OSB_REQUIRE(lora == nullptr || a.epilogue <= OSB_EPI_BIAS_GATE_RES,
+              "%s: epilogue %d is not built with a LoRA update", fn, a.epilogue);
   if (a.epilogue == OSB_EPI_BIAS_GATE_RES) {
     OSB_REQUIRE(a.R == nullptr || (a.ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(a.R) & 15) == 0),
                 "%s: R must be 16-byte aligned with ldr %% 8 == 0", fn);

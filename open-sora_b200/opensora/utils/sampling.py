@@ -229,6 +229,33 @@ def prepare_ids(img: Tensor, t5_embedding: Tensor, clip_embedding: Tensor) -> di
             "y_vec": _broadcast_batch(clip_embedding, bs).to(device, dtype)}
 
 
+def prepare_models(cfg, device, dtype, offload_model: bool = False):
+    """:511-559.  Builds (model, model_ae, model_t5, model_clip, optional_models) from the config's `model`, `ae`, `t5` and
+    `clip` dicts through the registry, with `device_map` / `torch_dtype` as the reference passes them;
+    `pretrained_lora_path` goes through `load_lora`.  The text-to-image-to-video models (`img_flux`, `img_flux_ae`) need
+    the Flux image autoencoder, which is not registered here."""
+    from opensora.registry import MODELS, build_module
+
+    if cfg.get("img_flux", None) is not None and "autoencoder_2d" not in MODELS:
+        raise KeyError("img_flux_ae needs the Flux image autoencoder (type 'autoencoder_2d'), which is not registered in "
+                       "this package")
+    model_device = "cpu" if offload_model and cfg.get("img_flux", None) is not None else device
+    model = build_module(cfg.get("model"), MODELS, device_map=model_device, torch_dtype=dtype).eval()
+    model_ae = build_module(cfg.get("ae"), MODELS, device_map=model_device, torch_dtype=dtype).eval()
+    model_t5 = build_module(cfg.get("t5"), MODELS, device_map=device, torch_dtype=dtype).eval()
+    model_clip = build_module(cfg.get("clip"), MODELS, device_map=device, torch_dtype=dtype).eval()
+    if cfg.get("pretrained_lora_path", None) is not None:
+        from opensora.utils.lora import load_lora
+
+        model = load_lora(model, cfg.get("pretrained_lora_path"))
+    optional_models = {}
+    if cfg.get("img_flux", None) is not None:
+        optional_models["img_flux"] = build_module(cfg.get("img_flux"), MODELS, device_map=device, torch_dtype=dtype).eval()
+        optional_models["img_flux_ae"] = build_module(cfg.get("img_flux_ae"), MODELS, device_map=device,
+                                                      torch_dtype=dtype).eval()
+    return model, model_ae, model_t5, model_clip, optional_models
+
+
 def prepare_api(model, model_ae, model_t5, model_clip, optional_models: dict):
     """:562-726.  Returns `api_fn(opt, cond_type="t2v", seed=None, sigma_min=1e-5, text=None, neg=None, patch_size=2,
     channel=16, **kwargs)`: noise -> schedule -> guidance prompts -> model inputs -> conditioning -> denoise -> unpack ->

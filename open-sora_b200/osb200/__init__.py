@@ -34,9 +34,12 @@ EXPORTS = (
     "osb_comm_barrier",
     "osb_rf_masked_step",
     "osb_gemm_lora",
+    "osb_attn_short_bias",
+    "osb_rms_norm",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
+EPI_GATED_GELU, EPI_BIAS_QUICK_GELU = 3, 4
 
 
 class OsbError(RuntimeError):
@@ -63,6 +66,8 @@ def _load() -> C.CDLL:
     lib.osb_gemm_bf16.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_gemm_lora.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
+    lib.osb_attn_short_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.osb_rms_norm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_void_p]
     lib.osb_conv3d_ndhwc.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_vae_prep.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_cfg_euler.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float,
@@ -311,6 +316,21 @@ def ln_modulate(x, shift, scale, *, group_rows: int, mod_index=None, eps: float 
     return out
 
 
+def rms_norm(x, w, *, eps: float = 1e-6, out=None):
+    """y = bf16(w * bf16(x * rsqrt(mean(x^2) + eps))) per row (osb_rms_norm, T5LayerNorm); x bf16 [rows, C], w bf16 [C]."""
+    import torch
+
+    _need(x, torch.bfloat16, "x"); _need(w, torch.bfloat16, "w")
+    if x.dim() != 2 or not x.is_contiguous() or w.shape != (x.shape[1],):
+        raise OsbError(f"rms_norm: x must be a contiguous [rows, C] tensor and w [C], got {tuple(x.shape)} and {tuple(w.shape)}")
+    if out is None:
+        out = torch.empty_like(x)
+    rows, Cdim = x.shape
+    with _Timed("rms_norm", 4.0 * rows * Cdim):  # algorithmic bytes: read x + write y (bf16)
+        _check(_lib.osb_rms_norm(_ptr(x), _ptr(w), _ptr(out), rows, Cdim, eps, _stream()), "osb_rms_norm")
+    return out
+
+
 def _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, cta_group, block_n):
     import torch
 
@@ -320,8 +340,8 @@ def _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out,
     assert a.dim() == 2 and w.dim() == 2 and a.shape[1] == w.shape[1]
     M, K = a.shape
     N = w.shape[0]
-    if out is None:
-        out = torch.empty((M, N), dtype=torch.bfloat16, device=a.device)
+    if out is None:   # the gated GELU writes one column per (wi_0, wi_1) row pair of w
+        out = torch.empty((M, N // 2 if epilogue == EPI_GATED_GELU else N), dtype=torch.bfloat16, device=a.device)
     _need(out, torch.bfloat16, "out")
     args = GemmArgs()
     args.A, args.W, args.bias, args.D = a.data_ptr(), w.data_ptr(), (bias.data_ptr() if bias is not None else None), out.data_ptr()
@@ -340,7 +360,9 @@ def _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out,
 def gemm(a, w, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None, group_rows: int = 0,
          mod_index=None, out=None, cta_group: int = 0, block_n: int = 0):
     """out = epilogue(a @ w.T + bias).  a bf16 [M,K] (row stride free), w bf16 [N,K], bias bf16 [N].
-    GATE_RES: out = residual + gate[g] * (a @ w.T + bias), gate fp32 [G, N] view, may be None."""
+    GATE_RES: out = residual + gate[g] * (a @ w.T + bias), gate fp32 [G, N] view, may be None.
+    GATED_GELU: out [M, N/2], out[:, c] = gelu_tanh(p[:, 2c]) * p[:, 2c+1], p = a @ w.T + bias (w's rows interleave
+    T5's wi_0 and wi_1, see interleave_gated).  BIAS_QUICK_GELU: out = p * sigmoid(1.702 p) (CLIP)."""
     args, out = _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, cta_group, block_n)
     with _Timed("gemm", 2.0 * args.M * args.N * args.K):  # algorithmic FLOPs
         _check(_lib.osb_gemm_bf16(C.byref(args), _stream()), "osb_gemm_bf16")
@@ -366,12 +388,16 @@ def gemm_lora(a, w, bias, u, b, *, epilogue: int = EPI_BIAS, residual=None, gate
     return out
 
 
-def attn_short(q, k, v, out, *, num_seqs: int, seqs_per_batch: int, q_strides, k_strides, Lq: int, Lk: int,
-               num_heads: int, head_dim: int, kv_lens=None, q_norm_w=None, k_norm_w=None, norm_eps: float = 1e-6,
-               rope_cos=None, rope_sin=None, softmax_scale: float | None = None, q_norm_w2=None, k_norm_w2=None,
-               norm_split: int = 0, impl: int = 0, rope_half: bool = False):
-    """softmax(q k^T * scale) v per (sequence, head) with optional fused QK-RMSNorm and RoPE.
-    q/k/v/out are 2-D bf16 views [rows, ld]; *_strides = (batch, seq, token) strides in rows."""
+def interleave_gated(wi_0, wi_1):
+    """[2 d_ff, d_model] weight of the gated-GELU GEMM: row 2c = wi_0[c], row 2c + 1 = wi_1[c]."""
+    import torch
+
+    return torch.stack((wi_0, wi_1), dim=1).reshape(2 * wi_0.shape[0], wi_0.shape[1]).contiguous()
+
+
+def _attn_short_struct(q, k, v, out, *, num_seqs, seqs_per_batch, q_strides, k_strides, Lq, Lk, num_heads, head_dim,
+                       kv_lens, q_norm_w, k_norm_w, norm_eps, rope_cos, rope_sin, softmax_scale, q_norm_w2, k_norm_w2,
+                       norm_split, impl, rope_half):
     import torch
 
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out"), (q_norm_w, "q_norm_w"), (k_norm_w, "k_norm_w")):
@@ -399,8 +425,45 @@ def attn_short(q, k, v, out, *, num_seqs: int, seqs_per_batch: int, q_strides, k
     a.norm_split = norm_split
     a.rope_half = int(rope_half)
     a.reserved = impl   # implementation switch of the C ABI; every value runs the one sm_90a kernel
+    return a
+
+
+def attn_short(q, k, v, out, *, num_seqs: int, seqs_per_batch: int, q_strides, k_strides, Lq: int, Lk: int,
+               num_heads: int, head_dim: int, kv_lens=None, q_norm_w=None, k_norm_w=None, norm_eps: float = 1e-6,
+               rope_cos=None, rope_sin=None, softmax_scale: float | None = None, q_norm_w2=None, k_norm_w2=None,
+               norm_split: int = 0, impl: int = 0, rope_half: bool = False):
+    """softmax(q k^T * scale) v per (sequence, head) with optional fused QK-RMSNorm and RoPE.
+    q/k/v/out are 2-D bf16 views [rows, ld]; *_strides = (batch, seq, token) strides in rows."""
+    a = _attn_short_struct(q, k, v, out, num_seqs=num_seqs, seqs_per_batch=seqs_per_batch, q_strides=q_strides,
+                           k_strides=k_strides, Lq=Lq, Lk=Lk, num_heads=num_heads, head_dim=head_dim, kv_lens=kv_lens,
+                           q_norm_w=q_norm_w, k_norm_w=k_norm_w, norm_eps=norm_eps, rope_cos=rope_cos, rope_sin=rope_sin,
+                           softmax_scale=softmax_scale, q_norm_w2=q_norm_w2, k_norm_w2=k_norm_w2, norm_split=norm_split,
+                           impl=impl, rope_half=rope_half)
     with _Timed("attn_short", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):  # QK^T + PV FLOPs
         _check(_lib.osb_attn_short(C.byref(a), _stream()), "osb_attn_short")
+    return out
+
+
+def attn_short_bias(q, k, v, out, bias, *, num_seqs: int, seqs_per_batch: int, q_strides, k_strides, Lq: int, Lk: int,
+                    num_heads: int, head_dim: int, kv_lens=None, softmax_scale: float | None = None):
+    """attn_short with an additive fp32 bias by relative position (osb_attn_short_bias): the score of query token i and
+    key token j is q.k * scale + bias[h, j - i + Lq - 1].  bias fp32 [num_heads, Lq + Lk - 1] (T5's relative attention
+    bias) or [Lq + Lk - 1] shared by all heads (0 / -inf: a causal mask)."""
+    import torch
+
+    _need(bias, torch.float32, "bias")
+    n = Lq + Lk - 1
+    if bias is None or not bias.is_contiguous() or bias.shape not in ((n,), (num_heads, n)):
+        raise OsbError(f"attn_short_bias: bias must be a contiguous fp32 [{n}] or [{num_heads}, {n}] tensor, got "
+                       f"{None if bias is None else tuple(bias.shape)}")
+    a = _attn_short_struct(q, k, v, out, num_seqs=num_seqs, seqs_per_batch=seqs_per_batch, q_strides=q_strides,
+                           k_strides=k_strides, Lq=Lq, Lk=Lk, num_heads=num_heads, head_dim=head_dim, kv_lens=kv_lens,
+                           q_norm_w=None, k_norm_w=None, norm_eps=1e-6, rope_cos=None, rope_sin=None,
+                           softmax_scale=softmax_scale, q_norm_w2=None, k_norm_w2=None, norm_split=0, impl=0,
+                           rope_half=False)
+    with _Timed("attn_short", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):
+        _check(_lib.osb_attn_short_bias(C.byref(a), _ptr(bias), n if bias.dim() == 2 else 0, _stream()),
+               "osb_attn_short_bias")
     return out
 
 
