@@ -107,6 +107,48 @@ typedef struct osb_lora_args {
  * Replaces the unmerged peft LoRA layer the reference wraps the denoiser with (opensora/utils/sampling.py:542-545). */
 int osb_gemm_lora(const osb_gemm_args* gemm, const osb_lora_args* lora, void* stream);
 
+/* ---- FP8 (e4m3) with per-row scales: the opt-in MLP path of STDiT3 ------------------------------------------------ */
+/* Quantization rule shared by the three entry points below: a row r of a matrix X gets s[r] = amax(|X[r, :]|) / 448
+ * (s = 1 for an all-zero row) and codes e4m3_rn_satfinite(X[r, k] / s[r]).  e4m3 tensors are one byte per element,
+ * row-major with an explicit leading dimension in elements (= bytes). */
+typedef struct osb_gemm_fp8_args {
+  const void* A;         /* e4m3 [M,K], row stride lda                                                 */
+  const void* W;         /* e4m3 [N,K], row stride ldw  (quantized nn.Linear.weight)                    */
+  const float* a_scale;  /* fp32 [M]: the row scales of A                                               */
+  const float* w_scale;  /* fp32 [N]: the row scales of W (per output channel)                          */
+  const void* bias;      /* bf16 [N] or NULL                                                            */
+  void* D;               /* bf16 [M,N], row stride ldd                                                  */
+  const void* R;         /* bf16 [M,N] residual (GATE_RES only), row stride ldr; may alias D            */
+  const float* gate;     /* fp32, row g at gate + g*gate_stride (GATE_RES only) or NULL                 */
+  const int32_t* mod_index; /* optional indirection for g, as in osb_ln_modulate                       */
+  int64_t M, N, K;
+  int64_t lda, ldw, ldd, ldr;
+  int64_t group_rows;    /* g = row / group_rows                                                        */
+  int64_t gate_stride;
+  int32_t epilogue;      /* OSB_EPI_BIAS, OSB_EPI_BIAS_GELU_TANH or OSB_EPI_BIAS_GATE_RES               */
+  int32_t block_n;       /* 0 = library default, else 64 or 128                                         */
+} osb_gemm_fp8_args;
+
+/* D = epilogue(acc * (a_scale[m] * w_scale[n]) + bias), acc = the sum of the e4m3 products of row m of A and row n of W:
+ * the tensor core (wgmma m64nNk32 e4m3) sums each 128-element k-block, whose partial is then added into an fp32
+ * register accumulator (the FP8 MMA's own accumulation keeps fewer mantissa bits than fp32 and is never carried across
+ * k-blocks).  The epilogues and their gate / residual / mod_index rules are those of osb_gemm_bf16, with one rounding
+ * to bf16.  Replaces the two Linear layers of the STDiT3 block MLP when FP8 is enabled.
+ * Requires K % 128 == 0, N % 8 == 0, lda, ldw multiples of 16 and 16-byte aligned A, W. */
+int osb_gemm_fp8(const osb_gemm_fp8_args* args, void* stream);
+
+/* osb_ln_modulate whose fp32 result row is quantized directly (no bf16 rounding) to e4m3 y8 [rows, C] (contiguous)
+ * with its scale in y_scale[row].  Same group_rows / mod_index / mod_stride / eps arguments; C % 8 == 0, C <= 4096. */
+int osb_ln_modulate_fp8(const void* x, const float* shift, const float* scale, void* y8, float* y_scale,
+                        int64_t rows, int C, int64_t group_rows, const int32_t* mod_index,
+                        int64_t mod_stride, float eps, void* stream);
+
+/* Row quantizer: bf16 x [rows, K] (row stride ldx) -> e4m3 y8 [rows, K] (row stride ldy) and fp32 y_scale [rows], in
+ * one pass over x (the row stays in registers between its amax and its codes).  K % 8 == 0, K <= 8192, ldx % 8 == 0,
+ * ldy % 16 == 0, 16-byte aligned x and y8. */
+int osb_quant_rows_fp8(const void* x, int64_t ldx, void* y8, int64_t ldy, float* y_scale, int64_t rows, int K,
+                       void* stream);
+
 /* ---- attention with short key sets (whole key set resident in one CTA) -------------------- */
 typedef struct osb_attn_short_args {
   const void* q; const void* k; const void* v; /* bf16; element (row, h*D + d) at ptr + row*ld + h*D + d */

@@ -39,7 +39,10 @@ int sm_count() { return g_sms; }
 // sequence-parallel rank with 2 048 tokens is host-bound on cuTensorMapEncodeTiled otherwise.
 struct TmapKey {
   uint64_t base, rows, cols, ld, box;
-  bool operator==(const TmapKey& o) const { return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box; }
+  uint32_t elem_bytes;
+  bool operator==(const TmapKey& o) const {
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box && elem_bytes == o.elem_bytes;
+  }
 };
 struct TmapKeyHash {
   size_t operator()(const TmapKey& k) const {
@@ -55,13 +58,14 @@ static std::mutex g_tmap_mu;
 static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> g_tmap_cache;
 static std::atomic<int64_t> g_tmap_hits{0}, g_tmap_misses{0};
 
-int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
-                      uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
+// elem_bytes 2: bf16, 1: e4m3 (ld and cols in elements; the swizzle row is 128 bytes either way)
+static int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                        uint32_t box_cols, uint32_t elem_bytes) {
   if (!g_encode) {
     set_error("osb_init() has not been called");
     return OSB_ERR_NOT_INIT;
   }
-  const TmapKey key{reinterpret_cast<uint64_t>(base), rows, cols, ld, ((uint64_t)box_rows << 32) | box_cols};
+  const TmapKey key{reinterpret_cast<uint64_t>(base), rows, cols, ld, ((uint64_t)box_rows << 32) | box_cols, elem_bytes};
   {
     std::lock_guard<std::mutex> lk(g_tmap_mu);
     auto it = g_tmap_cache.find(key);
@@ -72,16 +76,17 @@ int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_
     }
   }
   g_tmap_misses.fetch_add(1, std::memory_order_relaxed);
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * 2) & 15)) {
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * elem_bytes) & 15)) {
     set_error("TMA operand must be 16-byte aligned (base %p, ld %llu elements)", base,
               (unsigned long long)ld);
     return OSB_ERR_INVALID;
   }
   cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstride[1] = {ld * 2};  // bytes, dims 1..rank-1
+  cuuint64_t gstride[1] = {ld * elem_bytes};  // bytes, dims 1..rank-1
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estride[2] = {1, 1};
-  CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim,
+  CUresult r = g_encode(map, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                        const_cast<void*>(base), gdim,
                         gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -97,6 +102,16 @@ int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_
     g_tmap_cache.emplace(key, *map);
   }
   return OSB_OK;
+}
+
+int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
+                      uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(map, base, rows, cols, ld, box_rows, box_cols, 2);
+}
+
+int make_tmap_2d_e4m3(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
+                      uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(map, base, rows, cols, ld, box_rows, box_cols, 1);
 }
 
 int make_tmap_5d_bf16(CUtensorMap* map, const void* base, const uint64_t dims[5], const uint64_t strides_bytes[4],

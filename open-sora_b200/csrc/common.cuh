@@ -70,6 +70,9 @@ inline cudaLaunchConfig_t launch_config(dim3 grid, dim3 block, size_t smem, cuda
 
 int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
                       uint64_t ld, uint32_t box_rows, uint32_t box_cols);
+// the same over a one-byte e4m3 matrix (box_cols must be 128: one 128-byte swizzle row)
+int make_tmap_2d_e4m3(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
+                      uint64_t ld, uint32_t box_rows, uint32_t box_cols);
 
 struct RowScatter;
 // validates an osb_scatter and copies it into the kernel-parameter form; rows = rows the producer writes

@@ -5,6 +5,9 @@
 // algorithmic traffic = read x + write y = 4 bytes per element.
 // Replaces: opensora/models/mmdit/layers.py:205-206,223-224,248,252,312,400 and upstream v1.2
 // t2i_modulate(norm(x), shift, scale) (SURVEY.md §8a-S).
+//
+// osb_ln_modulate_fp8 / osb_quant_rows_fp8: the FP8 (e4m3) row quantization of the opt-in MLP path, s = amax / 448 per
+// row, codes e4m3_rn_satfinite(x / s); the row is register-resident, so its amax is one more warp reduction.
 #include "common.cuh"
 
 namespace osb {
@@ -96,6 +99,164 @@ ln_modulate_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict_
       t.z = pack_bf16x2(o[4], o[5]);
       t.w = pack_bf16x2(o[6], o[7]);
       yr[c] = t;
+    }
+  }
+}
+
+// ---- FP8 (e4m3) row quantization ----------------------------------------------------------------------------------
+// two e4m3 codes, round to nearest even, saturated to +-448 (`lo` in the low byte)
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// the row scale from the warp's partial amax values: amax / 448, 1 for an all-zero row
+__device__ __forceinline__ float fp8_row_scale(float amax) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  return amax > 0.f ? amax / 448.0f : 1.0f;
+}
+// eight values -> eight codes (x / s, IEEE division as the contract states it)
+__device__ __forceinline__ uint2 e4m3x8(const float (&o)[8], float s) {
+  uint2 q;
+  q.x = e4m3x2(o[0] / s, o[1] / s) | (e4m3x2(o[2] / s, o[3] / s) << 16);
+  q.y = e4m3x2(o[4] / s, o[5] / s) | (e4m3x2(o[6] / s, o[7] / s) << 16);
+  return q;
+}
+
+// osb_ln_modulate with the fp32 result quantized per row: the modulated row replaces the input row in registers, its
+// amax is reduced over the warp, and the codes go out as 8 bytes per 16-byte input chunk.
+template <int NCH>
+__global__ void __launch_bounds__(kLnWarpsPerBlock * 32)
+ln_modulate_fp8_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ shift,
+                       const float* __restrict__ scale, uint8_t* __restrict__ y8, float* __restrict__ y_scale, int64_t rows,
+                       int C, int64_t group_rows, const int32_t* __restrict__ mod_index, int64_t mod_stride, float eps) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * kLnWarpsPerBlock + (threadIdx.x >> 5);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (row >= rows) return;
+  const int nchunks = C >> 3;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + row * C);
+
+  float v[NCH][8];
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+      uint4 t;
+      asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+                   : "=r"(t.x), "=r"(t.y), "=r"(t.z), "=r"(t.w) : "l"(xr + c));
+      const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = unpack_bf16x2(tw[e]);
+        v[i][2 * e] = f.x;
+        v[i][2 * e + 1] = f.y;
+        sum += f.x + f.y;
+      }
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[i][e] = 0.f;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  const float mean = sum / (float)C;
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float d = v[i][e] - mean;
+        sq += d * d;
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  const float rstd = rsqrtf(sq / (float)C + eps);
+
+  int64_t g = row / group_rows;
+  if (mod_index) g = mod_index[g];
+  const float* sh = shift + g * mod_stride;
+  const float* sc = scale + g * mod_stride;
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+      const float4 s0 = __ldg(reinterpret_cast<const float4*>(sc + c * 8));
+      const float4 s1 = __ldg(reinterpret_cast<const float4*>(sc + c * 8 + 4));
+      const float4 h0 = __ldg(reinterpret_cast<const float4*>(sh + c * 8));
+      const float4 h1 = __ldg(reinterpret_cast<const float4*>(sh + c * 8 + 4));
+      const float s[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+      const float hh[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        v[i][e] = (v[i][e] - mean) * rstd * (1.0f + s[e]) + hh[e];
+        amax = fmaxf(amax, fabsf(v[i][e]));
+      }
+    }
+  }
+  const float rs = fp8_row_scale(amax);
+  if (lane == 0) y_scale[row] = rs;
+  uint2* yr = reinterpret_cast<uint2*>(y8 + row * C);
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) yr[c] = e4m3x8(v[i], rs);
+  }
+}
+
+// bf16 row -> e4m3 codes + fp32 scale in one read: the row is held as packed bf16 (4 registers per 8 elements) between
+// its amax reduction and the conversion.
+template <int NCH>
+__global__ void __launch_bounds__(kLnWarpsPerBlock * 32)
+quant_rows_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, uint8_t* __restrict__ y8, int64_t ldy,
+                      float* __restrict__ y_scale, int64_t rows, int K) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * kLnWarpsPerBlock + (threadIdx.x >> 5);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (row >= rows) return;
+  const int nchunks = K >> 3;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + row * ldx);
+  uint4 t[NCH];
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+      asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+                   : "=r"(t[i].x), "=r"(t[i].y), "=r"(t[i].z), "=r"(t[i].w) : "l"(xr + c));
+      const uint32_t tw[4] = {t[i].x, t[i].y, t[i].z, t[i].w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = unpack_bf16x2(tw[e]);
+        amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+      }
+    }
+  }
+  const float rs = fp8_row_scale(amax);
+  if (lane == 0) y_scale[row] = rs;
+  uint2* yr = reinterpret_cast<uint2*>(y8 + row * ldy);
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nchunks) {
+      const uint32_t tw[4] = {t[i].x, t[i].y, t[i].z, t[i].w};
+      float o[8];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = unpack_bf16x2(tw[e]);
+        o[2 * e] = f.x;
+        o[2 * e + 1] = f.y;
+      }
+      yr[c] = e4m3x8(o, rs);
     }
   }
 }
@@ -223,6 +384,73 @@ extern "C" int osb_ln_modulate(const void* x, const float* shift, const float* s
                                int64_t rows, int C, int64_t group_rows, const int32_t* mod_index,
                                int64_t mod_stride, float eps, void* stream) {
   return ln_modulate_launch(x, shift, scale, y, rows, C, group_rows, mod_index, mod_stride, eps, osb::RowScatter(), stream);
+}
+
+extern "C" int osb_ln_modulate_fp8(const void* x, const float* shift, const float* scale, void* y8, float* y_scale,
+                                   int64_t rows, int C, int64_t group_rows, const int32_t* mod_index,
+                                   int64_t mod_stride, float eps, void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(x && y8 && y_scale && shift && scale, "osb_ln_modulate_fp8: null tensor");
+  OSB_REQUIRE(rows > 0, "osb_ln_modulate_fp8: rows must be positive");
+  // (the fp32 row stays in registers until its amax is known: beyond 4096 columns it would spill)
+  OSB_REQUIRE(C > 0 && C % 8 == 0 && C <= 4096, "osb_ln_modulate_fp8: C must be a multiple of 8 and <= 4096 (got %d)", C);
+  OSB_REQUIRE(mod_stride % 4 == 0, "osb_ln_modulate_fp8: mod_stride must be a multiple of 4");
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y8) |
+                reinterpret_cast<uintptr_t>(shift) | reinterpret_cast<uintptr_t>(scale)) & 15) == 0 &&
+              (reinterpret_cast<uintptr_t>(y_scale) & 3) == 0,
+              "osb_ln_modulate_fp8: tensors must be 16-byte aligned (y_scale 4-byte)");
+  if (group_rows <= 0) group_rows = rows;
+  const int nch = (C / 8 + 31) / 32;
+  const unsigned blocks = (unsigned)((rows + kLnWarpsPerBlock - 1) / kLnWarpsPerBlock);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const __nv_bfloat16* xb = static_cast<const __nv_bfloat16*>(x);
+  uint8_t* yb = static_cast<uint8_t*>(y8);
+#define OSB_LN8_CASE(N)                                                                                  \
+  if (nch <= N) {                                                                                        \
+    cudaLaunchAttribute attr[2];                                                                         \
+    cudaLaunchConfig_t cfg = launch_config(dim3(blocks), dim3(kLnWarpsPerBlock * 32), 0, s, attr);       \
+    OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, ln_modulate_fp8_kernel<N>, xb, shift, scale, yb, y_scale, rows, \
+                                      C, group_rows, mod_index, mod_stride, eps));                       \
+    count_launch();                                                                                      \
+    return OSB_OK;                                                                                       \
+  }
+  OSB_LN8_CASE(1) OSB_LN8_CASE(2) OSB_LN8_CASE(3) OSB_LN8_CASE(5) OSB_LN8_CASE(8) OSB_LN8_CASE(16)
+#undef OSB_LN8_CASE
+  set_error("osb_ln_modulate_fp8: unsupported C %d", C);
+  return OSB_ERR_UNSUPPORTED;
+}
+
+extern "C" int osb_quant_rows_fp8(const void* x, int64_t ldx, void* y8, int64_t ldy, float* y_scale, int64_t rows, int K,
+                                  void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(x && y8 && y_scale, "osb_quant_rows_fp8: null tensor");
+  OSB_REQUIRE(rows > 0, "osb_quant_rows_fp8: rows must be positive");
+  OSB_REQUIRE(K > 0 && K % 8 == 0 && K <= 8192, "osb_quant_rows_fp8: K must be a multiple of 8 and <= 8192 (got %d)", K);
+  OSB_REQUIRE(ldx >= K && ldy >= K && ldx % 8 == 0 && ldy % 16 == 0,
+              "osb_quant_rows_fp8: ldx must be a multiple of 8 and ldy of 16, both >= K (ldx %lld ldy %lld K %d)",
+              (long long)ldx, (long long)ldy, K);
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y8)) & 15) == 0 &&
+              (reinterpret_cast<uintptr_t>(y_scale) & 3) == 0,
+              "osb_quant_rows_fp8: x and y8 must be 16-byte aligned (y_scale 4-byte)");
+  const int nch = (K / 8 + 31) / 32;
+  const unsigned blocks = (unsigned)((rows + kLnWarpsPerBlock - 1) / kLnWarpsPerBlock);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const __nv_bfloat16* xb = static_cast<const __nv_bfloat16*>(x);
+  uint8_t* yb = static_cast<uint8_t*>(y8);
+#define OSB_Q8_CASE(N)                                                                                   \
+  if (nch <= N) {                                                                                        \
+    cudaLaunchAttribute attr[2];                                                                         \
+    cudaLaunchConfig_t cfg = launch_config(dim3(blocks), dim3(kLnWarpsPerBlock * 32), 0, s, attr);       \
+    OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, quant_rows_fp8_kernel<N>, xb, ldx, yb, ldy, y_scale, rows, K)); \
+    count_launch();                                                                                      \
+    return OSB_OK;                                                                                       \
+  }
+  OSB_Q8_CASE(1) OSB_Q8_CASE(2) OSB_Q8_CASE(5) OSB_Q8_CASE(8) OSB_Q8_CASE(18) OSB_Q8_CASE(32)
+#undef OSB_Q8_CASE
+  set_error("osb_quant_rows_fp8: unsupported K %d", K);
+  return OSB_ERR_UNSUPPORTED;
 }
 
 extern "C" int osb_ln_modulate_scatter(const void* x, const float* shift, const float* scale, int64_t rows, int C,

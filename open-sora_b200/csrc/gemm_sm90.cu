@@ -18,6 +18,10 @@
 //   kText       nn.Linear with the text encoders' activations: T5's gated GELU gelu_tanh(x wi_0^T) * (x wi_1^T) over a
 //               weight whose rows interleave wi_0 and wi_1 (both halves of an output column sit in one thread's
 //               accumulator pair, the [M, 2 d_ff] product never leaves registers), and CLIP's bias + quick GELU.
+//   kFp8        kPlain on e4m3 operands with per-row scales: a k-block is 128 e4m3 elements (the same 128-byte swizzle row,
+//               box bytes and stage ring as 64 bf16), issued as 4 wgmma k32 steps into a partial accumulator that is added
+//               into the fp32 register accumulator after every k-block; the epilogue scales the accumulator by
+//               a_scale[row] * w_scale[col] before the unchanged bias / GELU / gate + residual code.  BLOCK_N 64 / 128.
 //
 // Replaces every nn.Linear on the denoiser block path of the reference
 // (opensora/models/mmdit/layers.py:209-214,247-252,277-281,314-334,401) and the fused epilogues
@@ -35,7 +39,7 @@ constexpr int kBlockK = 64;
 constexpr int kNumThreads = 384;            // producer warpgroup + two consumer warpgroups
 constexpr int kStageBudget = 200 * 1024;    // operand ring (one CTA per SM; 227 KB is the per-block limit)
 
-enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4 };
+enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4, kFp8 = 5 };
 
 struct GemmEpilogueParams {
   const __nv_bfloat16* bias;
@@ -97,9 +101,11 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                  const GemmEpilogueParams p, const ConvGeom cg, const HeadTileParams ht,
                  const __grid_constant__ CUtensorMap tmap_u, const __grid_constant__ CUtensorMap tmap_lb,
-                 const int32_t lora_k_blocks) {   // kLora only: U / s B maps and ceil(r / 64)
+                 const int32_t lora_k_blocks,     // kLora only: U / s B maps and ceil(r / 64)
+                 const float* a_scale, const float* w_scale) {   // kFp8 only: row scales of A and W
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::STAGES;
+  constexpr int kBK = kMode == kFp8 ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 1024-byte aligned
@@ -113,7 +119,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int tid_wg = threadIdx.x & 127;
   const int64_t num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int64_t m_blk = blockIdx.x / num_n_blocks, n_blk = blockIdx.x % num_n_blocks;
-  const int64_t num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
+  const int64_t num_k_blocks = (p.K + kBK - 1) / kBK;
   const int64_t total_k_blocks = kMode == kLora ? num_k_blocks + lora_k_blocks : num_k_blocks;
   // conv: m_blk -> (batch, t-tile, h-tile, w-tile); the box origin in OUTPUT coordinates
   int n_i = 0, t0 = 0, h0 = 0, w0 = 0;
@@ -152,7 +158,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       uint32_t phase = 0;
       for (int64_t kb = 0; kb < num_k_blocks; ++kb) {
         mbar_wait_notrace(empty_bar(stage), phase ^ 1);
-        const int32_t k0 = (int32_t)(kb * kBlockK);
+        const int32_t k0 = (int32_t)(kb * kBK);
         mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);   // out-of-bounds box elements are zero filled and counted
         if constexpr (kMode == kConv) {   // tap offsets in the padded input, output origin scaled by the stride
           const int tap = (int)(kb / cg.cin_chunks);
@@ -186,7 +192,34 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   float acc[BLOCK_N / 2];
 #pragma unroll
   for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-  {
+  if constexpr (kMode == kFp8) {
+    // FP8 wgmma adds into its accumulator with fewer mantissa bits than an fp32 add, so a K-long sum in the wgmma
+    // accumulator loses precision with K.  Each k-block (128 e4m3 elements) is summed into `part` by the tensor core and
+    // promoted into the fp32 register accumulator `acc` before the next one: acc is an fp32 sum of 128-element partials.
+    // (Two accumulators per thread: BLOCK_N <= 128 fits the 168-register budget of a 384-thread CTA.)
+    float part[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) part[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
+      mbar_wait_notrace(full_bar(stage), phase);
+      const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
+      const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
+      wgmma_fence_regs(part);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
+        WgmmaFp8<BLOCK_N>::mma(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();   // this k-block's partial is complete and its stage has been read
+      wgmma_fence_regs(part);
+      if (tid_wg == 0) mbar_arrive(empty_bar(stage));
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+  } else {
     int stage = 0, prev = 0;
     uint32_t phase = 0;
     for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
@@ -347,18 +380,25 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
       if (!row_ok) continue;
       const float* gate_row = nullptr;
-      if ((kMode == kPlain || kMode == kLora) && p.epilogue == OSB_EPI_BIAS_GATE_RES && p.gate != nullptr) {
+      if ((kMode == kPlain || kMode == kLora || kMode == kFp8) && p.epilogue == OSB_EPI_BIAS_GATE_RES && p.gate != nullptr) {
         int64_t gi = (uint32_t)row / group_rows32;
         if (p.mod_index) gi = p.mod_index[gi];
         gate_row = p.gate + gi * p.gate_stride;
       }
       __nv_bfloat16* drow = p.D + row * p.ldd;
       const __nv_bfloat16* rrow = p.R ? p.R + row * p.ldr : nullptr;
+      float sa = 0.f;
+      if constexpr (kMode == kFp8) sa = __ldg(a_scale + row);
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
         const int64_t n = n_blk * BLOCK_N + 8 * j + c_frag;
         if (n >= p.N) continue;   // N % 8 == 0: n < N implies n + 1 < N
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if constexpr (kMode == kFp8) {
+          const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+          v0 *= sa * sw.x;
+          v1 *= sa * sw.y;
+        }
         if (p.bias) {
           const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
           v0 += b.x;
@@ -391,13 +431,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 template <int BLOCK_N, int kMode>
 static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tw, const GemmEpilogueParams& p, const ConvGeom& cg,
                          const HeadTileParams& ht, int64_t tiles, cudaStream_t stream, const CUtensorMap* tu = nullptr,
-                         const CUtensorMap* tlb = nullptr, int32_t lora_k_blocks = 0) {
+                         const CUtensorMap* tlb = nullptr, int32_t lora_k_blocks = 0, const float* a_scale = nullptr,
+                         const float* w_scale = nullptr) {
   if (tiles >= (1ll << 31)) { set_error("osb gemm: too many output tiles (%lld)", (long long)tiles); return OSB_ERR_UNSUPPORTED; }
   cudaLaunchAttribute attr[2];
   cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)tiles), dim3(kNumThreads), GemmCfg<BLOCK_N>::SMEM_BYTES, stream, attr);
   // the LoRA maps are read by kLora only; every other mode gets the main maps as placeholders
   OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<BLOCK_N, kMode>, ta, tw, p, cg, ht, tu ? *tu : ta,
-                                    tlb ? *tlb : tw, lora_k_blocks));
+                                    tlb ? *tlb : tw, lora_k_blocks, a_scale, w_scale));
   count_launch();
   return OSB_OK;
 }
@@ -478,6 +519,8 @@ int gemm_init() {
   if ((rc = init_one<128, kText>())) return rc;
   if ((rc = init_one<192, kText>())) return rc;
   if ((rc = init_one<256, kText>())) return rc;
+  if ((rc = init_one<64, kFp8>())) return rc;
+  if ((rc = init_one<128, kFp8>())) return rc;
   return OSB_OK;
 }
 
@@ -496,6 +539,31 @@ static int pick_block_n(int64_t M, int64_t N) {
     if (cost < best_cost) { best_cost = cost; best = bn; }
   }
   return best;
+}
+
+template <int BLOCK_N>
+static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream) {
+  CUtensorMap ta, tw;
+  int rc = make_tmap_2d_e4m3(&ta, a.A, a.M, a.K, a.lda, kBlockM, 2 * kBlockK);
+  if (rc) return rc;
+  rc = make_tmap_2d_e4m3(&tw, a.W, a.N, a.K, a.ldw, BLOCK_N, 2 * kBlockK);
+  if (rc) return rc;
+  GemmEpilogueParams p = {};
+  p.bias = static_cast<const __nv_bfloat16*>(a.bias);
+  p.D = static_cast<__nv_bfloat16*>(a.D);
+  p.R = a.epilogue == OSB_EPI_BIAS_GATE_RES ? static_cast<const __nv_bfloat16*>(a.R) : nullptr;
+  p.gate = a.gate;
+  p.mod_index = a.mod_index;
+  p.M = a.M; p.N = a.N; p.K = a.K;
+  p.ldd = a.ldd;
+  p.ldr = a.ldr;
+  p.group_rows = a.group_rows > 0 ? a.group_rows : a.M;
+  p.gate_stride = a.gate_stride;
+  p.epilogue = a.epilogue;
+  const int64_t tiles = ((a.M + kBlockM - 1) / kBlockM) * ((a.N + BLOCK_N - 1) / BLOCK_N);
+  ConvGeom cg = {};
+  HeadTileParams ht = {};
+  return launch_kernel<BLOCK_N, kFp8>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, a.a_scale, a.w_scale);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -589,6 +657,42 @@ extern "C" int osb_gemm_bf16(const osb_gemm_args* args, void* stream) {
 extern "C" int osb_gemm_lora(const osb_gemm_args* gemm, const osb_lora_args* lora, void* stream) {
   if (lora == nullptr) { osb::set_error("osb_gemm_lora: null lora args"); return OSB_ERR_INVALID; }
   return osb::gemm_dispatch("osb_gemm_lora", gemm, lora, stream);
+}
+
+extern "C" int osb_gemm_fp8(const osb_gemm_fp8_args* args, void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(args != nullptr, "osb_gemm_fp8: null args");
+  const osb_gemm_fp8_args& a = *args;
+  OSB_REQUIRE(a.A && a.W && a.D && a.a_scale && a.w_scale, "osb_gemm_fp8: null operand or scale");
+  OSB_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "osb_gemm_fp8: empty problem (M %lld N %lld K %lld)",
+              (long long)a.M, (long long)a.N, (long long)a.K);
+  OSB_REQUIRE(a.K % 128 == 0, "osb_gemm_fp8: K must be a multiple of 128 (one e4m3 k-block), got %lld", (long long)a.K);
+  OSB_REQUIRE(a.N % 8 == 0, "osb_gemm_fp8: N must be a multiple of 8, got %lld", (long long)a.N);
+  OSB_REQUIRE(a.lda % 16 == 0 && a.ldw % 16 == 0 && a.lda >= a.K && a.ldw >= a.K,
+              "osb_gemm_fp8: lda and ldw must be >= K and multiples of 16 (lda %lld ldw %lld)", (long long)a.lda,
+              (long long)a.ldw);
+  OSB_REQUIRE(a.ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(a.D) & 15) == 0,
+              "osb_gemm_fp8: D must be 16-byte aligned with ldd %% 8 == 0");
+  OSB_REQUIRE(a.epilogue >= OSB_EPI_BIAS && a.epilogue <= OSB_EPI_BIAS_GATE_RES,
+              "osb_gemm_fp8: epilogue %d is not built for FP8 (bias, GELU-tanh, gate + residual)", a.epilogue);
+  OSB_REQUIRE((reinterpret_cast<uintptr_t>(a.w_scale) & 7) == 0 && (reinterpret_cast<uintptr_t>(a.a_scale) & 3) == 0,
+              "osb_gemm_fp8: a_scale must be 4-byte and w_scale 8-byte aligned");
+  if (a.epilogue == OSB_EPI_BIAS_GATE_RES) {
+    OSB_REQUIRE(a.R == nullptr || (a.ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(a.R) & 15) == 0),
+                "osb_gemm_fp8: R must be 16-byte aligned with ldr %% 8 == 0");
+    OSB_REQUIRE(a.gate == nullptr || (a.gate_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(a.gate) & 15) == 0),
+                "osb_gemm_fp8: gate must be 16-byte aligned with gate_stride %% 4 == 0");
+  }
+  OSB_REQUIRE(a.bias == nullptr || (reinterpret_cast<uintptr_t>(a.bias) & 15) == 0,
+              "osb_gemm_fp8: bias must be 16-byte aligned");
+  // the promoted accumulation holds two accumulators per thread: tiles wider than 128 columns would not fit
+  const int bn = a.block_n ? a.block_n : (a.N <= 64 ? 64 : 128);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (bn == 64) return launch_gemm_fp8<64>(a, s);
+  if (bn == 128) return launch_gemm_fp8<128>(a, s);
+  set_error("osb_gemm_fp8: unsupported block_n %d (64 or 128)", bn);
+  return OSB_ERR_UNSUPPORTED;
 }
 
 extern "C" int osb_conv3d_ndhwc(const osb_conv3d_args* args, void* stream) {

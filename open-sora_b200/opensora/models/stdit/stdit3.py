@@ -14,6 +14,8 @@ Per block (SURVEY.md §8a-S `STDiT3Block.forward`), 10 launches:
   -> proj GEMM (+gate, +residual) -> q GEMM (operand tiles) -> cross attention (kv_lens) -> proj GEMM (+residual)
   -> ln_modulate -> fc1 GEMM (+GELU-tanh) -> fc2 GEMM (+gate, +residual)
 The 2*depth kv_linear projections of the (block-invariant) text tokens are batched into one GEMM.
+With `enable_fp8()` the MLP runs on e4m3 operands with per-row scales instead (11 launches):
+  ln_modulate_fp8 -> fc1 gemm_fp8 (+GELU-tanh) -> quant_rows_fp8 -> fc2 gemm_fp8 (+gate, +residual)
 q / k / v never exist in token layout: the projection epilogue writes "head tiles" (include/osb200.h) that the
 attention kernel loads with one bulk copy per tile.  Head sizes the tile path is not built for (anything but
 64 / 72 / 128, or an odd head count) use the register-path kernel `osb_attn_short` on token-layout q / k / v.
@@ -166,6 +168,7 @@ class STDiT3(nn.Module):
         self._peer = None
         self._sp_exchange = "nccl"
         self._sp_config_checked = False
+        self._fp8 = False
         self.register_load_state_dict_post_hook(lambda m, k: m._cache.clear())
 
     # ---- construction helpers ---------------------------------------------------------------
@@ -253,6 +256,40 @@ class STDiT3(nn.Module):
                 self._sp_exchange = "nccl"
                 return None
         return self._peer
+
+    # ---- FP8 (e4m3) MLPs ---------------------------------------------------------------------------------------------
+    def enable_fp8(self) -> None:
+        """Run fc1 and fc2 of every block MLP (spatial and temporal) on FP8 (e4m3) tensor cores.  The weights are quantized
+        here, per output channel (s = amax / 448), into the per-model cache; the bf16 parameters and the state dict stay
+        as they are.  Activations are quantized per row: the fp32 LN+modulate result for fc1, the bf16 GELU output for fc2
+        (include/osb200.h, osb_gemm_fp8).  Needs hidden size and MLP width that are multiples of 128, a hidden size of at
+        most 4096 (the FP8 LN+modulate) and an MLP width of at most 8192 (the row quantizer)."""
+        C, hidden = self.hidden_size, self.spatial_blocks[0].mlp.fc1.out_features
+        if C % 128 or hidden % 128 or C > 4096 or hidden > 8192:
+            raise ValueError(f"FP8 MLPs need the hidden size ({C}) and the MLP width ({hidden}) to be multiples of 128 "
+                             "(one e4m3 k-block of osb_gemm_fp8), with hidden size <= 4096 and MLP width <= 8192")
+        w = self.x_embedder.proj.weight
+        if w.is_cuda:   # quantized now; a model not yet on the GPU quantizes at its first forward
+            self._fp8_weights(w.device)
+        self._fp8 = True
+
+    def disable_fp8(self) -> None:
+        """Back to the bf16 MLPs; the FP8 weight copies are released."""
+        self._fp8 = False
+        for k in [k for k in self._cache if k[0] == "fp8"]:
+            del self._cache[k]
+
+    def _fp8_weights(self, dev):
+        """Per block (spatial / temporal interleaved, as the block loop runs): (fc1 e4m3, fc1 scales, fc2 e4m3, fc2 scales)."""
+        key = ("fp8", dev)
+        if key not in self._cache:
+            import osb200 as osb
+
+            q = []
+            for b in (b for pair in zip(self.spatial_blocks, self.temporal_blocks) for b in pair):
+                q.append(osb.quant_rows_fp8(b.mlp.fc1.weight) + osb.quant_rows_fp8(b.mlp.fc2.weight))
+            self._cache[key] = q
+        return self._cache[key]
 
     # ---- CUDA-graph replay of one step (fixed shapes): removes the ~600 Python-issued launches from the critical
     # path.  Matters when the per-rank work is small (sequence parallel at 8 GPUs is host-bound otherwise). ----------
@@ -445,10 +482,10 @@ class STDiT3(nn.Module):
         # ---- workspaces reused by every block ------------------------------------------------------
         R = B * N
 
-        def wsbuf(name, *shape):   # block workspaces live with the model (no allocator traffic per step, graph-safe)
+        def wsbuf(name, *shape, dtype=bf):   # block workspaces live with the model (no allocator traffic per step, graph-safe)
             key = ("ws", name, shape, dev)
             if key not in self._cache:
-                self._cache[key] = torch.empty(*shape, dtype=bf, device=dev)
+                self._cache[key] = torch.empty(*shape, dtype=dtype, device=dev)
             return self._cache[key]
 
         xm_buf = wsbuf("xm", R, C)
@@ -457,6 +494,10 @@ class STDiT3(nn.Module):
         cos, sin = self._rope(T, dev)
         ws = dict(xm=xm_buf, ao=ao, hid=hid, cos=cos, sin=sin, kv=kv_all, kv_lens=kv_lens, tiles=use_tiles,
                   peer=self._peer_exchange(dev) if P > 1 else None)
+        if self._fp8:   # e4m3 codes + row scales of the fc1 input (C wide) and the fc2 input (hid wide)
+            f8 = torch.float8_e4m3fn
+            ws.update(fp8=self._fp8_weights(dev), xm8=wsbuf("xm8", R, C, dtype=f8), xm8_s=wsbuf("xm8_s", R, dtype=torch.float32),
+                      hid8=wsbuf("hid8", *hid.shape, dtype=f8), hid8_s=wsbuf("hid8_s", R, dtype=torch.float32))
         if use_tiles:
             Sl = S // P   # temporal attention runs on this rank's S/P columns of every frame
             ws["sp_t"] = self._tiles(osb, ("spatial", B, Tl, S), R, osb.tile_map(0, S), 3, dev)
@@ -601,6 +642,15 @@ class STDiT3(nn.Module):
                            k_strides=(Ly, 0, 1), Lq=N, Lk=Ly, num_heads=Hh, head_dim=D, kv_lens=ws["kv_lens"])
         osb.gemm(ao, ca.proj.weight, ca.proj.bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=xs, gate=None, out=xs)
         # 3. MLP
+        if "fp8" in ws:
+            w1, s1, w2, s2 = ws["fp8"][bi]
+            x8, xs8 = osb.ln_modulate_fp8(xs, m[:, 3], m[:, 4], group_rows=group_rows, mod_index=mod_index,
+                                          out=ws["xm8"], out_scale=ws["xm8_s"])
+            osb.gemm_fp8(x8, xs8, w1, s1, mlp.fc1.bias, epilogue=osb.EPI_BIAS_GELU_TANH, out=hid)
+            h8, hs8 = osb.quant_rows_fp8(hid, out=ws["hid8"], out_scale=ws["hid8_s"])
+            osb.gemm_fp8(h8, hs8, w2, s2, mlp.fc2.bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=xs, gate=m[:, 5],
+                         group_rows=group_rows, mod_index=mod_index, out=xs)
+            return
         osb.ln_modulate(xs, m[:, 3], m[:, 4], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
         osb.gemm(xm_buf, mlp.fc1.weight, mlp.fc1.bias, epilogue=osb.EPI_BIAS_GELU_TANH, out=hid)
         osb.gemm(hid, mlp.fc2.weight, mlp.fc2.bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=xs, gate=m[:, 5],

@@ -36,6 +36,9 @@ EXPORTS = (
     "osb_gemm_lora",
     "osb_attn_short_bias",
     "osb_rms_norm",
+    "osb_gemm_fp8",
+    "osb_ln_modulate_fp8",
+    "osb_quant_rows_fp8",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -65,6 +68,13 @@ def _load() -> C.CDLL:
     ]
     lib.osb_gemm_bf16.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_gemm_lora.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.osb_gemm_fp8.argtypes = [C.c_void_p, C.c_void_p]
+    lib.osb_ln_modulate_fp8.argtypes = [
+        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p,
+        C.c_int64, C.c_float, C.c_void_p,
+    ]
+    lib.osb_quant_rows_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int,
+                                       C.c_void_p]
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_attn_short_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     lib.osb_rms_norm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_void_p]
@@ -151,6 +161,17 @@ class GemmArgs(C.Structure):
 class LoraArgs(C.Structure):
     _fields_ = [("U", C.c_void_p), ("B", C.c_void_p), ("ldu", C.c_int64), ("ldb", C.c_int64), ("r", C.c_int32),
                 ("reserved", C.c_int32)]
+
+
+class GemmFp8Args(C.Structure):
+    _fields_ = [
+        ("A", C.c_void_p), ("W", C.c_void_p), ("a_scale", C.c_void_p), ("w_scale", C.c_void_p),
+        ("bias", C.c_void_p), ("D", C.c_void_p), ("R", C.c_void_p), ("gate", C.c_void_p), ("mod_index", C.c_void_p),
+        ("M", C.c_int64), ("N", C.c_int64), ("K", C.c_int64),
+        ("lda", C.c_int64), ("ldw", C.c_int64), ("ldd", C.c_int64), ("ldr", C.c_int64),
+        ("group_rows", C.c_int64), ("gate_stride", C.c_int64),
+        ("epilogue", C.c_int32), ("block_n", C.c_int32),
+    ]
 
 
 class AttnShortArgs(C.Structure):
@@ -386,6 +407,91 @@ def gemm_lora(a, w, bias, u, b, *, epilogue: int = EPI_BIAS, residual=None, gate
     with _Timed("gemm", 2.0 * args.M * args.N * (args.K + la.r)):
         _check(_lib.osb_gemm_lora(C.byref(args), C.byref(la), _stream()), "osb_gemm_lora")
     return out
+
+
+# ---- FP8 (e4m3) with per-row scales (include/osb200.h): s[r] = amax(|X[r, :]|) / 448 (1 for a zero row), codes
+# e4m3_rn_satfinite(X / s).  e4m3 tensors are torch.float8_e4m3fn, scales fp32. ---------------------------------------
+def gemm_fp8(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None,
+             group_rows: int = 0, mod_index=None, out=None, block_n: int = 0):
+    """out = epilogue(acc * (a_scale[m] * w_scale[n]) + bias), acc = a8 @ w8.T summed in fp32 (osb_gemm_fp8).
+    a8 e4m3 [M, K] (row stride free), w8 e4m3 [N, K], scales fp32 [M] / [N]; K % 128 == 0.  The epilogues BIAS,
+    BIAS_GELU_TANH and BIAS_GATE_RES behave as in `gemm`."""
+    import torch
+
+    _need(a8, torch.float8_e4m3fn, "a8"); _need(w8, torch.float8_e4m3fn, "w8")
+    _need(a_scale, torch.float32, "a_scale"); _need(w_scale, torch.float32, "w_scale")
+    _need(bias, torch.bfloat16, "bias"); _need(residual, torch.bfloat16, "residual"); _need(gate, torch.float32, "gate")
+    _need(mod_index, torch.int32, "mod_index")
+    if a8.dim() != 2 or w8.dim() != 2 or a8.shape[1] != w8.shape[1]:
+        raise OsbError(f"gemm_fp8: a8 [M, K] and w8 [N, K] expected, got {tuple(a8.shape)} and {tuple(w8.shape)}")
+    M, K = a8.shape
+    N = w8.shape[0]
+    if a_scale is None or w_scale is None or a_scale.shape != (M,) or w_scale.shape != (N,):
+        raise OsbError(f"gemm_fp8: a_scale must be [{M}] and w_scale [{N}]")
+    if out is None:
+        out = torch.empty((M, N), dtype=torch.bfloat16, device=a8.device)
+    _need(out, torch.bfloat16, "out")
+    g = GemmFp8Args()
+    g.A, g.W, g.a_scale, g.w_scale = a8.data_ptr(), w8.data_ptr(), a_scale.data_ptr(), w_scale.data_ptr()
+    g.bias = bias.data_ptr() if bias is not None else None
+    g.D = out.data_ptr()
+    g.R = residual.data_ptr() if residual is not None else None
+    g.gate = gate.data_ptr() if gate is not None else None
+    g.mod_index = mod_index.data_ptr() if mod_index is not None else None
+    g.M, g.N, g.K = M, N, K
+    g.lda, g.ldw, g.ldd = a8.stride(0), w8.stride(0), out.stride(0)
+    g.ldr = residual.stride(0) if residual is not None else 0
+    g.group_rows = group_rows if group_rows > 0 else M
+    g.gate_stride = gate.stride(0) if gate is not None else 0
+    g.epilogue, g.block_n = epilogue, block_n
+    with _Timed("gemm_fp8", 2.0 * M * N * K):
+        _check(_lib.osb_gemm_fp8(C.byref(g), _stream()), "osb_gemm_fp8")
+    return out
+
+
+def ln_modulate_fp8(x, shift, scale, *, group_rows: int, mod_index=None, eps: float = 1e-6, out=None, out_scale=None):
+    """`ln_modulate` with the fp32 result quantized per row (osb_ln_modulate_fp8): returns (e4m3 [rows, C], fp32 [rows])."""
+    import torch
+
+    _need(x, torch.bfloat16, "x"); _need(shift, torch.float32, "shift"); _need(scale, torch.float32, "scale")
+    _need(mod_index, torch.int32, "mod_index")
+    assert x.dim() == 2 and x.is_contiguous()
+    assert shift.dim() == 2 and scale.dim() == 2 and shift.stride(0) == scale.stride(0)
+    rows, Cdim = x.shape
+    if out is None:
+        out = torch.empty((rows, Cdim), dtype=torch.float8_e4m3fn, device=x.device)
+    if out_scale is None:
+        out_scale = torch.empty(rows, dtype=torch.float32, device=x.device)
+    _need(out, torch.float8_e4m3fn, "out"); _need(out_scale, torch.float32, "out_scale")
+    if out.shape != (rows, Cdim) or not out.is_contiguous() or out_scale.shape != (rows,):
+        raise OsbError(f"ln_modulate_fp8: out must be a contiguous [{rows}, {Cdim}] e4m3 tensor and out_scale [{rows}]")
+    with _Timed("ln_modulate", 3.0 * rows * Cdim):  # algorithmic bytes: read x (bf16) + write codes (e4m3)
+        _check(_lib.osb_ln_modulate_fp8(_ptr(x), _ptr(shift), _ptr(scale), _ptr(out), _ptr(out_scale), rows, Cdim,
+                                        group_rows, _ptr(mod_index), shift.stride(0), eps, _stream()),
+               "osb_ln_modulate_fp8")
+    return out, out_scale
+
+
+def quant_rows_fp8(x, *, out=None, out_scale=None):
+    """Per-row e4m3 quantization of bf16 x [rows, K] (row stride free) in one pass (osb_quant_rows_fp8): returns
+    (e4m3 [rows, K], fp32 [rows])."""
+    import torch
+
+    _need(x, torch.bfloat16, "x")
+    if x.dim() != 2:
+        raise OsbError(f"quant_rows_fp8: x must be [rows, K], got {tuple(x.shape)}")
+    rows, K = x.shape
+    if out is None:
+        out = torch.empty((rows, K), dtype=torch.float8_e4m3fn, device=x.device)
+    if out_scale is None:
+        out_scale = torch.empty(rows, dtype=torch.float32, device=x.device)
+    _need(out, torch.float8_e4m3fn, "out"); _need(out_scale, torch.float32, "out_scale")
+    if out.shape != (rows, K) or out_scale.shape != (rows,):
+        raise OsbError(f"quant_rows_fp8: out must be [{rows}, {K}] and out_scale [{rows}]")
+    with _Timed("quant_rows_fp8", 3.0 * rows * K):  # algorithmic bytes: read bf16 + write e4m3
+        _check(_lib.osb_quant_rows_fp8(_ptr(x), x.stride(0), _ptr(out), out.stride(0), _ptr(out_scale), rows, K,
+                                       _stream()), "osb_quant_rows_fp8")
+    return out, out_scale
 
 
 def interleave_gated(wi_0, wi_1):
