@@ -98,13 +98,23 @@ typedef struct osb_lora_args {
   int64_t ldu, ldb;
   int32_t r;      /* multiple of 8 (the host zero-pads smaller ranks)                    */
   int32_t reserved;
+  const float* col_scale; /* NULL, or fp32 [N], 8-byte aligned: DoRA's per-output-channel factor g */
 } osb_lora_args;
 
-/* D = epilogue(A W^T + U B^T + bias): osb_gemm_bf16 whose K loop is followed by ceil(r / 64) k-blocks of U and B
- * through the same wgmma pipeline, so the base product and the adapter's update share one fp32 accumulator and one
- * rounding to bf16 (merging the update into bf16 weights would round most of a small update away).  Every epilogue,
- * block_n and alignment rule of osb_gemm_bf16 applies.  The down projection U = x A^T is osb_gemm_bf16 with N = r.
- * Replaces the unmerged peft LoRA layer the reference wraps the denoiser with (opensora/utils/sampling.py:542-545). */
+/* D = epilogue(col_scale[n] * (A W^T + U B^T) + bias): osb_gemm_bf16 whose K loop is followed by ceil(r / 64) k-blocks
+ * of U and B through the same wgmma pipeline, so the base product and the adapter's update share one fp32 accumulator
+ * and one rounding to bf16 (merging the update into bf16 weights would round most of a small update away).  Every
+ * epilogue, block_n and alignment rule of osb_gemm_bf16 applies.  The down projection U = x A^T is osb_gemm_bf16 with
+ * N = r.  Replaces the unmerged peft LoRA layer the reference wraps the denoiser with (opensora/utils/sampling.py:542-545).
+ *
+ * col_scale (DoRA, weight-decomposed LoRA) multiplies the fp32 accumulator in registers, before the bias, GELU-tanh and
+ * the gate / residual / mod_index rules; NULL means no scale.  It replaces peft's DoRA forward (peft/tuners/lora/dora.py,
+ * DoraLinearLayer.forward at inference, dropout the identity):
+ *     weight_norm    = || W + scaling * (lora_B @ lora_A) ||_2 per output row
+ *     mag_norm_scale = lora_magnitude_vector / weight_norm
+ *     result         = base(x) + (mag_norm_scale - 1) * x W^T + mag_norm_scale * scaling * lora_B(lora_A(x))
+ * which equals g * (x W^T + scaling x A^T B^T) + bias with g = mag_norm_scale: the host computes g once per adapter and
+ * passes it here.  An all-ones col_scale gives the bits of col_scale == NULL (x * 1.0f is exact). */
 int osb_gemm_lora(const osb_gemm_args* gemm, const osb_lora_args* lora, void* stream);
 
 /* ---- FP8 (e4m3) with per-row scales: the opt-in MLP path of STDiT3 ------------------------------------------------ */

@@ -14,7 +14,8 @@
 //   kHeadTiles  q / k / v projection whose epilogue writes per-head operand tiles (tiles.cuh) with RMSNorm + RoPE;
 //   kLora       kPlain plus an unmerged low-rank update: after the K loop the producer streams ceil(r / 64) more
 //               k-blocks, U = x A^T [M, r] in the A slot and s B [N, r] in the W slot, through the same stage ring, so
-//               A W^T + U (s B)^T lands in one fp32 accumulator before the unchanged epilogue.
+//               A W^T + U (s B)^T lands in one fp32 accumulator before the unchanged epilogue; with a DoRA column
+//               scale the accumulator is multiplied by col_scale[n] in registers first.
 //   kText       nn.Linear with the text encoders' activations: T5's gated GELU gelu_tanh(x wi_0^T) * (x wi_1^T) over a
 //               weight whose rows interleave wi_0 and wi_1 (both halves of an output column sit in one thread's
 //               accumulator pair, the [M, 2 d_ff] product never leaves registers), and CLIP's bias + quick GELU.
@@ -102,7 +103,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const GemmEpilogueParams p, const ConvGeom cg, const HeadTileParams ht,
                  const __grid_constant__ CUtensorMap tmap_u, const __grid_constant__ CUtensorMap tmap_lb,
                  const int32_t lora_k_blocks,     // kLora only: U / s B maps and ceil(r / 64)
-                 const float* a_scale, const float* w_scale) {   // kFp8 only: row scales of A and W
+                 const float* a_scale, const float* w_scale) {   // kFp8: row scales of A and W; kLora: w_scale is the
+                                                                 // optional per-column (DoRA) scale, may be null
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::STAGES;
   constexpr int kBK = kMode == kFp8 ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
@@ -246,6 +248,24 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int warp_in = tid_wg >> 5, lane = tid_wg & 31;
   const int r_frag = cw * 64 + warp_in * 16 + (lane >> 2);
   const int c_frag = 2 * (lane & 3);
+
+  if constexpr (kMode == kLora) {
+    // DoRA: acc *= col_scale[n] (passed in the w_scale slot) before the epilogue adds the bias.  A thread's columns are
+    // the same for both of its rows, so each scale pair is loaded once per tile.  x * 1.0f is exact: an all-ones scale
+    // leaves the accumulator's bits as they are.  Columns >= N are never stored, so their index is clamped instead of
+    // branched around: the loads carry no control dependence and can all be in flight at once.
+    if (w_scale != nullptr) {
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);
+        const float2 cs = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+        acc[4 * j] *= cs.x;
+        acc[4 * j + 1] *= cs.y;
+        acc[4 * j + 2] *= cs.x;
+        acc[4 * j + 3] *= cs.y;
+      }
+    }
+  }
 
   if constexpr (kMode == kHeadTiles) {
     // ===================== epilogue: head tiles =====================
@@ -488,7 +508,8 @@ static int launch_gemm(const osb_gemm_args& a, bool has_res, cudaStream_t stream
   CUtensorMap tu, tlb;
   if ((rc = make_tmap_2d_bf16(&tu, lora->U, a.M, lora->r, lora->ldu, kBlockM, kBlockK))) return rc;
   if ((rc = make_tmap_2d_bf16(&tlb, lora->B, a.N, lora->r, lora->ldb, BLOCK_N, kBlockK))) return rc;
-  return launch_kernel<BLOCK_N, kLora>(ta, tw, p, cg, ht, tiles, stream, &tu, &tlb, (lora->r + kBlockK - 1) / kBlockK);
+  return launch_kernel<BLOCK_N, kLora>(ta, tw, p, cg, ht, tiles, stream, &tu, &tlb, (lora->r + kBlockK - 1) / kBlockK,
+                                       nullptr, lora->col_scale);
 }
 
 template <int BLOCK_N, int kMode>
@@ -636,6 +657,7 @@ static int gemm_dispatch(const char* fn, const osb_gemm_args* args, const osb_lo
                 ((reinterpret_cast<uintptr_t>(l.U) | reinterpret_cast<uintptr_t>(l.B)) & 15) == 0,
                 "%s: U and B must be 16-byte aligned with ldu, ldb >= r and multiples of 8 (r %d ldu %lld ldb %lld)", fn,
                 l.r, (long long)l.ldu, (long long)l.ldb);
+    OSB_REQUIRE((reinterpret_cast<uintptr_t>(l.col_scale) & 7) == 0, "%s: col_scale must be 8-byte aligned", fn);
   }
   const bool has_res = (a.epilogue == OSB_EPI_BIAS_GATE_RES) && a.R != nullptr;
   const int bn = a.block_n ? a.block_n : pick_block_n(a.M, a.N);

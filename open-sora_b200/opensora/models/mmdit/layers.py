@@ -13,9 +13,9 @@ Any joint sequence length (the flash attention variant streams key blocks), both
 interleaved pairs and `LigerEmbedND` rotate-half) and both QKV checkpoint layouts (`fused_qkv` True / False).
 
 LoRA (opensora/utils/lora.py): every Linear is read through `linear_parts` / `lora_pack`, which also return the active
-adapter's (A, scaling * B), if any.  Linears that read one input share one down GEMM U = x A_cat^T; each output weight
-then runs `osb_gemm_lora` (x W^T + U B^T in one accumulator).  Without an adapter the launches are those of the plain
-model."""
+adapter's (A, scaling * B, DoRA column scale or None), if any.  Linears that read one input share one down GEMM
+U = x A_cat^T; each output weight then runs `osb_gemm_lora` (g * (x W^T + U B^T) in one accumulator, g = 1 without
+DoRA).  Without an adapter the launches are those of the plain model."""
 from __future__ import annotations
 
 import math
@@ -76,20 +76,23 @@ def timestep_embedding(t: Tensor, dim, max_period=10000, time_factor: float = 10
 
 
 def linear_parts(lin: nn.Module, k_pad: int = 0):
-    """(weight, bias, lora) of a Linear the forward sends to osb200: lora is None, or (A [r, K + k_pad], scaling * B)
-    of its adapter (lora_pack)."""
+    """(weight, bias, lora) of a Linear the forward sends to osb200: lora is None, or (A [r, K + k_pad], scaling * B,
+    DoRA column scale or None) of its adapter (lora_pack)."""
     if adapter_of(lin) is None:
         return lin.weight, lin.bias, None
-    A, (B,) = lora_pack([[(lin, 0, lin.out_features)]], k_pad)
-    return lin.weight, lin.bias, (A, B)
+    A, (B,), (S,) = lora_pack([[(lin, 0, lin.out_features)]], k_pad)
+    return lin.weight, lin.bias, (A, B, S)
 
 
 def _gemm(osb, x2d: Tensor, w: Tensor, b, lora, u: Tensor | None = None, **kw) -> Tensor:
-    """osb.gemm, or with lora = (A, B) the fused base + update GEMM; `u` = x2d A^T when a shared down GEMM made it."""
+    """osb.gemm, or with lora = (A, B, col_scale) the fused base + update GEMM; `u` = x2d A^T when a shared down GEMM
+    made it."""
     if lora is None or lora[1] is None:
         return osb.gemm(x2d, w, b, **kw)
     if u is None:
         u = osb.gemm(x2d, lora[0])
+    if lora[2] is not None:
+        kw["col_scale"] = lora[2]
     return osb.gemm_lora(x2d, w, b, u, lora[1], **kw)
 
 
@@ -263,12 +266,12 @@ class _ProcessorBase:
 
     @staticmethod
     def _qkv_lora(sa: nn.Module):
-        """Adapters of the q|k|v projection in the row order of `_qkv`: (A_cat, B_cat) or None."""
+        """Adapters of the q|k|v projection in the row order of `_qkv`: (A_cat, B_cat, col_scale) or None."""
         if getattr(sa, "fused_qkv", hasattr(sa, "qkv")):
             return linear_parts(sa.qkv)[2]
         C = sa.q_proj.out_features
         p = lora_pack([[(sa.q_proj, 0, C), (sa.k_proj, 0, C), (sa.v_proj, 0, C)]])
-        return None if p is None else (p[0], p[1][0])
+        return None if p is None else (p[0], p[1][0], p[2][0])
 
     @staticmethod
     def _modulation(osb, mod: nn.Module, vec: Tensor):
@@ -329,7 +332,7 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
         pi, pt = attn.img_attn.proj, attn.txt_attn.proj
         lp = lora_pack([[(pi, 0, pi.out_features)], [(pt, 0, pt.out_features)]])
         up = None if lp is None else osb.gemm(ao, lp[0])
-        lpi, lpt = (None, None) if lp is None else ((lp[0], lp[1][0]), (lp[0], lp[1][1]))
+        lpi, lpt = (None, None) if lp is None else ((lp[0], lp[1][0], lp[2][0]), (lp[0], lp[1][1], lp[2][1]))
         for b in range(B):  # x + gate * proj(attn)   (layers.py:247, 251)
             if Li:
                 _gemm(osb, ao[b * L + Lt:(b + 1) * L], pi.weight, pi.bias, lpi,
@@ -397,15 +400,15 @@ class SingleStreamBlockProcessor(_ProcessorBase):
 
     @staticmethod
     def _split_lora(blk: nn.Module, M4: int):
-        """Adapters of the qkv and mlp parts of `_split_weights`, which read the same input: (A_cat, B_qkv, B_mlp) with
-        one A_cat for both, or None."""
+        """Adapters of the qkv and mlp parts of `_split_weights`, which read the same input: ((A_cat, B_qkv, S_qkv),
+        (A_cat, B_mlp, S_mlp)) with one A_cat for both, or None."""
         C = blk.linear2.out_features
         if getattr(blk, "fused_qkv", hasattr(blk, "linear1")):
             groups = [[(blk.linear1, 0, 3 * C)], [(blk.linear1, 3 * C, 3 * C + M4)]]
         else:
             groups = [[(blk.q_proj, 0, C), (blk.k_proj, 0, C), (blk.v_mlp, 0, C)], [(blk.v_mlp, C, C + M4)]]
         p = lora_pack(groups)
-        return None if p is None else (p[0], p[1][0], p[1][1])
+        return None if p is None else ((p[0], p[1][0], p[2][0]), (p[0], p[1][1], p[2][1]))
 
     def __call__(self, attn: nn.Module, x: Tensor, vec: Tensor, pe) -> Tensor:
         osb = _check(x)
@@ -417,8 +420,8 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         xm = osb.ln_modulate(x2, mod.shift, mod.scale, group_rows=L)
         wq, bq, wm, bm = self._split_weights(attn)
         lo = self._split_lora(attn, M4)
-        u = None if lo is None else osb.gemm(xm, lo[0])                          # shared down projection
-        lq, lm = (None, None) if lo is None else ((lo[0], lo[1]), (lo[0], lo[2]))
+        u = None if lo is None else osb.gemm(xm, lo[0][0])                       # shared down projection
+        lq, lm = (None, None) if lo is None else lo
         qkv = _gemm(osb, xm, wq, bq, lq, u)                                      # [B*L, 3C]
         cos, sin, half = _rope(pe)
         kw = dict(q_norm_w=attn.norm.query_norm.scale, k_norm_w=attn.norm.key_norm.scale, rope_cos=cos, rope_sin=sin,

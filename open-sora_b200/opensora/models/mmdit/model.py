@@ -10,7 +10,7 @@ from torch import Tensor, nn
 
 from opensora.registry import MODELS
 
-from opensora.utils.lora import adapter_of, lora_pack
+from opensora.utils.lora import adapter_of, dora_magnitude, lora_pack
 
 from .layers import (DoubleStreamBlock, EmbedND, LastLayer, LigerEmbedND, MLPEmbedder, SingleStreamBlock, _gemm,
                      linear_parts, timestep_embedding)
@@ -97,10 +97,15 @@ class MMDiTModel(nn.Module):
     def _grouped_modulation(self, vec: Tensor) -> None:
         """All 2*19 + 38 `Modulation.lin` projections of `vec` as ONE GEMM (the reference launches 76 tiny ones per step,
         layers.py:179-192).  The fp32 result and the column range of every layer ride on `vec`; the processors pick their
-        slice (a processor installed on a block this model does not own simply does its own projection)."""
+        slice (a processor installed on a block this model does not own simply does its own projection).  A layer with a
+        DoRA adapter stays out of the group: its magnitude factor scales its base product too, which one grouped launch
+        cannot do per layer, so the block projects it itself (osb_gemm_lora with col_scale)."""
         import osb200
 
         lins = [m.lin for b in self.double_blocks for m in (b.img_mod, b.txt_mod)] + [b.modulation.lin for b in self.single_blocks]
+        lins = [lin for lin in lins if dora_magnitude(lin) is None]
+        if not lins:
+            return
         adapted = [lin for lin in lins if adapter_of(lin) is not None]
         key = tuple((id(l), l.weight.data_ptr(), l.weight._version) for l in lins)
         if self._mod_pack is None or self._mod_pack[0] != key:
@@ -123,7 +128,7 @@ class MMDiTModel(nn.Module):
                 self._mod_lora = ml = (parts, torch.cat([p[0] for p in parts], 0).contiguous())
             u = osb200.gemm(sv, ml[1])
             ro = 0
-            for lin, (A, (lb,)) in zip(adapted, parts):
+            for lin, (A, (lb,), _) in zip(adapted, parts):
                 lo, hi = cols[id(lin)]
                 osb200.gemm(u[:, ro:ro + A.shape[0]], lb, None, epilogue=osb200.EPI_BIAS_GATE_RES, residual=out[:, lo:hi],
                             out=out[:, lo:hi])

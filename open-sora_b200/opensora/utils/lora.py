@@ -12,8 +12,13 @@ base weights.
 Restated from peft's LoraConfig semantics (peft is not a dependency): `target_modules` as a list matches a module whose
 name equals an entry or ends with "." + entry, as a string it is a regex full match; `rank_pattern` / `alpha_pattern`
 keys match a module name that ends with the pattern (regex) at a "." boundary; scaling = lora_alpha / r, or
-lora_alpha / sqrt(r) with `use_rslora`, times `scale`.  `lora_dropout` is inference-irrelevant and ignored.  Everything
-else an adapter could ask for (DoRA, trained biases, modules_to_save, layer selection, fan_in_fan_out) is refused."""
+lora_alpha / sqrt(r) with `use_rslora`, times `scale`.  `lora_dropout` is inference-irrelevant and ignored.
+
+DoRA (`use_dora`, weight-decomposed LoRA): peft's forward is base(x) + (g - 1) x W^T + g s x A^T B^T with
+g = m / ||W + s B A||_2 per output row (m = `lora_magnitude_vector`), i.e. g * (x W^T + s x A^T B^T) + bias.  g is
+computed once per pack, in fp32 on the weights' device, and the kernel multiplies its accumulator by it before the bias
+(osb_lora_args.col_scale).  Everything else an adapter could ask for (trained biases, modules_to_save, layer selection,
+fan_in_fan_out) is refused."""
 from __future__ import annotations
 
 import json
@@ -28,16 +33,28 @@ from torch import nn
 ADAPTER = "default"
 
 
-class LoraLinear(nn.Module):
-    """An `nn.Linear` with one unmerged low-rank adapter, in peft's `lora.Linear` attribute layout."""
+class DoraMagnitude(nn.Module):
+    """peft's `DoraLinearLayer` as far as inference reads it: the magnitude vector m [out_features] as `.weight`."""
 
-    def __init__(self, base: nn.Linear, r: int, scaling: float):
+    def __init__(self, out_features: int, device=None, dtype=None):
+        super().__init__()
+        self.weight = nn.Parameter(torch.ones(out_features, device=device, dtype=dtype))
+
+
+class LoraLinear(nn.Module):
+    """An `nn.Linear` with one unmerged low-rank adapter, in peft's `lora.Linear` attribute layout (with DoRA:
+    `use_dora[name]` and `lora_magnitude_vector[name].weight`)."""
+
+    def __init__(self, base: nn.Linear, r: int, scaling: float, use_dora: bool = False):
         super().__init__()
         self.base_layer = base
         kw = dict(bias=False, device=base.weight.device, dtype=base.weight.dtype)
         self.lora_A = nn.ModuleDict({ADAPTER: nn.Linear(base.in_features, r, **kw)})
         self.lora_B = nn.ModuleDict({ADAPTER: nn.Linear(r, base.out_features, **kw)})
         self.scaling = {ADAPTER: float(scaling)}
+        self.use_dora = {ADAPTER: bool(use_dora)}
+        self.lora_magnitude_vector = nn.ModuleDict(
+            {ADAPTER: DoraMagnitude(base.out_features, base.weight.device, base.weight.dtype)} if use_dora else {})
         self.active_adapters = [ADAPTER]
         self.in_features, self.out_features = base.in_features, base.out_features
 
@@ -55,7 +72,8 @@ class LoraLinear(nn.Module):
         return _linear(x.reshape(-1, x.shape[-1]).contiguous(), self).view(*x.shape[:-1], self.out_features)
 
     def extra_repr(self) -> str:
-        return f"r={self.lora_A[ADAPTER].out_features}, scaling={self.scaling[ADAPTER]}"
+        dora = ", use_dora=True" if self.use_dora[ADAPTER] else ""
+        return f"r={self.lora_A[ADAPTER].out_features}, scaling={self.scaling[ADAPTER]}{dora}"
 
 
 def is_wrapped(module: nn.Module) -> bool:
@@ -63,9 +81,8 @@ def is_wrapped(module: nn.Module) -> bool:
     return hasattr(module, "base_layer") and hasattr(module, "lora_A")
 
 
-def adapter_of(lin: nn.Module):
-    """(A [r, in], B [out, r], scaling) of the active adapter of a LoRA-wrapped Linear, or None for a plain Linear (and
-    for a peft layer whose adapters are disabled or already merged into the base weight)."""
+def _active(lin: nn.Module):
+    """Name of the active adapter of a LoRA-wrapped Linear, or None (plain Linear, adapters disabled or merged)."""
     la = getattr(lin, "lora_A", None)
     if la is None or getattr(lin, "merged", False) or getattr(lin, "disable_adapters", False):
         return None
@@ -74,19 +91,41 @@ def adapter_of(lin: nn.Module):
         return None
     if len(names) > 1:
         raise NotImplementedError(f"{len(names)} active LoRA adapters on one Linear: osb200 runs one at a time")
-    n = names[0]
-    if getattr(lin, "use_dora", {}).get(n, False):
-        raise NotImplementedError("DoRA adapters are not supported")
-    return la[n].weight, lin.lora_B[n].weight, float(lin.scaling[n])
+    return names[0]
+
+
+def adapter_of(lin: nn.Module):
+    """(A [r, in], B [out, r], scaling) of the active adapter of a LoRA-wrapped Linear, or None for a plain Linear (and
+    for a peft layer whose adapters are disabled or already merged into the base weight).  A DoRA adapter also has a
+    magnitude vector: `dora_magnitude`."""
+    n = _active(lin)
+    if n is None:
+        return None
+    return lin.lora_A[n].weight, lin.lora_B[n].weight, float(lin.scaling[n])
+
+
+def dora_magnitude(lin: nn.Module):
+    """The magnitude vector m [out_features] of the active adapter when it is a DoRA adapter, else None."""
+    n = _active(lin)
+    if n is None or not getattr(lin, "use_dora", {}).get(n, False):
+        return None
+    return lin.lora_magnitude_vector[n].weight
 
 
 def _state(lins):
-    """What a packed adapter depends on: identity and version of every A / B tensor and the scaling."""
+    """What a packed adapter depends on: identity and version of every A / B tensor and the scaling; for DoRA also of
+    the magnitude vector and the base weight, which g = m / ||W + s B A|| reads."""
     out = []
     for lin in lins:
         ad = adapter_of(lin)
-        out.append(None if ad is None else (id(lin), ad[0].data_ptr(), ad[0]._version, ad[1].data_ptr(), ad[1]._version,
-                                            ad[2], ad[0].dtype, ad[0].device))
+        if ad is None:
+            out.append(None)
+            continue
+        st = (id(lin), ad[0].data_ptr(), ad[0]._version, ad[1].data_ptr(), ad[1]._version, ad[2], ad[0].dtype, ad[0].device)
+        m = dora_magnitude(lin)
+        if m is not None:
+            st += (m.data_ptr(), m._version, lin.weight.data_ptr(), lin.weight._version)
+        out.append(st)
     return tuple(out)
 
 
@@ -96,10 +135,12 @@ _PACKS = weakref.WeakKeyDictionary()   # first Linear of a pack -> {layout: (ada
 def lora_pack(groups, k_pad: int = 0):
     """The adapters of Linears that read ONE input, for one down GEMM: `groups` lists, per weight the forward multiplies
     that input with, its output rows as (linear, row_lo, row_hi) slices (a packed q|k|v weight has three; linear1's qkv
-    part is (linear1, 0, 3C)).  Returns None when no member carries an adapter, else (A_cat, [B_cat or None per group]):
-    A_cat bf16 [R, K + k_pad] stacks every adapted member's A once (rank zero-padded to a multiple of 8, K zero-padded by
-    k_pad like the base weight); B_cat bf16 [rows, R] holds scaling * B in the member's rows and rank columns and zeros
-    elsewhere, None for a group without an adapted member.  Cached on the adapter state."""
+    part is (linear1, 0, 3C)).  Returns None when no member carries an adapter, else
+    (A_cat, [B_cat or None per group], [col_scale or None per group]): A_cat bf16 [R, K + k_pad] stacks every adapted
+    member's A once (rank zero-padded to a multiple of 8, K zero-padded by k_pad like the base weight); B_cat bf16
+    [rows, R] holds scaling * B in the member's rows and rank columns and zeros elsewhere, None for a group without an
+    adapted member; col_scale fp32 [rows] holds DoRA's g = m / ||W + s B A|| in a DoRA member's rows and 1.0 elsewhere,
+    None for a group without a DoRA member.  Cached on the adapter state."""
     lins = []
     for g in groups:
         for lin, _, _ in g:
@@ -145,7 +186,31 @@ def _build_pack(groups, lins, k_pad):
                     Bg[row:row + hi - lo, o:o + A.shape[0]] = s * Bw[lo:hi].float()
                 row += hi - lo
             Bs.append(Bg.to(torch.bfloat16).contiguous())   # bf16(s B): the scale is folded once per load / change
-    return A_cat, Bs
+        gs = {id(l): _dora_scale(l, *ads[id(l)]) for l in lins if ads[id(l)] is not None and dora_magnitude(l) is not None}
+        Ss = []
+        for g in groups:
+            if all(id(l) not in gs for l, _, _ in g):
+                Ss.append(None)
+                continue
+            Ss.append(torch.cat([gs[id(l)][lo:hi] if id(l) in gs else torch.ones(hi - lo, device=ref.device)
+                                 for l, lo, hi in g]).contiguous())
+    return A_cat, Bs, Ss
+
+
+_NORM_CHUNK = 1 << 24   # fp32 elements of W + s B A materialised at a time while g is computed (64 MB)
+
+
+def _dora_scale(lin, A, B, s):
+    """g = m / ||W + s B A||_2 over in_features, fp32 [out_features], on the weights' device; computed in row chunks so
+    the temporary stays bounded whatever the layer's size.  (peft's DoRA layer recomputes this on every forward.)"""
+    W = lin.weight
+    Af = A.float()
+    norm = torch.empty(W.shape[0], dtype=torch.float32, device=W.device)
+    step = max(1, _NORM_CHUNK // W.shape[1])
+    for lo in range(0, W.shape[0], step):
+        hi = min(lo + step, W.shape[0])
+        norm[lo:hi] = torch.linalg.vector_norm(W[lo:hi].float() + s * (B[lo:hi].float() @ Af), dim=1)
+    return dora_magnitude(lin).float() / norm
 
 
 # LoRA-wrapped modules registered into any parent module since import.  Wrapping (peft's and load_lora's) assigns the
@@ -179,8 +244,6 @@ def _read_config(path: str) -> dict:
         cfg = json.load(f)
     if cfg.get("peft_type", "LORA") != "LORA":
         raise ValueError(f"peft_type {cfg.get('peft_type')!r} is not supported: only LORA adapters can be loaded")
-    if cfg.get("use_dora"):
-        raise ValueError("use_dora: DoRA adapters are not supported")
     if cfg.get("bias", "none") != "none":
         raise ValueError(f"bias={cfg['bias']!r}: adapters with trained biases are not supported (only bias='none')")
     if cfg.get("modules_to_save"):
@@ -232,7 +295,9 @@ def _pattern_value(patterns: dict, name: str, default):
 
 def load_lora(model: nn.Module, path: str, scale: float = 1.0) -> nn.Module:
     """Load the PEFT LoRA adapter in directory `path` into the MMDiT `model`, in place, unmerged; `scale` multiplies
-    every layer's scaling (lora_alpha / r).  Returns the model.  One adapter at a time: `unload_lora` first."""
+    every layer's scaling (lora_alpha / r).  A DoRA adapter (`use_dora: true`) also carries one magnitude vector per
+    target, saved by peft as `base_model.model.<name>.lora_magnitude_vector` [out_features] (its state-dict export drops
+    the adapter name and the DoRA layer's `.weight`).  Returns the model.  One adapter at a time: `unload_lora` first."""
     from opensora.models.mmdit.model import MMDiTModel
 
     if not isinstance(model, MMDiTModel):
@@ -244,6 +309,7 @@ def load_lora(model: nn.Module, path: str, scale: float = 1.0) -> nn.Module:
     weights = _read_weights(path)
     prefix = "base_model.model."
     r0, alpha0 = int(cfg.get("r", 8)), float(cfg.get("lora_alpha", 8))
+    dora = bool(cfg.get("use_dora"))
     mods = dict(model.named_modules())
     plan, used = [], set()
     for name in _targets(model, cfg["target_modules"]):
@@ -260,15 +326,26 @@ def load_lora(model: nn.Module, path: str, scale: float = 1.0) -> nn.Module:
             if tuple(weights[k].shape) != shape:
                 raise ValueError(f"{k} has shape {tuple(weights[k].shape)}, expected {shape} (r = {r})")
         used |= {ka, kb}
-        plan.append((name, lin, r, s, weights[ka], weights[kb]))
+        mag = None
+        if dora:
+            km = f"{prefix}{name}.lora_magnitude_vector"
+            if km not in weights:
+                raise ValueError(f"use_dora: adapter weights miss the magnitude vector {km}")
+            if tuple(weights[km].shape) != (lin.out_features,):
+                raise ValueError(f"use_dora: {km} has shape {tuple(weights[km].shape)}, expected ({lin.out_features},)")
+            used.add(km)
+            mag = weights[km]
+        plan.append((name, lin, r, s, weights[ka], weights[kb], mag))
     extra = sorted(set(weights) - used)
     if extra:
         raise ValueError(f"adapter weights hold {len(extra)} tensors no target uses, e.g. {extra[:3]}")
     with torch.no_grad():
-        for name, lin, r, s, A, B in plan:
-            wrapped = LoraLinear(lin, r, s)
+        for name, lin, r, s, A, B, mag in plan:
+            wrapped = LoraLinear(lin, r, s, use_dora=mag is not None)
             wrapped.lora_A[ADAPTER].weight.copy_(A)
             wrapped.lora_B[ADAPTER].weight.copy_(B)
+            if mag is not None:
+                wrapped.lora_magnitude_vector[ADAPTER].weight.copy_(mag)
             parent, _, attr = name.rpartition(".")
             setattr(mods[parent] if parent else model, attr, wrapped)
     _drop_caches(model)

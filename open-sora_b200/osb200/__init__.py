@@ -160,7 +160,7 @@ class GemmArgs(C.Structure):
 
 class LoraArgs(C.Structure):
     _fields_ = [("U", C.c_void_p), ("B", C.c_void_p), ("ldu", C.c_int64), ("ldb", C.c_int64), ("r", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("reserved", C.c_int32), ("col_scale", C.c_void_p)]
 
 
 class GemmFp8Args(C.Structure):
@@ -391,19 +391,26 @@ def gemm(a, w, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None,
 
 
 def gemm_lora(a, w, bias, u, b, *, epilogue: int = EPI_BIAS, residual=None, gate=None, group_rows: int = 0,
-              mod_index=None, out=None, block_n: int = 0):
+              mod_index=None, out=None, block_n: int = 0, col_scale=None):
     """out = epilogue(a @ w.T + u @ b.T + bias) in one fp32 accumulator (osb_gemm_lora): `gemm` plus an unmerged LoRA
     update.  u bf16 [M, r] = x @ lora_A.T (the down projection, row stride free), b bf16 [N, r] = scaling * lora_B; r is
-    a multiple of 8 (zero-pad A's rows and B's columns)."""
+    a multiple of 8 (zero-pad A's rows and B's columns).  col_scale: None, or a contiguous fp32 [N] tensor g on a's
+    device: out = epilogue(g * (a @ w.T + u @ b.T) + bias), DoRA's per-output-channel factor."""
     import torch
 
     _need(u, torch.bfloat16, "u"); _need(b, torch.bfloat16, "b")
     if u.dim() != 2 or b.dim() != 2 or u.shape[0] != a.shape[0] or b.shape[0] != w.shape[0] or u.shape[1] != b.shape[1]:
         raise OsbError(f"gemm_lora: u must be [M, r] and b [N, r] for a {tuple(a.shape)} x {tuple(w.shape)} GEMM, got "
                        f"{tuple(u.shape)} and {tuple(b.shape)}")
+    if col_scale is not None:
+        if col_scale.dtype != torch.float32 or col_scale.shape != (w.shape[0],) or not col_scale.is_contiguous() \
+                or col_scale.device != a.device:
+            raise OsbError(f"gemm_lora: col_scale must be a contiguous float32 [{w.shape[0]}] tensor on {a.device}, got "
+                           f"{col_scale.dtype} {tuple(col_scale.shape)} on {col_scale.device}")
     args, out = _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, 0, block_n)
     la = LoraArgs()
     la.U, la.B, la.ldu, la.ldb, la.r = u.data_ptr(), b.data_ptr(), u.stride(0), b.stride(0), u.shape[1]
+    la.col_scale = None if col_scale is None else col_scale.data_ptr()
     with _Timed("gemm", 2.0 * args.M * args.N * (args.K + la.r)):
         _check(_lib.osb_gemm_lora(C.byref(args), C.byref(la), _stream()), "osb_gemm_lora")
     return out
