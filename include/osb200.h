@@ -64,7 +64,8 @@ typedef enum osb_epilogue {
                               /*                      layers.py:247-252, 333-334               */
   OSB_EPI_GATED_GELU = 3,     /* D[:, c] = gelu_tanh(P[:, 2c]) * P[:, 2c+1], P = A W^T + bias: W's rows interleave
                                  T5's wi_0 (even) and wi_1 (odd), D has N/2 columns (T5DenseGatedActDense)      */
-  OSB_EPI_BIAS_QUICK_GELU = 4 /* D = x * sigmoid(1.702 x), x = A W^T + bias (CLIP mlp.fc1 + quick_gelu)          */
+  OSB_EPI_BIAS_QUICK_GELU = 4, /* D = x * sigmoid(1.702 x), x = A W^T + bias (CLIP mlp.fc1 + quick_gelu)         */
+  OSB_EPI_BIAS_GELU_TANH_FP8 = 5 /* osb_gemm_fp8_blocks only: gelu_tanh(...) emitted as e4m3 with 1 x 128 block scales */
 } osb_epilogue;
 
 typedef struct osb_gemm_args {
@@ -158,6 +159,37 @@ int osb_ln_modulate_fp8(const void* x, const float* shift, const float* scale, v
  * ldy % 16 == 0, 16-byte aligned x and y8. */
 int osb_quant_rows_fp8(const void* x, int64_t ldx, void* y8, int64_t ldy, float* y_scale, int64_t rows, int K,
                        void* stream);
+
+/* ---- FP8 (e4m3) with 1 x 128 block scales: the opt-in MLP path of MMDiT -------------------------------------------- */
+/* Block quantization rule: the block (r, b) = X[r, 128 b .. 128 b + 127] gets s[r, b] = amax(|block|) / 448 (s = 1 for an
+ * all-zero block) and codes e4m3_rn_satfinite(X[r, k] / s[r, b]): the per-row rule applied per 128 columns. */
+typedef struct osb_fp8_blocks_args {
+  int64_t a_scale_ld;  /* 0: a_scale is fp32 [M] (per row); > 0: block mode, a_scale is fp32 [M, K/128] with this row
+                          stride (>= K / 128)                                                                        */
+  void* D8;            /* OSB_EPI_BIAS_GELU_TANH_FP8 only: e4m3 [M, N] codes, row stride ldd8 (D is not written)       */
+  float* d_scale;      /* OSB_EPI_BIAS_GELU_TANH_FP8 only: fp32 [M, N/128] block scales, row stride ld_dscale          */
+  int64_t ldd8, ld_dscale;
+} osb_fp8_blocks_args;
+
+/* osb_gemm_fp8 with the scales of A per (row, 128-element k-block): D = epilogue(w_scale[n] * sum_kb a_scale[m, kb] *
+ * acc_kb + bias), acc_kb = the tensor core's sum over k-block kb, multiplied by its scale as it is promoted into the fp32
+ * register accumulator.  Every epilogue of osb_gemm_fp8 (bias, GELU-tanh, gate + residual with group_rows / mod_index)
+ * works in block mode.  a_scale_ld == 0 (per-row scales) with one of those epilogues runs osb_gemm_fp8 itself (same
+ * kernel, same bits).
+ * OSB_EPI_BIAS_GELU_TANH_FP8 (per-row or block-scaled A): v = gelu_tanh(acc * scales + bias) in fp32, written as e4m3
+ * codes to D8 with one scale per (row, 128 columns) in d_scale, by the block quantization rule; no bf16 output.  Needs
+ * N % 128 == 0 and block_n 0 or 128 (one output tile row = one scale block).  With D8 / d_scale pointing into the
+ * columns of a wider buffer, it fills part of the A operand of a later block-mode GEMM.  Replaces fc1 -> GELU (and the
+ * mlp part of linear1 -> GELU) of the MMDiT blocks when FP8 is enabled; block mode replaces fc2 and linear2. */
+int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* gemm, const osb_fp8_blocks_args* blk, void* stream);
+
+/* Block quantizer: bf16 x [rows, K] (row stride ldx) -> e4m3 y8 [rows, K] (row stride ldy) with the scale of (row r,
+ * block b) at y_scale[r * lds + b].  block == 128: 1 x 128 block scales, one pass over x (the attention output of the
+ * MMDiT single blocks).  block == K: one scale per row for rows of any length (the MLP weights, per output channel, up
+ * to K = 5 x 4096; the row is read twice).  K % 128 == 0, ldx and ldy multiples of 8, 16-byte aligned x, 8-byte aligned
+ * y8, 4-byte aligned y_scale. */
+int osb_quant_blocks_fp8(const void* x, int64_t ldx, void* y8, int64_t ldy, float* y_scale, int64_t lds, int64_t rows,
+                         int K, int block, void* stream);
 
 /* ---- attention with short key sets (whole key set resident in one CTA) -------------------- */
 typedef struct osb_attn_short_args {

@@ -343,5 +343,12 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   return 0.5f * x * (1.0f + t);
 }
 
+// two e4m3 codes, round to nearest even, saturated to +-448 (`lo` in the low byte)
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
 #endif  // __CUDACC__
 }  // namespace osb

@@ -103,13 +103,7 @@ ln_modulate_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict_
   }
 }
 
-// ---- FP8 (e4m3) row quantization ----------------------------------------------------------------------------------
-// two e4m3 codes, round to nearest even, saturated to +-448 (`lo` in the low byte)
-__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
-  uint16_t r;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  return r;
-}
+// ---- FP8 (e4m3) row quantization (e4m3x2: common.cuh) ---------------------------------------------------------------
 // the row scale from the warp's partial amax values: amax / 448, 1 for an all-zero row
 __device__ __forceinline__ float fp8_row_scale(float amax) {
 #pragma unroll
@@ -258,6 +252,79 @@ quant_rows_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, uint8_t*
       }
       yr[c] = e4m3x8(o, rs);
     }
+  }
+}
+
+// bf16 -> e4m3 codes with one scale per (row, 128-column block): the 16 lanes of a half-warp hold one block, 8 elements
+// (one 16-byte load) each, so the block amax is four shuffles and every lane stores its 8 codes.  K / 8 is a multiple of
+// 16: a half-warp never straddles two blocks, and past the end whole half-warps leave together.
+__global__ void __launch_bounds__(kLnWarpsPerBlock * 32)
+quant_blocks_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, uint8_t* __restrict__ y8, int64_t ldy,
+                        float* __restrict__ y_scale, int64_t lds, int64_t rows, int K) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int64_t nchunks = K >> 3;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * nchunks) return;
+  const int64_t row = i / nchunks;
+  const int c = (int)(i - row * nchunks);
+  uint4 t;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(t.x), "=r"(t.y), "=r"(t.z), "=r"(t.w) : "l"(x + row * ldx + c * 8));
+  const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
+  float o[8];
+  float amax = 0.f;
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const float2 f = unpack_bf16x2(tw[e]);
+    o[2 * e] = f.x;
+    o[2 * e + 1] = f.y;
+    amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+  }
+  const unsigned half = (threadIdx.x & 16) ? 0xffff0000u : 0x0000ffffu;
+#pragma unroll
+  for (int m = 8; m > 0; m >>= 1) amax = fmaxf(amax, __shfl_xor_sync(half, amax, m));
+  const float s = amax > 0.f ? amax / 448.0f : 1.0f;
+  if ((c & 15) == 0) y_scale[row * lds + (c >> 4)] = s;
+  *reinterpret_cast<uint2*>(y8 + row * ldy + c * 8) = e4m3x8(o, s);
+}
+
+// Per-row quantization of rows of any length (the MLP weights at enable time, K up to 5 x 4096): one warp per row reads
+// it twice, once for the amax and once for the codes (the second read mostly hits L2).  Not on the per-step path.
+__global__ void __launch_bounds__(kLnWarpsPerBlock * 32)
+quant_rows_long_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, uint8_t* __restrict__ y8, int64_t ldy,
+                           float* __restrict__ y_scale, int64_t lds, int64_t rows, int K) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * kLnWarpsPerBlock + (threadIdx.x >> 5);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (row >= rows) return;
+  const int nchunks = K >> 3;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + row * ldx);
+  float amax = 0.f;
+  for (int c = lane; c < nchunks; c += 32) {
+    const uint4 t = xr[c];
+    const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 f = unpack_bf16x2(tw[e]);
+      amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+    }
+  }
+  const float rs = fp8_row_scale(amax);
+  if (lane == 0) y_scale[row * lds] = rs;
+  uint2* yr = reinterpret_cast<uint2*>(y8 + row * ldy);
+  for (int c = lane; c < nchunks; c += 32) {
+    const uint4 t = xr[c];
+    const uint32_t tw[4] = {t.x, t.y, t.z, t.w};
+    float o[8];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 f = unpack_bf16x2(tw[e]);
+      o[2 * e] = f.x;
+      o[2 * e + 1] = f.y;
+    }
+    yr[c] = e4m3x8(o, rs);
   }
 }
 
@@ -451,6 +518,39 @@ extern "C" int osb_quant_rows_fp8(const void* x, int64_t ldx, void* y8, int64_t 
 #undef OSB_Q8_CASE
   set_error("osb_quant_rows_fp8: unsupported K %d", K);
   return OSB_ERR_UNSUPPORTED;
+}
+
+extern "C" int osb_quant_blocks_fp8(const void* x, int64_t ldx, void* y8, int64_t ldy, float* y_scale, int64_t lds,
+                                    int64_t rows, int K, int block, void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(x && y8 && y_scale, "osb_quant_blocks_fp8: null tensor");
+  OSB_REQUIRE(rows > 0, "osb_quant_blocks_fp8: rows must be positive");
+  OSB_REQUIRE(K > 0 && K % 128 == 0, "osb_quant_blocks_fp8: K must be a positive multiple of 128 (got %d)", K);
+  OSB_REQUIRE(block == 128 || block == K, "osb_quant_blocks_fp8: block must be 128 or K (got %d, K %d)", block, K);
+  OSB_REQUIRE(ldx >= K && ldy >= K && ldx % 8 == 0 && ldy % 8 == 0 && lds >= K / block,
+              "osb_quant_blocks_fp8: ldx and ldy must be >= K and multiples of 8, lds >= K / block (ldx %lld ldy %lld "
+              "lds %lld K %d)", (long long)ldx, (long long)ldy, (long long)lds, K);
+  OSB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y8) & 7) == 0 &&
+              (reinterpret_cast<uintptr_t>(y_scale) & 3) == 0,
+              "osb_quant_blocks_fp8: x must be 16-byte, y8 8-byte and y_scale 4-byte aligned");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const __nv_bfloat16* xb = static_cast<const __nv_bfloat16*>(x);
+  uint8_t* yb = static_cast<uint8_t*>(y8);
+  cudaLaunchAttribute attr[2];
+  if (block == 128) {
+    const int64_t threads = rows * (K / 8);
+    const int64_t blocks = (threads + kLnWarpsPerBlock * 32 - 1) / (kLnWarpsPerBlock * 32);
+    OSB_REQUIRE(blocks < (1ll << 31), "osb_quant_blocks_fp8: too many rows (%lld)", (long long)rows);
+    cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)blocks), dim3(kLnWarpsPerBlock * 32), 0, s, attr);
+    OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, quant_blocks_fp8_kernel, xb, ldx, yb, ldy, y_scale, lds, rows, K));
+  } else {
+    const unsigned blocks = (unsigned)((rows + kLnWarpsPerBlock - 1) / kLnWarpsPerBlock);
+    cudaLaunchConfig_t cfg = launch_config(dim3(blocks), dim3(kLnWarpsPerBlock * 32), 0, s, attr);
+    OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, quant_rows_long_fp8_kernel, xb, ldx, yb, ldy, y_scale, lds, rows, K));
+  }
+  count_launch();
+  return OSB_OK;
 }
 
 extern "C" int osb_ln_modulate_scatter(const void* x, const float* shift, const float* scale, int64_t rows, int C,

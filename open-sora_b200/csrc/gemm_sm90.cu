@@ -23,6 +23,11 @@
 //               box bytes and stage ring as 64 bf16), issued as 4 wgmma k32 steps into a partial accumulator that is added
 //               into the fp32 register accumulator after every k-block; the epilogue scales the accumulator by
 //               a_scale[row] * w_scale[col] before the unchanged bias / GELU / gate + residual code.  BLOCK_N 64 / 128.
+//   kFp8Blk     kFp8 with 1 x 128 block scales on A: each k-block's partial is multiplied by a_scale[row, kb] as it is
+//               promoted into the fp32 accumulator (per-row scales are a zero k-stride), the epilogue applies w_scale[col].
+//               With BLOCK_N = 128 it also has the FP8-emitting GELU epilogue: one output tile row is exactly one
+//               128-column scale block, held by the 4 lanes of a quad, so the block amax is two shuffles; the codes and
+//               the scale go out instead of bf16.
 //
 // Replaces every nn.Linear on the denoiser block path of the reference
 // (opensora/models/mmdit/layers.py:209-214,247-252,277-281,314-334,401) and the fused epilogues
@@ -40,7 +45,16 @@ constexpr int kBlockK = 64;
 constexpr int kNumThreads = 384;            // producer warpgroup + two consumer warpgroups
 constexpr int kStageBudget = 200 * 1024;    // operand ring (one CTA per SM; 227 KB is the per-block limit)
 
-enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4, kFp8 = 5 };
+enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4, kFp8 = 5, kFp8Blk = 6 };
+
+// kFp8Blk only: where the scale of (row m, k-block kb) of A is (a_scale + m * a_ld + kb * a_kstride; a_kstride = 0 for
+// per-row scales), and the e4m3 output of the FP8-emitting GELU epilogue (codes d8 [M, N], ldd8; scales [M, N / 128]).
+struct Fp8BlockParams {
+  int64_t a_ld, a_kstride;
+  uint8_t* d8;
+  float* d_scale;
+  int64_t ldd8, ld_dscale;
+};
 
 struct GemmEpilogueParams {
   const __nv_bfloat16* bias;
@@ -103,11 +117,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const GemmEpilogueParams p, const ConvGeom cg, const HeadTileParams ht,
                  const __grid_constant__ CUtensorMap tmap_u, const __grid_constant__ CUtensorMap tmap_lb,
                  const int32_t lora_k_blocks,     // kLora only: U / s B maps and ceil(r / 64)
-                 const float* a_scale, const float* w_scale) {   // kFp8: row scales of A and W; kLora: w_scale is the
+                 const float* a_scale, const float* w_scale,     // kFp8: row scales of A and W; kLora: w_scale is the
                                                                  // optional per-column (DoRA) scale, may be null
+                 const Fp8BlockParams fb) {                      // kFp8Blk only
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::STAGES;
-  constexpr int kBK = kMode == kFp8 ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
+  constexpr int kBK = (kMode == kFp8 || kMode == kFp8Blk) ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 1024-byte aligned
@@ -194,7 +209,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   float acc[BLOCK_N / 2];
 #pragma unroll
   for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-  if constexpr (kMode == kFp8) {
+  if constexpr (kMode == kFp8 || kMode == kFp8Blk) {
     // FP8 wgmma adds into its accumulator with fewer mantissa bits than an fp32 add, so a K-long sum in the wgmma
     // accumulator loses precision with K.  Each k-block (128 e4m3 elements) is summed into `part` by the tensor core and
     // promoted into the fp32 register accumulator `acc` before the next one: acc is an fp32 sum of 128-element partials.
@@ -202,9 +217,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     float part[BLOCK_N / 2];
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) part[i] = 0.f;
+    // kFp8Blk: the scale rows of this thread's two accumulator rows (clamped: rows >= M are computed but never stored)
+    const float* sa_row0 = a_scale;
+    const float* sa_row1 = a_scale;
+    if constexpr (kMode == kFp8Blk) {
+      const int64_t r0 = m_blk * kBlockM + cw * 64 + (tid_wg >> 5) * 16 + ((tid_wg & 31) >> 2);
+      sa_row0 = a_scale + min(r0, p.M - 1) * fb.a_ld;
+      sa_row1 = a_scale + min(r0 + 8, p.M - 1) * fb.a_ld;
+    }
     int stage = 0;
     uint32_t phase = 0;
     for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
+      float s0 = 1.f, s1 = 1.f;
+      if constexpr (kMode == kFp8Blk) {   // issued before the wait: the loads overlap the TMA and the tensor core
+        s0 = __ldg(sa_row0 + kb * fb.a_kstride);
+        s1 = __ldg(sa_row1 + kb * fb.a_kstride);
+      }
       mbar_wait_notrace(full_bar(stage), phase);
       const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
       const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
@@ -217,8 +245,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       wgmma_wait<0>();   // this k-block's partial is complete and its stage has been read
       wgmma_fence_regs(part);
       if (tid_wg == 0) mbar_arrive(empty_bar(stage));
+      if constexpr (kMode == kFp8Blk) {   // acc[4 j + 2 h + e] belongs to row h of the fragment
 #pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          acc[4 * j] = fmaf(part[4 * j], s0, acc[4 * j]);
+          acc[4 * j + 1] = fmaf(part[4 * j + 1], s0, acc[4 * j + 1]);
+          acc[4 * j + 2] = fmaf(part[4 * j + 2], s1, acc[4 * j + 2]);
+          acc[4 * j + 3] = fmaf(part[4 * j + 3], s1, acc[4 * j + 3]);
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
+      }
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
   } else {
@@ -264,6 +302,48 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         acc[4 * j + 2] *= cs.x;
         acc[4 * j + 3] *= cs.y;
       }
+    }
+  }
+
+  if constexpr (kMode == kFp8Blk && BLOCK_N == 128) {
+    if (p.epilogue == OSB_EPI_BIAS_GELU_TANH_FP8) {
+      // ===================== epilogue: GELU-tanh -> e4m3 codes + one scale per (row, 128 columns) =====================
+      // N % 128 == 0 (host check): every column of the tile exists.  Rows >= M take part in the quad shuffles (all lanes
+      // must) and store nothing.
+      const int64_t n0 = n_blk * BLOCK_N + c_frag;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
+        float amax = 0.f;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int64_t n = n0 + 8 * j;
+          const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+          float v0 = acc[4 * j + 2 * h] * sw.x, v1 = acc[4 * j + 2 * h + 1] * sw.y;
+          if (p.bias) {
+            const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+            v0 += b.x;
+            v1 += b.y;
+          }
+          v0 = gelu_tanh(v0);
+          v1 = gelu_tanh(v1);
+          acc[4 * j + 2 * h] = v0;
+          acc[4 * j + 2 * h + 1] = v1;
+          amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+        }
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+        const float s = amax > 0.f ? amax / 448.0f : 1.0f;
+        if (row < p.M) {
+          uint8_t* drow = fb.d8 + row * fb.ldd8;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j)   // x / s, IEEE division as the contract states it
+            *reinterpret_cast<uint16_t*>(drow + n0 + 8 * j) =
+                (uint16_t)e4m3x2(acc[4 * j + 2 * h] / s, acc[4 * j + 2 * h + 1] / s);
+          if (c_frag == 0) fb.d_scale[row * fb.ld_dscale + n_blk] = s;
+        }
+      }
+      return;
     }
   }
 
@@ -400,7 +480,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
       if (!row_ok) continue;
       const float* gate_row = nullptr;
-      if ((kMode == kPlain || kMode == kLora || kMode == kFp8) && p.epilogue == OSB_EPI_BIAS_GATE_RES && p.gate != nullptr) {
+      if ((kMode == kPlain || kMode == kLora || kMode == kFp8 || kMode == kFp8Blk) && p.epilogue == OSB_EPI_BIAS_GATE_RES &&
+          p.gate != nullptr) {
         int64_t gi = (uint32_t)row / group_rows32;
         if (p.mod_index) gi = p.mod_index[gi];
         gate_row = p.gate + gi * p.gate_stride;
@@ -418,6 +499,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
           v0 *= sa * sw.x;
           v1 *= sa * sw.y;
+        } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator
+          const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+          v0 *= sw.x;
+          v1 *= sw.y;
         }
         if (p.bias) {
           const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
@@ -452,13 +537,13 @@ template <int BLOCK_N, int kMode>
 static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tw, const GemmEpilogueParams& p, const ConvGeom& cg,
                          const HeadTileParams& ht, int64_t tiles, cudaStream_t stream, const CUtensorMap* tu = nullptr,
                          const CUtensorMap* tlb = nullptr, int32_t lora_k_blocks = 0, const float* a_scale = nullptr,
-                         const float* w_scale = nullptr) {
+                         const float* w_scale = nullptr, const Fp8BlockParams& fb = Fp8BlockParams{}) {
   if (tiles >= (1ll << 31)) { set_error("osb gemm: too many output tiles (%lld)", (long long)tiles); return OSB_ERR_UNSUPPORTED; }
   cudaLaunchAttribute attr[2];
   cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)tiles), dim3(kNumThreads), GemmCfg<BLOCK_N>::SMEM_BYTES, stream, attr);
   // the LoRA maps are read by kLora only; every other mode gets the main maps as placeholders
   OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<BLOCK_N, kMode>, ta, tw, p, cg, ht, tu ? *tu : ta,
-                                    tlb ? *tlb : tw, lora_k_blocks, a_scale, w_scale));
+                                    tlb ? *tlb : tw, lora_k_blocks, a_scale, w_scale, fb));
   count_launch();
   return OSB_OK;
 }
@@ -542,6 +627,8 @@ int gemm_init() {
   if ((rc = init_one<256, kText>())) return rc;
   if ((rc = init_one<64, kFp8>())) return rc;
   if ((rc = init_one<128, kFp8>())) return rc;
+  if ((rc = init_one<64, kFp8Blk>())) return rc;
+  if ((rc = init_one<128, kFp8Blk>())) return rc;
   return OSB_OK;
 }
 
@@ -562,8 +649,8 @@ static int pick_block_n(int64_t M, int64_t N) {
   return best;
 }
 
-template <int BLOCK_N>
-static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream) {
+template <int BLOCK_N, int kMode = kFp8>
+static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream, const Fp8BlockParams& fb = Fp8BlockParams{}) {
   CUtensorMap ta, tw;
   int rc = make_tmap_2d_e4m3(&ta, a.A, a.M, a.K, a.lda, kBlockM, 2 * kBlockK);
   if (rc) return rc;
@@ -584,7 +671,7 @@ static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream) {
   const int64_t tiles = ((a.M + kBlockM - 1) / kBlockM) * ((a.N + BLOCK_N - 1) / BLOCK_N);
   ConvGeom cg = {};
   HeadTileParams ht = {};
-  return launch_kernel<BLOCK_N, kFp8>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, a.a_scale, a.w_scale);
+  return launch_kernel<BLOCK_N, kMode>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, a.a_scale, a.w_scale, fb);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -681,39 +768,94 @@ extern "C" int osb_gemm_lora(const osb_gemm_args* gemm, const osb_lora_args* lor
   return osb::gemm_dispatch("osb_gemm_lora", gemm, lora, stream);
 }
 
-extern "C" int osb_gemm_fp8(const osb_gemm_fp8_args* args, void* stream) {
-  using namespace osb;
+namespace osb {
+
+// Argument checks shared by osb_gemm_fp8 and osb_gemm_fp8_blocks (`fn` names the entry point in errors); fp8_out: the
+// FP8-emitting epilogue, whose output is checked by the caller instead of D.
+static int check_fp8_args(const char* fn, const osb_gemm_fp8_args* args, bool fp8_out) {
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
-  OSB_REQUIRE(args != nullptr, "osb_gemm_fp8: null args");
+  OSB_REQUIRE(args != nullptr, "%s: null args", fn);
   const osb_gemm_fp8_args& a = *args;
-  OSB_REQUIRE(a.A && a.W && a.D && a.a_scale && a.w_scale, "osb_gemm_fp8: null operand or scale");
-  OSB_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "osb_gemm_fp8: empty problem (M %lld N %lld K %lld)",
+  OSB_REQUIRE(a.A && a.W && (a.D || fp8_out) && a.a_scale && a.w_scale, "%s: null operand or scale", fn);
+  OSB_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "%s: empty problem (M %lld N %lld K %lld)", fn,
               (long long)a.M, (long long)a.N, (long long)a.K);
-  OSB_REQUIRE(a.K % 128 == 0, "osb_gemm_fp8: K must be a multiple of 128 (one e4m3 k-block), got %lld", (long long)a.K);
-  OSB_REQUIRE(a.N % 8 == 0, "osb_gemm_fp8: N must be a multiple of 8, got %lld", (long long)a.N);
+  OSB_REQUIRE(a.K % 128 == 0, "%s: K must be a multiple of 128 (one e4m3 k-block), got %lld", fn, (long long)a.K);
+  OSB_REQUIRE(a.N % 8 == 0, "%s: N must be a multiple of 8, got %lld", fn, (long long)a.N);
   OSB_REQUIRE(a.lda % 16 == 0 && a.ldw % 16 == 0 && a.lda >= a.K && a.ldw >= a.K,
-              "osb_gemm_fp8: lda and ldw must be >= K and multiples of 16 (lda %lld ldw %lld)", (long long)a.lda,
+              "%s: lda and ldw must be >= K and multiples of 16 (lda %lld ldw %lld)", fn, (long long)a.lda,
               (long long)a.ldw);
-  OSB_REQUIRE(a.ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(a.D) & 15) == 0,
-              "osb_gemm_fp8: D must be 16-byte aligned with ldd %% 8 == 0");
-  OSB_REQUIRE(a.epilogue >= OSB_EPI_BIAS && a.epilogue <= OSB_EPI_BIAS_GATE_RES,
-              "osb_gemm_fp8: epilogue %d is not built for FP8 (bias, GELU-tanh, gate + residual)", a.epilogue);
+  if (!fp8_out) {
+    OSB_REQUIRE(a.ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(a.D) & 15) == 0,
+                "%s: D must be 16-byte aligned with ldd %% 8 == 0", fn);
+    OSB_REQUIRE(a.epilogue >= OSB_EPI_BIAS && a.epilogue <= OSB_EPI_BIAS_GATE_RES,
+                "%s: epilogue %d is not built for FP8 (bias, GELU-tanh, gate + residual)", fn, a.epilogue);
+  }
   OSB_REQUIRE((reinterpret_cast<uintptr_t>(a.w_scale) & 7) == 0 && (reinterpret_cast<uintptr_t>(a.a_scale) & 3) == 0,
-              "osb_gemm_fp8: a_scale must be 4-byte and w_scale 8-byte aligned");
+              "%s: a_scale must be 4-byte and w_scale 8-byte aligned", fn);
   if (a.epilogue == OSB_EPI_BIAS_GATE_RES) {
     OSB_REQUIRE(a.R == nullptr || (a.ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(a.R) & 15) == 0),
-                "osb_gemm_fp8: R must be 16-byte aligned with ldr %% 8 == 0");
+                "%s: R must be 16-byte aligned with ldr %% 8 == 0", fn);
     OSB_REQUIRE(a.gate == nullptr || (a.gate_stride % 4 == 0 && (reinterpret_cast<uintptr_t>(a.gate) & 15) == 0),
-                "osb_gemm_fp8: gate must be 16-byte aligned with gate_stride %% 4 == 0");
+                "%s: gate must be 16-byte aligned with gate_stride %% 4 == 0", fn);
   }
-  OSB_REQUIRE(a.bias == nullptr || (reinterpret_cast<uintptr_t>(a.bias) & 15) == 0,
-              "osb_gemm_fp8: bias must be 16-byte aligned");
+  OSB_REQUIRE(a.bias == nullptr || (reinterpret_cast<uintptr_t>(a.bias) & 15) == 0, "%s: bias must be 16-byte aligned", fn);
+  return OSB_OK;
+}
+
+}  // namespace osb
+
+extern "C" int osb_gemm_fp8(const osb_gemm_fp8_args* args, void* stream) {
+  using namespace osb;
+  if (int rc = check_fp8_args("osb_gemm_fp8", args, false)) return rc;
+  const osb_gemm_fp8_args& a = *args;
   // the promoted accumulation holds two accumulators per thread: tiles wider than 128 columns would not fit
   const int bn = a.block_n ? a.block_n : (a.N <= 64 ? 64 : 128);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (bn == 64) return launch_gemm_fp8<64>(a, s);
   if (bn == 128) return launch_gemm_fp8<128>(a, s);
   set_error("osb_gemm_fp8: unsupported block_n %d (64 or 128)", bn);
+  return OSB_ERR_UNSUPPORTED;
+}
+
+extern "C" int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* args, const osb_fp8_blocks_args* blk, void* stream) {
+  using namespace osb;
+  if (blk == nullptr) { set_error("osb_gemm_fp8_blocks: null block args"); return OSB_ERR_INVALID; }
+  const bool fp8_out = args != nullptr && args->epilogue == OSB_EPI_BIAS_GELU_TANH_FP8;
+  if (int rc = check_fp8_args("osb_gemm_fp8_blocks", args, fp8_out)) return rc;
+  const osb_gemm_fp8_args& a = *args;
+  const osb_fp8_blocks_args& b = *blk;
+  OSB_REQUIRE(b.a_scale_ld == 0 || b.a_scale_ld >= a.K / 128,
+              "osb_gemm_fp8_blocks: a_scale_ld must be 0 (per-row scales) or >= K / 128 (got %lld, K %lld)",
+              (long long)b.a_scale_ld, (long long)a.K);
+  int bn = a.block_n ? a.block_n : (a.N <= 64 ? 64 : 128);
+  if (fp8_out) {
+    // one 128-column output tile = one scale block per row
+    OSB_REQUIRE(a.N % 128 == 0, "osb_gemm_fp8_blocks: the FP8 GELU epilogue needs N %% 128 == 0, got %lld", (long long)a.N);
+    OSB_REQUIRE(a.block_n == 0 || a.block_n == 128, "osb_gemm_fp8_blocks: the FP8 GELU epilogue needs block_n 128, got %d",
+                a.block_n);
+    OSB_REQUIRE(b.D8 && b.d_scale, "osb_gemm_fp8_blocks: the FP8 GELU epilogue needs D8 and d_scale");
+    OSB_REQUIRE(b.ldd8 >= a.N && b.ldd8 % 2 == 0 && (reinterpret_cast<uintptr_t>(b.D8) & 1) == 0 &&
+                b.ld_dscale >= a.N / 128 && (reinterpret_cast<uintptr_t>(b.d_scale) & 3) == 0,
+                "osb_gemm_fp8_blocks: D8 must be 2-byte aligned with even ldd8 >= N, d_scale 4-byte aligned with "
+                "ld_dscale >= N / 128 (ldd8 %lld ld_dscale %lld)", (long long)b.ldd8, (long long)b.ld_dscale);
+    bn = 128;
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (b.a_scale_ld == 0 && !fp8_out) {   // per-row scales and a bf16 epilogue: exactly osb_gemm_fp8
+    if (bn == 64) return launch_gemm_fp8<64>(a, s);
+    if (bn == 128) return launch_gemm_fp8<128>(a, s);
+  } else {
+    Fp8BlockParams fb = {};
+    fb.a_ld = b.a_scale_ld ? b.a_scale_ld : 1;
+    fb.a_kstride = b.a_scale_ld ? 1 : 0;
+    fb.d8 = static_cast<uint8_t*>(b.D8);
+    fb.d_scale = b.d_scale;
+    fb.ldd8 = b.ldd8;
+    fb.ld_dscale = b.ld_dscale;
+    if (bn == 64) return launch_gemm_fp8<64, kFp8Blk>(a, s, fb);
+    if (bn == 128) return launch_gemm_fp8<128, kFp8Blk>(a, s, fb);
+  }
+  set_error("osb_gemm_fp8_blocks: unsupported block_n %d (64 or 128)", bn);
   return OSB_ERR_UNSUPPORTED;
 }
 

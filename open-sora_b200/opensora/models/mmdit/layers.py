@@ -15,7 +15,14 @@ interleaved pairs and `LigerEmbedND` rotate-half) and both QKV checkpoint layout
 LoRA (opensora/utils/lora.py): every Linear is read through `linear_parts` / `lora_pack`, which also return the active
 adapter's (A, scaling * B, DoRA column scale or None), if any.  Linears that read one input share one down GEMM
 U = x A_cat^T; each output weight then runs `osb_gemm_lora` (g * (x W^T + U B^T) in one accumulator, g = 1 without
-DoRA).  Without an adapter the launches are those of the plain model."""
+DoRA).  Without an adapter the launches are those of the plain model.
+
+FP8 (MMDiTModel.enable_fp8): the MLPs run on e4m3 operands.  Double blocks: ln_modulate_fp8 -> fc1 on
+`osb_gemm_fp8_blocks` whose GELU epilogue emits e4m3 codes with 1 x 128 block scales -> fc2 on block-scaled A (gate +
+residual).  Single blocks: the qkv part of linear1 stays bf16; the mlp part runs on ln_modulate_fp8 and its GELU epilogue
+writes columns C.. of an e4m3 [rows, 5C] cat buffer, `osb_quant_blocks_fp8` fills columns 0..C-1 from the attention
+output, and linear2 is one block-scaled FP8 GEMM with K = 5C.  The model hands the quantized weights and workspaces to the
+processors on `vec` (`_osb_fp8`, an `Fp8State`)."""
 from __future__ import annotations
 
 import math
@@ -235,6 +242,62 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
     return ao
 
 
+class Fp8State:
+    """What the FP8 MLP path of one MMDiTModel keeps: e4m3 weights with per-output-channel scales, quantized once per
+    block and MLP (`weights`), and e4m3 / scale workspaces reused by every block, one per shape (`buf`)."""
+
+    def __init__(self):
+        self._w, self._ws = {}, {}
+
+    @staticmethod
+    def mlp_linears(blk: nn.Module, kind: str):
+        """(fc1-side Linear, its row range, fc2-side Linear) of an MLP: kind "img" / "txt" (double block) or "single"."""
+        if kind != "single":
+            mlp = blk.img_mlp if kind == "img" else blk.txt_mlp
+            return mlp[0], (0, mlp[0].out_features), mlp[2]
+        C = blk.linear2.out_features
+        lin1 = blk.linear1 if getattr(blk, "fused_qkv", hasattr(blk, "linear1")) else blk.v_mlp
+        off = 3 * C if lin1 is getattr(blk, "linear1", None) else C
+        return lin1, (off, lin1.out_features), blk.linear2
+
+    def weights(self, osb, blk: nn.Module, kind: str):
+        """(fc1 e4m3 [hid, C], fc1 scales [hid], fc1 bias, fc2 e4m3 [C, K2], fc2 scales [C], fc2 bias) of one MLP."""
+        key = (id(blk), kind)
+        hit = self._w.get(key)
+        if hit is None or hit[0] is not blk:
+            l1, (lo, hi), l2 = self.mlp_linears(blk, kind)
+            for lin in (l1, l2):
+                if adapter_of(lin) is not None:
+                    raise ValueError("FP8 MLPs: a LoRA / DoRA adapter on an MLP Linear cannot run on the FP8 path; "
+                                     "unload_lora or disable_fp8 first")
+            w1, s1 = osb.quant_blocks_fp8(l1.weight[lo:hi], block=l1.in_features)
+            w2, s2 = osb.quant_blocks_fp8(l2.weight, block=l2.in_features)
+            b1 = None if l1.bias is None else l1.bias[lo:hi]
+            hit = self._w[key] = (blk, (w1, s1.view(-1), b1, w2, s2.view(-1), l2.bias))
+        return hit[1]
+
+    def buf(self, name: str, *shape, dtype=torch.float32, device=None) -> Tensor:
+        key = (name, shape, dtype, device)
+        t = self._ws.get(key)
+        if t is None:
+            t = self._ws[key] = torch.empty(shape, dtype=dtype, device=device)
+        return t
+
+
+def _mlp_fp8(osb, fp8: Fp8State, blk: nn.Module, kind: str, x: Tensor, mod, n: int) -> None:
+    """x += gate * MLP((1 + scale) * LN(x) + shift) in place, on FP8 operands (x: [rows, C] bf16, group_rows = n)."""
+    w1, s1, b1, w2, s2, b2 = fp8.weights(osb, blk, kind)
+    rows, C = x.shape
+    hid, dev, f8 = w1.shape[0], x.device, torch.float8_e4m3fn
+    x8, xs = osb.ln_modulate_fp8(x, mod.shift, mod.scale, group_rows=n, out=fp8.buf("x8", rows, C, dtype=f8, device=dev),
+                                 out_scale=fp8.buf("xs", rows, device=dev))
+    h8, hs = osb.gemm_fp8_blocks(x8, xs, w1, s1, b1, epilogue=osb.EPI_BIAS_GELU_TANH_FP8,
+                                 out=fp8.buf("h8", rows, hid, dtype=f8, device=dev),
+                                 out_scale=fp8.buf("hs", rows, hid // 128, device=dev))
+    osb.gemm_fp8_blocks(h8, hs, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x, gate=mod.gate, group_rows=n,
+                        out=x)
+
+
 class _ProcessorBase:
     """What both processors share.  A processor holds NO model weights and touches only attributes the reference's own
     block classes have (`opensora/models/mmdit/layers.py:138-176,256-306,337-388`), so it can be installed with
@@ -344,8 +407,12 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
                       epilogue=osb.EPI_BIAS_GATE_RES, residual=txt2[b * Lt:(b + 1) * Lt], gate=tm1.gate[b:b + 1],
                       out=txt_o[b * Lt:(b + 1) * Lt])
         # x + gate * MLP((1 + scale) * LN(x) + shift)   (layers.py:248, 252)
-        for x_o, mod, mlp, n in ((img_o, im2, attn.img_mlp, Li), (txt_o, tm2, attn.txt_mlp, Lt)):
+        fp8 = getattr(vec, "_osb_fp8", None)
+        for x_o, mod, mlp, n, kind in ((img_o, im2, attn.img_mlp, Li, "img"), (txt_o, tm2, attn.txt_mlp, Lt, "txt")):
             if n == 0:
+                continue
+            if fp8 is not None:
+                _mlp_fp8(osb, fp8, attn, kind, x_o, mod, n)
                 continue
             xm = osb.ln_modulate(x_o, mod.shift, mod.scale, group_rows=n)
             hid = _gemm(osb, xm, *linear_parts(mlp[0]), epilogue=osb.EPI_BIAS_GELU_TANH)
@@ -426,12 +493,34 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         cos, sin, half = _rope(pe)
         kw = dict(q_norm_w=attn.norm.query_norm.scale, k_norm_w=attn.norm.key_norm.scale, rope_cos=cos, rope_sin=sin,
                   rope_half=half)
+        fp8 = getattr(vec, "_osb_fp8", None)
+        if fp8 is not None:
+            return self._fp8_tail(osb, fp8, attn, x2, qkv, mod, B, L, C, H, D, kw).view(B, L, C)
         # [attn | gelu(mlp)] side by side: the attention output and the GELU GEMM write one [rows, C + 4C] buffer
         cat = _sp_attention(osb, qkv, C + M4, B, L, H, D, kw, 0, x.dtype, x.device)
         _gemm(osb, xm, wm, bm, lm, u, epilogue=osb.EPI_BIAS_GELU_TANH, out=cat[:, C:])
         out = _gemm(osb, cat, *linear_parts(attn.linear2), epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
                     group_rows=L)
         return out.view(B, L, C)
+
+    @staticmethod
+    def _fp8_tail(osb, fp8: Fp8State, attn: nn.Module, x2: Tensor, qkv: Tensor, mod, B: int, L: int, C: int, H: int,
+                  D: int, kw: dict) -> Tensor:
+        """x + gate * linear2(cat(attn, gelu(mlp))) with the cat buffer in e4m3: the attention output is block-quantized
+        into columns 0..C-1, the mlp part of linear1 (on its own FP8 LN+modulate) emits its GELU codes into columns C..,
+        and linear2 is one block-scaled FP8 GEMM."""
+        wm, sm, bm, w2, s2, b2 = fp8.weights(osb, attn, "single")
+        rows, M4, dev, f8 = B * L, wm.shape[0], x2.device, torch.float8_e4m3fn
+        cat8 = fp8.buf("cat8", rows, C + M4, dtype=f8, device=dev)
+        cats = fp8.buf("cats", rows, (C + M4) // 128, device=dev)
+        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, 0, x2.dtype, dev)
+        osb.quant_blocks_fp8(ao, out=cat8[:, :C], out_scale=cats[:, :C // 128])
+        x8, xs = osb.ln_modulate_fp8(x2, mod.shift, mod.scale, group_rows=L,
+                                     out=fp8.buf("x8", rows, C, dtype=f8, device=dev), out_scale=fp8.buf("xs", rows, device=dev))
+        osb.gemm_fp8_blocks(x8, xs, wm, sm, bm, epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=cat8[:, C:],
+                            out_scale=cats[:, C // 128:])
+        return osb.gemm_fp8_blocks(cat8, cats, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
+                                   group_rows=L)
 
 
 class SingleStreamBlock(nn.Module):

@@ -12,8 +12,8 @@ from opensora.registry import MODELS
 
 from opensora.utils.lora import adapter_of, dora_magnitude, lora_pack
 
-from .layers import (DoubleStreamBlock, EmbedND, LastLayer, LigerEmbedND, MLPEmbedder, SingleStreamBlock, _gemm,
-                     linear_parts, timestep_embedding)
+from .layers import (DoubleStreamBlock, EmbedND, Fp8State, LastLayer, LigerEmbedND, MLPEmbedder, SingleStreamBlock,
+                     _gemm, linear_parts, timestep_embedding)
 
 
 @dataclass
@@ -84,10 +84,13 @@ class MMDiTModel(nn.Module):
         self._mod_lora = None
         self._pe_cache = None
         self._sp_group = None
+        self._fp8 = False
+        self._fp8_state = None
         self.register_load_state_dict_post_hook(lambda m, k: m._drop_caches())
 
     def _drop_caches(self):
         self._cond_w = self._mod_pack = self._mod_lora = self._pe_cache = None
+        self._fp8_state = None   # quantized again from the current parameters at the next forward
 
     def _apply(self, fn, *a, **k):
         self._drop_caches()
@@ -188,6 +191,48 @@ class MMDiTModel(nn.Module):
         pe = self._pe(txt_ids, img_ids)
         return img, txt, vec, pe
 
+    # ---- FP8 (e4m3) MLPs -------------------------------------------------------------------------------------------
+    def _mlps(self):
+        """(block, kind) of every MLP: "img" / "txt" of the double blocks, "single" of the single blocks."""
+        return [(b, k) for b in self.double_blocks for k in ("img", "txt")] + [(b, "single") for b in self.single_blocks]
+
+    def fp8_mlp_linears(self) -> list[str]:
+        """Names of the Linears the FP8 path replaces: fc1 / fc2 of the double-block MLPs, and linear1 (or v_mlp) and
+        linear2 of the single blocks, which hold their MLP's weights."""
+        names = {id(m): n for n, m in self.named_modules()}
+        return [names[id(lin)] for blk, kind in self._mlps() for lin in Fp8State.mlp_linears(blk, kind)[::2]]
+
+    def enable_fp8(self) -> None:
+        """Run the MLPs of every double and single block on FP8 (e4m3) tensor cores.  The weights are quantized per output
+        channel (s = amax / 448) into a per-model cache; the bf16 parameters and the state dict stay as they are.  The fc1
+        input is the fp32 LN+modulate row, quantized per row; the fc2 / linear2 input is quantized per 1 x 128 block by
+        the fc1 GELU epilogue (and, for the attention half of linear2's input, by osb_quant_blocks_fp8)
+        (include/osb200.h, osb_gemm_fp8_blocks).  Needs a hidden size and an MLP width that are multiples of 128 and a
+        hidden size of at most 4096 (the FP8 LN+modulate); LoRA / DoRA adapters on the MLP Linears are refused."""
+        C, hid = self.hidden_size, int(self.hidden_size * self.config.mlp_ratio)
+        if C % 128 or hid % 128:
+            raise ValueError(f"FP8 MLPs need the hidden size ({C}) and the MLP width ({hid}) to be multiples of 128 "
+                             "(one e4m3 k-block / scale block of osb_gemm_fp8_blocks)")
+        if C > 4096:
+            raise ValueError(f"FP8 MLPs need a hidden size <= 4096 (the FP8 LN+modulate holds one row), got {C}")
+        mods = dict(self.named_modules())
+        adapted = [n for n in self.fp8_mlp_linears() if adapter_of(mods[n]) is not None]
+        if adapted:
+            raise ValueError(f"FP8 MLPs cannot run LoRA / DoRA adapters on MLP Linears ({adapted[0]} has one): "
+                             "unload_lora first")
+        state = Fp8State()
+        w = self.img_in.weight
+        if w.is_cuda:   # quantized now; a model not yet on the GPU quantizes at its first forward
+            import osb200
+
+            for blk, kind in self._mlps():
+                state.weights(osb200, blk, kind)
+        self._fp8_state, self._fp8 = state, True
+
+    def disable_fp8(self) -> None:
+        """Back to the bf16 MLPs; the FP8 weight copies and workspaces are released."""
+        self._fp8, self._fp8_state = False, None
+
     def enable_sequence_parallel(self, group) -> None:
         """Ulysses sequence parallelism over `group` (the reference's `all_to_all` mode, opensora/models/mmdit/
         distributed.py:473-495,598-634,671-679): the joint txt|img sequence is split into P equal chunks (a rank holds the tail
@@ -221,6 +266,10 @@ class MMDiTModel(nn.Module):
 
         img, txt, vec, pe = self.prepare_block_inputs(img, img_ids, txt, txt_ids, timesteps, y_vec, cond, guidance)
         self._grouped_modulation(vec)
+        if self._fp8:
+            if self._fp8_state is None:
+                self._fp8_state = Fp8State()
+            vec._osb_fp8 = self._fp8_state
         Lt, Li = txt.shape[1], img.shape[1]
         sp = self._sp_splits(Lt, Li)
         vec._osb_txt_len = Lt   # joint positions >= Lt take the image stream's QK-norm weights on every rank

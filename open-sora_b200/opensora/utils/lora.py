@@ -336,6 +336,11 @@ def load_lora(model: nn.Module, path: str, scale: float = 1.0) -> nn.Module:
             used.add(km)
             mag = weights[km]
         plan.append((name, lin, r, s, weights[ka], weights[kb], mag))
+    if getattr(model, "_fp8", False):
+        on_mlp = sorted({p[0] for p in plan} & set(model.fp8_mlp_linears()))
+        if on_mlp:
+            raise ValueError(f"the model runs FP8 MLPs, which take no LoRA / DoRA adapter on an MLP Linear "
+                             f"(target '{on_mlp[0]}'): disable_fp8 first")
     extra = sorted(set(weights) - used)
     if extra:
         raise ValueError(f"adapter weights hold {len(extra)} tensors no target uses, e.g. {extra[:3]}")

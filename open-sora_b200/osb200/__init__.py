@@ -39,10 +39,13 @@ EXPORTS = (
     "osb_gemm_fp8",
     "osb_ln_modulate_fp8",
     "osb_quant_rows_fp8",
+    "osb_gemm_fp8_blocks",
+    "osb_quant_blocks_fp8",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
 EPI_GATED_GELU, EPI_BIAS_QUICK_GELU = 3, 4
+EPI_BIAS_GELU_TANH_FP8 = 5   # gemm_fp8_blocks only: GELU-tanh emitted as e4m3 codes with 1 x 128 block scales
 
 
 class OsbError(RuntimeError):
@@ -75,6 +78,9 @@ def _load() -> C.CDLL:
     ]
     lib.osb_quant_rows_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int,
                                        C.c_void_p]
+    lib.osb_gemm_fp8_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.osb_quant_blocks_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64,
+                                         C.c_int, C.c_int, C.c_void_p]
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_attn_short_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     lib.osb_rms_norm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_void_p]
@@ -172,6 +178,11 @@ class GemmFp8Args(C.Structure):
         ("group_rows", C.c_int64), ("gate_stride", C.c_int64),
         ("epilogue", C.c_int32), ("block_n", C.c_int32),
     ]
+
+
+class Fp8BlocksArgs(C.Structure):
+    _fields_ = [("a_scale_ld", C.c_int64), ("D8", C.c_void_p), ("d_scale", C.c_void_p), ("ldd8", C.c_int64),
+                ("ld_dscale", C.c_int64)]
 
 
 class AttnShortArgs(C.Structure):
@@ -498,6 +509,103 @@ def quant_rows_fp8(x, *, out=None, out_scale=None):
     with _Timed("quant_rows_fp8", 3.0 * rows * K):  # algorithmic bytes: read bf16 + write e4m3
         _check(_lib.osb_quant_rows_fp8(_ptr(x), x.stride(0), _ptr(out), out.stride(0), _ptr(out_scale), rows, K,
                                        _stream()), "osb_quant_rows_fp8")
+    return out, out_scale
+
+
+# ---- FP8 (e4m3) with 1 x 128 block scales (include/osb200.h): the block (r, b) = X[r, 128 b : 128 b + 128] gets
+# s[r, b] = amax(|block|) / 448 (1 for a zero block), codes e4m3_rn_satfinite(X / s).  Scale tensors may be column views
+# of wider buffers (row stride free, unit column stride). ---------------------------------------------------------------
+def _scale_view(t, rows: int, cols: int, name: str):
+    import torch
+
+    _need(t, torch.float32, name)
+    if t is None or t.dim() != 2 or t.shape != (rows, cols):
+        raise OsbError(f"{name} must be a float32 [{rows}, {cols}] tensor (row stride free), got "
+                       f"{None if t is None else tuple(t.shape)}")
+    return t.stride(0)
+
+
+def gemm_fp8_blocks(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None,
+                    group_rows: int = 0, mod_index=None, out=None, out_scale=None, block_n: int = 0):
+    """`gemm_fp8` with block-scaled A (osb_gemm_fp8_blocks).  a_scale: fp32 [M] (per row: with a bf16 epilogue this is
+    exactly `gemm_fp8`) or [M, K / 128] (block mode, row stride free): out = epilogue(w_scale[n] * sum_kb a_scale[m, kb]
+    * acc_kb + bias).  EPI_BIAS, EPI_BIAS_GELU_TANH and EPI_BIAS_GATE_RES write bf16 `out` as in `gemm`.
+    EPI_BIAS_GELU_TANH_FP8 writes e4m3 `out` [M, N] and fp32 `out_scale` [M, N / 128] (both row stride free, e.g. column
+    slices of a wider buffer) and returns (out, out_scale); N % 128 == 0."""
+    import torch
+
+    _need(a8, torch.float8_e4m3fn, "a8"); _need(w8, torch.float8_e4m3fn, "w8"); _need(w_scale, torch.float32, "w_scale")
+    _need(bias, torch.bfloat16, "bias"); _need(residual, torch.bfloat16, "residual"); _need(gate, torch.float32, "gate")
+    _need(mod_index, torch.int32, "mod_index")
+    if a8.dim() != 2 or w8.dim() != 2 or a8.shape[1] != w8.shape[1]:
+        raise OsbError(f"gemm_fp8_blocks: a8 [M, K] and w8 [N, K] expected, got {tuple(a8.shape)} and {tuple(w8.shape)}")
+    M, K = a8.shape
+    N = w8.shape[0]
+    if w_scale is None or w_scale.shape != (N,):
+        raise OsbError(f"gemm_fp8_blocks: w_scale must be [{N}]")
+    b = Fp8BlocksArgs()
+    if a_scale is not None and a_scale.dim() == 1:
+        _need(a_scale, torch.float32, "a_scale")
+        if a_scale.shape != (M,):
+            raise OsbError(f"gemm_fp8_blocks: a per-row a_scale must be [{M}], got {tuple(a_scale.shape)}")
+    else:
+        b.a_scale_ld = _scale_view(a_scale, M, K // 128, "a_scale")
+    fp8_out = epilogue == EPI_BIAS_GELU_TANH_FP8
+    if fp8_out:
+        if out is None:
+            out = torch.empty((M, N), dtype=torch.float8_e4m3fn, device=a8.device)
+        if out_scale is None:
+            out_scale = torch.empty((M, N // 128), dtype=torch.float32, device=a8.device)
+        _need(out, torch.float8_e4m3fn, "out")
+        if out.shape != (M, N):
+            raise OsbError(f"gemm_fp8_blocks: out must be e4m3 [{M}, {N}], got {tuple(out.shape)}")
+        b.D8, b.ldd8 = out.data_ptr(), out.stride(0)
+        b.d_scale, b.ld_dscale = out_scale.data_ptr(), _scale_view(out_scale, M, N // 128, "out_scale")
+    else:
+        if out is None:
+            out = torch.empty((M, N), dtype=torch.bfloat16, device=a8.device)
+        _need(out, torch.bfloat16, "out")
+    g = GemmFp8Args()
+    g.A, g.W, g.a_scale, g.w_scale = a8.data_ptr(), w8.data_ptr(), a_scale.data_ptr(), w_scale.data_ptr()
+    g.bias = bias.data_ptr() if bias is not None else None
+    g.D = None if fp8_out else out.data_ptr()
+    g.R = residual.data_ptr() if residual is not None else None
+    g.gate = gate.data_ptr() if gate is not None else None
+    g.mod_index = mod_index.data_ptr() if mod_index is not None else None
+    g.M, g.N, g.K = M, N, K
+    g.lda, g.ldw, g.ldd = a8.stride(0), w8.stride(0), 0 if fp8_out else out.stride(0)
+    g.ldr = residual.stride(0) if residual is not None else 0
+    g.group_rows = group_rows if group_rows > 0 else M
+    g.gate_stride = gate.stride(0) if gate is not None else 0
+    g.epilogue, g.block_n = epilogue, block_n
+    with _Timed("gemm_fp8", 2.0 * M * N * K):
+        _check(_lib.osb_gemm_fp8_blocks(C.byref(g), C.byref(b), _stream()), "osb_gemm_fp8_blocks")
+    return (out, out_scale) if fp8_out else out
+
+
+def quant_blocks_fp8(x, *, block: int = 128, out=None, out_scale=None):
+    """e4m3 quantization of bf16 x [rows, K] (row stride free) with one scale per (row, `block` columns)
+    (osb_quant_blocks_fp8): block 128 (one pass) or K (per row, any K; the MLP weights).  Returns (e4m3 [rows, K],
+    fp32 [rows, K / block]); `out` / `out_scale` may be column views of wider buffers."""
+    import torch
+
+    _need(x, torch.bfloat16, "x")
+    if x.dim() != 2:
+        raise OsbError(f"quant_blocks_fp8: x must be [rows, K], got {tuple(x.shape)}")
+    rows, K = x.shape
+    if block <= 0 or K % block:
+        raise OsbError(f"quant_blocks_fp8: block {block} does not divide K = {K}")
+    if out is None:
+        out = torch.empty((rows, K), dtype=torch.float8_e4m3fn, device=x.device)
+    if out_scale is None:
+        out_scale = torch.empty((rows, K // block), dtype=torch.float32, device=x.device)
+    _need(out, torch.float8_e4m3fn, "out")
+    if out.shape != (rows, K):
+        raise OsbError(f"quant_blocks_fp8: out must be [{rows}, {K}], got {tuple(out.shape)}")
+    lds = _scale_view(out_scale, rows, K // block, "out_scale")
+    with _Timed("quant_blocks_fp8", 3.0 * rows * K):  # algorithmic bytes: read bf16 + write e4m3
+        _check(_lib.osb_quant_blocks_fp8(_ptr(x), x.stride(0), _ptr(out), out.stride(0), _ptr(out_scale), lds, rows, K,
+                                         block, _stream()), "osb_quant_blocks_fp8")
     return out, out_scale
 
 
