@@ -363,15 +363,36 @@ def rms_norm(x, w, *, eps: float = 1e-6, out=None):
     return out
 
 
-def _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, cta_group, block_n):
+def _epilogue_shapes(fn, M, N, out_cols, out, bias, residual, gate, group_rows, mod_index):
+    """Extents of the optional GEMM operands.  The kernels address out, bias, residual, gate and mod_index by (row,
+    column) with only a row stride, so a tensor smaller than the problem would be read or written out of bounds: refuse
+    it here.  mod_index's values live on the device and are not checked."""
+    if out is not None and tuple(out.shape) != (M, out_cols):
+        raise OsbError(f"{fn}: out must be [{M}, {out_cols}], got {tuple(out.shape)}")
+    if bias is not None and tuple(bias.shape) != (N,):
+        raise OsbError(f"{fn}: bias must be [{N}], got {tuple(bias.shape)}")
+    if residual is not None and tuple(residual.shape) != (M, N):
+        raise OsbError(f"{fn}: residual must be [{M}, {N}], got {tuple(residual.shape)}")
+    groups = -(-M // (group_rows if group_rows > 0 else M))
+    if gate is not None and (gate.dim() != 2 or gate.shape[1] != N or (mod_index is None and gate.shape[0] < groups)):
+        raise OsbError(f"{fn}: gate must be [G, {N}] with G >= {groups} row groups (or indexed by mod_index), got "
+                       f"{tuple(gate.shape)}")
+    if mod_index is not None and (mod_index.dim() != 1 or mod_index.shape[0] < groups):
+        raise OsbError(f"{fn}: mod_index must be 1-D with at least {groups} entries, got {tuple(mod_index.shape)}")
+
+
+def _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, cta_group, block_n, fn="gemm"):
     import torch
 
     _need(a, torch.bfloat16, "a"); _need(w, torch.bfloat16, "w"); _need(bias, torch.bfloat16, "bias")
     _need(residual, torch.bfloat16, "residual"); _need(gate, torch.float32, "gate")
     _need(mod_index, torch.int32, "mod_index")
-    assert a.dim() == 2 and w.dim() == 2 and a.shape[1] == w.shape[1]
+    if a.dim() != 2 or w.dim() != 2 or a.shape[1] != w.shape[1]:
+        raise OsbError(f"{fn}: a [M, K] and w [N, K] expected, got {tuple(a.shape)} and {tuple(w.shape)}")
     M, K = a.shape
     N = w.shape[0]
+    _epilogue_shapes(fn, M, N, N // 2 if epilogue == EPI_GATED_GELU else N, out, bias, residual, gate, group_rows,
+                     mod_index)
     if out is None:   # the gated GELU writes one column per (wi_0, wi_1) row pair of w
         out = torch.empty((M, N // 2 if epilogue == EPI_GATED_GELU else N), dtype=torch.bfloat16, device=a.device)
     _need(out, torch.bfloat16, "out")
@@ -418,7 +439,7 @@ def gemm_lora(a, w, bias, u, b, *, epilogue: int = EPI_BIAS, residual=None, gate
                 or col_scale.device != a.device:
             raise OsbError(f"gemm_lora: col_scale must be a contiguous float32 [{w.shape[0]}] tensor on {a.device}, got "
                            f"{col_scale.dtype} {tuple(col_scale.shape)} on {col_scale.device}")
-    args, out = _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, 0, block_n)
+    args, out = _gemm_args(a, w, bias, epilogue, residual, gate, group_rows, mod_index, out, 0, block_n, "gemm_lora")
     la = LoraArgs()
     la.U, la.B, la.ldu, la.ldb, la.r = u.data_ptr(), b.data_ptr(), u.stride(0), b.stride(0), u.shape[1]
     la.col_scale = None if col_scale is None else col_scale.data_ptr()
@@ -446,6 +467,7 @@ def gemm_fp8(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_BIAS, r
     N = w8.shape[0]
     if a_scale is None or w_scale is None or a_scale.shape != (M,) or w_scale.shape != (N,):
         raise OsbError(f"gemm_fp8: a_scale must be [{M}] and w_scale [{N}]")
+    _epilogue_shapes("gemm_fp8", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if out is None:
         out = torch.empty((M, N), dtype=torch.bfloat16, device=a8.device)
     _need(out, torch.bfloat16, "out")
@@ -551,6 +573,7 @@ def gemm_fp8_blocks(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_
     else:
         b.a_scale_ld = _scale_view(a_scale, M, K // 128, "a_scale")
     fp8_out = epilogue == EPI_BIAS_GELU_TANH_FP8
+    _epilogue_shapes("gemm_fp8_blocks", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if fp8_out:
         if out is None:
             out = torch.empty((M, N), dtype=torch.float8_e4m3fn, device=a8.device)

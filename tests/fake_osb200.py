@@ -68,6 +68,21 @@ def _need(t, dtype, name):
         raise OsbError(f"{name} must have unit stride in the last dimension")
 
 
+def _epilogue_shapes(fn, M, N, out_cols, out, bias, residual, gate, group_rows, mod_index):
+    """The binding's extent checks of the optional GEMM operands (osb200._epilogue_shapes), raised before any math."""
+    if out is not None and tuple(out.shape) != (M, out_cols):
+        raise OsbError(f"{fn}: out must be [{M}, {out_cols}], got {tuple(out.shape)}")
+    if bias is not None and tuple(bias.shape) != (N,):
+        raise OsbError(f"{fn}: bias must be [{N}], got {tuple(bias.shape)}")
+    if residual is not None and tuple(residual.shape) != (M, N):
+        raise OsbError(f"{fn}: residual must be [{M}, {N}], got {tuple(residual.shape)}")
+    groups = -(-M // (group_rows if group_rows > 0 else M))
+    if gate is not None and (gate.dim() != 2 or gate.shape[1] != N or (mod_index is None and gate.shape[0] < groups)):
+        raise OsbError(f"{fn}: gate must be [G, {N}] with G >= {groups} row groups, got {tuple(gate.shape)}")
+    if mod_index is not None and (mod_index.dim() != 1 or mod_index.shape[0] < groups):
+        raise OsbError(f"{fn}: mod_index must be 1-D with at least {groups} entries, got {tuple(mod_index.shape)}")
+
+
 def _groups(rows, group_rows, mod_index, device):
     g = torch.arange(rows, device=device) // max(int(group_rows), 1)
     if mod_index is not None:
@@ -124,9 +139,11 @@ def gemm(a, w, bias=None, *, epilogue: int = EPI_BIAS, residual=None, gate=None,
     for t, n in ((a, "a"), (w, "w"), (bias, "bias"), (residual, "residual"), (out, "out")):
         _need(t, torch.bfloat16, n)
     _need(gate, torch.float32, "gate"); _need(mod_index, torch.int32, "mod_index")
-    assert a.dim() == 2 and w.dim() == 2 and a.shape[1] == w.shape[1]
+    if a.dim() != 2 or w.dim() != 2 or a.shape[1] != w.shape[1]:
+        raise OsbError(f"gemm: a [M, K] and w [N, K] expected, got {tuple(a.shape)} and {tuple(w.shape)}")
     M, K = a.shape
     N = w.shape[0]
+    _epilogue_shapes("gemm", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if K % 8 or N % 8:
         raise OsbError(f"osb_gemm_bf16 failed (-1): osb_gemm_bf16: K and N must be multiples of 8 (K {K} N {N})")
     acc = a.to(ACC_DTYPE) @ w.to(ACC_DTYPE).t()

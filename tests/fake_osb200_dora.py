@@ -39,8 +39,11 @@ def gemm_lora(a, w, bias, u, b, *, epilogue=base.EPI_BIAS, residual=None, gate=N
     for t, n in ((a, "a"), (w, "w"), (bias, "bias"), (u, "u"), (b, "b"), (residual, "residual"), (out, "out")):
         base._need(t, torch.bfloat16, n)
     base._need(gate, torch.float32, "gate"); base._need(mod_index, torch.int32, "mod_index")
+    if a.dim() != 2 or w.dim() != 2 or a.shape[1] != w.shape[1]:
+        raise base.OsbError(f"gemm_lora: a [M, K] and w [N, K] expected, got {tuple(a.shape)} and {tuple(w.shape)}")
     M, K = a.shape
     N = w.shape[0]
+    base._epilogue_shapes("gemm_lora", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if K % 8 or N % 8:
         raise base.OsbError(f"osb_gemm_lora failed (-1): K and N must be multiples of 8 (K {K} N {N})")
     if u.shape[0] != M or b.shape[0] != N or u.shape[1] != b.shape[1] or u.shape[1] % 8:

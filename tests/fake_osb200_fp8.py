@@ -80,6 +80,7 @@ def gemm_fp8(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = base.EPI_BI
     N = w8.shape[0]
     if a_scale is None or w_scale is None or a_scale.shape != (M,) or w_scale.shape != (N,):
         raise OsbError(f"gemm_fp8: a_scale must be [{M}] and w_scale [{N}]")
+    base._epilogue_shapes("gemm_fp8", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if K % 128:
         raise OsbError(f"osb_gemm_fp8 failed (-1): osb_gemm_fp8: K must be a multiple of 128 (one e4m3 k-block), got {K}")
     if N % 8:

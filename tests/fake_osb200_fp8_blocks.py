@@ -68,7 +68,10 @@ def gemm_fp8_blocks(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = base
     KB = K // 128
     if a_scale is None or w_scale is None or w_scale.shape != (N,) or a_scale.shape not in ((M,), (M, KB)):
         raise OsbError(f"gemm_fp8_blocks: a_scale must be [{M}] or [{M}, {KB}] and w_scale [{N}]")
+    base._epilogue_shapes("gemm_fp8_blocks", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     fp8_out = epilogue == EPI_BIAS_GELU_TANH_FP8
+    if fp8_out and out_scale is not None and tuple(out_scale.shape) != (M, N // 128):
+        raise OsbError(f"out_scale must be a float32 [{M}, {N // 128}] tensor (row stride free)")
     if block_n not in ((0, 128) if fp8_out else (0, 64, 128)):
         raise OsbError(f"osb_gemm_fp8_blocks failed (-3): unsupported block_n {block_n}")
     if not (fp8_out or base.EPI_BIAS <= epilogue <= base.EPI_BIAS_GATE_RES):

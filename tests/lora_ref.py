@@ -34,8 +34,12 @@ def gemm_lora(a, w, bias, u, b, *, epilogue=EPI_BIAS, residual=None, gate=None, 
 
     for t, n in ((a, "a"), (w, "w"), (bias, "bias"), (u, "u"), (b, "b"), (residual, "residual"), (out, "out")):
         F_._need(t, torch.bfloat16, n)
+    F_._need(gate, torch.float32, "gate"); F_._need(mod_index, torch.int32, "mod_index")
+    if a.dim() != 2 or w.dim() != 2 or a.shape[1] != w.shape[1]:
+        raise F_.OsbError(f"gemm_lora: a [M, K] and w [N, K] expected, got {tuple(a.shape)} and {tuple(w.shape)}")
     M, K = a.shape
     N = w.shape[0]
+    F_._epilogue_shapes("gemm_lora", M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if K % 8 or N % 8:
         raise F_.OsbError(f"osb_gemm_lora failed (-1): K and N must be multiples of 8 (K {K} N {N})")
     if u.shape[0] != M or b.shape[0] != N or u.shape[1] != b.shape[1] or u.shape[1] % 8:

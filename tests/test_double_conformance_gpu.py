@@ -877,6 +877,55 @@ def _refusals():
                                                                            osb_ht(m, d, 64, m.tile_map(0, 16), 3, 2, 64),
                                                                            b(64, 128).to(d), Lk=16, num_seqs=4,
                                                                            kv_lens=torch.full((4,), 16, dtype=torch.int32).to(d))),
+    ] + _shape_refusals()
+
+
+def _shape_refusals():
+    """Wrong-shaped optional GEMM operands (out, bias, residual, gate, mod_index) and a K mismatch.  Each wrong-shaped
+    tensor is a view into an allocation large enough for what a launch would touch, so a missing check shows as "did
+    not raise", never as an out-of-bounds access."""
+    from tests import fake_osb200_dora, fake_osb200_fp8, fake_osb200_fp8_blocks
+
+    b = lambda *s: torch.zeros(*s, dtype=torch.bfloat16)  # noqa: E731
+    f = lambda *s: torch.zeros(*s, dtype=torch.float32)  # noqa: E731
+    e = lambda *s: torch.zeros(*s, dtype=torch.float8_e4m3fn)  # noqa: E731
+    gr = dict(epilogue=F_.EPI_BIAS_GATE_RES, group_rows=8)
+    lora = lambda m: fake_gemm_lora if m is F_ else m.gemm_lora  # noqa: E731
+    dora = lambda m: fake_osb200_dora.gemm_lora if m is F_ else m.gemm_lora  # noqa: E731
+    fp8 = lambda m: fake_osb200_fp8.gemm_fp8 if m is F_ else m.gemm_fp8  # noqa: E731
+    blk = lambda m: fake_osb200_fp8_blocks.gemm_fp8_blocks if m is F_ else m.gemm_fp8_blocks  # noqa: E731
+    lo = lambda d: (b(16, 8).to(d), b(16, 8).to(d))  # noqa: E731   u [M, r], b [N, r]
+    s8 = lambda d: (f(16).to(d) + 1, f(16).to(d) + 1)  # noqa: E731   a_scale [M], w_scale [N]
+    return [
+        ("gemm out [M, N-8]", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), out=b(16, 16).to(d)[:, :8])),
+        ("gemm bias [N-8]", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), b(16).to(d)[:8])),
+        ("gemm residual [M-1, N]", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), residual=b(16, 16).to(d)[:15],
+                                                       epilogue=F_.EPI_BIAS_GATE_RES)),
+        ("gemm gate [G, N-8]", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), gate=f(2, 16).to(d)[:, :8], **gr)),
+        ("gemm gate rows < groups", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), gate=f(2, 16).to(d)[:1], **gr)),
+        ("gemm mod_index short", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), gate=f(2, 16).to(d),
+                                                     mod_index=torch.zeros(2, dtype=torch.int32).to(d)[:1], **gr)),
+        ("gemm K mismatch", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 24).to(d))),
+        ("gemm_lora out [M-1, N]", lambda m, d: lora(m)(b(16, 16).to(d), b(16, 16).to(d), None, *lo(d),
+                                                        out=b(16, 16).to(d)[:15])),
+        ("gemm_lora gate [G, N-8]", lambda m, d: lora(m)(b(16, 16).to(d), b(16, 16).to(d), None, *lo(d),
+                                                         gate=f(2, 16).to(d)[:, :8], **gr)),
+        ("gemm_lora col_scale bias [N-8]", lambda m, d: dora(m)(b(16, 16).to(d), b(16, 16).to(d), b(16).to(d)[:8], *lo(d),
+                                                                col_scale=f(16).to(d) + 1)),
+        ("gemm_fp8 out [M, N-8]", lambda m, d: fp8(m)(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
+                                                      out=b(16, 16).to(d)[:, :8])),
+        ("gemm_fp8 residual [M, N-8]", lambda m, d: fp8(m)(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
+                                                           residual=b(16, 16).to(d)[:, :8], epilogue=F_.EPI_BIAS_GATE_RES)),
+        ("gemm_fp8 gate rows < groups", lambda m, d: fp8(m)(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
+                                                            gate=f(2, 16).to(d)[:1], **gr)),
+        ("gemm_fp8_blocks out [M-1, N]", lambda m, d: blk(m)(e(16, 128).to(d), f(16, 1).to(d) + 1, e(16, 128).to(d),
+                                                             s8(d)[1], out=b(16, 16).to(d)[:15])),
+        ("gemm_fp8_blocks FP8 GELU bias [N-8]", lambda m, d: blk(m)(e(16, 128).to(d), f(16, 1).to(d) + 1, e(128, 128).to(d),
+                                                                    f(128).to(d) + 1, b(128).to(d)[:120],
+                                                                    epilogue=fake_osb200_fp8_blocks.EPI_BIAS_GELU_TANH_FP8)),
+        ("gemm_fp8_blocks mod_index short", lambda m, d: blk(m)(e(16, 128).to(d), f(16, 1).to(d) + 1, e(16, 128).to(d),
+                                                                s8(d)[1], gate=f(2, 16).to(d),
+                                                                mod_index=torch.zeros(2, dtype=torch.int32).to(d)[:1], **gr)),
     ]
 
 
