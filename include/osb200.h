@@ -191,6 +191,47 @@ int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* gemm, const osb_fp8_blocks_args
 int osb_quant_blocks_fp8(const void* x, int64_t ldx, void* y8, int64_t ldy, float* y_scale, int64_t lds, int64_t rows,
                          int K, int block, void* stream);
 
+/* ---- FP8 (e4m3) attention: the opt-in attention path of MMDiT -------------------------------------------------------- */
+/* Self-attention of the joint txt|img sequence of MMDiT on e4m3 operands.  Inputs are described by osb_attn_short_args
+ * with head_dim == 128, Lq == Lk == L (any L >= 1), seqs_per_batch == 1, kv_lens == NULL, any number of heads.  Per
+ * sequence b, head h (bh = b * num_heads + h) and token t:
+ *   q, k:  q~ = the bf16 row osb_attn_short stages (RMSNorm with the weight of the token's stream, RoPE, one rounding);
+ *          s_q[bh, t] = amax(|q~|) / 448 (1 for a zero row), codes e4m3_rn_satfinite(q~ / s_q): the per-row rule of the
+ *          FP8 GEMMs applied per (token, head).  k likewise.
+ *   v:     one scale per channel over the sequence: s_v[bh, c] = amax_t(|v[t, c]|) / 448 (1 for a zero column), codes
+ *          e4m3_rn_satfinite(v / s_v).
+ *   scores (log2 units, fp32):  S_ij = s_q[i] * s_k[j] * (sum_d q8[i, d] k8[j, d]) * softmax_scale * log2(e).
+ *   softmax: online over key blocks of 128, p = exp2(S - m_running) in fp32, l = fp32 sum of p.
+ *   PV:    P8 = e4m3_rn_satfinite(256 * p) (2^8: p down to ~2^-17 keeps a nonzero code, nothing saturates); each key
+ *          block's P8 V8 is summed by the tensor core into a partial that is promoted into the fp32 accumulator as
+ *          O = alpha * O + partial (the FP8 MMA accumulates with fewer mantissa bits than fp32).
+ *   out[row of (b, i), h * 128 + c] = bf16(O_ic * s_v[c] / (256 * l_i)), rows and columns as osb_attn_short writes them.
+ *
+ * Workspace (caller-owned, device memory; Lpad = L rounded up to a multiple of 128, the key block):
+ *   q8, k8   e4m3 [B*H, Lpad, 128], rows t >= L hold zero codes with scale 1
+ *   vt8      e4m3 [B*H, 128, Lpad]: V transposed (keys contiguous: FP8 wgmma reads B K-major only), and within every group
+ *            of 32 keys g*32 + j the key at position p is j(p) = 16*(p/16) + 2*((p%16)/4) + (p%2) + 8*((p%4)/2), so that
+ *            the S accumulator registers of a thread are the register A fragment of the PV product as they are; pad keys
+ *            hold zero codes
+ *   s_q, s_k fp32 [B*H, Lpad]
+ *   s_v      fp32 [B*H, 128]
+ *   v_amax   fp32 [B*H, 128] scratch: must be all zero before the first call (each call leaves it zero again, on the
+ *            stream, so the path has no host synchronisation and is graph-capturable)
+ * All pointers 16-byte aligned; capacity_bh >= B*H and capacity_lpad >= Lpad describe the buffers' extents, and the
+ * strides above are those of the CALL's Lpad (the buffers are viewed densely for each call). */
+typedef struct osb_attn_fp8_workspace {
+  void* q8; void* k8; void* vt8;
+  float* s_q; float* s_k; float* s_v;
+  float* v_amax;
+  int64_t capacity_bh, capacity_lpad;
+} osb_attn_fp8_workspace;
+
+/* Three launches: prep (q / k quantized rows with their scales, v's channel amax by atomicMax on the non-negative
+ * float bits), V pack (scales, transposed permuted codes), attention (wgmma e4m3 x e4m3 -> fp32, TMA-fed).  Refuses
+ * head_dim != 128, Lq != Lk, kv_lens, seqs_per_batch != 1, misaligned pointers and a workspace too small. */
+struct osb_attn_short_args;   /* defined with osb_attn_short below */
+int osb_attn_fp8(const struct osb_attn_short_args* args, const osb_attn_fp8_workspace* ws, void* stream);
+
 /* ---- attention with short key sets (whole key set resident in one CTA) -------------------- */
 typedef struct osb_attn_short_args {
   const void* q; const void* k; const void* v; /* bf16; element (row, h*D + d) at ptr + row*ld + h*D + d */

@@ -1,0 +1,437 @@
+// FP8 (e4m3) self-attention of MMDiT's joint txt|img sequence on sm_90a (include/osb200.h, osb_attn_fp8).
+//
+// Three launches, each with PDL:
+//   attn_fp8_prep_kernel   one CTA per (64 tokens, sequence x head).  Each of 128 threads stages one q or k row exactly
+//                          as osb_attn_short does (stage.cuh: RMSNorm with the stream's weight, RoPE, one rounding to
+//                          bf16), then writes its e4m3 codes and per-row scale.  The same CTA reduces v's per-channel
+//                          amax over its 64 tokens and publishes it with atomicMax on the float bits (non-negative floats
+//                          order like their bit patterns, so the result does not depend on the order of the atomics).
+//   attn_fp8_vpack_kernel  one CTA per (128 keys, sequence x head): v / s_v as e4m3, transposed through shared memory
+//                          to [channel][key] with the key permutation of the header inside every 32-key group.
+//   attn_fp8_kernel        one CTA per (128 queries, sequence x head), 3 warpgroups.  Warpgroup 0 (24 registers) has
+//                          one thread that loads Q once and streams K, V^T (TMA, 128-byte swizzle rows = 128 e4m3) and
+//                          the 128 key scales (bulk copy) through a 4-stage mbarrier ring.  Warpgroups 1 and 2 (240
+//                          registers) own 64 query rows each: S = Q K^T by wgmma with both operands in shared memory,
+//                          the online softmax in registers, P8 = e4m3(256 p) packed straight from the S accumulator into
+//                          the register A fragment of the PV wgmma (the vt8 key permutation makes the two layouts
+//                          agree), PV into a partial accumulator that is promoted into the fp32 O as O = alpha O + partial.
+//                          This kernel also zeroes the v amax scratch for the next call, after the V pack read it.
+#include "common.cuh"
+#include "stage.cuh"
+#include "tiles.cuh"
+#include "wgmma.cuh"
+
+namespace osb {
+
+constexpr int kF8D = 128;          // head_dim
+constexpr int kF8KB = 128;         // keys per block, and the granularity of Lpad
+constexpr int kF8Stages = 4;
+constexpr int kF8Threads = 384;    // producer warpgroup + two consumer warpgroups
+constexpr int kF8TileBytes = 128 * 128;
+constexpr int kF8Smem = 1024 + kF8TileBytes + kF8Stages * (2 * kF8TileBytes + 512) + 8 * (1 + 2 * kF8Stages);
+
+struct Fp8AttnPrep {
+  const __nv_bfloat16* q; const __nv_bfloat16* k; const __nv_bfloat16* v;
+  int64_t q_ld, k_ld, v_ld;
+  int64_t q_bs, q_ts, k_bs, k_ts;   // row of token t of sequence b: b * bs + t * ts (k's map also addresses v)
+  int32_t L, Lpad, H;
+  const __nv_bfloat16* qw; const __nv_bfloat16* kw;
+  const __nv_bfloat16* qw2; const __nv_bfloat16* kw2;
+  int32_t norm_split;
+  float eps;
+  const float* cos; const float* sin;
+  int32_t rope_half;
+  uint8_t* q8; uint8_t* k8; uint8_t* vt8;
+  float* s_q; float* s_k; float* s_v; float* v_amax;
+};
+
+struct Fp8AttnMain {
+  const float* s_q; const float* s_k; const float* s_v;
+  float* v_amax;
+  __nv_bfloat16* out;
+  int64_t out_ld, q_bs, q_ts;
+  int32_t L, Lpad, H, nkb;
+  float sc;   // softmax_scale * log2(e)
+};
+
+__global__ void __launch_bounds__(128) attn_fp8_prep_kernel(const Fp8AttnPrep p) {
+  __shared__ float s_amax[4][kF8D];
+  const int tid = threadIdx.x;
+  const int bh = blockIdx.y, b = bh / p.H, h = bh - b * p.H;
+  const int t0 = blockIdx.x * 64;
+  pdl_wait();   // q, k, v were written by the previous kernel
+  {   // ---- one q (threads 0..63) or k (64..127) row: stage, quantize per row ----
+    const int kind = tid >> 6, t = t0 + (tid & 63);
+    const bool ok = t < p.L;
+    const int64_t row = ok ? (int64_t)b * (kind ? p.k_bs : p.q_bs) + (int64_t)t * (kind ? p.k_ts : p.q_ts) : 0;
+    const uint4* src = reinterpret_cast<const uint4*>((kind ? p.k : p.q) + row * (kind ? p.k_ld : p.q_ld) + (int64_t)h * kF8D);
+    uint4 raw[kF8D / 8];
+#pragma unroll
+    for (int u = 0; u < kF8D / 8; ++u) raw[u] = ok ? __ldg(src + u) : make_uint4(0, 0, 0, 0);
+    const __nv_bfloat16* w1 = kind ? p.kw : p.qw;
+    const __nv_bfloat16* w2 = kind ? p.kw2 : p.qw2;
+    const __nv_bfloat16* w = (w2 != nullptr && t >= p.norm_split) ? w2 : w1;
+    const bool rope = ok && p.cos != nullptr;
+    norm_rope_row<kF8D, kF8D / 8>(raw, ok && w1 != nullptr, p.eps, w, rope ? p.cos + (int64_t)t * (kF8D / 2) : nullptr,
+                                  rope ? p.sin + (int64_t)t * (kF8D / 2) : nullptr, p.rope_half != 0);
+    float amax = 0.f;
+#pragma unroll
+    for (int u = 0; u < kF8D / 8; ++u) {
+      float x[8];
+      unpack8(raw[u], x);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) amax = fmaxf(amax, fabsf(x[e]));
+    }
+    const float s = amax > 0.f ? amax / 448.0f : 1.0f;   // rows t >= L: zero codes, scale 1
+    const int64_t r8 = (int64_t)bh * p.Lpad + t;
+    uint4* dst = reinterpret_cast<uint4*>((kind ? p.k8 : p.q8) + r8 * kF8D);
+#pragma unroll
+    for (int u = 0; u < kF8D / 16; ++u) {
+      float x[16];
+      unpack8(raw[2 * u], x);
+      unpack8(raw[2 * u + 1], x + 8);
+      uint4 o;
+      o.x = e4m3x2(x[0] / s, x[1] / s) | (e4m3x2(x[2] / s, x[3] / s) << 16);
+      o.y = e4m3x2(x[4] / s, x[5] / s) | (e4m3x2(x[6] / s, x[7] / s) << 16);
+      o.z = e4m3x2(x[8] / s, x[9] / s) | (e4m3x2(x[10] / s, x[11] / s) << 16);
+      o.w = e4m3x2(x[12] / s, x[13] / s) | (e4m3x2(x[14] / s, x[15] / s) << 16);
+      dst[u] = o;
+    }
+    (kind ? p.s_k : p.s_q)[r8] = s;
+  }
+  {   // ---- v: per-channel amax of the CTA's 64 tokens; thread = (channel unit tid % 16, rows tid / 16 + 8 i) ----
+    const int u = tid & 15, r0 = tid >> 4;
+    float m[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int t = t0 + r0 + 8 * i;
+      if (t < p.L) {
+        float x[8];
+        unpack8(__ldg(reinterpret_cast<const uint4*>(p.v + ((int64_t)b * p.k_bs + (int64_t)t * p.k_ts) * p.v_ld +
+                                                     (int64_t)h * kF8D) + u), x);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) m[e] = fmaxf(m[e], fabsf(x[e]));
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m[e] = fmaxf(m[e], __shfl_xor_sync(0xffffffffu, m[e], 16));   // lane l ^ 16: same u
+    if ((tid & 31) < 16) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) s_amax[tid >> 5][8 * u + e] = m[e];
+    }
+    __syncthreads();
+    const float a = fmaxf(fmaxf(s_amax[0][tid], s_amax[1][tid]), fmaxf(s_amax[2][tid], s_amax[3][tid]));
+    if (a > 0.f) atomicMax(reinterpret_cast<unsigned int*>(p.v_amax) + (int64_t)bh * kF8D + tid, __float_as_uint(a));
+  }
+  pdl_launch_dependents();
+}
+
+// position p (0..31) of a 32-key group of vt8 holds key j(p) = 16 (p/16) + 2 ((p%16)/4) + p%2 + 8 ((p%4)/2): the order in
+// which a thread's S accumulator registers (columns 2 (lane%4) + {0, 1, 8, 9, 16, 17, 24, 25}) fill its FP8 A fragment
+// (k = 4 (lane%4) + {0..3, 16..19})
+__device__ __forceinline__ int vt8_key(int pos) {
+  return (pos & ~31) + 16 * ((pos >> 4) & 1) + 2 * ((pos >> 2) & 3) + (pos & 1) + 8 * ((pos >> 1) & 1);
+}
+
+__global__ void __launch_bounds__(256) attn_fp8_vpack_kernel(const Fp8AttnPrep p) {
+  __shared__ __align__(16) __nv_bfloat16 tile[kF8KB][kF8D];   // [key][channel]
+  const int tid = threadIdx.x;
+  const int bh = blockIdx.y, b = bh / p.H, h = bh - b * p.H;
+  const int key0 = blockIdx.x * kF8KB;
+  pdl_wait();   // the channel amax of the prep kernel
+  for (int i = tid; i < kF8KB * kF8D / 8; i += 256) {
+    const int key = i >> 4, u = i & 15, t = key0 + key;
+    uint4 x = make_uint4(0, 0, 0, 0);
+    if (t < p.L)
+      x = __ldg(reinterpret_cast<const uint4*>(p.v + ((int64_t)b * p.k_bs + (int64_t)t * p.k_ts) * p.v_ld +
+                                               (int64_t)h * kF8D) + u);
+    *reinterpret_cast<uint4*>(&tile[key][8 * u]) = x;
+  }
+  const int c = tid & 127, half = tid >> 7;
+  const float a = p.v_amax[(int64_t)bh * kF8D + c];
+  const float s = a > 0.f ? a / 448.0f : 1.0f;
+  if (blockIdx.x == 0 && half == 0) p.s_v[(int64_t)bh * kF8D + c] = s;
+  __syncthreads();
+  uint4* dst = reinterpret_cast<uint4*>(p.vt8 + ((int64_t)bh * kF8D + c) * p.Lpad + key0 + 64 * half);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {   // 16 key positions per store
+    uint32_t w[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int pos = 64 * half + 16 * q + 4 * r;
+      const float x0 = __bfloat162float(tile[vt8_key(pos)][c]), x1 = __bfloat162float(tile[vt8_key(pos + 1)][c]);
+      const float x2 = __bfloat162float(tile[vt8_key(pos + 2)][c]), x3 = __bfloat162float(tile[vt8_key(pos + 3)][c]);
+      w[r] = e4m3x2(x0 / s, x1 / s) | (e4m3x2(x2 / s, x3 / s) << 16);   // pad keys were loaded as zeros
+    }
+    dst[q] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+  pdl_launch_dependents();
+}
+
+__device__ __forceinline__ void fence_regs_u32(uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+
+__global__ void __launch_bounds__(kF8Threads, 1)
+attn_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                const __grid_constant__ CUtensorMap tmap_vt, const Fp8AttnMain p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw0 = smem_u32(smem_raw);
+  const uint32_t base = (raw0 + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 1024-byte aligned
+  const uint32_t sQ = base;
+  auto sK = [&](int s) { return base + (uint32_t)kF8TileBytes + (uint32_t)s * 2u * kF8TileBytes; };
+  auto sV = [&](int s) { return sK(s) + (uint32_t)kF8TileBytes; };
+  const uint32_t sScale = base + (uint32_t)kF8TileBytes * (1 + 2 * kF8Stages);
+  auto sSk = [&](int s) { return sScale + 512u * s; };
+  const uint32_t bar = sScale + 512u * kF8Stages;
+  const uint32_t q_full = bar;
+  auto full_bar = [&](int s) { return bar + 8u + 8u * s; };
+  auto empty_bar = [&](int s) { return bar + 8u + 8u * (kF8Stages + s); };
+
+  const int wg = threadIdx.x >> 7, tid_wg = threadIdx.x & 127;
+  const int qt = blockIdx.x, bh = blockIdx.y;
+  const int32_t row0 = bh * p.Lpad;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_q);
+    tma_prefetch_desc(&tmap_k);
+    tma_prefetch_desc(&tmap_vt);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < kF8Stages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();   // the prep and V pack kernels have completed
+
+  if (wg == 0) {
+    // ===================== producer =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+    if (qt == 0) p.v_amax[(int64_t)bh * kF8D + tid_wg] = 0.f;   // read by this call's V pack only: ready for the next call
+    if (tid_wg == 0) {
+      mbar_expect_tx(q_full, kF8TileBytes);
+      tma_load_2d(&tmap_q, q_full, sQ, 0, row0 + qt * kF8KB);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kb = 0; kb < p.nkb; ++kb) {
+        mbar_wait_notrace(empty_bar(stage), phase ^ 1);
+        mbar_expect_tx(full_bar(stage), 2 * kF8TileBytes + 512);
+        tma_load_2d(&tmap_k, full_bar(stage), sK(stage), 0, row0 + kb * kF8KB);
+        tma_load_2d(&tmap_vt, full_bar(stage), sV(stage), kb * kF8KB, bh * kF8D);
+        bulk_load_1d(sSk(stage), p.s_k + row0 + kb * kF8KB, 512, full_bar(stage));
+        if (++stage == kF8Stages) { stage = 0; phase ^= 1; }
+      }
+      pdl_launch_dependents();
+    }
+    return;
+  }
+
+  // ===================== consumers: 64 query rows each =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;\n" ::: "memory");
+  const int cw = wg - 1;
+  const int lane = tid_wg & 31, quad = lane & 3;
+  const int r_loc = cw * 64 + (tid_wg >> 5) * 16 + (lane >> 2);   // rows r_loc and r_loc + 8 of the query tile
+  float sq[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) sq[hh] = __ldg(p.s_q + row0 + qt * kF8KB + r_loc + 8 * hh) * p.sc;
+  // accumulator fragment: x[4 j + 2 hh + e] = (row r_loc + 8 hh, column 8 j + 2 quad + e)
+  float o[64], part[64], s[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = part[i] = s[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const float* sk_gen = reinterpret_cast<const float*>(smem_raw + (sSk(0) - raw0));
+
+  mbar_wait_notrace(q_full, 0);
+  const uint64_t dq = make_sw128_kmajor_desc(sQ + (uint32_t)(cw * 64 * 128));
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < p.nkb; ++kb) {
+    mbar_wait_notrace(full_bar(stage), phase);
+    // ---- S = Q K^T: 4 k32 steps (+32 bytes = +2 in the descriptors) ----
+    const uint64_t dk = make_sw128_kmajor_desc(sK(stage));
+    wgmma_fence_regs(s);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) WgmmaFp8<128>::mma(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // ---- scores in log2 units, mask of the ragged last block, running maximum ----
+    const float* skp = sk_gen + 128 * stage;
+    const int kvalid = p.L - kb * kF8KB;   // < 128 only in the last block
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float2 sk = *reinterpret_cast<const float2*>(skp + 8 * j + 2 * quad);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v = s[4 * j + 2 * hh + e] * sq[hh] * (e ? sk.y : sk.x);
+          if (8 * j + 2 * quad + e >= kvalid) v = -INFINITY;
+          s[4 * j + 2 * hh + e] = v;
+          mx[hh] = fmaxf(mx[hh], v);
+        }
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+      const float mn = fmaxf(m[hh], mx[hh]);   // finite: every block holds a valid key
+      alpha[hh] = fast_exp2(m[hh] - mn);       // m == -inf (first block): 0
+      m[hh] = mn;
+      l[hh] *= alpha[hh];
+    }
+    // ---- p = exp2(S - m) (masked: 0), l += p, P8 = e4m3(256 p) in the A fragment order ----
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const float pv = fast_exp2(s[i] - m[(i >> 1) & 1]);
+      l[(i >> 1) & 1] += pv;
+      s[i] = 256.f * pv;
+    }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+      pa[g][0] = e4m3x2(s[16 * g + 0], s[16 * g + 1]) | (e4m3x2(s[16 * g + 4], s[16 * g + 5]) << 16);
+      pa[g][1] = e4m3x2(s[16 * g + 2], s[16 * g + 3]) | (e4m3x2(s[16 * g + 6], s[16 * g + 7]) << 16);
+      pa[g][2] = e4m3x2(s[16 * g + 8], s[16 * g + 9]) | (e4m3x2(s[16 * g + 12], s[16 * g + 13]) << 16);
+      pa[g][3] = e4m3x2(s[16 * g + 10], s[16 * g + 11]) | (e4m3x2(s[16 * g + 14], s[16 * g + 15]) << 16);
+    }
+    // ---- partial = P8 V8 (tensor core), then O = alpha O + partial in fp32 ----
+    const uint64_t dv = make_sw128_kmajor_desc(sV(stage));
+    wgmma_fence_regs(part);
+    wgmma_fence();
+#pragma unroll
+    for (int g = 0; g < 4; ++g) WgmmaFp8RegA128::mma(part, pa[g], dv + (uint64_t)(2 * g), g > 0 ? 1u : 0u);
+    wgmma_commit();
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {   // overlaps the PV product
+      o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
+      o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(part);
+#pragma unroll
+    for (int g = 0; g < 4; ++g) fence_regs_u32(pa[g]);   // the A registers stay untouched until the product retired
+    if (tid_wg == 0) mbar_arrive(empty_bar(stage));
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] += part[i];
+    if (++stage == kF8Stages) { stage = 0; phase ^= 1; }
+  }
+
+  // ---- out = O s_v / (256 l), rows < L ----
+  float inv[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    inv[hh] = __fdividef(1.0f, 256.f * l[hh]);   // l >= 1: the row maximum contributes exp2(0)
+  }
+  const int b = bh / p.H, head = bh - b * p.H;
+  const float* sv = p.s_v + (int64_t)bh * kF8D;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int i = qt * kF8KB + r_loc + 8 * hh;
+    if (i >= p.L) continue;
+    __nv_bfloat16* dst = p.out + ((int64_t)b * p.q_bs + (int64_t)i * p.q_ts) * p.out_ld + (int64_t)head * kF8D;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = 8 * j + 2 * quad;
+      const float2 v = __ldg(reinterpret_cast<const float2*>(sv + c));
+      *reinterpret_cast<uint32_t*>(dst + c) =
+          pack_bf16x2(o[4 * j + 2 * hh] * v.x * inv[hh], o[4 * j + 2 * hh + 1] * v.y * inv[hh]);
+    }
+  }
+}
+
+int attn_fp8_init() {
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kF8Smem));
+  return OSB_OK;
+}
+
+}  // namespace osb
+
+extern "C" int osb_attn_fp8(const osb_attn_short_args* a, const osb_attn_fp8_workspace* ws, void* stream) {
+  using namespace osb;
+  if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
+  OSB_REQUIRE(a != nullptr && ws != nullptr, "osb_attn_fp8: null args");
+  OSB_REQUIRE(a->q && a->k && a->v && a->out, "osb_attn_fp8: null tensor");
+  OSB_REQUIRE(a->head_dim == kF8D, "osb_attn_fp8: head_dim %d not built (128)", a->head_dim);
+  OSB_REQUIRE(a->Lq == a->Lk, "osb_attn_fp8: self-attention only (Lq %d != Lk %d)", a->Lq, a->Lk);
+  OSB_REQUIRE(a->kv_lens == nullptr, "osb_attn_fp8: kv_lens is not supported");
+  OSB_REQUIRE(a->seqs_per_batch == 1, "osb_attn_fp8: one sequence per batch element (seqs_per_batch %lld)",
+              (long long)a->seqs_per_batch);
+  OSB_REQUIRE(a->Lq > 0 && a->num_seqs > 0 && a->num_heads > 0, "osb_attn_fp8: empty problem");
+  OSB_REQUIRE((a->q_ld % 8) == 0 && (a->k_ld % 8) == 0 && (a->v_ld % 8) == 0 && (a->out_ld % 8) == 0,
+              "osb_attn_fp8: leading dimensions must be multiples of 8 elements");
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(a->q) | reinterpret_cast<uintptr_t>(a->k) |
+                reinterpret_cast<uintptr_t>(a->v) | reinterpret_cast<uintptr_t>(a->out)) & 15) == 0,
+              "osb_attn_fp8: tensors must be 16-byte aligned");
+  OSB_REQUIRE((a->q_norm_w == nullptr) == (a->k_norm_w == nullptr), "osb_attn_fp8: q/k norm weights must come together");
+  OSB_REQUIRE((a->rope_cos == nullptr) == (a->rope_sin == nullptr), "osb_attn_fp8: rope cos/sin must come together");
+  OSB_REQUIRE((a->q_norm_w2 == nullptr) == (a->k_norm_w2 == nullptr) && (a->q_norm_w2 == nullptr || a->q_norm_w != nullptr),
+              "osb_attn_fp8: the second norm weight pair needs the first");
+  OSB_REQUIRE(a->rope_cos == nullptr || ((reinterpret_cast<uintptr_t>(a->rope_cos) | reinterpret_cast<uintptr_t>(a->rope_sin)) & 15) == 0,
+              "osb_attn_fp8: rope tables must be 16-byte aligned");
+  const int64_t BH = a->num_seqs * a->num_heads;
+  const int32_t L = a->Lq, Lpad = (L + kF8KB - 1) / kF8KB * kF8KB;
+  OSB_REQUIRE(ws->q8 && ws->k8 && ws->vt8 && ws->s_q && ws->s_k && ws->s_v && ws->v_amax, "osb_attn_fp8: null workspace buffer");
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(ws->q8) | reinterpret_cast<uintptr_t>(ws->k8) | reinterpret_cast<uintptr_t>(ws->vt8) |
+                reinterpret_cast<uintptr_t>(ws->s_q) | reinterpret_cast<uintptr_t>(ws->s_k) | reinterpret_cast<uintptr_t>(ws->s_v) |
+                reinterpret_cast<uintptr_t>(ws->v_amax)) & 15) == 0, "osb_attn_fp8: workspace buffers must be 16-byte aligned");
+  OSB_REQUIRE(BH <= ws->capacity_bh && Lpad <= ws->capacity_lpad,
+              "osb_attn_fp8: workspace for %lld x %lld holds less than %lld sequence-heads x %d padded tokens",
+              (long long)ws->capacity_bh, (long long)ws->capacity_lpad, (long long)BH, Lpad);
+  OSB_REQUIRE(BH <= 65535 && BH * Lpad < (1ll << 31), "osb_attn_fp8: problem too large (%lld sequence-heads of %d)",
+              (long long)BH, Lpad);
+
+  Fp8AttnPrep pp = {};
+  pp.q = static_cast<const __nv_bfloat16*>(a->q);
+  pp.k = static_cast<const __nv_bfloat16*>(a->k);
+  pp.v = static_cast<const __nv_bfloat16*>(a->v);
+  pp.q_ld = a->q_ld; pp.k_ld = a->k_ld; pp.v_ld = a->v_ld;
+  pp.q_bs = a->q_batch_stride; pp.q_ts = a->q_tok_stride;
+  pp.k_bs = a->k_batch_stride; pp.k_ts = a->k_tok_stride;
+  pp.L = L; pp.Lpad = Lpad; pp.H = a->num_heads;
+  pp.qw = static_cast<const __nv_bfloat16*>(a->q_norm_w);
+  pp.kw = static_cast<const __nv_bfloat16*>(a->k_norm_w);
+  pp.qw2 = static_cast<const __nv_bfloat16*>(a->q_norm_w2);
+  pp.kw2 = static_cast<const __nv_bfloat16*>(a->k_norm_w2);
+  pp.norm_split = a->norm_split;
+  pp.eps = a->norm_eps;
+  pp.cos = a->rope_cos; pp.sin = a->rope_sin;
+  pp.rope_half = a->rope_cos != nullptr && a->rope_half ? 1 : 0;
+  pp.q8 = static_cast<uint8_t*>(ws->q8); pp.k8 = static_cast<uint8_t*>(ws->k8); pp.vt8 = static_cast<uint8_t*>(ws->vt8);
+  pp.s_q = ws->s_q; pp.s_k = ws->s_k; pp.s_v = ws->s_v; pp.v_amax = ws->v_amax;
+
+  CUtensorMap tq, tk, tv;
+  int rc = make_tmap_2d_e4m3(&tq, ws->q8, (uint64_t)BH * Lpad, kF8D, kF8D, kF8KB, kF8D);
+  if (rc) return rc;
+  rc = make_tmap_2d_e4m3(&tk, ws->k8, (uint64_t)BH * Lpad, kF8D, kF8D, kF8KB, kF8D);
+  if (rc) return rc;
+  rc = make_tmap_2d_e4m3(&tv, ws->vt8, (uint64_t)BH * kF8D, Lpad, Lpad, kF8D, kF8KB);
+  if (rc) return rc;
+
+  Fp8AttnMain pm = {};
+  pm.s_q = ws->s_q; pm.s_k = ws->s_k; pm.s_v = ws->s_v; pm.v_amax = ws->v_amax;
+  pm.out = static_cast<__nv_bfloat16*>(a->out);
+  pm.out_ld = a->out_ld; pm.q_bs = a->q_batch_stride; pm.q_ts = a->q_tok_stride;
+  pm.L = L; pm.Lpad = Lpad; pm.H = a->num_heads; pm.nkb = Lpad / kF8KB;
+  pm.sc = a->softmax_scale * 1.4426950408889634f;
+
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  cudaLaunchAttribute attr[2];
+  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)(Lpad / 64), (unsigned)BH), dim3(128), 0, s, attr);
+  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_prep_kernel, pp));
+  cfg = launch_config(dim3((unsigned)(Lpad / kF8KB), (unsigned)BH), dim3(256), 0, s, attr);
+  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_vpack_kernel, pp));
+  cfg = launch_config(dim3((unsigned)(Lpad / kF8KB), (unsigned)BH), dim3(kF8Threads), kF8Smem, s, attr);
+  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_kernel, tq, tk, tv, pm));
+  count_launch(3);
+  return OSB_OK;
+}

@@ -22,7 +22,11 @@ FP8 (MMDiTModel.enable_fp8): the MLPs run on e4m3 operands.  Double blocks: ln_m
 residual).  Single blocks: the qkv part of linear1 stays bf16; the mlp part runs on ln_modulate_fp8 and its GELU epilogue
 writes columns C.. of an e4m3 [rows, 5C] cat buffer, `osb_quant_blocks_fp8` fills columns 0..C-1 from the attention
 output, and linear2 is one block-scaled FP8 GEMM with K = 5C.  The model hands the quantized weights and workspaces to the
-processors on `vec` (`_osb_fp8`, an `Fp8State`)."""
+processors on `vec` (`_osb_fp8`, an `Fp8State`).
+
+FP8 attention (MMDiTModel.enable_fp8_attention, independent of the FP8 MLPs): the joint self-attention runs on
+`osb_attn_fp8` (q / k quantized per token and head after QK-norm and RoPE, v per channel, P as e4m3(256 p)) instead of
+`osb_attn_short`, with the workspaces on `vec` (`_osb_fp8_attn`, an `Fp8AttnState`).  No Linear changes."""
 from __future__ import annotations
 
 import math
@@ -207,11 +211,38 @@ def _sp_group():
     return _SP["group"]
 
 
+class Fp8AttnState:
+    """What the FP8 attention path of one MMDiTModel keeps: the workspaces of `osb200.attn_fp8`, one per (B, L, heads,
+    device), reused by every block."""
+
+    def __init__(self):
+        self._ws = {}
+
+    def workspace(self, osb, B: int, L: int, H: int, device):
+        key = (B, L, H, device)
+        ws = self._ws.get(key)
+        if ws is None:
+            ws = self._ws[key] = osb.attn_fp8_workspace(B, L, H, device)
+        return ws
+
+
+def _attention(osb, fp8_attn: Fp8AttnState | None, q, k, v, out, B: int, L: int, H: int, D: int, norm_split: int,
+               attn_kw: dict) -> None:
+    """Joint self-attention of B sequences of L tokens: `osb_attn_short`, or `osb_attn_fp8` when FP8 attention is on."""
+    kw = dict(num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H,
+              head_dim=D, norm_split=norm_split, **attn_kw)
+    if fp8_attn is None:
+        osb.attn_short(q, k, v, out, **kw)
+    else:
+        osb.attn_fp8(q, k, v, out, workspace=fp8_attn.workspace(osb, B, L, H, q.device), **kw)
+
+
 def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D: int, attn_kw: dict, norm_split_full: int,
-                  dtype, device) -> Tensor:
+                  dtype, device, fp8_attn: Fp8AttnState | None = None) -> Tensor:
     """softmax(q k^T) v over the FULL joint sequence from this rank's [B*Lloc, 3*H*D] q|k|v rows: heads are scattered and
     the sequence gathered with one all-to-all (q, k, v travel together), attention runs on H/P heads, and the output comes
-    back with the inverse exchange.  Without a group it is the plain local attention."""
+    back with the inverse exchange.  Without a group it is the plain local attention.  With `fp8_attn` the attention
+    itself runs on FP8 operands (it sees the whole sequence of its heads either way)."""
     import torch.distributed as dist
 
     from opensora.acceleration.communications import all_to_all
@@ -221,9 +252,8 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
     C = H * D
     if P == 1:
         ao = torch.empty(B * Lloc, out_cols, dtype=dtype, device=device)
-        osb.attn_short(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ao[:, :C], num_seqs=B, seqs_per_batch=1,
-                       q_strides=(Lloc, 0, 1), k_strides=(Lloc, 0, 1), Lq=Lloc, Lk=Lloc, num_heads=H, head_dim=D,
-                       norm_split=norm_split_full, **attn_kw)
+        _attention(osb, fp8_attn, qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ao[:, :C], B, Lloc, H, D,
+                   norm_split_full, attn_kw)
         return ao
     if H % P:
         raise ValueError(f"sequence parallel size {P} must divide the head count {H} (distributed.py:477-479)")
@@ -231,9 +261,8 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
     full = all_to_all(qkv.view(B, Lloc, 3, H, D), g, scatter_dim=3, gather_dim=1).reshape(B * L, 3 * Hp * D)
     Cp = Hp * D
     ao_full = torch.empty(B * L, Cp, dtype=dtype, device=device)
-    osb.attn_short(full[:, :Cp], full[:, Cp:2 * Cp], full[:, 2 * Cp:], ao_full, num_seqs=B, seqs_per_batch=1,
-                   q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=Hp, head_dim=D,
-                   norm_split=norm_split_full, **attn_kw)
+    _attention(osb, fp8_attn, full[:, :Cp], full[:, Cp:2 * Cp], full[:, 2 * Cp:], ao_full, B, L, Hp, D, norm_split_full,
+               attn_kw)
     back = all_to_all(ao_full.view(B, L, Hp, D), g, scatter_dim=1, gather_dim=2).reshape(B * Lloc, C)
     if out_cols == C:
         return back
@@ -389,7 +418,8 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
                   rope_cos=cos, rope_sin=sin, rope_half=half)
         # tokens at joint position >= the FULL text length take the image stream's QK-norm weights
         split_full = getattr(vec, "_osb_txt_len", Lt)
-        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img.dtype, img.device)
+        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img.dtype, img.device,
+                           getattr(vec, "_osb_fp8_attn", None))
         img_o, txt_o = torch.empty_like(img2), torch.empty_like(txt2)
         # both output projections read `ao`: one down projection for their adapters
         pi, pt = attn.img_attn.proj, attn.txt_attn.proj
@@ -495,9 +525,9 @@ class SingleStreamBlockProcessor(_ProcessorBase):
                   rope_half=half)
         fp8 = getattr(vec, "_osb_fp8", None)
         if fp8 is not None:
-            return self._fp8_tail(osb, fp8, attn, x2, qkv, mod, B, L, C, H, D, kw).view(B, L, C)
+            return self._fp8_tail(osb, fp8, attn, x2, qkv, mod, B, L, C, H, D, kw, vec).view(B, L, C)
         # [attn | gelu(mlp)] side by side: the attention output and the GELU GEMM write one [rows, C + 4C] buffer
-        cat = _sp_attention(osb, qkv, C + M4, B, L, H, D, kw, 0, x.dtype, x.device)
+        cat = _sp_attention(osb, qkv, C + M4, B, L, H, D, kw, 0, x.dtype, x.device, getattr(vec, "_osb_fp8_attn", None))
         _gemm(osb, xm, wm, bm, lm, u, epilogue=osb.EPI_BIAS_GELU_TANH, out=cat[:, C:])
         out = _gemm(osb, cat, *linear_parts(attn.linear2), epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
                     group_rows=L)
@@ -505,7 +535,7 @@ class SingleStreamBlockProcessor(_ProcessorBase):
 
     @staticmethod
     def _fp8_tail(osb, fp8: Fp8State, attn: nn.Module, x2: Tensor, qkv: Tensor, mod, B: int, L: int, C: int, H: int,
-                  D: int, kw: dict) -> Tensor:
+                  D: int, kw: dict, vec: Tensor) -> Tensor:
         """x + gate * linear2(cat(attn, gelu(mlp))) with the cat buffer in e4m3: the attention output is block-quantized
         into columns 0..C-1, the mlp part of linear1 (on its own FP8 LN+modulate) emits its GELU codes into columns C..,
         and linear2 is one block-scaled FP8 GEMM."""
@@ -513,7 +543,7 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         rows, M4, dev, f8 = B * L, wm.shape[0], x2.device, torch.float8_e4m3fn
         cat8 = fp8.buf("cat8", rows, C + M4, dtype=f8, device=dev)
         cats = fp8.buf("cats", rows, (C + M4) // 128, device=dev)
-        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, 0, x2.dtype, dev)
+        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, 0, x2.dtype, dev, getattr(vec, "_osb_fp8_attn", None))
         osb.quant_blocks_fp8(ao, out=cat8[:, :C], out_scale=cats[:, :C // 128])
         x8, xs = osb.ln_modulate_fp8(x2, mod.shift, mod.scale, group_rows=L,
                                      out=fp8.buf("x8", rows, C, dtype=f8, device=dev), out_scale=fp8.buf("xs", rows, device=dev))

@@ -12,8 +12,8 @@ from opensora.registry import MODELS
 
 from opensora.utils.lora import adapter_of, dora_magnitude, lora_pack
 
-from .layers import (DoubleStreamBlock, EmbedND, Fp8State, LastLayer, LigerEmbedND, MLPEmbedder, SingleStreamBlock,
-                     _gemm, linear_parts, timestep_embedding)
+from .layers import (DoubleStreamBlock, EmbedND, Fp8AttnState, Fp8State, LastLayer, LigerEmbedND, MLPEmbedder,
+                     SingleStreamBlock, _gemm, linear_parts, timestep_embedding)
 
 
 @dataclass
@@ -86,11 +86,14 @@ class MMDiTModel(nn.Module):
         self._sp_group = None
         self._fp8 = False
         self._fp8_state = None
+        self._fp8_attn = False
+        self._fp8_attn_state = None
         self.register_load_state_dict_post_hook(lambda m, k: m._drop_caches())
 
     def _drop_caches(self):
         self._cond_w = self._mod_pack = self._mod_lora = self._pe_cache = None
         self._fp8_state = None   # quantized again from the current parameters at the next forward
+        self._fp8_attn_state = None   # workspaces: allocated again on the current device at the next forward
 
     def _apply(self, fn, *a, **k):
         self._drop_caches()
@@ -233,6 +236,21 @@ class MMDiTModel(nn.Module):
         """Back to the bf16 MLPs; the FP8 weight copies and workspaces are released."""
         self._fp8, self._fp8_state = False, None
 
+    # ---- FP8 (e4m3) attention -------------------------------------------------------------------------------------
+    def enable_fp8_attention(self) -> None:
+        """Run the joint self-attention of every double and single block on FP8 (e4m3) tensor cores (osb_attn_fp8,
+        include/osb200.h): q and k quantized per token and head after QK-norm and RoPE, v per channel over the sequence,
+        the softmax probabilities as e4m3(256 p).  Independent of `enable_fp8()` (the MLPs): the two compose in either
+        order.  No parameter, Linear or adapter changes.  Needs heads of 128 channels."""
+        D = self.hidden_size // self.num_heads
+        if D != 128:
+            raise ValueError(f"FP8 attention needs a head size of 128 (osb_attn_fp8), got {D}")
+        self._fp8_attn, self._fp8_attn_state = True, Fp8AttnState()
+
+    def disable_fp8_attention(self) -> None:
+        """Back to the bf16 attention (osb_attn_short); the FP8 attention workspaces are released."""
+        self._fp8_attn, self._fp8_attn_state = False, None
+
     def enable_sequence_parallel(self, group) -> None:
         """Ulysses sequence parallelism over `group` (the reference's `all_to_all` mode, opensora/models/mmdit/
         distributed.py:473-495,598-634,671-679): the joint txt|img sequence is split into P equal chunks (a rank holds the tail
@@ -270,6 +288,10 @@ class MMDiTModel(nn.Module):
             if self._fp8_state is None:
                 self._fp8_state = Fp8State()
             vec._osb_fp8 = self._fp8_state
+        if self._fp8_attn:
+            if self._fp8_attn_state is None:
+                self._fp8_attn_state = Fp8AttnState()
+            vec._osb_fp8_attn = self._fp8_attn_state
         Lt, Li = txt.shape[1], img.shape[1]
         sp = self._sp_splits(Lt, Li)
         vec._osb_txt_len = Lt   # joint positions >= Lt take the image stream's QK-norm weights on every rank

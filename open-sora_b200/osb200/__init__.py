@@ -41,6 +41,7 @@ EXPORTS = (
     "osb_quant_rows_fp8",
     "osb_gemm_fp8_blocks",
     "osb_quant_blocks_fp8",
+    "osb_attn_fp8",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -83,6 +84,7 @@ def _load() -> C.CDLL:
                                          C.c_int, C.c_int, C.c_void_p]
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_attn_short_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.osb_attn_fp8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_rms_norm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_void_p]
     lib.osb_conv3d_ndhwc.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_vae_prep.argtypes = [C.c_void_p, C.c_void_p]
@@ -708,6 +710,67 @@ def attn_short_bias(q, k, v, out, bias, *, num_seqs: int, seqs_per_batch: int, q
     with _Timed("attn_short", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):
         _check(_lib.osb_attn_short_bias(C.byref(a), _ptr(bias), n if bias.dim() == 2 else 0, _stream()),
                "osb_attn_short_bias")
+    return out
+
+
+# ---- FP8 (e4m3) attention (include/osb200.h, osb_attn_fp8) ------------------------------------------------------------
+ATTN_FP8_KEY_BLOCK = 128   # keys per block; the workspace pads L to a multiple of it
+
+
+class AttnFp8WorkspaceArgs(C.Structure):
+    _fields_ = [("q8", C.c_void_p), ("k8", C.c_void_p), ("vt8", C.c_void_p), ("s_q", C.c_void_p), ("s_k", C.c_void_p),
+                ("s_v", C.c_void_p), ("v_amax", C.c_void_p), ("capacity_bh", C.c_int64), ("capacity_lpad", C.c_int64)]
+
+
+class AttnFp8Workspace:
+    """Device buffers of `attn_fp8` for B sequences of L tokens and H heads (Lpad = L rounded up to 128): q8 / k8 e4m3
+    [B*H, Lpad, 128], vt8 e4m3 [B*H, 128, Lpad] (V transposed, keys permuted inside 32-key groups, include/osb200.h),
+    s_q / s_k fp32 [B*H, Lpad], s_v fp32 [B*H, 128] and the zero-initialised v amax scratch [B*H, 128]."""
+
+    def __init__(self, B: int, L: int, H: int, device):
+        import torch
+
+        self.B, self.L, self.H = B, L, H
+        BH, Lp = B * H, -(-L // ATTN_FP8_KEY_BLOCK) * ATTN_FP8_KEY_BLOCK
+        self.Lpad = Lp
+        f8 = torch.float8_e4m3fn
+        self.q8 = torch.empty(BH, Lp, 128, dtype=f8, device=device)
+        self.k8 = torch.empty(BH, Lp, 128, dtype=f8, device=device)
+        self.vt8 = torch.empty(BH, 128, Lp, dtype=f8, device=device)
+        self.s_q = torch.empty(BH, Lp, dtype=torch.float32, device=device)
+        self.s_k = torch.empty(BH, Lp, dtype=torch.float32, device=device)
+        self.s_v = torch.empty(BH, 128, dtype=torch.float32, device=device)
+        self.v_amax = torch.zeros(BH, 128, dtype=torch.float32, device=device)
+        a = self.args = AttnFp8WorkspaceArgs()
+        a.q8, a.k8, a.vt8 = self.q8.data_ptr(), self.k8.data_ptr(), self.vt8.data_ptr()
+        a.s_q, a.s_k, a.s_v, a.v_amax = self.s_q.data_ptr(), self.s_k.data_ptr(), self.s_v.data_ptr(), self.v_amax.data_ptr()
+        a.capacity_bh, a.capacity_lpad = BH, Lp
+
+
+def attn_fp8_workspace(B: int, L: int, H: int, device) -> AttnFp8Workspace:
+    """Allocate the workspace of `attn_fp8` for B sequences of L tokens with H heads of 128."""
+    return AttnFp8Workspace(B, L, H, device)
+
+
+def attn_fp8(q, k, v, out, *, workspace: AttnFp8Workspace, num_seqs: int, seqs_per_batch: int, q_strides, k_strides,
+             Lq: int, Lk: int, num_heads: int, head_dim: int, kv_lens=None, q_norm_w=None, k_norm_w=None,
+             norm_eps: float = 1e-6, rope_cos=None, rope_sin=None, softmax_scale: float | None = None, q_norm_w2=None,
+             k_norm_w2=None, norm_split: int = 0, impl: int = 0, rope_half: bool = False):
+    """`attn_short` on e4m3 operands (osb_attn_fp8): q / k quantized per (token, head) after QK-norm and RoPE, v per
+    channel, P as e4m3(256 p).  Self-attention of one sequence per batch element with heads of 128 (Lq == Lk,
+    seqs_per_batch == 1, no kv_lens); the keywords are those of `attn_short`.  `workspace` (attn_fp8_workspace) must
+    hold num_seqs * num_heads sequence-heads of Lq tokens; after the call it holds the quantized operands."""
+    if not isinstance(workspace, AttnFp8Workspace):
+        raise OsbError("attn_fp8: workspace must come from attn_fp8_workspace()")
+    a = _attn_short_struct(q, k, v, out, num_seqs=num_seqs, seqs_per_batch=seqs_per_batch, q_strides=q_strides,
+                           k_strides=k_strides, Lq=Lq, Lk=Lk, num_heads=num_heads, head_dim=head_dim, kv_lens=kv_lens,
+                           q_norm_w=q_norm_w, k_norm_w=k_norm_w, norm_eps=norm_eps, rope_cos=rope_cos, rope_sin=rope_sin,
+                           softmax_scale=softmax_scale, q_norm_w2=q_norm_w2, k_norm_w2=k_norm_w2, norm_split=norm_split,
+                           impl=impl, rope_half=rope_half)
+    if workspace.q8.device != q.device:
+        raise OsbError(f"attn_fp8: the workspace is on {workspace.q8.device}, q on {q.device}")
+    with _Timed("attn_fp8", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):  # QK^T + PV FLOPs
+        _check(_lib.osb_attn_fp8(C.byref(a), C.byref(workspace.args), _stream()), "osb_attn_fp8")
     return out
 
 
