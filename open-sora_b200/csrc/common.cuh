@@ -235,6 +235,28 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint32_t bar, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
+// tile stores from this CTA's smem (box elements outside the tensor map's extents are not written); the smem writes they
+// read must be made visible to the async proxy first (fence_proxy_async_smem + a barrier over the writing threads)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t src, int32_t c0, int32_t c1, int32_t c2,
+                                             int32_t c3, int32_t c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed bulk store has finished READING its smem source (the smem may be reused or released)
+__device__ __forceinline__ void bulk_wait_group_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// named barrier `id` (1..15) over `count` threads (a multiple of 32)
+__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 // ---- wgmma (warpgroup MMA) ----------------------------------------------------------------
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -7,6 +7,10 @@
 // epilogue runs on those registers, so the accumulator never goes through memory before its single rounding to bf16.
 // One wgmma group stays in flight while the next stage is waited for; a stage is handed back to the producer as soon
 // as the group that read it has retired.
+// Every mode whose output is a bf16 [rows, N] tile (all but kHeadTiles, kText and the FP8-emitting GELU) stages its
+// epilogue through shared memory: the producer TMA-loads the residual tile into an epilogue buffer before the main loop,
+// the consumers round each result once into that buffer, over the residual, and one thread writes the tile with TMA
+// stores clipped to the output's extents.  No global load then waits behind a global store.
 //
 // The same main loop serves five front ends (template kMode):
 //   kPlain      nn.Linear with fused bias / GELU(tanh) / gate * x + residual epilogues;
@@ -34,6 +38,8 @@
 // replace the separate bias / GELU(tanh) / gate*x+residual elementwise kernels.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "tiles.cuh"
 #include "wgmma.cuh"
@@ -43,7 +49,8 @@ namespace osb {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kNumThreads = 384;            // producer warpgroup + two consumer warpgroups
-constexpr int kStageBudget = 200 * 1024;    // operand ring (one CTA per SM; 227 KB is the per-block limit)
+constexpr int kStageBudget = 200 * 1024;    // operand ring of the register-epilogue modes (one CTA per SM)
+constexpr int kSmemLimit = 227 * 1024;      // sm_90 per-block dynamic shared memory limit
 
 enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4, kFp8 = 5, kFp8Blk = 6 };
 
@@ -98,17 +105,27 @@ struct ConvGeom {
   int32_t cin_chunks;                    // 64-wide channel chunks per tap
 };
 
-template <int BLOCK_N>
+// Modes whose output is a bf16 [rows, N] tile go through the staged epilogue: the 128 x BLOCK_N tile is assembled in a
+// shared-memory buffer (the residual tile is TMA-loaded into it during the main loop) and leaves by TMA tile stores.
+__host__ __device__ constexpr bool staged_epilogue(int mode) { return mode == kPlain || mode == kConv || mode == kLora || mode == kFp8 || mode == kFp8Blk; }
+
+template <int BLOCK_N, bool kStaged = false>
 struct GemmCfg {
   static constexpr int A_BYTES = kBlockM * kBlockK * 2;
   static constexpr int B_BYTES = BLOCK_N * kBlockK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES_RAW = kStageBudget / STAGE_BYTES;
+  // epilogue buffer: BLOCK_N / 64 boxes of 128 rows x 64 columns (one 128-byte swizzle row per tile row)
+  static constexpr int EPI_BYTES = kStaged ? kBlockM * BLOCK_N * 2 : 0;
+  static constexpr int RING_BUDGET = kStaged ? kSmemLimit - 1024 - 256 - EPI_BYTES : kStageBudget;
+  static constexpr int STAGES_RAW = RING_BUDGET / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 2 * 8 * STAGES;  // +1024 alignment slack
+  static constexpr int NUM_BARS = 2 * STAGES + (kStaged ? 1 : 0);   // full / empty per stage (+ residual tile)
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 + 8 * NUM_BARS;  // +1024 alignment slack
   static_assert(STAGES >= 2, "pipeline needs at least two stages");
+  static_assert(SMEM_BYTES <= kSmemLimit, "shared memory");
   static_assert(B_BYTES % 1024 == 0, "W tile must keep 1024-byte swizzle-atom alignment");
   static_assert(BLOCK_N % 16 == 0 && BLOCK_N <= 256, "wgmma N");
+  static_assert(!kStaged || BLOCK_N % 64 == 0, "the staged epilogue moves 64-column boxes");
 };
 
 template <int BLOCK_N, int kMode>
@@ -119,16 +136,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const int32_t lora_k_blocks,     // kLora only: U / s B maps and ceil(r / 64)
                  const float* a_scale, const float* w_scale,     // kFp8: row scales of A and W; kLora: w_scale is the
                                                                  // optional per-column (DoRA) scale, may be null
-                 const Fp8BlockParams fb) {                      // kFp8Blk only
-  using Cfg = GemmCfg<BLOCK_N>;
+                 const Fp8BlockParams fb,                        // kFp8Blk only
+                 const __grid_constant__ CUtensorMap tmap_r,     // staged epilogue: residual (read only when p.R)
+                 const __grid_constant__ CUtensorMap tmap_d) {   //   and output, extents exactly those of the output
+  constexpr bool kStaged = staged_epilogue(kMode);
+  using Cfg = GemmCfg<BLOCK_N, kStaged>;
   constexpr int kStages = Cfg::STAGES;
   constexpr int kBK = (kMode == kFp8 || kMode == kFp8Blk) ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
+  constexpr uint32_t kEpiBoxBytes = kBlockM * 128;   // one 128-row x 64-column box of the epilogue buffer
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 1024-byte aligned
-  const uint32_t bar_base = smem_base + kStages * Cfg::STAGE_BYTES;
+  const uint32_t epi_base = smem_base + kStages * Cfg::STAGE_BYTES;   // staged epilogue buffer (1024-byte aligned)
+  const uint32_t bar_base = epi_base + Cfg::EPI_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
+  const uint32_t res_bar = bar_base + 8u * (2 * kStages);   // staged epilogue: the residual tile has landed
   auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
   auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
 
@@ -157,6 +180,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       tma_prefetch_desc(&tmap_u);
       tma_prefetch_desc(&tmap_lb);
     }
+    if constexpr (kStaged) {
+      if (p.R != nullptr) tma_prefetch_desc(&tmap_r);
+      tma_prefetch_desc(&tmap_d);
+      mbar_init(res_bar, 1);
+    }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
@@ -171,6 +199,21 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (tid_wg == 0) {
       const int32_t a_row = (int32_t)(m_blk * kBlockM);
       const int32_t w_row = (int32_t)(n_blk * BLOCK_N);
+      if constexpr (kStaged) {
+        // The residual tile goes first, into the epilogue buffer: its latency hides behind the whole main loop.  R may
+        // alias D (in-place update): only this CTA reads or writes this tile.  Boxes past N are not issued; the
+        // out-of-bounds part of a box is zero filled and counted.
+        if (p.R != nullptr) {
+          const int live = (int)min((int64_t)(BLOCK_N / 64), (p.N - w_row + 63) / 64);
+          mbar_expect_tx(res_bar, (uint32_t)live * kEpiBoxBytes);
+          for (int c = 0; c < live; ++c) {
+            if constexpr (kMode == kConv)
+              tma_load_5d(&tmap_r, res_bar, epi_base + c * kEpiBoxBytes, w_row + 64 * c, w0, h0, t0, n_i);
+            else
+              tma_load_2d(&tmap_r, res_bar, epi_base + c * kEpiBoxBytes, w_row + 64 * c, a_row);
+          }
+        }
+      }
       int stage = 0;
       uint32_t phase = 0;
       for (int64_t kb = 0; kb < num_k_blocks; ++kb) {
@@ -464,68 +507,95 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
     }
   } else {
-    // ===================== epilogue: bias / GELU / gate + residual =====================
-    const uint32_t group_rows32 = (uint32_t)(p.group_rows > 0xffffffffll ? 0xffffffffu : p.group_rows);
+    // ===================== staged epilogue: bias / GELU / gate + residual =====================
+    // The tile is assembled in the epilogue buffer and leaves by TMA: the buffer row of tile row li is li (for kConv the
+    // 5-D output box orders its 128 positions exactly like the A box, so li is also its row there), column c of the tile
+    // sits in box c / 64 at 16-byte chunk (c % 64) / 8 XOR (li % 8) - the 128-byte swizzle.  A quad's four lanes cover
+    // one 16-byte chunk of a row and the eight rows of a warp's fragment land in eight different chunks: conflict free.
+    // Rows >= M and columns >= N are computed like the others and clipped by the tensor map on the store, so the only
+    // global reads left are the per-column bias / scale / gate vectors (clamped indices, no control dependence: they can
+    // all be in flight at once) and nothing is read after the first store.  The arithmetic per element is the register
+    // epilogue's, in its order and with its roundings (explicit _rn operations: no contraction into an FMA).
+    static_assert(kStaged, "every other mode has its own epilogue");
+    const float* gate_row[2] = {nullptr, nullptr};
+    float sa[2] = {0.f, 0.f};
+    if constexpr (kMode != kConv) {
+      const uint32_t group_rows32 = (uint32_t)(p.group_rows > 0xffffffffll ? 0xffffffffu : p.group_rows);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int li = r_frag + 8 * h;   // row inside the tile
-      int64_t row = m_blk * kBlockM + li;
-      bool row_ok = row < p.M;
-      if constexpr (kMode == kConv) {  // box-local row -> (t, h, w) output position -> flattened NDHWC row
-        const int w = w0 + (li & ((1 << cg.wt_log2) - 1));
-        const int hy = h0 + ((li >> cg.wt_log2) & ((1 << cg.ht_log2) - 1));
-        const int t = t0 + (li >> (cg.wt_log2 + cg.ht_log2));
-        row_ok = w < cg.w_out && hy < cg.h_out && t < cg.t_out;
-        row = (((int64_t)n_i * cg.t_out + t) * cg.h_out + hy) * cg.w_out + w;
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = min(m_blk * kBlockM + r_frag + 8 * h, p.M - 1);
+        if (p.epilogue == OSB_EPI_BIAS_GATE_RES && p.gate != nullptr) {   // modulation group per row: tiles may straddle
+          int64_t gi = (uint32_t)row / group_rows32;
+          if (p.mod_index) gi = p.mod_index[gi];
+          gate_row[h] = p.gate + gi * p.gate_stride;
+        }
+        if constexpr (kMode == kFp8) sa[h] = __ldg(a_scale + row);
       }
-      if (!row_ok) continue;
-      const float* gate_row = nullptr;
-      if ((kMode == kPlain || kMode == kLora || kMode == kFp8 || kMode == kFp8Blk) && p.epilogue == OSB_EPI_BIAS_GATE_RES &&
-          p.gate != nullptr) {
-        int64_t gi = (uint32_t)row / group_rows32;
-        if (p.mod_index) gi = p.mod_index[gi];
-        gate_row = p.gate + gi * p.gate_stride;
-      }
-      __nv_bfloat16* drow = p.D + row * p.ldd;
-      const __nv_bfloat16* rrow = p.R ? p.R + row * p.ldr : nullptr;
-      float sa = 0.f;
-      if constexpr (kMode == kFp8) sa = __ldg(a_scale + row);
+    }
+    uint8_t* const epi = smem_raw + (epi_base - smem_u32(smem_raw));
+    const bool gate_res = p.epilogue == OSB_EPI_BIAS_GATE_RES;
+    if (!gate_res) gate_row[0] = gate_row[1] = nullptr;
+    const bool has_res = gate_res && p.R != nullptr;
+    if (p.R != nullptr) mbar_wait_notrace(res_bar, 0);
+    // One straight-line body per activation, with the optional operands folded into identities that leave every bit of
+    // the value as it is (x + -0 = x, x * 1 = x): no branch splits the unrolled loop, so the loads are not held behind one.
+    auto body = [&](auto gelu) {
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int64_t n = n_blk * BLOCK_N + 8 * j + c_frag;
-        if (n >= p.N) continue;   // N % 8 == 0: n < N implies n + 1 < N
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if constexpr (kMode == kFp8) {
-          const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
-          v0 *= sa * sw.x;
-          v1 *= sa * sw.y;
-        } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator
-          const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
-          v0 *= sw.x;
-          v1 *= sw.y;
-        }
-        if (p.bias) {
-          const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
-          v0 += b.x;
-          v1 += b.y;
-        }
-        if (p.epilogue == OSB_EPI_BIAS_GELU_TANH) {
-          v0 = gelu_tanh(v0);
-          v1 = gelu_tanh(v1);
-        } else if (p.epilogue == OSB_EPI_BIAS_GATE_RES) {
-          if (gate_row != nullptr) {
-            const float2 g = __ldg(reinterpret_cast<const float2*>(gate_row + n));
-            v0 *= g.x;
-            v1 *= g.y;
+        const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);   // N % 8 == 0: n < N implies n + 1 < N
+        float2 sw = make_float2(1.f, 1.f), b = make_float2(-0.f, -0.f);
+        if constexpr (kMode == kFp8 || kMode == kFp8Blk) sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+        if (p.bias) b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int li = r_frag + 8 * h;
+          uint32_t* const cell = reinterpret_cast<uint32_t*>(epi + (j >> 3) * kEpiBoxBytes + li * 128 +
+                                                             (((j & 7) ^ (li & 7)) << 4) + c_frag * 2);
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if constexpr (kMode == kFp8) {
+            v0 = __fmul_rn(v0, __fmul_rn(sa[h], sw.x));
+            v1 = __fmul_rn(v1, __fmul_rn(sa[h], sw.y));
+          } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator
+            v0 = __fmul_rn(v0, sw.x);
+            v1 = __fmul_rn(v1, sw.y);
           }
-          if (rrow != nullptr) {   // R may alias D: the element is read before this thread overwrites it
-            const float2 rv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(rrow + n));
-            v0 += rv.x;
-            v1 += rv.y;
+          v0 = __fadd_rn(v0, b.x);
+          v1 = __fadd_rn(v1, b.y);
+          if constexpr (decltype(gelu)::value) {
+            v0 = gelu_tanh(v0);
+            v1 = gelu_tanh(v1);
+          } else {
+            // the residual element is read before this thread overwrites it with the result
+            const float2 g = gate_row[h] ? __ldg(reinterpret_cast<const float2*>(gate_row[h] + n)) : make_float2(1.f, 1.f);
+            const float2 rv = has_res ? unpack_bf16x2(*cell) : make_float2(-0.f, -0.f);
+            v0 = __fadd_rn(__fmul_rn(v0, g.x), rv.x);
+            v1 = __fadd_rn(__fmul_rn(v1, g.y), rv.y);
           }
+          *cell = pack_bf16x2(v0, v1);
         }
-        *reinterpret_cast<uint32_t*>(drow + n) = pack_bf16x2(v0, v1);
       }
+    };
+    if (p.epilogue == OSB_EPI_BIAS_GELU_TANH)
+      body(std::true_type{});
+    else
+      body(std::false_type{});
+    // Both consumer warpgroups' writes, made visible to the async proxy, then one thread stores the tile.  It waits only
+    // until the stores have READ the buffer, which is all the CTA needs before it exits and its shared memory is reused.
+    // The writes themselves belong to this grid's memory operations, which a dependent kernel's griddepcontrol.wait (PDL)
+    // or an ordinary stream-ordered launch waits for in full before it reads the output.
+    fence_proxy_async_smem();
+    named_barrier_sync(1, 256);
+    if (threadIdx.x == 128) {
+      const int32_t n0 = (int32_t)(n_blk * BLOCK_N);
+      const int live = (int)min((int64_t)(BLOCK_N / 64), (p.N - n0 + 63) / 64);
+      for (int c = 0; c < live; ++c) {
+        if constexpr (kMode == kConv)
+          tma_store_5d(&tmap_d, epi_base + c * kEpiBoxBytes, n0 + 64 * c, w0, h0, t0, n_i);
+        else
+          tma_store_2d(&tmap_d, epi_base + c * kEpiBoxBytes, n0 + 64 * c, (int32_t)(m_blk * kBlockM));
+      }
+      bulk_commit_group();
+      bulk_wait_group_read_all();
     }
   }
 }
@@ -537,14 +607,27 @@ template <int BLOCK_N, int kMode>
 static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tw, const GemmEpilogueParams& p, const ConvGeom& cg,
                          const HeadTileParams& ht, int64_t tiles, cudaStream_t stream, const CUtensorMap* tu = nullptr,
                          const CUtensorMap* tlb = nullptr, int32_t lora_k_blocks = 0, const float* a_scale = nullptr,
-                         const float* w_scale = nullptr, const Fp8BlockParams& fb = Fp8BlockParams{}) {
+                         const float* w_scale = nullptr, const Fp8BlockParams& fb = Fp8BlockParams{},
+                         const CUtensorMap* tr = nullptr, const CUtensorMap* td = nullptr) {
   if (tiles >= (1ll << 31)) { set_error("osb gemm: too many output tiles (%lld)", (long long)tiles); return OSB_ERR_UNSUPPORTED; }
   cudaLaunchAttribute attr[2];
-  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)tiles), dim3(kNumThreads), GemmCfg<BLOCK_N>::SMEM_BYTES, stream, attr);
-  // the LoRA maps are read by kLora only; every other mode gets the main maps as placeholders
+  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)tiles), dim3(kNumThreads),
+                                         GemmCfg<BLOCK_N, staged_epilogue(kMode)>::SMEM_BYTES, stream, attr);
+  // the LoRA maps are read by kLora only, the residual / output maps by the staged epilogue only (the residual map only
+  // when p.R is set); where a map is not read the main maps are passed as placeholders
   OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<BLOCK_N, kMode>, ta, tw, p, cg, ht, tu ? *tu : ta,
-                                    tlb ? *tlb : tw, lora_k_blocks, a_scale, w_scale, fb));
+                                    tlb ? *tlb : tw, lora_k_blocks, a_scale, w_scale, fb, tr ? *tr : ta, td ? *td : ta));
   count_launch();
+  return OSB_OK;
+}
+
+// Staged epilogue maps over the output D and the residual R (when p.R is set; *tr is left unset otherwise): [M, N] with
+// the row strides ldd / ldr, boxes of 128 rows x 64 columns.  The extents are exactly M x N, never ldd columns or a
+// padded M: the tile stores clip to them, so no byte outside the output view is written.
+static int make_epilogue_maps(const GemmEpilogueParams& p, CUtensorMap* tr, CUtensorMap* td) {
+  if (int rc = make_tmap_2d_bf16(td, p.D, p.M, p.N, p.ldd, kBlockM, 64)) return rc;
+  if (p.R != nullptr) return make_tmap_2d_bf16(tr, p.R, p.M, p.N, p.ldr, kBlockM, 64);
+  *tr = *td;
   return OSB_OK;
 }
 
@@ -589,18 +672,22 @@ static int launch_gemm(const osb_gemm_args& a, bool has_res, cudaStream_t stream
   ConvGeom cg = {};
   HeadTileParams ht = {};
   if (lora == nullptr && a.epilogue >= OSB_EPI_GATED_GELU) return launch_kernel<BLOCK_N, kText>(ta, tw, p, cg, ht, tiles, stream);
-  if (lora == nullptr) return launch_kernel<BLOCK_N, kPlain>(ta, tw, p, cg, ht, tiles, stream);
+  CUtensorMap tr, td;
+  if ((rc = make_epilogue_maps(p, &tr, &td))) return rc;
+  if (lora == nullptr)
+    return launch_kernel<BLOCK_N, kPlain>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, nullptr, nullptr,
+                                          Fp8BlockParams{}, &tr, &td);
   CUtensorMap tu, tlb;
   if ((rc = make_tmap_2d_bf16(&tu, lora->U, a.M, lora->r, lora->ldu, kBlockM, kBlockK))) return rc;
   if ((rc = make_tmap_2d_bf16(&tlb, lora->B, a.N, lora->r, lora->ldb, BLOCK_N, kBlockK))) return rc;
   return launch_kernel<BLOCK_N, kLora>(ta, tw, p, cg, ht, tiles, stream, &tu, &tlb, (lora->r + kBlockK - 1) / kBlockK,
-                                       nullptr, lora->col_scale);
+                                       nullptr, lora->col_scale, Fp8BlockParams{}, &tr, &td);
 }
 
 template <int BLOCK_N, int kMode>
 static int init_one() {
   OSB_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<BLOCK_N, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      GemmCfg<BLOCK_N>::SMEM_BYTES));
+                                      GemmCfg<BLOCK_N, staged_epilogue(kMode)>::SMEM_BYTES));
   return OSB_OK;
 }
 
@@ -671,7 +758,10 @@ static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream, cons
   const int64_t tiles = ((a.M + kBlockM - 1) / kBlockM) * ((a.N + BLOCK_N - 1) / BLOCK_N);
   ConvGeom cg = {};
   HeadTileParams ht = {};
-  return launch_kernel<BLOCK_N, kMode>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, a.a_scale, a.w_scale, fb);
+  CUtensorMap tr = ta, td = ta;   // the FP8-emitting GELU epilogue writes no bf16 D (it may be null)
+  if (a.epilogue != OSB_EPI_BIAS_GELU_TANH_FP8 && (rc = make_epilogue_maps(p, &tr, &td))) return rc;
+  return launch_kernel<BLOCK_N, kMode>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, a.a_scale, a.w_scale, fb,
+                                       &tr, &td);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -704,7 +794,20 @@ static int launch_conv(const osb_conv3d_args& a, const ConvGeom& cg, const uint3
   p.epilogue = a.residual ? OSB_EPI_BIAS_GATE_RES : OSB_EPI_BIAS;
   const int64_t tiles = (int64_t)cg.nb * cg.tiles_t * cg.tiles_h * cg.tiles_w * ((a.cout + BLOCK_N - 1) / BLOCK_N);
   HeadTileParams ht = {};
-  return launch_kernel<BLOCK_N, kConv>(ta, tw, p, cg, ht, tiles, stream);
+  // output and residual: the NDHWC [nb, t_out, h_out, w_out, cout] tensor, one box = the CTA's Wt x Ht x Tt positions x
+  // 64 channels, ordered like the A box (its 128 rows); boxes past the output's edges are clipped on store
+  const uint64_t cout = (uint64_t)a.cout;
+  const uint64_t odims[5] = {cout, (uint64_t)a.w_out, (uint64_t)a.h_out, (uint64_t)a.t_out, (uint64_t)a.nb};
+  const uint64_t ostr[4] = {cout * 2, (uint64_t)a.w_out * cout * 2, (uint64_t)a.h_out * a.w_out * cout * 2,
+                            (uint64_t)a.t_out * a.h_out * a.w_out * cout * 2};
+  const uint32_t obox[5] = {64, 1u << cg.wt_log2, 1u << cg.ht_log2, 128u >> (cg.wt_log2 + cg.ht_log2), 1};
+  const uint32_t ones[5] = {1, 1, 1, 1, 1};
+  CUtensorMap tr, td;
+  if ((rc = make_tmap_5d_bf16(&td, a.y, odims, ostr, obox, ones))) return rc;
+  tr = td;
+  if (a.residual && (rc = make_tmap_5d_bf16(&tr, a.residual, odims, ostr, obox, ones))) return rc;
+  return launch_kernel<BLOCK_N, kConv>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, nullptr, nullptr,
+                                       Fp8BlockParams{}, &tr, &td);
 }
 
 }  // namespace osb
