@@ -353,6 +353,63 @@ typedef struct osb_attn_tiles_args {
  * with the next key tile in flight (open-sora_b200/csrc/attn_sm90.cu).  Replaces mmdit/math.py:22-36. */
 int osb_attn_tiles(const osb_attn_tiles_args* args, void* stream);
 
+/* ---- FP8 (e4m3) head-tile attention: the opt-in attention path of STDiT3 ---------------------------------------------- */
+/* The bf16 head tiles written by osb_gemm_head_tiles (bias, QK-RMSNorm and RoPE applied, rounded once) are converted to
+ * e4m3 tiles, and osb_attn_tiles_fp8 computes every set shape of osb_attn_tiles on them.  head_dim 72 or 64 only.
+ *   q, k:  one scale per (token, head): s = amax(|row|) / 448 (1 for an all-zero row), codes e4m3_rn_satfinite(row / s):
+ *          the per-row rule of the FP8 GEMMs.
+ *   v:     one scale per (key tile, head, channel) over the tile's rows, by the same rule.  A packed temporal tile
+ *          shares one scale among its G short sequences; no reduction crosses tiles.
+ *   scores (log2 units, fp32):  S_ij = s_q[i] * s_k[j] * (sum_d q8[i, d] k8[j, d]) * softmax_scale * log2(e).
+ *   softmax: online over key tiles, p = exp2(S - m_running) in fp32, l = fp32 sum of p.
+ *   PV:    P8 = e4m3_rn_satfinite(256 * p); each key tile's P8 V8 is summed by the tensor core into a partial promoted as
+ *          O = alpha * O + s_v[tile] (.) partial (per channel).
+ *   out = bf16(O / (256 * l)), rows addressed as osb_attn_tiles addresses them (inverse q_map, optional out_scatter).
+ *   Masks: packed sequences (G > 1) are block-diagonal inside a tile, kv_lens applies when G == 1, the last tile may be
+ *   ragged, and an empty key set writes zeros (as osb_attn_tiles does).
+ *
+ * Tile format (open-sora_b200/csrc/tiles.cuh): every tile is 128 rows x 128 bytes of e4m3 codes (16384 bytes) in the
+ * 128-byte swizzle (byte c of row r at r * 128 + (((c / 16) ^ (r % 8)) * 16) + c % 16) plus 128 fp32 scales.
+ *   q / k tile: row = tile row, byte = channel (channels >= head_dim and rows >= tile_rows: zero codes, scale 1).
+ *   v tile:     row = channel (rows >= head_dim unused), byte p = key j(p) of the tile with the osb_attn_fp8 vt8 order
+ *               j(p) = 32*(p/32) + 16*((p%32)/16) + 2*((p%16)/4) + (p%2) + 8*((p%4)/2); scales per channel (1 past
+ *               head_dim).
+ * Tile (kind, head, t) sits at index (kind * num_heads + head) * tiles_per_head + t of both arrays, t the tile index of
+ * the bf16 buffer it came from. */
+typedef struct osb_tiles_fp8 {
+  void* codes;              /* e4m3, 16384 bytes per tile, 16-byte aligned                                           */
+  float* scales;            /* fp32 [tiles][128], 16-byte aligned                                                    */
+  int64_t tiles_per_head;
+  int32_t num_heads, reserved;
+} osb_tiles_fp8;
+
+typedef struct osb_head_tiles_fp8_args {
+  const void* tiles;        /* bf16 head tiles of the first kind converted (osb_head_tiles_args layout)              */
+  int64_t kind_stride, head_stride;   /* bytes, as in osb_head_tiles_args                                            */
+  osb_tiles_fp8 dst;        /* e4m3 tiles: dst tile (k, head, t) <- source tile (k, head, t), k < nkinds             */
+  int32_t tile_rows, head_dim;
+  int32_t nkinds;           /* kinds converted in this launch                                                        */
+  int32_t v_period, v_slot; /* kind k is a value kind iff v_period > 0 and k % v_period == v_slot (q|k|v: 3, 2;
+                               the k|v pairs of all blocks: 2, 1; queries only: 0, 0)                                */
+  int32_t reserved;
+} osb_head_tiles_fp8_args;
+
+/* One launch, one CTA per (tile, head, kind): q / k tiles get per-row codes and scales, v tiles are transposed and
+ * scaled per channel.  Any run of kinds converts in one launch (the text keys / values of all 2*depth blocks at once). */
+int osb_head_tiles_fp8(const osb_head_tiles_fp8_args* args, void* stream);
+
+typedef struct osb_attn_tiles_fp8_operands {
+  const void* q8; const void* k8; const void* v8;     /* e4m3 tile 0 of head 0 of the q, k and v kinds               */
+  const float* s_q; const float* s_k; const float* s_v; /* the scales of the same tiles                               */
+  int64_t q_head_tiles, kv_head_tiles;                /* tiles between heads (tiles_per_head of each buffer)         */
+} osb_attn_tiles_fp8_operands;
+
+/* osb_attn_tiles on e4m3 tiles: every field of `args` keeps its meaning except q_tiles / k_tiles / v_tiles and the two
+ * head strides, which are not read (`ops` gives the e4m3 tiles).  head_dim 72 or 64.  One CTA of three warpgroups per
+ * (query tile, head): a producer streams K / V tiles and their scales with bulk copies through an mbarrier ring, two
+ * consumers run S = Q K^T and P8 V8 on wgmma e4m3. */
+int osb_attn_tiles_fp8(const osb_attn_tiles_args* args, const osb_attn_tiles_fp8_operands* ops, void* stream);
+
 /* ---- sequence-parallel exchange over peer memory (NVLink / NVSwitch; SURVEY.md §8b, §8e) ------------------------- */
 /* The T-shard <-> S-shard transposition around temporal attention (the reference's all_to_all,
  * opensora/acceleration/communications.py:8-18,57-63) is done by the PRODUCING kernel: it stores every output row

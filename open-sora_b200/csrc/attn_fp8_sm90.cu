@@ -126,13 +126,6 @@ __global__ void __launch_bounds__(128) attn_fp8_prep_kernel(const Fp8AttnPrep p)
   pdl_launch_dependents();
 }
 
-// position p (0..31) of a 32-key group of vt8 holds key j(p) = 16 (p/16) + 2 ((p%16)/4) + p%2 + 8 ((p%4)/2): the order in
-// which a thread's S accumulator registers (columns 2 (lane%4) + {0, 1, 8, 9, 16, 17, 24, 25}) fill its FP8 A fragment
-// (k = 4 (lane%4) + {0..3, 16..19})
-__device__ __forceinline__ int vt8_key(int pos) {
-  return (pos & ~31) + 16 * ((pos >> 4) & 1) + 2 * ((pos >> 2) & 3) + (pos & 1) + 8 * ((pos >> 1) & 1);
-}
-
 __global__ void __launch_bounds__(256) attn_fp8_vpack_kernel(const Fp8AttnPrep p) {
   __shared__ __align__(16) __nv_bfloat16 tile[kF8KB][kF8D];   // [key][channel]
   const int tid = threadIdx.x;
@@ -166,11 +159,6 @@ __global__ void __launch_bounds__(256) attn_fp8_vpack_kernel(const Fp8AttnPrep p
     dst[q] = make_uint4(w[0], w[1], w[2], w[3]);
   }
   pdl_launch_dependents();
-}
-
-__device__ __forceinline__ void fence_regs_u32(uint32_t (&a)[4]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 __global__ void __launch_bounds__(kF8Threads, 1)

@@ -11,6 +11,17 @@
 // The same bytes serve as the operand of S = Q K^T (ldmatrix) and of O = P V (ldmatrix.trans).
 // Producers: the head-tile epilogue of gemm_bf16_kernel (bias + per-head RMSNorm + RoPE fused, gemm_sm90.cu) and the
 // staging step of attn_short_kernel.  Consumers: attn_tiles_kernel / attn_short_kernel (attn_sm90.cu).
+//
+// FP8 head tiles (osb_head_tiles_fp8 -> osb_attn_tiles_fp8, attn_tiles_fp8_sm90.cu): every bf16 tile has an e4m3 twin
+// of 128 rows x 128 bytes (kTileF8Bytes), again the shared-memory image of a wgmma operand: K-major rows of 128 bytes
+// in the 128-byte swizzle (byte c of row r at r * 128 + (((c / 16) ^ (r % 8)) * 16) + c % 16), loaded by one bulk copy.
+//   q / k tile: row = tile row (token), byte = channel; channels >= D and rows >= tile_rows hold zero codes.  The head
+//               dim is padded to 128 bytes but the QK^T product runs ceil(D / 32) k32 steps only (3 for D = 72).
+//   v tile:     row = channel (< D; later rows unused), byte p = key vt8_key(p) of the tile (below), so the
+//               S accumulator registers are the A fragment of the PV product as they are.
+// Next to the codes, 128 fp32 scales per tile (kTileF8Scales): per row for q / k (1 past the tile's rows), per
+// channel for v (1 for channels >= D).  Tile (kind, head, t) has index (kind * heads + head) * tiles_per_head + t in
+// both arrays, the indexing of the bf16 buffer it was converted from.
 #pragma once
 
 #include "common.cuh"
@@ -28,6 +39,9 @@ struct HeadTileCfg {
   static_assert(TAIL == 0 || TAIL == 16, "head_dim tail must be one MMA K step");
   static_assert(D % 8 == 0, "head_dim must be a multiple of 8");
 };
+
+constexpr int kTileF8Bytes = 128 * 128;
+constexpr int kTileF8Scales = 128;
 
 // How GEMM rows (tokens) map to (tile, row in tile); shared by the producing epilogue and by the attention kernel's
 // output addressing (the inverse map).
@@ -85,6 +99,12 @@ template <int MAIN>
 __device__ __forceinline__ uint32_t tile_unit_off(int r, int u, uint32_t chunk_bytes) {
   return u < MAIN * 8 ? (uint32_t)(u >> 3) * chunk_bytes + sw128_off(r, u & 7)
                       : (uint32_t)MAIN * chunk_bytes + tail_off(r, u - MAIN * 8);
+}
+// position p (0..31) of a 32-key group of vt8 holds key j(p) = 16 (p/16) + 2 ((p%16)/4) + p%2 + 8 ((p%4)/2): the order in
+// which a thread's S accumulator registers (columns 2 (lane%4) + {0, 1, 8, 9, 16, 17, 24, 25}) fill its FP8 A fragment
+// (k = 4 (lane%4) + {0..3, 16..19})
+__device__ __forceinline__ int vt8_key(int pos) {
+  return (pos & ~31) + 16 * ((pos >> 4) & 1) + 2 * ((pos >> 2) & 3) + (pos & 1) + 8 * ((pos >> 1) & 1);
 }
 // 1-D bulk copy global -> this CTA's shared memory, completion (bytes) on an mbarrier.  size % 16 == 0.
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {

@@ -16,6 +16,8 @@ Per block (SURVEY.md §8a-S `STDiT3Block.forward`), 10 launches:
 The 2*depth kv_linear projections of the (block-invariant) text tokens are batched into one GEMM.
 With `enable_fp8()` the MLP runs on e4m3 operands with per-row scales instead (11 launches):
   ln_modulate_fp8 -> fc1 gemm_fp8 (+GELU-tanh) -> quant_rows_fp8 -> fc2 gemm_fp8 (+gate, +residual)
+With `enable_fp8_attention()` each attention reads e4m3 copies of its head tiles: head_tiles_fp8 -> attn_tiles_fp8 in
+place of attn_tiles (12 launches per block; the text keys / values of all blocks convert once per forward).
 q / k / v never exist in token layout: the projection epilogue writes "head tiles" (include/osb200.h) that the
 attention kernel loads with one bulk copy per tile.  Head sizes the tile path is not built for (anything but
 64 / 72 / 128, or an odd head count) use the register-path kernel `osb_attn_short` on token-layout q / k / v.
@@ -169,6 +171,7 @@ class STDiT3(nn.Module):
         self._sp_exchange = "nccl"
         self._sp_config_checked = False
         self._fp8 = False
+        self._fp8_attn = False
         self.register_load_state_dict_post_hook(lambda m, k: m._cache.clear())
 
     # ---- construction helpers ---------------------------------------------------------------
@@ -277,6 +280,23 @@ class STDiT3(nn.Module):
         """Back to the bf16 MLPs; the FP8 weight copies are released."""
         self._fp8 = False
         for k in [k for k in self._cache if k[0] == "fp8"]:
+            del self._cache[k]
+
+    # ---- FP8 (e4m3) attention ----------------------------------------------------------------------------------------
+    def enable_fp8_attention(self) -> None:
+        """Run every self-attention (spatial and temporal) and every cross-attention on FP8 (e4m3) tensor cores: the bf16
+        head tiles of each attention are converted to e4m3 tiles (q / k per row, v per key tile and channel) and
+        osb_attn_tiles_fp8 replaces osb_attn_tiles (include/osb200.h).  The text keys / values of all blocks convert once per
+        forward.  Composes with enable_fp8().  Head sizes 72 and 64 only; the forward raises if the head-tile attention
+        path is off (OSB_ATTN_TILES=0, or an odd head count)."""
+        if self.head_dim not in (64, 72):
+            raise ValueError(f"FP8 attention is built for head sizes 72 and 64, not {self.head_dim}")
+        self._fp8_attn = True
+
+    def disable_fp8_attention(self) -> None:
+        """Back to the bf16 attention; the e4m3 tile workspaces are released."""
+        self._fp8_attn = False
+        for k in [k for k in self._cache if k[0] == "fp8attn"]:
             del self._cache[k]
 
     def _fp8_weights(self, dev):
@@ -455,9 +475,16 @@ class STDiT3(nn.Module):
         yh = osb.gemm(yt, yp.fc1.weight, yp.fc1.bias, epilogue=osb.EPI_BIAS_GELU_TANH)
         ye = osb.gemm(yh, yp.fc2.weight, yp.fc2.bias)                                    # [B*Ly, C]
         use_tiles = self._use_tiles()
+        fp8_attn = self._fp8_attn
+        if fp8_attn and not use_tiles:
+            raise RuntimeError("FP8 attention runs on the head-tile attention path, which is off here (OSB_ATTN_TILES=0 "
+                               f"or an odd head count, {self.num_heads}); disable_fp8_attention() for the bf16 path")
+        kv8 = None
         if use_tiles:   # keys / values of all 2*depth blocks as attention operand tiles: [block][k|v][head][tile]
             kv_all = self._tiles(osb, ("kv", B, Ly), B * Ly, osb.tile_map(0, Ly, keys_only=True), 2 * nb, dev)
             osb.gemm_head_tiles(ye, cst["kv_w"], cst["kv_b"], kv_all, nkinds=2)
+            if fp8_attn:   # every block's text k | v pair in one conversion launch
+                kv8 = osb.head_tiles_fp8(kv_all, self._tiles_fp8(osb, kv_all), v_period=2, v_slot=1)
         else:
             kv_all = osb.gemm(ye, cst["kv_w"], cst["kv_b"])                              # [B*Ly, nb*2C]
         if mask is not None:
@@ -493,7 +520,7 @@ class STDiT3(nn.Module):
         hid = wsbuf("hid", R, int(C * self.config.mlp_ratio))
         cos, sin = self._rope(T, dev)
         ws = dict(xm=xm_buf, ao=ao, hid=hid, cos=cos, sin=sin, kv=kv_all, kv_lens=kv_lens, tiles=use_tiles,
-                  peer=self._peer_exchange(dev) if P > 1 else None)
+                  fp8_attn=fp8_attn, kv8=kv8, peer=self._peer_exchange(dev) if P > 1 else None)
         if self._fp8:   # e4m3 codes + row scales of the fc1 input (C wide) and the fc2 input (hid wide)
             f8 = torch.float8_e4m3fn
             ws.update(fp8=self._fp8_weights(dev), xm8=wsbuf("xm8", R, C, dtype=f8), xm8_s=wsbuf("xm8_s", R, dtype=torch.float32),
@@ -549,6 +576,22 @@ class STDiT3(nn.Module):
             self._cache[key] = osb.HeadTiles(rows, tmap, kinds, self.num_heads, self.head_dim, dev)
         return self._cache[key]
 
+    def _tiles_fp8(self, osb, tiles):
+        """The e4m3 twin of a cached bf16 tile workspace, cached with it (freed by disable_fp8_attention)."""
+        key = ("fp8attn", id(tiles))
+        hit = self._cache.get(key)
+        if hit is None or hit[0] is not tiles:
+            hit = self._cache[key] = (tiles, osb.HeadTilesFp8(tiles))
+        return hit[1]
+
+    def _self_attn(self, osb, tiles, out, ws, **kw):
+        """Self-attention over the q | k | v head tiles: osb_attn_tiles, or with FP8 attention on, one conversion of the three
+        kinds and osb_attn_tiles_fp8."""
+        if ws["fp8_attn"]:
+            t8 = osb.head_tiles_fp8(tiles, self._tiles_fp8(osb, tiles), v_period=3, v_slot=2)
+            return osb.attn_tiles_fp8(t8, t8, out, **kw)
+        return osb.attn_tiles(tiles, tiles, out, **kw)
+
     def _block(self, osb, blk, bi, xs, m, mod_index, group_rows, Ly, B, T, Tl, S, ws, sp):
         C, Hh, D = self.hidden_size, self.num_heads, self.head_dim
         N = Tl * S
@@ -571,8 +614,8 @@ class STDiT3(nn.Module):
             tt = ws["tm_t"]
             osb.gemm_head_tiles(xt, a.qkv.weight, a.qkv.bias, tt, nkinds=3, norm_w=(qn, kn, None), rope=(cos, sin),
                                 rope_kinds=0b011)
-            osb.attn_tiles(tt, tt, None, Lk=T, num_seqs=B * Sl, out_map=ws["tm_out"],
-                           out_scatter=peer.scatter(2, T, Sl, ar_ptrs), out_ld=C)
+            self._self_attn(osb, tt, None, ws, Lk=T, num_seqs=B * Sl, out_map=ws["tm_out"],
+                            out_scatter=peer.scatter(2, T, Sl, ar_ptrs), out_ld=C)
             peer.barrier()
             ao = ar
         elif blk.temporal and tiles and sp is None:
@@ -583,7 +626,7 @@ class STDiT3(nn.Module):
                             scatter=osb.make_scatter(3, 1, 0, T, S, [xm_t]))
             osb.gemm_head_tiles(xm_t, a.qkv.weight, a.qkv.bias, tt, nkinds=3, norm_w=(qn, kn, None), rope=(cos, sin),
                                 rope_kinds=0b011)
-            osb.attn_tiles(tt, tt, ao, Lk=T, num_seqs=B * S, out_map=ws["tm_out"])
+            self._self_attn(osb, tt, ao, ws, Lk=T, num_seqs=B * S, out_map=ws["tm_out"])
         elif blk.temporal:
             osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
             if sp is not None:
@@ -602,7 +645,7 @@ class STDiT3(nn.Module):
                 tt = self._tiles(osb, ("temporal-fm", B, T, Sl), B * T * Sl, ws["tm_out"], 3, xs.device)
                 osb.gemm_head_tiles(xt, a.qkv.weight, a.qkv.bias, tt, nkinds=3, norm_w=(qn, kn, None), rope=(cos, sin),
                                     rope_kinds=0b011)
-                osb.attn_tiles(tt, tt, ao_t, Lk=T, num_seqs=B * Sl)
+                self._self_attn(osb, tt, ao_t, ws, Lk=T, num_seqs=B * Sl)
             else:
                 qkv = ws["qkv"]
                 osb.gemm(xt, a.qkv.weight, a.qkv.bias, out=qkv)
@@ -616,7 +659,7 @@ class STDiT3(nn.Module):
             osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
             st = ws["sp_t"]
             osb.gemm_head_tiles(xm_buf, a.qkv.weight, a.qkv.bias, st, nkinds=3, norm_w=(qn, kn, None))
-            osb.attn_tiles(st, st, ao, Lk=S, num_seqs=B * Tl)
+            self._self_attn(osb, st, ao, ws, Lk=S, num_seqs=B * Tl)
         else:
             osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
             qkv = ws["qkv"]
@@ -632,8 +675,13 @@ class STDiT3(nn.Module):
         if tiles:
             qt = ws["q_t"]
             osb.gemm_head_tiles(xs, ca.q_linear.weight, ca.q_linear.bias, qt, nkinds=1)
-            osb.attn_tiles(qt, ws["kv"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
-                           kv_lens=ws["kv_lens"])
+            if ws["fp8_attn"]:   # q per block; the text keys / values were converted once per forward
+                q8 = osb.head_tiles_fp8(qt, self._tiles_fp8(osb, qt))
+                osb.attn_tiles_fp8(q8, ws["kv8"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
+                                   kv_lens=ws["kv_lens"])
+            else:
+                osb.attn_tiles(qt, ws["kv"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
+                               kv_lens=ws["kv_lens"])
         else:
             qc = ws["qc"]
             kv = ws["kv"][:, bi * 2 * C:(bi + 1) * 2 * C]

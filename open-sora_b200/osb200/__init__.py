@@ -42,6 +42,8 @@ EXPORTS = (
     "osb_gemm_fp8_blocks",
     "osb_quant_blocks_fp8",
     "osb_attn_fp8",
+    "osb_head_tiles_fp8",
+    "osb_attn_tiles_fp8",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -96,6 +98,8 @@ def _load() -> C.CDLL:
     lib.osb_group_stats_workspace_bytes.restype = C.c_int64
     lib.osb_gemm_head_tiles.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_attn_tiles.argtypes = [C.c_void_p, C.c_void_p]
+    lib.osb_head_tiles_fp8.argtypes = [C.c_void_p, C.c_void_p]
+    lib.osb_attn_tiles_fp8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_head_tiles_per_head.argtypes = [C.c_void_p, C.c_int64]
     lib.osb_head_tiles_per_head.restype = C.c_int64
     lib.osb_tmap_cache_stats.argtypes = [C.c_void_p, C.c_void_p]
@@ -888,17 +892,28 @@ def attn_tiles(q: HeadTiles, kv: HeadTiles, out, *, q_kind: int = 0, k_kind: int
     are the same buffer (kinds 0, 1, 2); cross-attention: kv holds the text keys / values (`keys_only` map).
     `out_map`: the token order of `out` when it differs from the order the q tiles were written from (temporal attention:
     tiles from the transposed [B, S, T] stream (mode 0), output rows frame-major (mode 1))."""
+    a = _attn_tiles_struct(q, kv, out, Lk=Lk, num_seqs=num_seqs, kv_lens=kv_lens, softmax_scale=softmax_scale,
+                           out_scatter=out_scatter, out_ld=out_ld, out_map=out_map, who="attn_tiles")
+    a.q_tiles, a.k_tiles, a.v_tiles = q.kind_ptr(q_kind), kv.kind_ptr(k_kind), kv.kind_ptr(v_kind)
+    a.q_head_stride, a.kv_head_stride = q.head_stride, kv.head_stride
+    with _Timed("attn_tiles", 4.0 * num_seqs * q.map.L * Lk * q.heads * q.head_dim):
+        _check(_lib.osb_attn_tiles(C.byref(a), _stream()), "osb_attn_tiles")
+    return out
+
+
+def _attn_tiles_struct(q, kv, out, *, Lk, num_seqs, kv_lens, softmax_scale, out_scatter, out_ld, out_map, who):
+    """osb_attn_tiles_args without the tile pointers: maps, key sets and output routing (shared by the bf16 and the FP8
+    tile attention)."""
     import torch
 
     _need(out, torch.bfloat16, "out"); _need(kv_lens, torch.int32, "kv_lens")
     assert (out is None) != (out_scatter is None), "exactly one of out / out_scatter"
     if kv_lens is not None and q.map.G > 1:   # the kernel reads kv_lens for unpacked query maps only
-        raise OsbError("attn_tiles: kv_lens applies to unpacked query maps only (G == 1); packed sequences see all Lk keys")
+        raise OsbError(f"{who}: kv_lens applies to unpacked query maps only (G == 1); packed sequences see all Lk keys")
     a = AttnTilesArgs()
-    a.q_tiles, a.k_tiles, a.v_tiles = q.kind_ptr(q_kind), kv.kind_ptr(k_kind), kv.kind_ptr(v_kind)
     if out_map is not None:   # output rows in another order than the rows the tiles were written from (same tiling)
         assert out_map.key()[4:] == q.map.key()[4:] and out_map.L == q.map.L
-    a.q_head_stride, a.kv_head_stride, a.q_map = q.head_stride, kv.head_stride, (out_map if out_map is not None else q.map)
+    a.q_map = out_map if out_map is not None else q.map
     a.kv_tile_rows = kv.map.tile_rows
     a.kv_tiles_per_set = kv.map.tps
     a.Lk, a.num_heads, a.head_dim = Lk, q.heads, q.head_dim
@@ -910,8 +925,93 @@ def attn_tiles(q: HeadTiles, kv: HeadTiles, out, *, q_kind: int = 0, k_kind: int
     else:
         a.out, a.out_ld = out.data_ptr(), out.stride(0)
     a.softmax_scale = softmax_scale if softmax_scale is not None else q.head_dim ** -0.5
-    with _Timed("attn_tiles", 4.0 * num_seqs * q.map.L * Lk * q.heads * q.head_dim):
-        _check(_lib.osb_attn_tiles(C.byref(a), _stream()), "osb_attn_tiles")
+    return a
+
+
+# ---- FP8 (e4m3) head tiles (include/osb200.h, osb_head_tiles_fp8 / osb_attn_tiles_fp8) ---------------------------------
+TILE_FP8_BYTES = 128 * 128   # one e4m3 tile: 128 rows of 128 bytes, 128-byte swizzle
+TILE_FP8_SCALES = 128        # fp32 scales per tile (per row for q / k, per channel for v)
+
+
+class TilesFp8(C.Structure):
+    _fields_ = [("codes", C.c_void_p), ("scales", C.c_void_p), ("tiles_per_head", C.c_int64), ("num_heads", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class HeadTilesFp8Args(C.Structure):
+    _fields_ = [
+        ("tiles", C.c_void_p), ("kind_stride", C.c_int64), ("head_stride", C.c_int64), ("dst", TilesFp8),
+        ("tile_rows", C.c_int32), ("head_dim", C.c_int32), ("nkinds", C.c_int32), ("v_period", C.c_int32),
+        ("v_slot", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+
+class AttnTilesFp8Operands(C.Structure):
+    _fields_ = [("q8", C.c_void_p), ("k8", C.c_void_p), ("v8", C.c_void_p), ("s_q", C.c_void_p), ("s_k", C.c_void_p),
+                ("s_v", C.c_void_p), ("q_head_tiles", C.c_int64), ("kv_head_tiles", C.c_int64)]
+
+
+class HeadTilesFp8:
+    """The e4m3 twin of a HeadTiles buffer: the same kinds x heads x tiles, each tile 128 rows x 128 bytes of codes
+    (`codes`, uint8 [kinds, heads, tiles, 128, 128] in the 128-byte swizzle) and 128 fp32 scales (`scales`, [kinds, heads,
+    tiles, 128]).  Zero-filled once, like HeadTiles."""
+
+    def __init__(self, tiles: HeadTiles):
+        import torch
+
+        if tiles.head_dim not in (64, 72):
+            raise OsbError(f"FP8 head tiles are built for head_dim 64 and 72, not {tiles.head_dim}")
+        self.src, self.map, self.kinds, self.heads, self.head_dim = tiles, tiles.map, tiles.kinds, tiles.heads, tiles.head_dim
+        self.tiles_per_head = tiles.tiles_per_head
+        n = tiles.kinds * tiles.heads * tiles.tiles_per_head
+        dev = tiles.buf.device
+        self.codes = torch.zeros(tiles.kinds, tiles.heads, tiles.tiles_per_head, 128, 128, dtype=torch.uint8, device=dev)
+        self.scales = torch.zeros(tiles.kinds, tiles.heads, tiles.tiles_per_head, TILE_FP8_SCALES, dtype=torch.float32,
+                                  device=dev)
+        assert self.codes.numel() == n * TILE_FP8_BYTES
+
+    def codes_ptr(self, kind: int) -> int:
+        return self.codes[kind].data_ptr()
+
+    def scales_ptr(self, kind: int) -> int:
+        return self.scales[kind].data_ptr()
+
+
+def head_tiles_fp8(tiles: HeadTiles, dst: HeadTilesFp8, *, kind0: int = 0, nkinds: int | None = None, v_period: int = 0,
+                   v_slot: int = 0) -> HeadTilesFp8:
+    """dst[kind0 + k] = e4m3(tiles[kind0 + k]) for k < nkinds, in one launch (osb_head_tiles_fp8): kind k (counted from
+    kind0) is converted as a value kind (transposed, per-channel scales) iff v_period > 0 and k % v_period == v_slot,
+    else as a query / key kind (per-row scales)."""
+    if dst.src is not tiles:
+        raise OsbError("head_tiles_fp8: dst must be HeadTilesFp8(tiles) of the same bf16 tiles")
+    nkinds = tiles.kinds - kind0 if nkinds is None else nkinds
+    if not (0 <= kind0 and nkinds >= 1 and kind0 + nkinds <= tiles.kinds):
+        raise OsbError(f"head_tiles_fp8: kinds [{kind0}, {kind0 + nkinds}) outside the {tiles.kinds} of the buffer")
+    a = HeadTilesFp8Args()
+    a.tiles, a.kind_stride, a.head_stride = tiles.kind_ptr(kind0), tiles.kind_stride, tiles.head_stride
+    a.dst.codes, a.dst.scales = dst.codes_ptr(kind0), dst.scales_ptr(kind0)
+    a.dst.tiles_per_head, a.dst.num_heads = dst.tiles_per_head, dst.heads
+    a.tile_rows, a.head_dim, a.nkinds, a.v_period, a.v_slot = tiles.map.tile_rows, tiles.head_dim, nkinds, v_period, v_slot
+    with _Timed("head_tiles_fp8", float(nkinds * tiles.heads * tiles.tiles_per_head * (tiles.tile_bytes + TILE_FP8_BYTES))):
+        _check(_lib.osb_head_tiles_fp8(C.byref(a), _stream()), "osb_head_tiles_fp8")
+    return dst
+
+
+def attn_tiles_fp8(q: HeadTilesFp8, kv: HeadTilesFp8, out, *, q_kind: int = 0, k_kind: int = 1, v_kind: int = 2, Lk: int,
+                   num_seqs: int, kv_lens=None, softmax_scale: float | None = None, out_scatter: Scatter | None = None,
+                   out_ld: int | None = None, out_map: TileMap | None = None):
+    """`attn_tiles` on e4m3 head tiles (osb_attn_tiles_fp8): the same keywords and set shapes, operands from
+    head_tiles_fp8.  head_dim 64 or 72."""
+    if not isinstance(q, HeadTilesFp8) or not isinstance(kv, HeadTilesFp8):
+        raise OsbError("attn_tiles_fp8: q and kv must be HeadTilesFp8 buffers")
+    a = _attn_tiles_struct(q, kv, out, Lk=Lk, num_seqs=num_seqs, kv_lens=kv_lens, softmax_scale=softmax_scale,
+                           out_scatter=out_scatter, out_ld=out_ld, out_map=out_map, who="attn_tiles_fp8")
+    o = AttnTilesFp8Operands()
+    o.q8, o.k8, o.v8 = q.codes_ptr(q_kind), kv.codes_ptr(k_kind), kv.codes_ptr(v_kind)
+    o.s_q, o.s_k, o.s_v = q.scales_ptr(q_kind), kv.scales_ptr(k_kind), kv.scales_ptr(v_kind)
+    o.q_head_tiles, o.kv_head_tiles = q.tiles_per_head, kv.tiles_per_head
+    with _Timed("attn_tiles_fp8", 4.0 * num_seqs * q.map.L * Lk * q.heads * q.head_dim):
+        _check(_lib.osb_attn_tiles_fp8(C.byref(a), C.byref(o), _stream()), "osb_attn_tiles_fp8")
     return out
 
 
