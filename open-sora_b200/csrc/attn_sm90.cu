@@ -1,17 +1,19 @@
 // Attention on sm_90a: softmax(q k^T * scale) v per (sequence, head), non-causal, exact online softmax.
 //
-// All entry points run the same flash-attention core.  One CTA (8 warps) owns 128 query rows of one head; every
-// warp owns 16 rows and keeps its Q fragments, the running row maximum / sum and the fp32 O accumulator in
-// registers.  Key / value tiles sit in shared memory in the head-tile layout (tiles.cuh: 64-column chunks with the
-// 128-byte swizzle plus the head-dim tail), so the 16-byte rows that ldmatrix gathers are bank-conflict free for
-// K (S = Q K^T) and for V read transposed (O = P V); the tensor core work is mma.sync m16n8k16 (bf16 in, fp32
-// accumulate).  P is rounded to bf16 straight from the S accumulator registers, which already have the layout of
-// the A operand of the PV product, so S and P never touch shared memory.
+// Key / value tiles sit in shared memory in the head-tile layout (tiles.cuh: 64-column chunks with the 128-byte swizzle
+// plus the head-dim tail).  P is rounded to bf16 straight from the S accumulator registers, which already have the
+// layout of the A operand of the PV product, so S and P never touch shared memory.
 //
 //   osb_attn_tiles: q / k / v arrive as operand-tile images written by the projection GEMM's head-tile epilogue
-//                   (bias, RMSNorm and RoPE applied there); every load is ONE cp.async.bulk of a whole tile completing
-//                   on an mbarrier, with the next key tile in flight while the current one is consumed.
-//   osb_attn_short: q / k / v are token-layout rows (any strides); the CTA stages them into the same tile layout,
+//                   (bias, RMSNorm and RoPE applied there).  attn_tiles_kernel is persistent and warp-specialized: a
+//                   producer warpgroup bulk-copies Q tiles and a ring of K / V tiles (kept resident while consecutive
+//                   work items share them) and two consumer warpgroups run S = Q K^T and O += P V on wgmma, reading the
+//                   tile images as shared-memory descriptors.
+//   osb_attn_short: the flash core below.  One CTA (8 warps) owns 128 query rows of one head; every warp owns 16 rows
+//                   and keeps its Q fragments, the running row maximum / sum and the fp32 O accumulator in registers;
+//                   the 16-byte rows that ldmatrix gathers are bank-conflict free for K and for V read transposed, and
+//                   the tensor core work is mma.sync m16n8k16 (bf16 in, fp32 accumulate).
+//                   q / k / v are token-layout rows (any strides); the CTA stages them into the same tile layout,
 //                   applying per-head RMSNorm and RoPE in fp32 on the way, so q / k / v are read exactly once.
 //   osb_attn_short_bias: the osb_attn_short kernel (template kBias) with an fp32 additive bias indexed by the relative
 //                   position, bias[h][j - i + Lq - 1], added to the scaled score before the running max (T5's relative
@@ -25,6 +27,7 @@
 #include "common.cuh"
 #include "stage.cuh"
 #include "tiles.cuh"
+#include "wgmma.cuh"
 
 namespace osb {
 
@@ -166,10 +169,10 @@ struct TileAttnParams {
   const uint8_t* q; const uint8_t* k; const uint8_t* v;   // first tile of head 0
   int64_t q_head_stride, kv_head_stride;                  // bytes
   TileMap qmap;                                           // q tiles <-> rows of `out`
-  int32_t q_tile_bytes, q_slot_bytes;                     // TRq * ROW_BYTES; slot: 128 rows
-  int32_t kv_tile_bytes, kv_slot_bytes;
+  int32_t q_tile_bytes, kv_tile_bytes;                    // TRq * ROW_BYTES, BK * ROW_BYTES
   int32_t BK, nkb, Lk;                                    // key-tile rows, key tiles per set, keys per sequence
   int64_t num_seqs, num_sets;
+  int64_t items;                                          // heads x sets x query tiles per set
   const int32_t* kv_lens;
   __nv_bfloat16* out;
   int64_t out_ld;
@@ -177,123 +180,280 @@ struct TileAttnParams {
   RowScatter out_sc;        // sequence parallel: output rows go straight to the consuming rank's buffer
 };
 
+// Shared-memory carve-up of attn_tiles_kernel<D>: two Q slots and a ring of K / V stages, every slot sized for 128 rows
+// whatever the tile rows are (the wgmma products read 64 query rows per consumer and 128 key rows per tile), then the
+// mbarriers.  One CTA per SM: the carve-up is more than half of the 227 KB an SM offers.
 template <int D>
-__global__ void __launch_bounds__(kAttnThreads, 1) attn_tiles_kernel(const TileAttnParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t s0 = smem_u32(smem);
-  const uint32_t sQ = s0;
-  auto sK = [&](int st) { return s0 + (uint32_t)(p.q_slot_bytes + st * 2 * p.kv_slot_bytes); };
-  auto sV = [&](int st) { return sK(st) + (uint32_t)p.kv_slot_bytes; };
-  const uint32_t bar = s0 + (uint32_t)(p.q_slot_bytes + 4 * p.kv_slot_bytes);
-  const uint32_t q_full = bar;
-  auto kv_full = [&](int st) { return bar + 8u + 8u * st; };
+struct TileAttnSmem {
+  static constexpr int kSlot = 128 * HeadTileCfg<D>::ROW_BYTES;   // 1024-byte multiple
+  static constexpr int kStages = D == 128 ? 2 : (D == 72 ? 4 : 5);
+  static constexpr int kData = 2 * kSlot + kStages * 2 * kSlot;
+  static constexpr int kBytes = 1024 + kData + 8 * (4 + 2 * kStages);   // + alignment slack
+  static_assert(kBytes <= 227 * 1024 && 2 * kBytes > 228 * 1024, "one resident CTA per SM");
+};
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t qtile = blockIdx.x;
-  const int head = blockIdx.y;
-  const int64_t set = qtile / p.qmap.tps;
-  const int qt = (int)(qtile - set * p.qmap.tps);
+constexpr int kTileAttnThreads = 384;   // producer warpgroup + two consumer warpgroups of 64 query rows
 
-  // valid key slots of the set (packed tiles: G * Lk, one key range per packed sequence)
+// key tiles of a set that hold valid keys (packed tiles: G * Lk keys, else Lk clipped by kv_lens)
+__device__ __forceinline__ int tile_set_keys(const TileAttnParams& p, int64_t set) {
   int keys = p.qmap.G > 1 ? p.qmap.G * p.Lk : p.Lk;
   if (p.qmap.G == 1 && p.kv_lens) { const int l = __ldg(p.kv_lens + set); keys = l < keys ? (l < 0 ? 0 : l) : keys; }
-  const int nkt = (keys + p.BK - 1) / p.BK;   // key tiles holding valid keys
+  return keys;
+}
 
-  if (tid == 0) {
-    mbar_init(q_full, 1);
-    mbar_init(kv_full(0), 1);
-    mbar_init(kv_full(1), 1);
+// Persistent: CTA b owns the work items [b * items / grid, (b + 1) * items / grid), item = (head * sets + set) * tps + q
+// tile, so consecutive items mostly share a (head, set).  Warpgroup 0 (one thread) bulk-copies each item's Q tile into
+// one of two slots and its key / value tiles into the stage ring while the consumers work on the item before; when an
+// item has the (head, set) of the item before and the set's key tiles fit the ring, they are still resident and are
+// not loaded again.  Warpgroups 1 and 2 own 64 query rows each: S = Q K^T on wgmma (both operands shared-memory
+// descriptors over the tile images), masks and the exact online softmax over one 128-key tile at a time in registers,
+// P rounded to bf16 into the register A fragment of O += P V (V read MN-major from the same tile image).  A stage is
+// released once the PV product that read it retired, unless the next item reuses it.
+template <int D>
+__global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const TileAttnParams p) {
+  using Cfg = HeadTileCfg<D>;
+  using Sm = TileAttnSmem<D>;
+  constexpr int MAIN = Cfg::MAIN, TAIL = Cfg::TAIL, STAGES = Sm::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B atoms are 1024-byte aligned
+  auto sQ = [&](int b) { return base + (uint32_t)(b * Sm::kSlot); };
+  auto sK = [&](int s) { return base + (uint32_t)((2 + 2 * s) * Sm::kSlot); };
+  auto sV = [&](int s) { return sK(s) + (uint32_t)Sm::kSlot; };
+  const uint32_t bar = base + (uint32_t)Sm::kData;
+  auto q_full = [&](int b) { return bar + 8u * b; };
+  auto q_empty = [&](int b) { return bar + 16u + 8u * b; };
+  auto full_bar = [&](int s) { return bar + 32u + 8u * s; };
+  auto empty_bar = [&](int s) { return bar + 32u + 8u * (STAGES + s); };
+
+  const int wg = threadIdx.x >> 7, tid_wg = threadIdx.x & 127;
+  const int64_t begin = (int64_t)blockIdx.x * p.items / gridDim.x, end = (int64_t)(blockIdx.x + 1) * p.items / gridDim.x;
+  const int tps = p.qmap.tps;
+
+  // Rows past a tile's rows are read by the products (key rows up to 128 for every tile, query rows up to 64 per
+  // consumer) and must be finite: P = 0 times a NaN left in shared memory would still be a NaN.
+  {
+    uint4* z = reinterpret_cast<uint4*>(smem_raw + (base - smem_u32(smem_raw)));
+    for (int i = threadIdx.x; i < Sm::kData / 16; i += kTileAttnThreads) z[i] = make_uint4(0, 0, 0, 0);
+  }
+  fence_proxy_async_smem();   // the zeros are ordered before the bulk copies into the same bytes
+  if (threadIdx.x == 0) {
+    for (int b = 0; b < 2; ++b) { mbar_init(q_full(b), 1); mbar_init(q_empty(b), 2); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }   // 2: one per consumer
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();   // the tiles were written by the previous kernel
-  const uint8_t* kbase = p.k + (int64_t)head * p.kv_head_stride + set * p.nkb * (int64_t)p.kv_tile_bytes;
-  const uint8_t* vbase = p.v + (int64_t)head * p.kv_head_stride + set * p.nkb * (int64_t)p.kv_tile_bytes;
-  if (tid == 0) {
-    mbar_expect_tx(q_full, (uint32_t)p.q_tile_bytes);
-    bulk_load_1d(sQ, p.q + (int64_t)head * p.q_head_stride + qtile * p.q_tile_bytes, (uint32_t)p.q_tile_bytes, q_full);
-    for (int st = 0; st < 2 && st < nkt; ++st) {
-      mbar_expect_tx(kv_full(st), 2u * (uint32_t)p.kv_tile_bytes);
-      bulk_load_1d(sK(st), kbase + (int64_t)st * p.kv_tile_bytes, (uint32_t)p.kv_tile_bytes, kv_full(st));
-      bulk_load_1d(sV(st), vbase + (int64_t)st * p.kv_tile_bytes, (uint32_t)p.kv_tile_bytes, kv_full(st));
+  pdl_wait();   // the tiles were written by the previous kernel, which may also still read `out`
+
+  if (wg == 0) {
+    // ===================== producer =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (tid_wg == 0) {
+      uint32_t kv_it = 0;   // K / V tile loads so far: stage kv_it % STAGES, ring pass kv_it / STAGES
+      for (int64_t it = begin; it < end; ++it) {
+        const uint32_t n = (uint32_t)(it - begin);
+        const int64_t hs = it / tps, head = hs / p.num_sets, set = hs - head * p.num_sets;
+        const int qs = n & 1;
+        mbar_wait_notrace(q_empty(qs), ((n >> 1) & 1u) ^ 1u);
+        mbar_expect_tx(q_full(qs), (uint32_t)p.q_tile_bytes);
+        bulk_load_1d(sQ(qs), p.q + head * p.q_head_stride + (it - head * p.num_sets * tps) * p.q_tile_bytes,
+                     (uint32_t)p.q_tile_bytes, q_full(qs));
+        const int nkt = (tile_set_keys(p, set) + p.BK - 1) / p.BK;
+        if (it > begin && (it - 1) / tps == hs && nkt <= STAGES) continue;   // the set's key tiles are resident
+        const int64_t off = head * p.kv_head_stride + set * p.nkb * (int64_t)p.kv_tile_bytes;
+        for (int t = 0; t < nkt; ++t, ++kv_it) {
+          const int s = (int)(kv_it % STAGES);
+          mbar_wait_notrace(empty_bar(s), ((kv_it / STAGES) & 1u) ^ 1u);
+          mbar_expect_tx(full_bar(s), 2u * (uint32_t)p.kv_tile_bytes);
+          bulk_load_1d(sK(s), p.k + off + (int64_t)t * p.kv_tile_bytes, (uint32_t)p.kv_tile_bytes, full_bar(s));
+          bulk_load_1d(sV(s), p.v + off + (int64_t)t * p.kv_tile_bytes, (uint32_t)p.kv_tile_bytes, full_bar(s));
+        }
+      }
+      pdl_launch_dependents();   // every load of this CTA is issued
     }
+    return;
   }
 
-  // my two query rows: sequence, position, valid key range [lo, hi) in the set's key slots
-  int64_t seq[2];
-  int pos[2], lo[2], hi[2];
-  bool valid[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int r = warp * 16 + (lane >> 2) + 8 * i;
-    lo[i] = hi[i] = 0;
-    if (p.qmap.G > 1) {
-      const int g = r / p.qmap.L;
-      pos[i] = r - g * p.qmap.L;
-      seq[i] = set * p.qmap.G + g;
-      valid[i] = g < p.qmap.G && seq[i] < p.num_seqs;
-      if (valid[i]) { lo[i] = g * p.Lk; hi[i] = lo[i] + p.Lk; }
-    } else {
-      pos[i] = qt * p.qmap.TR + r;
-      seq[i] = set;
-      valid[i] = r < p.qmap.TR && pos[i] < p.qmap.L;
-      if (valid[i]) hi[i] = keys;
-    }
-  }
-
-  FlashState<D> f;
-  mbar_wait(q_full, 0);
-  // rows >= TR of the slot are not part of the tile: they only feed S rows that are never stored
-  flash_load_q<D>(f, sQ, (uint32_t)p.qmap.TR * 128u);
+  // ===================== consumers: 64 query rows each =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const int cw = wg - 1;
+  const int lane = tid_wg & 31, quad = lane & 3;
+  const int r_loc = cw * 64 + (tid_wg >> 5) * 16 + (lane >> 2);   // rows r_loc and r_loc + 8 of the query tile
   const float sc = p.scale_log2;
-  for (int kb = 0; kb < nkt; ++kb) {
-    const int st = kb & 1;
-    mbar_wait(kv_full(st), (uint32_t)(kb >> 1) & 1u);
-    for (int k0 = 0; k0 < p.BK; k0 += kKeyBlock) {
-      int n = keys - (kb * p.BK + k0);
-      const int cap = p.BK - k0 < kKeyBlock ? p.BK - k0 : kKeyBlock;
-      n = n > cap ? cap : n;
-      if (n <= 0) break;
-      const int lo_b[2] = {lo[0], lo[1]}, hi_b[2] = {hi[0], hi[1]};
-      flash_block<D>(f, sK(st), sV(st), (uint32_t)p.BK * 128u, k0, (n + 15) >> 4, kb * p.BK + k0, lo_b, hi_b, sc);
-    }
-    __syncthreads();   // every warp is done with this stage
-    if (tid == 0 && kb + 2 < nkt) {
-      mbar_expect_tx(kv_full(st), 2u * (uint32_t)p.kv_tile_bytes);
-      bulk_load_1d(sK(st), kbase + (int64_t)(kb + 2) * p.kv_tile_bytes, (uint32_t)p.kv_tile_bytes, kv_full(st));
-      bulk_load_1d(sV(st), vbase + (int64_t)(kb + 2) * p.kv_tile_bytes, (uint32_t)p.kv_tile_bytes, kv_full(st));
-    }
-  }
-  pdl_launch_dependents();
-
-  __nv_bfloat16* dst[2] = {nullptr, nullptr};
+  // accumulator fragments: x[4 j + 2 hh + e] = (row r_loc + 8 hh, column 8 j + 2 quad + e)
+  float s[64], o[MAIN][32], ot[TAIL ? 8 : 1];
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    if (!valid[i]) continue;
-    int64_t orow = row_of_token(p.qmap, seq[i], pos[i]);
-    __nv_bfloat16* obase = p.out;
-    if (p.out_sc.mode != 0) {
-      int peer;
-      scatter_row(p.out_sc, orow, peer, orow);
-      obase = static_cast<__nv_bfloat16*>(scatter_base(p.out_sc, peer));
+  for (int i = 0; i < 64; ++i) s[i] = 0.f;
+  uint32_t kv_it = 0, kv0 = 0;   // the producer's count of K / V tile loads; kv0: first load of the current set
+  for (int64_t it = begin; it < end; ++it) {
+    const uint32_t n = (uint32_t)(it - begin);
+    const int64_t hs = it / tps, head = hs / p.num_sets, set = hs - head * p.num_sets;
+    const int qt = (int)(it - hs * tps), qs = n & 1;
+    const int keys = tile_set_keys(p, set);
+    const int nkt = (keys + p.BK - 1) / p.BK;
+    if (!(it > begin && (it - 1) / tps == hs && nkt <= STAGES)) { kv0 = kv_it; kv_it += nkt; }
+    const bool keep = it + 1 < end && (it + 1) / tps == hs && nkt <= STAGES;   // the next item reads these stages
+
+    // my two query rows: sequence, position, valid key range [lo, hi) in the set's key slots
+    int64_t seq[2];
+    int pos[2], lo[2], hi[2];
+    bool valid[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int r = r_loc + 8 * hh;
+      lo[hh] = hi[hh] = 0;
+      if (p.qmap.G > 1) {
+        const int g = r / p.qmap.L;
+        pos[hh] = r - g * p.qmap.L;
+        seq[hh] = set * p.qmap.G + g;
+        valid[hh] = g < p.qmap.G && seq[hh] < p.num_seqs;
+        if (valid[hh]) { lo[hh] = g * p.Lk; hi[hh] = lo[hh] + p.Lk; }
+      } else {
+        pos[hh] = qt * p.qmap.TR + r;
+        seq[hh] = set;
+        valid[hh] = r < p.qmap.TR && pos[hh] < p.qmap.L;
+        if (valid[hh]) hi[hh] = keys;
+      }
     }
-    dst[i] = obase + orow * p.out_ld + (int64_t)head * D;
+#pragma unroll
+    for (int c = 0; c < MAIN; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (TAIL ? 8 : 1); ++i) ot[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+
+    // Q rows [64 cw, 64 cw + 64) of the slot; 64-column chunks TR * 128 bytes apart, then the tail
+    const uint32_t q_chunk = (uint32_t)p.qmap.TR * 128u, kv_chunk = (uint32_t)p.BK * 128u;
+    const uint32_t qa = sQ(qs) + (uint32_t)(cw * 64 * 128), qa_tail = sQ(qs) + MAIN * q_chunk + (uint32_t)(cw * 8 * 256);
+    mbar_wait_notrace(q_full(qs), (n >> 1) & 1u);
+    for (int t = 0; t < nkt; ++t) {
+      const uint32_t u = kv0 + (uint32_t)t;
+      const int st = (int)(u % STAGES);
+      mbar_wait_notrace(full_bar(st), (u / STAGES) & 1u);
+      // ---- S = Q K^T over 128 key rows (rows past BK are masked) ----
+      const uint32_t ka = sK(st), va = sV(st);
+      wgmma_fence_regs(s);
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < MAIN; ++c)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          Wgmma<128>::mma(s, make_sw128_kmajor_desc(qa + c * q_chunk + 32u * k),
+                          make_sw128_kmajor_desc(ka + c * kv_chunk + 32u * k), (c | k) ? 1u : 0u);
+      if constexpr (TAIL != 0)
+        Wgmma<128>::mma(s, make_noswizzle_desc(qa_tail, 128u, 256u), make_noswizzle_desc(ka + MAIN * kv_chunk, 128u, 256u), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      if (t == nkt - 1 && tid_wg == 0) mbar_arrive(q_empty(qs));   // the item's last read of its Q slot retired
+      // ---- mask, tile maximum ----
+      const int slot0 = t * p.BK;
+      // 16-key groups of the tile before the set's last valid key (>= 1): later groups have P = 0 in every row, so
+      // their exp2 is skipped (the text keys of a cross-attention end 4 keys into their third tile).  Their PV k steps
+      // still run: a branch around them would make ptxas serialise every wgmma of the kernel (C7520).
+      const int n16 = ((keys - slot0 < p.BK ? keys - slot0 : p.BK) + 15) >> 4;
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        const int hh = (i >> 1) & 1;
+        const int col = 8 * (i >> 2) + 2 * quad + (i & 1), key = slot0 + col;
+        if (col >= p.BK || key < lo[hh] || key >= hi[hh]) s[i] = -INFINITY;
+        mx[hh] = fmaxf(mx[hh], s[i]);
+      }
+      float alpha[2], ms[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+        const float mn = fmaxf(m[hh], mx[hh]);
+        alpha[hh] = (mn == -INFINITY) ? 1.f : fast_exp2((m[hh] - mn) * sc);   // m == -inf: exp2(-inf) = 0
+        ms[hh] = (mn == -INFINITY) ? 0.f : mn * sc;
+        m[hh] = mn;
+        l[hh] *= alpha[hh];
+      }
+#pragma unroll
+      for (int c = 0; c < MAIN; ++c)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[c][i] *= alpha[(i >> 1) & 1];
+      if constexpr (TAIL != 0) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) ot[i] *= alpha[(i >> 1) & 1];
+      }
+      // ---- P = exp2(S * sc - max) (masked scores are -inf and give 0), bf16 A fragments of the 8 k16 steps ----
+      uint32_t pa[8][4];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        s[i] = (i >> 3) < n16 ? fast_exp2(fmaf(s[i], sc, -ms[(i >> 1) & 1])) : 0.f;
+        l[(i >> 1) & 1] += s[i];
+      }
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        pa[g][0] = pack_bf16x2(s[8 * g + 0], s[8 * g + 1]);
+        pa[g][1] = pack_bf16x2(s[8 * g + 2], s[8 * g + 3]);
+        pa[g][2] = pack_bf16x2(s[8 * g + 4], s[8 * g + 5]);
+        pa[g][3] = pack_bf16x2(s[8 * g + 6], s[8 * g + 7]);
+      }
+      // ---- O += P V: V MN-major, 16 keys per k step = two 8-row swizzle atoms (2048 B) / tail groups (512 B) ----
+#pragma unroll
+      for (int c = 0; c < MAIN; ++c) wgmma_fence_regs(o[c]);
+      if constexpr (TAIL != 0) wgmma_fence_regs(ot);
+      wgmma_fence();
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+#pragma unroll
+        for (int c = 0; c < MAIN; ++c)
+          WgmmaRegAT<64>::mma(o[c], pa[g], make_sw128_kmajor_desc(va + c * kv_chunk + 2048u * g), 1u);
+        if constexpr (TAIL != 0)
+          WgmmaRegAT<16>::mma(ot, pa[g], make_noswizzle_desc(va + MAIN * kv_chunk + 512u * g, 256u, 128u), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < MAIN; ++c) wgmma_fence_regs(o[c]);
+      if constexpr (TAIL != 0) wgmma_fence_regs(ot);
+#pragma unroll
+      for (int g = 0; g < 8; ++g) fence_regs_u32(pa[g]);   // the A registers stay untouched until the product retired
+      if (!keep && tid_wg == 0) mbar_arrive(empty_bar(st));
+    }
+    if (nkt == 0 && tid_wg == 0) mbar_arrive(q_empty(qs));
+
+    // ---- normalise, round once to bf16, store through the inverse q map ----
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float lt = l[hh];
+      lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+      lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+      const float inv = lt > 0.f ? 1.0f / lt : 0.f;   // no valid key: zeros, never 0 * garbage
+      if (!valid[hh]) continue;
+      int64_t orow = row_of_token(p.qmap, seq[hh], pos[hh]);
+      __nv_bfloat16* obase = p.out;
+      if (p.out_sc.mode != 0) {
+        int peer;
+        scatter_row(p.out_sc, orow, peer, orow);
+        obase = static_cast<__nv_bfloat16*>(scatter_base(p.out_sc, peer));
+      }
+      __nv_bfloat16* dst = obase + orow * p.out_ld + head * D + 2 * quad;
+#pragma unroll
+      for (int c = 0; c < MAIN; ++c)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint32_t*>(dst + 64 * c + 8 * j) = pack_bf16x2(o[c][4 * j + 2 * hh] * inv, o[c][4 * j + 2 * hh + 1] * inv);
+      if constexpr (TAIL != 0)   // columns 64 MAIN .. + 7 (the rest of the tail is padding)
+        *reinterpret_cast<uint32_t*>(dst + 64 * MAIN) = pack_bf16x2(ot[2 * hh] * inv, ot[2 * hh + 1] * inv);
+    }
   }
-  flash_store<D>(f, dst[0], dst[1]);
 }
 
 template <int D>
 static int attn_tiles_launch(TileAttnParams& p, int H, cudaStream_t stream) {
   using Cfg = HeadTileCfg<D>;
   p.q_tile_bytes = p.qmap.TR * Cfg::ROW_BYTES;
-  p.q_slot_bytes = 128 * Cfg::ROW_BYTES;   // the Q fragments are read for 128 rows whatever TR is
   p.kv_tile_bytes = p.BK * Cfg::ROW_BYTES;
-  p.kv_slot_bytes = (p.kv_tile_bytes + 127) / 128 * 128;
-  const int smem = p.q_slot_bytes + 4 * p.kv_slot_bytes + 64;
-  const int64_t qtiles = p.num_sets * p.qmap.tps;
-  if (qtiles >= (1ll << 31) || H > 65535) { set_error("osb_attn_tiles: problem too large (%lld query tiles)", (long long)qtiles); return OSB_ERR_UNSUPPORTED; }
+  p.items = (int64_t)H * p.num_sets * p.qmap.tps;
+  if (p.items >= (1ll << 31)) { set_error("osb_attn_tiles: problem too large (%lld work items)", (long long)p.items); return OSB_ERR_UNSUPPORTED; }
+  const int64_t grid = p.items < sm_count() ? p.items : sm_count();   // every CTA resident at once
   cudaLaunchAttribute attr[2];
-  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)qtiles, (unsigned)H), dim3(kAttnThreads), smem, stream, attr);
+  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)grid), dim3(kTileAttnThreads), TileAttnSmem<D>::kBytes, stream, attr);
   OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_tiles_kernel<D>, p));
   count_launch();
   return OSB_OK;
@@ -476,14 +636,14 @@ static int attn_short_launch(const AttnParams& p, int64_t units, int H, cudaStre
 }
 
 int attn_init() {
-  constexpr int kMax = 200 * 1024;   // largest carve-up: 128-row Q slot + two K/V stages of 128-row D = 128 tiles
+  constexpr int kMax = 200 * 1024;   // attn_short: a 128-row Q tile and a 64-row K / V block (64 KB at D = 128)
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<72, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_short_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<72>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMax));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileAttnSmem<64>::kBytes));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<72>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileAttnSmem<72>::kBytes));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TileAttnSmem<128>::kBytes));
   return OSB_OK;
 }
 

@@ -8,9 +8,11 @@
 //   bytes [.., + TR * 32)         head-dim tail (D % 64 != 0: columns 64*MAIN .. +15, zero padded) in the
 //                                 no-swizzle core-matrix layout (8 rows x 16 B; K-adjacent matrices 128 B apart,
 //                                 8-row groups 256 B apart)
-// The same bytes serve as the operand of S = Q K^T (ldmatrix) and of O = P V (ldmatrix.trans).
+// The same bytes serve as the operand of S = Q K^T and of O = P V: as wgmma shared-memory descriptors (the chunks
+// K-major / MN-major with the 128-byte swizzle, the tail as no-swizzle core matrices) or through ldmatrix / .trans.
 // Producers: the head-tile epilogue of gemm_bf16_kernel (bias + per-head RMSNorm + RoPE fused, gemm_sm90.cu) and the
-// staging step of attn_short_kernel.  Consumers: attn_tiles_kernel / attn_short_kernel (attn_sm90.cu).
+// staging step of attn_short_kernel.  Consumers: attn_tiles_kernel (wgmma), attn_short_kernel (ldmatrix + mma.sync),
+// both in attn_sm90.cu, and head_tiles_fp8_kernel (attn_tiles_fp8_sm90.cu).
 //
 // FP8 head tiles (osb_head_tiles_fp8 -> osb_attn_tiles_fp8, attn_tiles_fp8_sm90.cu): every bf16 tile has an e4m3 twin
 // of 128 rows x 128 bytes (kTileF8Bytes), again the shared-memory image of a wgmma operand: K-major rows of 128 bytes
