@@ -173,7 +173,6 @@ int make_row_scatter(RowScatter* dst, const osb_scatter* src, int64_t rows, cons
 int gemm_init();   // gemm_sm90.cu
 int attn_init();   // attn_sm90.cu
 int attn_fp8_init();   // attn_fp8_sm90.cu
-int attn_tiles_fp8_init();   // attn_tiles_fp8_sm90.cu
 
 }  // namespace osb
 
@@ -218,8 +217,6 @@ int osb_init(int device) {
   rc = attn_init();
   if (rc) return rc;
   rc = attn_fp8_init();
-  if (rc) return rc;
-  rc = attn_tiles_fp8_init();
   if (rc) return rc;
   g_init = true;
   return OSB_OK;

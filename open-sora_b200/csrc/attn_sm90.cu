@@ -168,16 +168,10 @@ __device__ __forceinline__ void flash_store(FlashState<D>& f, __nv_bfloat16* dst
 struct TileAttnParams {
   const uint8_t* q; const uint8_t* k; const uint8_t* v;   // first tile of head 0
   int64_t q_head_stride, kv_head_stride;                  // bytes
-  TileMap qmap;                                           // q tiles <-> rows of `out`
   int32_t q_tile_bytes, kv_tile_bytes;                    // TRq * ROW_BYTES, BK * ROW_BYTES
-  int32_t BK, nkb, Lk;                                    // key-tile rows, key tiles per set, keys per sequence
-  int64_t num_seqs, num_sets;
   int64_t items;                                          // heads x sets x query tiles per set
-  const int32_t* kv_lens;
-  __nv_bfloat16* out;
-  int64_t out_ld;
   float scale_log2;
-  RowScatter out_sc;        // sequence parallel: output rows go straight to the consuming rank's buffer
+  TileSets ts;
 };
 
 // Shared-memory carve-up of attn_tiles_kernel<D>: two Q slots and a ring of K / V stages, every slot sized for 128 rows
@@ -193,13 +187,6 @@ struct TileAttnSmem {
 };
 
 constexpr int kTileAttnThreads = 384;   // producer warpgroup + two consumer warpgroups of 64 query rows
-
-// key tiles of a set that hold valid keys (packed tiles: G * Lk keys, else Lk clipped by kv_lens)
-__device__ __forceinline__ int tile_set_keys(const TileAttnParams& p, int64_t set) {
-  int keys = p.qmap.G > 1 ? p.qmap.G * p.Lk : p.Lk;
-  if (p.qmap.G == 1 && p.kv_lens) { const int l = __ldg(p.kv_lens + set); keys = l < keys ? (l < 0 ? 0 : l) : keys; }
-  return keys;
-}
 
 // Persistent: CTA b owns the work items [b * items / grid, (b + 1) * items / grid), item = (head * sets + set) * tps + q
 // tile, so consecutive items mostly share a (head, set).  Warpgroup 0 (one thread) bulk-copies each item's Q tile into
@@ -227,7 +214,8 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
 
   const int wg = threadIdx.x >> 7, tid_wg = threadIdx.x & 127;
   const int64_t begin = (int64_t)blockIdx.x * p.items / gridDim.x, end = (int64_t)(blockIdx.x + 1) * p.items / gridDim.x;
-  const int tps = p.qmap.tps;
+  const TileSets& ts = p.ts;
+  const int tps = ts.qmap.tps;
 
   // Rows past a tile's rows are read by the products (key rows up to 128 for every tile, query rows up to 64 per
   // consumer) and must be finite: P = 0 times a NaN left in shared memory would still be a NaN.
@@ -251,15 +239,15 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
       uint32_t kv_it = 0;   // K / V tile loads so far: stage kv_it % STAGES, ring pass kv_it / STAGES
       for (int64_t it = begin; it < end; ++it) {
         const uint32_t n = (uint32_t)(it - begin);
-        const int64_t hs = it / tps, head = hs / p.num_sets, set = hs - head * p.num_sets;
+        const int64_t hs = it / tps, head = hs / ts.num_sets, set = hs - head * ts.num_sets;
         const int qs = n & 1;
         mbar_wait_notrace(q_empty(qs), ((n >> 1) & 1u) ^ 1u);
         mbar_expect_tx(q_full(qs), (uint32_t)p.q_tile_bytes);
-        bulk_load_1d(sQ(qs), p.q + head * p.q_head_stride + (it - head * p.num_sets * tps) * p.q_tile_bytes,
+        bulk_load_1d(sQ(qs), p.q + head * p.q_head_stride + (it - head * ts.num_sets * tps) * p.q_tile_bytes,
                      (uint32_t)p.q_tile_bytes, q_full(qs));
-        const int nkt = (tile_set_keys(p, set) + p.BK - 1) / p.BK;
+        const int nkt = (tile_set_keys(ts, set) + ts.BK - 1) / ts.BK;
         if (it > begin && (it - 1) / tps == hs && nkt <= STAGES) continue;   // the set's key tiles are resident
-        const int64_t off = head * p.kv_head_stride + set * p.nkb * (int64_t)p.kv_tile_bytes;
+        const int64_t off = head * p.kv_head_stride + set * ts.nkb * (int64_t)p.kv_tile_bytes;
         for (int t = 0; t < nkt; ++t, ++kv_it) {
           const int s = (int)(kv_it % STAGES);
           mbar_wait_notrace(empty_bar(s), ((kv_it / STAGES) & 1u) ^ 1u);
@@ -286,10 +274,10 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
   uint32_t kv_it = 0, kv0 = 0;   // the producer's count of K / V tile loads; kv0: first load of the current set
   for (int64_t it = begin; it < end; ++it) {
     const uint32_t n = (uint32_t)(it - begin);
-    const int64_t hs = it / tps, head = hs / p.num_sets, set = hs - head * p.num_sets;
+    const int64_t hs = it / tps, head = hs / ts.num_sets, set = hs - head * ts.num_sets;
     const int qt = (int)(it - hs * tps), qs = n & 1;
-    const int keys = tile_set_keys(p, set);
-    const int nkt = (keys + p.BK - 1) / p.BK;
+    const int keys = tile_set_keys(ts, set);
+    const int nkt = (keys + ts.BK - 1) / ts.BK;
     if (!(it > begin && (it - 1) / tps == hs && nkt <= STAGES)) { kv0 = kv_it; kv_it += nkt; }
     const bool keep = it + 1 < end && (it + 1) / tps == hs && nkt <= STAGES;   // the next item reads these stages
 
@@ -298,22 +286,7 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
     int pos[2], lo[2], hi[2];
     bool valid[2];
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int r = r_loc + 8 * hh;
-      lo[hh] = hi[hh] = 0;
-      if (p.qmap.G > 1) {
-        const int g = r / p.qmap.L;
-        pos[hh] = r - g * p.qmap.L;
-        seq[hh] = set * p.qmap.G + g;
-        valid[hh] = g < p.qmap.G && seq[hh] < p.num_seqs;
-        if (valid[hh]) { lo[hh] = g * p.Lk; hi[hh] = lo[hh] + p.Lk; }
-      } else {
-        pos[hh] = qt * p.qmap.TR + r;
-        seq[hh] = set;
-        valid[hh] = r < p.qmap.TR && pos[hh] < p.qmap.L;
-        if (valid[hh]) hi[hh] = keys;
-      }
-    }
+    for (int hh = 0; hh < 2; ++hh) tile_query_row(ts, set, qt, keys, r_loc + 8 * hh, seq[hh], pos[hh], valid[hh], lo[hh], hi[hh]);
 #pragma unroll
     for (int c = 0; c < MAIN; ++c)
 #pragma unroll
@@ -323,7 +296,7 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
     // Q rows [64 cw, 64 cw + 64) of the slot; 64-column chunks TR * 128 bytes apart, then the tail
-    const uint32_t q_chunk = (uint32_t)p.qmap.TR * 128u, kv_chunk = (uint32_t)p.BK * 128u;
+    const uint32_t q_chunk = (uint32_t)ts.qmap.TR * 128u, kv_chunk = (uint32_t)ts.BK * 128u;
     const uint32_t qa = sQ(qs) + (uint32_t)(cw * 64 * 128), qa_tail = sQ(qs) + MAIN * q_chunk + (uint32_t)(cw * 8 * 256);
     mbar_wait_notrace(q_full(qs), (n >> 1) & 1u);
     for (int t = 0; t < nkt; ++t) {
@@ -347,17 +320,17 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
       wgmma_fence_regs(s);
       if (t == nkt - 1 && tid_wg == 0) mbar_arrive(q_empty(qs));   // the item's last read of its Q slot retired
       // ---- mask, tile maximum ----
-      const int slot0 = t * p.BK;
+      const int slot0 = t * ts.BK;
       // 16-key groups of the tile before the set's last valid key (>= 1): later groups have P = 0 in every row, so
       // their exp2 is skipped (the text keys of a cross-attention end 4 keys into their third tile).  Their PV k steps
       // still run: a branch around them would make ptxas serialise every wgmma of the kernel (C7520).
-      const int n16 = ((keys - slot0 < p.BK ? keys - slot0 : p.BK) + 15) >> 4;
+      const int n16 = ((keys - slot0 < ts.BK ? keys - slot0 : ts.BK) + 15) >> 4;
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
         const int hh = (i >> 1) & 1;
         const int col = 8 * (i >> 2) + 2 * quad + (i & 1), key = slot0 + col;
-        if (col >= p.BK || key < lo[hh] || key >= hi[hh]) s[i] = -INFINITY;
+        if (col >= ts.BK || key < lo[hh] || key >= hi[hh]) s[i] = -INFINITY;
         mx[hh] = fmaxf(mx[hh], s[i]);
       }
       float alpha[2], ms[2];
@@ -425,14 +398,7 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
       lt += __shfl_xor_sync(0xffffffffu, lt, 2);
       const float inv = lt > 0.f ? 1.0f / lt : 0.f;   // no valid key: zeros, never 0 * garbage
       if (!valid[hh]) continue;
-      int64_t orow = row_of_token(p.qmap, seq[hh], pos[hh]);
-      __nv_bfloat16* obase = p.out;
-      if (p.out_sc.mode != 0) {
-        int peer;
-        scatter_row(p.out_sc, orow, peer, orow);
-        obase = static_cast<__nv_bfloat16*>(scatter_base(p.out_sc, peer));
-      }
-      __nv_bfloat16* dst = obase + orow * p.out_ld + head * D + 2 * quad;
+      __nv_bfloat16* dst = tile_out_row(ts, seq[hh], pos[hh]) + head * D + 2 * quad;
 #pragma unroll
       for (int c = 0; c < MAIN; ++c)
 #pragma unroll
@@ -447,9 +413,9 @@ __global__ void __launch_bounds__(kTileAttnThreads, 1) attn_tiles_kernel(const T
 template <int D>
 static int attn_tiles_launch(TileAttnParams& p, int H, cudaStream_t stream) {
   using Cfg = HeadTileCfg<D>;
-  p.q_tile_bytes = p.qmap.TR * Cfg::ROW_BYTES;
-  p.kv_tile_bytes = p.BK * Cfg::ROW_BYTES;
-  p.items = (int64_t)H * p.num_sets * p.qmap.tps;
+  p.q_tile_bytes = p.ts.qmap.TR * Cfg::ROW_BYTES;
+  p.kv_tile_bytes = p.ts.BK * Cfg::ROW_BYTES;
+  p.items = (int64_t)H * p.ts.num_sets * p.ts.qmap.tps;
   if (p.items >= (1ll << 31)) { set_error("osb_attn_tiles: problem too large (%lld work items)", (long long)p.items); return OSB_ERR_UNSUPPORTED; }
   const int64_t grid = p.items < sm_count() ? p.items : sm_count();   // every CTA resident at once
   cudaLaunchAttribute attr[2];
@@ -647,6 +613,57 @@ int attn_init() {
   return OSB_OK;
 }
 
+int make_tile_map(TileMap* dst, const osb_tile_map& m, const char* who) {
+  OSB_REQUIRE(m.mode == 0 || m.mode == 1, "%s: unknown tile map mode %d", who, m.mode);
+  OSB_REQUIRE(m.L > 0 && m.G >= 1 && m.tile_rows > 0 && m.tile_rows <= 128 && m.tile_rows % 8 == 0,
+              "%s: bad tile map (L %d G %d rows %d)", who, m.L, m.G, m.tile_rows);
+  OSB_REQUIRE(m.G == 1 ? (m.tps == (m.L + m.tile_rows - 1) / m.tile_rows) : (m.G * m.L <= m.tile_rows && m.tps == 1),
+              "%s: tile map inconsistent (L %d G %d tps %d rows %d)", who, m.L, m.G, m.tps, m.tile_rows);
+  OSB_REQUIRE(m.mode == 0 || (m.S > 0 && m.T == m.L), "%s: temporal map needs S > 0 and T == L", who);
+  dst->mode = m.mode; dst->L = m.L; dst->S = m.S; dst->T = m.T; dst->G = m.G; dst->tps = m.tps; dst->TR = m.tile_rows;
+  return OSB_OK;
+}
+
+int make_tile_sets(TileSets* dst, const osb_attn_tiles_args* a, const char* who) {
+  OSB_REQUIRE(a->out || a->out_scatter, "%s: null tensor", who);
+  const int rc = make_tile_map(&dst->qmap, a->q_map, who);
+  if (rc) return rc;
+  const int G = a->q_map.G;
+  OSB_REQUIRE(a->kv_tile_rows >= 16 && a->kv_tile_rows <= 128 && a->kv_tile_rows % 16 == 0,
+              "%s: key tiles must have 16..128 rows in multiples of 16, got %d", who, a->kv_tile_rows);
+  OSB_REQUIRE(a->Lk > 0 && a->kv_tiles_per_set >= 1 && (int64_t)a->kv_tiles_per_set * a->kv_tile_rows >= (int64_t)(G > 1 ? G : 1) * a->Lk,
+              "%s: %d key tiles of %d rows cannot hold %d keys", who, a->kv_tiles_per_set, a->kv_tile_rows, a->Lk);
+  OSB_REQUIRE(G == 1 || (a->kv_tiles_per_set == 1), "%s: packed sequences use one key tile per set", who);
+  OSB_REQUIRE(a->num_seqs > 0 && a->num_heads > 0, "%s: empty problem", who);
+  OSB_REQUIRE(a->out_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(a->out) & 15) == 0, "%s: out must be 16-byte aligned", who);
+  dst->BK = a->kv_tile_rows; dst->nkb = a->kv_tiles_per_set; dst->Lk = a->Lk;
+  dst->num_seqs = a->num_seqs;
+  dst->num_sets = G > 1 ? (a->num_seqs + G - 1) / G : a->num_seqs;
+  dst->kv_lens = a->kv_lens;
+  dst->out = static_cast<__nv_bfloat16*>(a->out);
+  dst->out_ld = a->out_ld;
+  return make_row_scatter(&dst->out_sc, a->out_scatter, a->num_seqs * a->q_map.L, who);
+}
+
+int check_attn_short_args(const osb_attn_short_args* a, const char* who) {
+  OSB_REQUIRE(a != nullptr, "%s: null args", who);
+  OSB_REQUIRE(a->q && a->k && a->v && a->out, "%s: null tensor", who);
+  OSB_REQUIRE(a->Lq > 0 && a->Lk > 0 && a->num_seqs > 0 && a->num_heads > 0, "%s: empty problem", who);
+  OSB_REQUIRE(a->seqs_per_batch > 0, "%s: seqs_per_batch must be positive", who);
+  OSB_REQUIRE((a->q_ld % 8) == 0 && (a->k_ld % 8) == 0 && (a->v_ld % 8) == 0 && (a->out_ld % 8) == 0,
+              "%s: leading dimensions must be multiples of 8 elements", who);
+  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(a->q) | reinterpret_cast<uintptr_t>(a->k) |
+                reinterpret_cast<uintptr_t>(a->v) | reinterpret_cast<uintptr_t>(a->out)) & 15) == 0,
+              "%s: tensors must be 16-byte aligned", who);
+  OSB_REQUIRE((a->q_norm_w == nullptr) == (a->k_norm_w == nullptr), "%s: q/k norm weights must come together", who);
+  OSB_REQUIRE((a->rope_cos == nullptr) == (a->rope_sin == nullptr), "%s: rope cos/sin must come together", who);
+  OSB_REQUIRE((a->q_norm_w2 == nullptr) == (a->k_norm_w2 == nullptr) && (a->q_norm_w2 == nullptr || a->q_norm_w != nullptr),
+              "%s: the second norm weight pair needs the first", who);
+  OSB_REQUIRE(a->rope_cos == nullptr || ((reinterpret_cast<uintptr_t>(a->rope_cos) | reinterpret_cast<uintptr_t>(a->rope_sin)) & 15) == 0,
+              "%s: rope tables must be 16-byte aligned", who);
+  return OSB_OK;
+}
+
 }  // namespace osb
 
 extern "C" int64_t osb_head_tiles_per_head(const osb_tile_map* m, int64_t rows) {
@@ -660,44 +677,20 @@ extern "C" int osb_attn_tiles(const osb_attn_tiles_args* a, void* stream) {
   using namespace osb;
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
   OSB_REQUIRE(a != nullptr, "osb_attn_tiles: null args");
-  OSB_REQUIRE(a->q_tiles && a->k_tiles && a->v_tiles && (a->out || a->out_scatter), "osb_attn_tiles: null tensor");
+  OSB_REQUIRE(a->q_tiles && a->k_tiles && a->v_tiles, "osb_attn_tiles: null tensor");
   const int D = a->head_dim;
   OSB_REQUIRE(D == 64 || D == 72 || D == 128, "osb_attn_tiles: head_dim %d not built (64, 72, 128)", D);
-  const osb_tile_map& m = a->q_map;
-  OSB_REQUIRE(m.mode == 0 || m.mode == 1, "osb_attn_tiles: unknown tile map mode %d", m.mode);
-  OSB_REQUIRE(m.L > 0 && m.G >= 1 && m.tile_rows > 0 && m.tile_rows <= 128 && m.tile_rows % 8 == 0,
-              "osb_attn_tiles: bad q tile map (L %d G %d rows %d)", m.L, m.G, m.tile_rows);
-  OSB_REQUIRE(m.G == 1 ? (m.tps == (m.L + m.tile_rows - 1) / m.tile_rows) : (m.G * m.L <= m.tile_rows && m.tps == 1),
-              "osb_attn_tiles: q tile map inconsistent (L %d G %d tps %d rows %d)", m.L, m.G, m.tps, m.tile_rows);
-  OSB_REQUIRE(m.mode == 0 || (m.S > 0 && m.T == m.L), "osb_attn_tiles: temporal map needs S > 0 and T == L");
-  OSB_REQUIRE(a->kv_tile_rows >= 16 && a->kv_tile_rows <= 128 && a->kv_tile_rows % 16 == 0,
-              "osb_attn_tiles: key tiles must have 16..128 rows in multiples of 16, got %d", a->kv_tile_rows);
-  OSB_REQUIRE(a->Lk > 0 && a->kv_tiles_per_set >= 1 && (int64_t)a->kv_tiles_per_set * a->kv_tile_rows >= (int64_t)(m.G > 1 ? m.G : 1) * a->Lk,
-              "osb_attn_tiles: %d key tiles of %d rows cannot hold %d keys", a->kv_tiles_per_set, a->kv_tile_rows, a->Lk);
-  OSB_REQUIRE(m.G == 1 || (a->kv_tiles_per_set == 1), "osb_attn_tiles: packed sequences use one key tile per set");
-  OSB_REQUIRE(a->num_seqs > 0 && a->num_heads > 0, "osb_attn_tiles: empty problem");
-  OSB_REQUIRE(a->out_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(a->out) & 15) == 0, "osb_attn_tiles: out must be 16-byte aligned");
   OSB_REQUIRE(((reinterpret_cast<uintptr_t>(a->q_tiles) | reinterpret_cast<uintptr_t>(a->k_tiles) | reinterpret_cast<uintptr_t>(a->v_tiles)) & 15) == 0 &&
               a->q_head_stride % 16 == 0 && a->kv_head_stride % 16 == 0, "osb_attn_tiles: tile buffers must be 16-byte aligned");
 
   TileAttnParams p = {};
+  const int rc = make_tile_sets(&p.ts, a, "osb_attn_tiles");
+  if (rc) return rc;
   p.q = static_cast<const uint8_t*>(a->q_tiles);
   p.k = static_cast<const uint8_t*>(a->k_tiles);
   p.v = static_cast<const uint8_t*>(a->v_tiles);
   p.q_head_stride = a->q_head_stride; p.kv_head_stride = a->kv_head_stride;
-  p.qmap.mode = m.mode; p.qmap.L = m.L; p.qmap.S = m.S; p.qmap.T = m.T; p.qmap.G = m.G; p.qmap.tps = m.tps; p.qmap.TR = m.tile_rows;
-  p.BK = a->kv_tile_rows; p.nkb = a->kv_tiles_per_set; p.Lk = a->Lk;
-  p.num_seqs = a->num_seqs;
-  p.num_sets = m.G > 1 ? (a->num_seqs + m.G - 1) / m.G : a->num_seqs;
-  p.kv_lens = a->kv_lens;
-  p.out = static_cast<__nv_bfloat16*>(a->out);
-  p.out_ld = a->out_ld;
   p.scale_log2 = a->softmax_scale * 1.4426950408889634f;
-  {
-    const int64_t out_rows = a->num_seqs * m.L;
-    const int rc = make_row_scatter(&p.out_sc, a->out_scatter, out_rows, "osb_attn_tiles");
-    if (rc) return rc;
-  }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (D == 64) return attn_tiles_launch<64>(p, a->num_heads, s);
   if (D == 72) return attn_tiles_launch<72>(p, a->num_heads, s);
@@ -708,24 +701,10 @@ extern "C" int osb_attn_tiles(const osb_attn_tiles_args* a, void* stream) {
 static int attn_short_entry(const osb_attn_short_args* a, const float* bias, int64_t bias_head_stride, void* stream) {
   using namespace osb;
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
-  OSB_REQUIRE(a != nullptr, "osb_attn_short: null args");
-  OSB_REQUIRE(a->q && a->k && a->v && a->out, "osb_attn_short: null tensor");
-  OSB_REQUIRE(a->Lq > 0 && a->Lk > 0 && a->num_seqs > 0 && a->num_heads > 0,
-              "osb_attn_short: empty problem");
-  OSB_REQUIRE(a->seqs_per_batch > 0, "osb_attn_short: seqs_per_batch must be positive");
+  const int rc = check_attn_short_args(a, "osb_attn_short");
+  if (rc) return rc;
   const int D = a->head_dim;
   OSB_REQUIRE(D == 64 || D == 72 || D == 128, "osb_attn_short: head_dim %d not built (64, 72, 128)", D);
-  OSB_REQUIRE((a->q_ld % 8) == 0 && (a->k_ld % 8) == 0 && (a->v_ld % 8) == 0 && (a->out_ld % 8) == 0,
-              "osb_attn_short: leading dimensions must be multiples of 8 elements");
-  OSB_REQUIRE(((reinterpret_cast<uintptr_t>(a->q) | reinterpret_cast<uintptr_t>(a->k) |
-                reinterpret_cast<uintptr_t>(a->v) | reinterpret_cast<uintptr_t>(a->out)) & 15) == 0,
-              "osb_attn_short: tensors must be 16-byte aligned");
-  OSB_REQUIRE((a->q_norm_w == nullptr) == (a->k_norm_w == nullptr), "osb_attn_short: q/k norm weights must come together");
-  OSB_REQUIRE((a->rope_cos == nullptr) == (a->rope_sin == nullptr), "osb_attn_short: rope cos/sin must come together");
-  OSB_REQUIRE((a->q_norm_w2 == nullptr) == (a->k_norm_w2 == nullptr) && (a->q_norm_w2 == nullptr || a->q_norm_w != nullptr),
-              "osb_attn_short: the second norm weight pair needs the first");
-  OSB_REQUIRE(a->rope_cos == nullptr || ((reinterpret_cast<uintptr_t>(a->rope_cos) | reinterpret_cast<uintptr_t>(a->rope_sin)) & 15) == 0,
-              "osb_attn_short: rope tables must be 16-byte aligned");
 
   AttnParams p;
   p.q = static_cast<const __nv_bfloat16*>(a->q);

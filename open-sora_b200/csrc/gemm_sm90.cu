@@ -403,30 +403,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     for (int h = 0; h < 2; ++h) {
       const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
       const bool row_ok = row < p.M;
-      // token row -> (position in its sequence, tile, row in tile)  (32-bit arithmetic: the host checks M < 2^31)
-      uint32_t pos = 0, tile_i = 0, seq;
+      // token row -> (tile, position in its sequence, row in tile)  (the host checks M < 2^31)
+      uint32_t pos = 0, tile_i = 0;
       int r = 0;
-      if (row_ok) {
-        const uint32_t row32 = (uint32_t)row;
-        if (ht.map.mode == 0) {
-          seq = row32 / (uint32_t)ht.map.L;
-          pos = row32 - seq * (uint32_t)ht.map.L;
-        } else {
-          const uint32_t ts = (uint32_t)ht.map.T * (uint32_t)ht.map.S;
-          const uint32_t b = row32 / ts;
-          const uint32_t rem = row32 - b * ts;
-          pos = rem / (uint32_t)ht.map.S;
-          seq = b * (uint32_t)ht.map.S + (rem - pos * (uint32_t)ht.map.S);
-        }
-        if (ht.map.G > 1) {
-          tile_i = seq / (uint32_t)ht.map.G;
-          r = (int)((seq - tile_i * (uint32_t)ht.map.G) * (uint32_t)ht.map.L + pos);
-        } else {
-          const uint32_t jt = pos / (uint32_t)ht.map.TR;
-          tile_i = seq * (uint32_t)ht.map.tps + jt;
-          r = (int)(pos - jt * (uint32_t)ht.map.TR);
-        }
-      }
+      if (row_ok) tile_of_row(ht.map, (uint32_t)row, tile_i, pos, r);
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int64_t col0 = n_blk * BLOCK_N + hh * D;
@@ -1034,12 +1014,10 @@ extern "C" int osb_gemm_head_tiles(const osb_gemm_args* args, const osb_head_til
               (long long)a.N, t.num_heads, D);
   OSB_REQUIRE(t.nkinds >= 1 && t.nkinds <= 4, "osb_gemm_head_tiles: nkinds must be 1..4");
   const osb_tile_map& m = t.map;
-  OSB_REQUIRE(m.mode == 0 || m.mode == 1, "osb_gemm_head_tiles: unknown tile map mode %d", m.mode);
-  OSB_REQUIRE(m.L > 0 && m.G >= 1 && m.tile_rows > 0 && m.tile_rows <= 128 && m.tile_rows % 8 == 0,
-              "osb_gemm_head_tiles: bad tile map (L %d G %d rows %d)", m.L, m.G, m.tile_rows);
-  OSB_REQUIRE(m.G == 1 ? (m.tps == (m.L + m.tile_rows - 1) / m.tile_rows) : (m.G * m.L <= m.tile_rows && m.tps == 1),
-              "osb_gemm_head_tiles: tile map inconsistent (L %d G %d tps %d rows %d)", m.L, m.G, m.tps, m.tile_rows);
-  OSB_REQUIRE(m.mode == 0 ? (a.M % m.L == 0) : (m.S > 0 && m.T == m.L && a.M % ((int64_t)m.S * m.T) == 0),
+  HeadTileParams ht = {};
+  const int rc = make_tile_map(&ht.map, m, "osb_gemm_head_tiles");
+  if (rc) return rc;
+  OSB_REQUIRE(a.M % (m.mode == 0 ? m.L : (int64_t)m.S * m.T) == 0,
               "osb_gemm_head_tiles: M (%lld) is not a whole number of sequences", (long long)a.M);
   OSB_REQUIRE((reinterpret_cast<uintptr_t>(t.tiles) & 15) == 0 && t.kind_stride % 16 == 0 && t.head_stride % 16 == 0,
               "osb_gemm_head_tiles: tile buffer must be 16-byte aligned");
@@ -1050,10 +1028,8 @@ extern "C" int osb_gemm_head_tiles(const osb_gemm_args* args, const osb_head_til
   OSB_REQUIRE(t.head_stride >= tph * tile_bytes, "osb_gemm_head_tiles: head_stride %lld < %lld tiles of %lld bytes",
               (long long)t.head_stride, (long long)tph, (long long)tile_bytes);
   OSB_REQUIRE(tph < (1ll << 31), "osb_gemm_head_tiles: too many tiles");
-  HeadTileParams ht = {};
   ht.base = static_cast<uint8_t*>(t.tiles);
   ht.kind_stride = t.kind_stride; ht.head_stride = t.head_stride;
-  ht.map.mode = m.mode; ht.map.L = m.L; ht.map.S = m.S; ht.map.T = m.T; ht.map.G = m.G; ht.map.tps = m.tps; ht.map.TR = m.tile_rows;
   ht.tile_bytes = (int32_t)tile_bytes;
   ht.heads = t.num_heads; ht.nkinds = t.nkinds;
   ht.norm_mask = t.norm_mask; ht.rope_mask = t.rope_mask;

@@ -7,6 +7,10 @@
 
 namespace osb {
 
+// Checks of osb_attn_short_args shared by osb_attn_short and osb_attn_fp8 (attn_sm90.cu): null and empty problems, the
+// norm-weight and RoPE pairs, leading dimensions and alignment.  `who` names the entry point in the error message.
+int check_attn_short_args(const osb_attn_short_args* a, const char* who);
+
 #ifdef __CUDACC__
 __device__ __forceinline__ void unpack8(const uint4& t, float* x) {
   const uint32_t tw[4] = {t.x, t.y, t.z, t.w};

@@ -12,9 +12,9 @@
 // K-major / MN-major with the 128-byte swizzle, the tail as no-swizzle core matrices) or through ldmatrix / .trans.
 // Producers: the head-tile epilogue of gemm_bf16_kernel (bias + per-head RMSNorm + RoPE fused, gemm_sm90.cu) and the
 // staging step of attn_short_kernel.  Consumers: attn_tiles_kernel (wgmma), attn_short_kernel (ldmatrix + mma.sync),
-// both in attn_sm90.cu, and head_tiles_fp8_kernel (attn_tiles_fp8_sm90.cu).
+// both in attn_sm90.cu, and head_tiles_fp8_kernel (attn_fp8_sm90.cu).
 //
-// FP8 head tiles (osb_head_tiles_fp8 -> osb_attn_tiles_fp8, attn_tiles_fp8_sm90.cu): every bf16 tile has an e4m3 twin
+// FP8 head tiles (osb_head_tiles_fp8 -> osb_attn_tiles_fp8, attn_fp8_sm90.cu): every bf16 tile has an e4m3 twin
 // of 128 rows x 128 bytes (kTileF8Bytes), again the shared-memory image of a wgmma operand: K-major rows of 128 bytes
 // in the 128-byte swizzle (byte c of row r at r * 128 + (((c / 16) ^ (r % 8)) * 16) + c % 16), loaded by one bulk copy.
 //   q / k tile: row = tile row (token), byte = channel; channels >= D and rows >= tile_rows hold zero codes.  The head
@@ -55,27 +55,26 @@ struct TileMap {
   int32_t mode, L, S, T, G, tps, TR;
 };
 
-__host__ __device__ inline void tile_of_row(const TileMap& m, int64_t row, int64_t& tile, int& r) {
-  int64_t seq;
-  int pos;
+// 32-bit arithmetic: the host requires fewer than 2^31 token rows
+__host__ __device__ __forceinline__ void tile_of_row(const TileMap& m, uint32_t row, uint32_t& tile, uint32_t& pos, int& r) {
+  uint32_t seq;
   if (m.mode == 0) {
-    seq = row / m.L;
-    pos = (int)(row - seq * m.L);
+    seq = row / (uint32_t)m.L;
+    pos = row - seq * (uint32_t)m.L;
   } else {
-    const int64_t ts = (int64_t)m.T * m.S;
-    const int64_t b = row / ts;
-    const int64_t rem = row - b * ts;
-    const int t = (int)(rem / m.S);
-    seq = b * m.S + (rem - (int64_t)t * m.S);
-    pos = t;
+    const uint32_t ts = (uint32_t)m.T * (uint32_t)m.S;
+    const uint32_t b = row / ts;
+    const uint32_t rem = row - b * ts;
+    pos = rem / (uint32_t)m.S;
+    seq = b * (uint32_t)m.S + (rem - pos * (uint32_t)m.S);
   }
   if (m.G > 1) {
-    tile = seq / m.G;
-    r = (int)(seq - tile * m.G) * m.L + pos;
+    tile = seq / (uint32_t)m.G;
+    r = (int)((seq - tile * (uint32_t)m.G) * (uint32_t)m.L + pos);
   } else {
-    const int j = pos / m.TR;
-    tile = seq * m.tps + j;
-    r = pos - j * m.TR;
+    const uint32_t jt = pos / (uint32_t)m.TR;
+    tile = seq * (uint32_t)m.tps + jt;
+    r = (int)(pos - jt * (uint32_t)m.TR);
   }
 }
 
@@ -115,6 +114,63 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst_smem, const void* src,
       "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
       : "memory");
 }
+
+// Key sets and output rows of the head-tile attention kernels (osb_attn_tiles, osb_attn_tiles_fp8).  Key set i belongs
+// to sequence i (G == 1: qmap.tps query tiles, nkb key tiles, Lk key slots clipped by kv_lens) or to query tile i
+// (G > 1: one key tile, the keys of its sequence g in the slots [g Lk, g Lk + Lk)).
+struct TileSets {
+  TileMap qmap;             // q tiles <-> rows of `out`
+  int32_t BK, nkb, Lk;      // key-tile rows, key tiles per set, keys per sequence
+  int64_t num_seqs, num_sets;
+  const int32_t* kv_lens;
+  __nv_bfloat16* out;
+  int64_t out_ld;
+  RowScatter out_sc;        // sequence parallel: output rows go straight to the consuming rank's buffer
+};
+
+// valid key slots of a set: packed tiles G * Lk, else Lk clipped by kv_lens
+__device__ __forceinline__ int tile_set_keys(const TileSets& t, int64_t set) {
+  int keys = t.qmap.G > 1 ? t.qmap.G * t.Lk : t.Lk;
+  if (t.qmap.G == 1 && t.kv_lens) { const int l = __ldg(t.kv_lens + set); keys = l < keys ? (l < 0 ? 0 : l) : keys; }
+  return keys;
+}
+
+// row r of query tile qt of `set` (keys = tile_set_keys(t, set)): its sequence and position, whether it holds a token,
+// and the key slots [lo, hi) it attends to (empty when it holds none)
+__device__ __forceinline__ void tile_query_row(const TileSets& t, int64_t set, int qt, int keys, int r, int64_t& seq,
+                                               int& pos, bool& valid, int& lo, int& hi) {
+  lo = hi = 0;
+  if (t.qmap.G > 1) {
+    const int g = r / t.qmap.L;
+    pos = r - g * t.qmap.L;
+    seq = set * t.qmap.G + g;
+    valid = g < t.qmap.G && seq < t.num_seqs;
+    if (valid) { lo = g * t.Lk; hi = lo + t.Lk; }
+  } else {
+    pos = qt * t.qmap.TR + r;
+    seq = set;
+    valid = r < t.qmap.TR && pos < t.qmap.L;
+    if (valid) hi = keys;
+  }
+}
+
+// first element of the output row of token `pos` of sequence `seq`: the inverse q map, then the optional scatter
+__device__ __forceinline__ __nv_bfloat16* tile_out_row(const TileSets& t, int64_t seq, int pos) {
+  int64_t orow = row_of_token(t.qmap, seq, pos);
+  __nv_bfloat16* obase = t.out;
+  if (t.out_sc.mode != 0) {
+    int peer;
+    scatter_row(t.out_sc, orow, peer, orow);
+    obase = static_cast<__nv_bfloat16*>(scatter_base(t.out_sc, peer));
+  }
+  return obase + orow * t.out_ld;
+}
+
+// Host checks shared by the entry points (attn_sm90.cu).  `who` names the entry point in the error message.
+// osb_tile_map -> TileMap
+int make_tile_map(TileMap* dst, const osb_tile_map& m, const char* who);
+// the key-set and output fields of osb_attn_tiles_args -> TileSets
+int make_tile_sets(TileSets* dst, const osb_attn_tiles_args* a, const char* who);
 #endif
 
 }  // namespace osb
