@@ -276,6 +276,36 @@ int osb_attn_short(const osb_attn_short_args* args, void* stream);
  * (opensora/models/text/conditioner.py:10-53). */
 int osb_attn_short_bias(const osb_attn_short_args* args, const float* bias, int64_t bias_head_stride, void* stream);
 
+/* ---- frame-causal attention of one 512-wide head (causal VAE mid block) ---------------------------------------------- */
+typedef struct osb_attn_frames_args {
+  const void* q; const void* k; const void* v;   /* bf16; element (row, d) at ptr + row * ld + d, d < 512            */
+  void* out;                                     /* bf16, rows mapped like q                                        */
+  int64_t q_ld, k_ld, v_ld, out_ld;              /* >= 512, multiples of 8 (q | k | v may be slices of one buffer)  */
+  int64_t q_batch_stride, k_batch_stride;        /* rows between samples (out uses q's, v uses k's)                 */
+  int64_t Lq, Lk;                                /* query / key tokens per sample                                   */
+  int32_t batch, head_dim;                       /* head_dim: 512, anything else is refused                         */
+  int32_t frame_tokens;                          /* hw: tokens per latent frame, any value >= 1                     */
+  int32_t q_frame0;                              /* global frame of query token 0 (frame-sharded VAE: `first`)      */
+  float softmax_scale;                           /* 512^-0.5                                                        */
+  int32_t reserved;
+} osb_attn_frames_args;
+
+/* out = softmax(q k^T * softmax_scale + frame mask) v for ONE head of 512 channels.  Query token i of a sample sees key
+ * j iff j < min(Lk, (q_frame0 + i / frame_tokens + 1) * frame_tokens): the mask of `prepare_causal_attention_mask` as a
+ * predicate, never a tensor; key blocks past a query tile's last visible key are not read.  With Lk > Lq and q_frame0 > 0
+ * the queries are a run of frames of a longer video whose keys / values were gathered (frame-sharded VAE).
+ * Arithmetic: scores in fp32 in log2 units, exact online softmax over 128-key blocks with a guarded running maximum,
+ * P rounded to bf16 unnormalised, O accumulated and rescaled in fp32, one rounding at the output.  Deterministic (no
+ * atomics, keys are never split across CTAs).  One CTA per 64 query rows: wgmma for both products, q / k / v loaded by TMA
+ * as they lie in memory (v is never transposed).
+ * Refused before any launch: head_dim != 512, an ld below 512 or not a multiple of 8, pointers not 16-byte aligned,
+ * frame_tokens < 1, batch < 1, Lq < 1, batch strides that are negative or shorter than the sample, softmax_scale <= 0,
+ * and q_frame0 < 0 or Lk < 1 (some query would see no key).
+ * Replaces the mid-block attention of the reference's causal VAE: the mask of
+ * opensora/models/hunyuan_vae/unet_causal_3d_blocks.py:52-60, the one-head Attention built at :311-325 and its call at
+ * :349-352 (diffusers' AttnProcessor2_0 -> scaled_dot_product_attention with that mask). */
+int osb_attn_frames(const osb_attn_frames_args* args, void* stream);
+
 /* ---- RMSNorm with weight (T5LayerNorm) ----------------------------------------------------------------------------- */
 /* y[r,:] = bf16(w * bf16(x[r,:] * rsqrt(mean(x[r,:]^2) + eps))): fp32 mean of squares, the reference's two roundings
  * (opensora/acceleration/shardformer/modeling/t5.py:14-27).  x, y: bf16 [rows, C] contiguous, w: bf16 [C].

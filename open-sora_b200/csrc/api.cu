@@ -40,8 +40,10 @@ int sm_count() { return g_sms; }
 struct TmapKey {
   uint64_t base, rows, cols, ld, box;
   uint32_t elem_bytes;
+  uint64_t batch, batch_ld;   // 3D maps (one matrix per sample); 0, 0 for a 2D map
   bool operator==(const TmapKey& o) const {
-    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box && elem_bytes == o.elem_bytes;
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box && elem_bytes == o.elem_bytes &&
+           batch == o.batch && batch_ld == o.batch_ld;
   }
 };
 struct TmapKeyHash {
@@ -51,6 +53,8 @@ struct TmapKeyHash {
     h ^= (k.cols + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
     h ^= (k.ld + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
     h ^= (k.box + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
+    h ^= (k.batch + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
+    h ^= (k.batch_ld + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
     return (size_t)h;
   }
 };
@@ -58,14 +62,15 @@ static std::mutex g_tmap_mu;
 static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> g_tmap_cache;
 static std::atomic<int64_t> g_tmap_hits{0}, g_tmap_misses{0};
 
-// elem_bytes 2: bf16, 1: e4m3 (ld and cols in elements; the swizzle row is 128 bytes either way)
+// elem_bytes 2: bf16, 1: e4m3 (ld and cols in elements; the swizzle row is 128 bytes either way).  batch > 0: a 3D map
+// over `batch` matrices batch_ld elements apart, the box one sample deep.
 static int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
-                        uint32_t box_cols, uint32_t elem_bytes) {
+                        uint32_t box_cols, uint32_t elem_bytes, uint64_t batch = 0, uint64_t batch_ld = 0) {
   if (!g_encode) {
     set_error("osb_init() has not been called");
     return OSB_ERR_NOT_INIT;
   }
-  const TmapKey key{reinterpret_cast<uint64_t>(base), rows, cols, ld, ((uint64_t)box_rows << 32) | box_cols, elem_bytes};
+  const TmapKey key{reinterpret_cast<uint64_t>(base), rows, cols, ld, ((uint64_t)box_rows << 32) | box_cols, elem_bytes, batch, batch_ld};
   {
     std::lock_guard<std::mutex> lk(g_tmap_mu);
     auto it = g_tmap_cache.find(key);
@@ -76,24 +81,24 @@ static int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint6
     }
   }
   g_tmap_misses.fetch_add(1, std::memory_order_relaxed);
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * elem_bytes) & 15)) {
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((ld * elem_bytes) & 15) || ((batch_ld * elem_bytes) & 15)) {
     set_error("TMA operand must be 16-byte aligned (base %p, ld %llu elements)", base,
               (unsigned long long)ld);
     return OSB_ERR_INVALID;
   }
-  cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstride[1] = {ld * elem_bytes};  // bytes, dims 1..rank-1
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estride[2] = {1, 1};
-  CUresult r = g_encode(map, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+  cuuint64_t gdim[3] = {cols, rows, batch};
+  cuuint64_t gstride[2] = {ld * elem_bytes, batch_ld * elem_bytes};  // bytes, dims 1..rank-1
+  cuuint32_t box[3] = {box_cols, box_rows, 1};
+  cuuint32_t estride[3] = {1, 1, 1};
+  CUresult r = g_encode(map, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, batch ? 3 : 2,
                         const_cast<void*>(base), gdim,
                         gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows %llu cols %llu ld %llu box %ux%u)",
+    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows %llu cols %llu ld %llu box %ux%u batch %llu x %llu)",
               (int)r, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld,
-              box_rows, box_cols);
+              box_rows, box_cols, (unsigned long long)batch, (unsigned long long)batch_ld);
     return OSB_ERR_CUDA;
   }
   {
@@ -112,6 +117,11 @@ int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_
 int make_tmap_2d_e4m3(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
                       uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
   return make_tmap_2d(map, base, rows, cols, ld, box_rows, box_cols, 1);
+}
+
+int make_tmap_3d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint64_t batch,
+                      uint64_t batch_ld, uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(map, base, rows, cols, ld, box_rows, box_cols, 2, batch, batch_ld);
 }
 
 int make_tmap_5d_bf16(CUtensorMap* map, const void* base, const uint64_t dims[5], const uint64_t strides_bytes[4],
@@ -173,6 +183,7 @@ int make_row_scatter(RowScatter* dst, const osb_scatter* src, int64_t rows, cons
 int gemm_init();   // gemm_sm90.cu
 int attn_init();   // attn_sm90.cu
 int attn_fp8_init();   // attn_fp8_sm90.cu
+int attn_frames_init();   // attn_frames_sm90.cu
 
 }  // namespace osb
 
@@ -217,6 +228,8 @@ int osb_init(int device) {
   rc = attn_init();
   if (rc) return rc;
   rc = attn_fp8_init();
+  if (rc) return rc;
+  rc = attn_frames_init();
   if (rc) return rc;
   g_init = true;
   return OSB_OK;

@@ -74,6 +74,11 @@ int make_tmap_2d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_
 int make_tmap_2d_e4m3(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
                       uint64_t ld, uint32_t box_rows, uint32_t box_cols);
 
+// `batch` such bf16 matrices `batch_ld` ELEMENTS apart as a 3D map (column, row, sample): rows past `rows` of a sample
+// are zero filled, never the next sample's.  Box = box_rows x 64 columns of one sample, 128-byte swizzle.
+int make_tmap_3d_bf16(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint64_t batch,
+                      uint64_t batch_ld, uint32_t box_rows, uint32_t box_cols);
+
 struct RowScatter;
 // validates an osb_scatter and copies it into the kernel-parameter form; rows = rows the producer writes
 int make_row_scatter(RowScatter* dst, const osb_scatter* src, int64_t rows, const char* who);
@@ -224,6 +229,15 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint32_t bar, 
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes "
       "[%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
+}
+// 3D tile load (a [rows, ld] matrix per sample: coordinates column, row, sample)
+__device__ __forceinline__ void tma_load_3d(const CUtensorMap* m, uint32_t bar, uint32_t dst, int32_t c0, int32_t c1,
+                                            int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 // 5D tile loads (NDHWC activations of the causal-conv VAE: coordinates c, w, h, t, n)

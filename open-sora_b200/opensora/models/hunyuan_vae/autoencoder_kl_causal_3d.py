@@ -114,6 +114,26 @@ class AutoencoderKLCausal3D(nn.Module):
         self.decoder.shard_group = process_group
         self.encoder.shard_group = process_group
 
+    def _mid_attentions(self):
+        return [a for part in (self.encoder, self.decoder) for a in part.mid_block.attentions if a is not None]
+
+    def enable_native_attention(self):
+        """Run the mid block's frame-causal attention (encoder and decoder, untiled, tiled and frame-sharded) as ONE
+        `osb_attn_frames` launch instead of one torch SDPA call per latent frame.  The kernel is built for one head of
+        512 channels - the width of every released checkpoint's mid block; any other width is refused here, never run
+        on another path.  Off by default: the default path still calls SDPA."""
+        for a in self._mid_attentions():
+            width = a.to_q.in_features
+            if width != 512:
+                raise ValueError(f"enable_native_attention: osb_attn_frames is built for a 512-wide mid block, this "
+                                 f"model's is {width} wide (block_out_channels[-1])")
+        for a in self._mid_attentions():
+            a.native = True
+
+    def disable_native_attention(self):
+        for a in self._mid_attentions():
+            a.native = False
+
     # ---- helpers -------------------------------------------------------------------------------------
     def _check(self):
         import osb200

@@ -250,6 +250,7 @@ class _MidAttention(nn.Module):
         self.to_k = nn.Linear(channels, channels)
         self.to_v = nn.Linear(channels, channels)
         self.to_out = nn.ModuleList([nn.Linear(channels, channels), nn.Dropout(0.0)])
+        self.native = False   # set by AutoencoderKLCausal3D.enable_native_attention: one osb_attn_frames call, no SDPA
 
     def forward(self, x):
         osb = _osb()
@@ -270,13 +271,18 @@ class _MidAttention(nn.Module):
             # per token) and the causal prefix of local frame f ends at global frame first + f
             k, v, first = _gather_frames(k, v, T, hw, shard)
         # Frame-causal attention (prepare_causal_attention_mask, :52-60): frame f attends to frames <= f, so the
-        # mask is never materialised - one un-masked SDPA per query frame over the key prefix.  LIBRARY kernel
-        # (torch SDPA, head_dim 512): the osb200 streaming attention for D=512 is the next kernel on this row.
-        o = torch.empty_like(q)
-        for f in range(T):
-            keys = (first + f + 1) * hw
-            o[:, :, f * hw:(f + 1) * hw] = torch.nn.functional.scaled_dot_product_attention(
-                q[:, :, f * hw:(f + 1) * hw], k[:, :, :keys], v[:, :, :keys])
+        # mask is never materialised.
+        if self.native:
+            # one osb_attn_frames launch (wgmma, head_dim 512): the mask is a predicate on (query frame, key) in the kernel
+            o = osb.attn_frames(q[:, 0], k[:, 0], v[:, 0], frame_tokens=hw, q_frame0=first).unsqueeze(1)
+        else:
+            # the default: one un-masked SDPA per query frame over the key prefix.  LIBRARY kernel (torch SDPA, head_dim
+            # 512), kept as the default until the native path has been measured against it on the benchmark's VAE leg.
+            o = torch.empty_like(q)
+            for f in range(T):
+                keys = (first + f + 1) * hw
+                o[:, :, f * hw:(f + 1) * hw] = torch.nn.functional.scaled_dot_product_attention(
+                    q[:, :, f * hw:(f + 1) * hw], k[:, :, :keys], v[:, :, :keys])
         out = osb.gemm(o.view(nb * T * hw, C), self.to_out[0].weight, self.to_out[0].bias, epilogue=osb.EPI_BIAS_GATE_RES,
                        residual=x.reshape(nb * T * hw, C))
         return out.view(nb, T, H, W, C)

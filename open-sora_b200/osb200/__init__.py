@@ -44,6 +44,7 @@ EXPORTS = (
     "osb_attn_fp8",
     "osb_head_tiles_fp8",
     "osb_attn_tiles_fp8",
+    "osb_attn_frames",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -87,6 +88,7 @@ def _load() -> C.CDLL:
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_attn_short_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     lib.osb_attn_fp8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.osb_attn_frames.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_rms_norm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_void_p]
     lib.osb_conv3d_ndhwc.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_vae_prep.argtypes = [C.c_void_p, C.c_void_p]
@@ -207,6 +209,17 @@ class AttnShortArgs(C.Structure):
         ("softmax_scale", C.c_float),
         ("q_norm_w2", C.c_void_p), ("k_norm_w2", C.c_void_p), ("norm_split", C.c_int32), ("reserved", C.c_int32),
         ("rope_half", C.c_int32), ("reserved2", C.c_int32),
+    ]
+
+
+class AttnFramesArgs(C.Structure):
+    _fields_ = [
+        ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("out", C.c_void_p),
+        ("q_ld", C.c_int64), ("k_ld", C.c_int64), ("v_ld", C.c_int64), ("out_ld", C.c_int64),
+        ("q_batch_stride", C.c_int64), ("k_batch_stride", C.c_int64),
+        ("Lq", C.c_int64), ("Lk", C.c_int64),
+        ("batch", C.c_int32), ("head_dim", C.c_int32), ("frame_tokens", C.c_int32), ("q_frame0", C.c_int32),
+        ("softmax_scale", C.c_float), ("reserved", C.c_int32),
     ]
 
 
@@ -714,6 +727,49 @@ def attn_short_bias(q, k, v, out, bias, *, num_seqs: int, seqs_per_batch: int, q
     with _Timed("attn_short", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):
         _check(_lib.osb_attn_short_bias(C.byref(a), _ptr(bias), n if bias.dim() == 2 else 0, _stream()),
                "osb_attn_short_bias")
+    return out
+
+
+def attn_frames(q, k, v, *, frame_tokens: int, q_frame0: int = 0, out=None, softmax_scale: float | None = None):
+    """Frame-causal attention of one head (osb_attn_frames): q [batch, Lq, D], k / v [batch, Lk, D] bf16, unit stride in
+    D, any row stride (column slices of one buffer are fine), k and v with the same batch stride.  Query token i sees key
+    j iff j < min(Lk, (q_frame0 + i // frame_tokens + 1) * frame_tokens).  Returns out [batch, Lq, D]."""
+    import torch
+
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
+        _need(t, torch.bfloat16, n)
+    if q.dim() != 3 or k.dim() != 3 or k.shape != v.shape or q.shape[0] != k.shape[0] or q.shape[2] != k.shape[2]:
+        raise OsbError(f"attn_frames: q [batch, Lq, D] and k, v [batch, Lk, D] expected, got {tuple(q.shape)}, "
+                       f"{tuple(k.shape)}, {tuple(v.shape)}")
+    nb, Lq, D = q.shape
+    if out is None:
+        out = torch.empty((nb, Lq, D), dtype=q.dtype, device=q.device)
+    if out.shape != q.shape:
+        raise OsbError(f"attn_frames: out must have q's shape {tuple(q.shape)}, got {tuple(out.shape)}")
+
+    def strides(t, name):
+        ld, bs = t.stride(1), t.stride(0)
+        if t.shape[1] == 1:
+            ld = max(ld, D)
+        if nb > 1 and bs % ld:
+            raise OsbError(f"attn_frames: the batch stride of {name} ({bs}) is not a multiple of its row stride ({ld})")
+        return ld, (bs // ld if nb > 1 else t.shape[1])
+
+    (q_ld, q_bs), (k_ld, k_bs), (v_ld, v_bs), (o_ld, o_bs) = strides(q, "q"), strides(k, "k"), strides(v, "v"), strides(out, "out")
+    if nb > 1 and (v_bs != k_bs or o_bs != q_bs):
+        raise OsbError("attn_frames: v must have k's batch stride and out q's (in rows)")
+    a = AttnFramesArgs()
+    a.q, a.k, a.v, a.out = q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr()
+    a.q_ld, a.k_ld, a.v_ld, a.out_ld = q_ld, k_ld, v_ld, o_ld
+    a.q_batch_stride, a.k_batch_stride = q_bs, k_bs
+    a.Lq, a.Lk = Lq, k.shape[1]
+    a.batch, a.head_dim, a.frame_tokens, a.q_frame0 = nb, D, frame_tokens, q_frame0
+    a.softmax_scale = softmax_scale if softmax_scale is not None else D ** -0.5
+    # FLOPs of the visible part only: row i multiplies min(Lk, (q_frame0 + i // hw + 1) hw) keys
+    full, rem = divmod(Lq, max(frame_tokens, 1))
+    keys = sum(min(k.shape[1], (q_frame0 + f + 1) * frame_tokens) * (frame_tokens if f < full else rem) for f in range(full + (rem > 0)))
+    with _Timed("attn_frames", 4.0 * nb * keys * D):
+        _check(_lib.osb_attn_frames(C.byref(a), _stream()), "osb_attn_frames")
     return out
 
 
