@@ -232,6 +232,25 @@ typedef struct osb_attn_fp8_workspace {
 struct osb_attn_short_args;   /* defined with osb_attn_short below */
 int osb_attn_fp8(const struct osb_attn_short_args* args, const osb_attn_fp8_workspace* ws, void* stream);
 
+/* Block-scaled e4m3 output of osb_attn_fp8.  With head_dim 128 one (row, head) of the output is one 1 x 128 block of
+ * the block quantization rule (osb_fp8_blocks_args): v = O_ic * s_v[c] / (256 * l_i) in fp32 (the value osb_attn_fp8
+ * rounds to bf16), s = amax_c(|v|) / 448 (1 for an all-zero block), codes e4m3_rn_satfinite(v / s) (IEEE division).
+ * Rows follow the row mapping of args->out:
+ *   codes   e4m3, element (row, h * 128 + c) at codes + row * codes_ld + h * 128 + c
+ *   scales  fp32, the scale of (row, h) at scales[row * scales_ld + h]
+ * With codes / scales pointing into the columns of a wider buffer the output fills part of the block-scaled A operand
+ * of osb_gemm_fp8_blocks (the attention half of linear2's input, or the input of an attention-output projection). */
+typedef struct osb_attn_fp8_out {
+  void* codes;       /* 16-byte aligned, codes_ld a multiple of 8           */
+  float* scales;     /* 4-byte aligned, scales_ld >= num_heads              */
+  int64_t codes_ld, scales_ld;
+} osb_attn_fp8_out;
+
+/* osb_attn_fp8 writing `out` instead of args->out (which is not read): the same three launches, workspace and refusals;
+ * the attention kernel quantizes in its epilogue. */
+int osb_attn_fp8_blocks(const struct osb_attn_short_args* args, const osb_attn_fp8_workspace* ws,
+                        const osb_attn_fp8_out* out, void* stream);
+
 /* ---- attention with short key sets (whole key set resident in one CTA) -------------------- */
 typedef struct osb_attn_short_args {
   const void* q; const void* k; const void* v; /* bf16; element (row, h*D + d) at ptr + row*ld + h*D + d */

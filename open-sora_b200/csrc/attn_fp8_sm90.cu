@@ -199,6 +199,11 @@ struct Fp8AttnMain {
   int64_t out_ld, q_bs, q_ts;
   int32_t L, Lpad, H, nkb;
   float sc;   // softmax_scale * log2(e)
+  // e4m3 output (osb_attn_fp8_blocks): codes of (row, head) at out8 + row * out8_ld + head * 128, scale at
+  // out_scale[row * scale_ld + head]
+  uint8_t* out8;
+  float* out_scale;
+  int64_t out8_ld, scale_ld;
 };
 
 __global__ void __launch_bounds__(128) attn_fp8_prep_kernel(const Fp8AttnPrep p) {
@@ -293,6 +298,8 @@ __global__ void __launch_bounds__(256) attn_fp8_vpack_kernel(const Fp8AttnPrep p
   pdl_launch_dependents();
 }
 
+// kOut8: the output leaves as e4m3 codes with one scale per (row, head) instead of bf16
+template <bool kOut8>
 __global__ void __launch_bounds__(kF8Threads, 1)
 attn_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_vt, const Fp8AttnMain p) {
@@ -389,17 +396,45 @@ attn_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   const int b = bh / p.H, head = bh - b * p.H;
   const float* sv = p.s_v + (int64_t)bh * kF8D;
+  if constexpr (kOut8) {
+    // The row's 128 channels (one 1 x 128 scale block) live in the 4 lanes of a quad: block amax by quad shuffles,
+    // s = amax / 448 (1 for a zero block), codes e4m3_rn_satfinite(v / s) with IEEE division.
 #pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    const int i = qt * kF8KB + r_loc + 8 * hh;
-    if (i >= p.L) continue;
-    __nv_bfloat16* dst = p.out + ((int64_t)b * p.q_bs + (int64_t)i * p.q_ts) * p.out_ld + (int64_t)head * kF8D;
+    for (int hh = 0; hh < 2; ++hh) {
+      const int i = qt * kF8KB + r_loc + 8 * hh;
+      float amax = 0.f;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int c = 8 * j + 2 * quad;
-      const float2 v = __ldg(reinterpret_cast<const float2*>(sv + c));
-      *reinterpret_cast<uint32_t*>(dst + c) =
-          pack_bf16x2(o[4 * j + 2 * hh] * v.x * inv[hh], o[4 * j + 2 * hh + 1] * v.y * inv[hh]);
+      for (int j = 0; j < 16; ++j) {
+        const float2 v = __ldg(reinterpret_cast<const float2*>(sv + 8 * j + 2 * quad));
+        o[4 * j + 2 * hh] = o[4 * j + 2 * hh] * v.x * inv[hh];
+        o[4 * j + 2 * hh + 1] = o[4 * j + 2 * hh + 1] * v.y * inv[hh];
+        amax = fmaxf(amax, fmaxf(fabsf(o[4 * j + 2 * hh]), fabsf(o[4 * j + 2 * hh + 1])));
+      }
+      amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+      amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+      if (i >= p.L) continue;
+      const float s = amax > 0.f ? amax / 448.0f : 1.0f;
+      const int64_t row = (int64_t)b * p.q_bs + (int64_t)i * p.q_ts;
+      uint8_t* dst = p.out8 + row * p.out8_ld + (int64_t)head * kF8D;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<uint16_t*>(dst + 8 * j + 2 * quad) =
+            (uint16_t)e4m3x2(o[4 * j + 2 * hh] / s, o[4 * j + 2 * hh + 1] / s);
+      if (quad == 0) p.out_scale[row * p.scale_ld + head] = s;
+    }
+  } else {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int i = qt * kF8KB + r_loc + 8 * hh;
+      if (i >= p.L) continue;
+      __nv_bfloat16* dst = p.out + ((int64_t)b * p.q_bs + (int64_t)i * p.q_ts) * p.out_ld + (int64_t)head * kF8D;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + 2 * quad;
+        const float2 v = __ldg(reinterpret_cast<const float2*>(sv + c));
+        *reinterpret_cast<uint32_t*>(dst + c) =
+            pack_bf16x2(o[4 * j + 2 * hh] * v.x * inv[hh], o[4 * j + 2 * hh + 1] * v.y * inv[hh]);
+      }
     }
   }
 }
@@ -602,7 +637,8 @@ __global__ void __launch_bounds__(kF8Threads, 1) attn_tiles_fp8_kernel(const Til
 }
 
 int attn_fp8_init() {
-  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kF8Smem));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_fp8_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF8Smem));
+  OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_fp8_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF8Smem));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_fp8_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTF8Smem));
   OSB_CHECK_CUDA(cudaFuncSetAttribute(attn_tiles_fp8_kernel<72>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTF8Smem));
   return OSB_OK;
@@ -610,27 +646,43 @@ int attn_fp8_init() {
 
 }  // namespace osb
 
-extern "C" int osb_attn_fp8(const osb_attn_short_args* a, const osb_attn_fp8_workspace* ws, void* stream) {
-  using namespace osb;
+namespace osb {
+namespace {
+
+// osb_attn_fp8 (o8 == nullptr: bf16 out) and osb_attn_fp8_blocks (e4m3 codes + block scales through o8)
+int attn_fp8_launch(const osb_attn_short_args* a, const osb_attn_fp8_workspace* ws, const osb_attn_fp8_out* o8,
+                    void* stream, const char* who) {
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
-  const int rc0 = check_attn_short_args(a, "osb_attn_fp8");
+  osb_attn_short_args chk;
+  if (o8 != nullptr) {   // the codes take the place of out in the argument checks
+    OSB_REQUIRE(a != nullptr, "%s: null args", who);
+    OSB_REQUIRE(o8->codes && o8->scales, "%s: null output codes or scales", who);
+    OSB_REQUIRE((reinterpret_cast<uintptr_t>(o8->scales) & 3) == 0 && o8->scales_ld >= a->num_heads,
+                "%s: scales must be 4-byte aligned with a row stride >= num_heads (%lld < %d)", who,
+                (long long)o8->scales_ld, a->num_heads);
+    chk = *a;
+    chk.out = o8->codes;
+    chk.out_ld = o8->codes_ld;
+    a = &chk;
+  }
+  const int rc0 = check_attn_short_args(a, who);
   if (rc0) return rc0;
-  OSB_REQUIRE(ws != nullptr, "osb_attn_fp8: null workspace");
-  OSB_REQUIRE(a->head_dim == kF8D, "osb_attn_fp8: head_dim %d not built (128)", a->head_dim);
-  OSB_REQUIRE(a->Lq == a->Lk, "osb_attn_fp8: self-attention only (Lq %d != Lk %d)", a->Lq, a->Lk);
-  OSB_REQUIRE(a->kv_lens == nullptr, "osb_attn_fp8: kv_lens is not supported");
-  OSB_REQUIRE(a->seqs_per_batch == 1, "osb_attn_fp8: one sequence per batch element (seqs_per_batch %lld)",
+  OSB_REQUIRE(ws != nullptr, "%s: null workspace", who);
+  OSB_REQUIRE(a->head_dim == kF8D, "%s: head_dim %d not built (128)", who, a->head_dim);
+  OSB_REQUIRE(a->Lq == a->Lk, "%s: self-attention only (Lq %d != Lk %d)", who, a->Lq, a->Lk);
+  OSB_REQUIRE(a->kv_lens == nullptr, "%s: kv_lens is not supported", who);
+  OSB_REQUIRE(a->seqs_per_batch == 1, "%s: one sequence per batch element (seqs_per_batch %lld)", who,
               (long long)a->seqs_per_batch);
   const int64_t BH = a->num_seqs * a->num_heads;
   const int32_t L = a->Lq, Lpad = (L + kF8KB - 1) / kF8KB * kF8KB;
-  OSB_REQUIRE(ws->q8 && ws->k8 && ws->vt8 && ws->s_q && ws->s_k && ws->s_v && ws->v_amax, "osb_attn_fp8: null workspace buffer");
+  OSB_REQUIRE(ws->q8 && ws->k8 && ws->vt8 && ws->s_q && ws->s_k && ws->s_v && ws->v_amax, "%s: null workspace buffer", who);
   OSB_REQUIRE(((reinterpret_cast<uintptr_t>(ws->q8) | reinterpret_cast<uintptr_t>(ws->k8) | reinterpret_cast<uintptr_t>(ws->vt8) |
                 reinterpret_cast<uintptr_t>(ws->s_q) | reinterpret_cast<uintptr_t>(ws->s_k) | reinterpret_cast<uintptr_t>(ws->s_v) |
-                reinterpret_cast<uintptr_t>(ws->v_amax)) & 15) == 0, "osb_attn_fp8: workspace buffers must be 16-byte aligned");
+                reinterpret_cast<uintptr_t>(ws->v_amax)) & 15) == 0, "%s: workspace buffers must be 16-byte aligned", who);
   OSB_REQUIRE(BH <= ws->capacity_bh && Lpad <= ws->capacity_lpad,
-              "osb_attn_fp8: workspace for %lld x %lld holds less than %lld sequence-heads x %d padded tokens",
-              (long long)ws->capacity_bh, (long long)ws->capacity_lpad, (long long)BH, Lpad);
-  OSB_REQUIRE(BH <= 65535 && BH * Lpad < (1ll << 31), "osb_attn_fp8: problem too large (%lld sequence-heads of %d)",
+              "%s: workspace for %lld x %lld holds less than %lld sequence-heads x %d padded tokens",
+              who, (long long)ws->capacity_bh, (long long)ws->capacity_lpad, (long long)BH, Lpad);
+  OSB_REQUIRE(BH <= 65535 && BH * Lpad < (1ll << 31), "%s: problem too large (%lld sequence-heads of %d)", who,
               (long long)BH, Lpad);
 
   Fp8AttnPrep pp = {};
@@ -666,6 +718,13 @@ extern "C" int osb_attn_fp8(const osb_attn_short_args* a, const osb_attn_fp8_wor
   pm.out_ld = a->out_ld; pm.q_bs = a->q_batch_stride; pm.q_ts = a->q_tok_stride;
   pm.L = L; pm.Lpad = Lpad; pm.H = a->num_heads; pm.nkb = Lpad / kF8KB;
   pm.sc = a->softmax_scale * 1.4426950408889634f;
+  if (o8 != nullptr) {
+    pm.out = nullptr;
+    pm.out8 = static_cast<uint8_t*>(o8->codes);
+    pm.out_scale = o8->scales;
+    pm.out8_ld = o8->codes_ld;
+    pm.scale_ld = o8->scales_ld;
+  }
 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   cudaLaunchAttribute attr[2];
@@ -674,9 +733,24 @@ extern "C" int osb_attn_fp8(const osb_attn_short_args* a, const osb_attn_fp8_wor
   cfg = launch_config(dim3((unsigned)(Lpad / kF8KB), (unsigned)BH), dim3(256), 0, s, attr);
   OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_vpack_kernel, pp));
   cfg = launch_config(dim3((unsigned)(Lpad / kF8KB), (unsigned)BH), dim3(kF8Threads), kF8Smem, s, attr);
-  OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_kernel, tq, tk, tv, pm));
+  if (o8 != nullptr) { OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_kernel<true>, tq, tk, tv, pm)); }
+  else { OSB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn_fp8_kernel<false>, tq, tk, tv, pm)); }
   count_launch(3);
   return OSB_OK;
+}
+
+}  // namespace
+}  // namespace osb
+
+extern "C" int osb_attn_fp8(const osb_attn_short_args* a, const osb_attn_fp8_workspace* ws, void* stream) {
+  return osb::attn_fp8_launch(a, ws, nullptr, stream, "osb_attn_fp8");
+}
+
+extern "C" int osb_attn_fp8_blocks(const osb_attn_short_args* a, const osb_attn_fp8_workspace* ws,
+                                   const osb_attn_fp8_out* out, void* stream) {
+  using namespace osb;
+  OSB_REQUIRE(out != nullptr, "osb_attn_fp8_blocks: null output args");
+  return attn_fp8_launch(a, ws, out, stream, "osb_attn_fp8_blocks");
 }
 
 extern "C" int osb_head_tiles_fp8(const osb_head_tiles_fp8_args* a, void* stream) {

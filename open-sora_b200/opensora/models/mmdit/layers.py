@@ -26,7 +26,14 @@ processors on `vec` (`_osb_fp8`, an `Fp8State`).
 
 FP8 attention (MMDiTModel.enable_fp8_attention, independent of the FP8 MLPs): the joint self-attention runs on
 `osb_attn_fp8` (q / k quantized per token and head after QK-norm and RoPE, v per channel, P as e4m3(256 p)) instead of
-`osb_attn_short`, with the workspaces on `vec` (`_osb_fp8_attn`, an `Fp8AttnState`).  No Linear changes."""
+`osb_attn_short`, with the workspaces on `vec` (`_osb_fp8_attn`, an `Fp8AttnState`).  No Linear changes.
+
+FP8 projections (MMDiTModel.enable_fp8(projections=True), `Fp8State.proj`): every block Linear runs on e4m3.  Double
+blocks, per stream: ln_modulate_fp8 -> the q|k|v GEMM on per-row A (`osb_gemm_fp8_blocks`, bf16 out) -> attention whose
+output leaves as e4m3 codes with 1 x 128 block scales (`osb_attn_fp8_blocks` with FP8 attention on, else the bf16
+attention and `osb_quant_blocks_fp8`) -> `proj` on block-scaled A (gate + residual).  Single blocks: ONE ln_modulate_fp8
+pass feeds the qkv GEMM and the mlp GEMM, the attention output fills columns 0..C-1 of the e4m3 cat buffer the same
+way, and no bf16 LN pass runs."""
 from __future__ import annotations
 
 import math
@@ -227,22 +234,41 @@ class Fp8AttnState:
 
 
 def _attention(osb, fp8_attn: Fp8AttnState | None, q, k, v, out, B: int, L: int, H: int, D: int, norm_split: int,
-               attn_kw: dict) -> None:
-    """Joint self-attention of B sequences of L tokens: `osb_attn_short`, or `osb_attn_fp8` when FP8 attention is on."""
+               attn_kw: dict, out_scale: Tensor | None = None) -> None:
+    """Joint self-attention of B sequences of L tokens: `osb_attn_short`, or `osb_attn_fp8` when FP8 attention is on
+    (`osb_attn_fp8_blocks` with `out_scale`: e4m3 `out`, one scale per (token, head))."""
     kw = dict(num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H,
               head_dim=D, norm_split=norm_split, **attn_kw)
     if fp8_attn is None:
         osb.attn_short(q, k, v, out, **kw)
+    elif out_scale is not None:
+        osb.attn_fp8_blocks(q, k, v, out, out_scale, workspace=fp8_attn.workspace(osb, B, L, H, q.device), **kw)
     else:
         osb.attn_fp8(q, k, v, out, workspace=fp8_attn.workspace(osb, B, L, H, q.device), **kw)
 
 
+def _attention_e4m3(osb, fp8_attn: Fp8AttnState | None, q, k, v, out8, B: int, L: int, H: int, D: int,
+                    norm_split: int, attn_kw: dict) -> None:
+    """`_attention` written as e4m3 codes with 1 x 128 block scales into out8 = (codes [rows, H*D], scales
+    [rows, H*D / 128]): by the FP8 attention kernel itself, or after the bf16 attention by `osb_quant_blocks_fp8`."""
+    if fp8_attn is not None:
+        _attention(osb, fp8_attn, q, k, v, out8[0], B, L, H, D, norm_split, attn_kw, out_scale=out8[1])
+        return
+    ao = torch.empty(B * L, H * D, dtype=q.dtype, device=q.device)
+    _attention(osb, None, q, k, v, ao, B, L, H, D, norm_split, attn_kw)
+    osb.quant_blocks_fp8(ao, out=out8[0], out_scale=out8[1])
+
+
 def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D: int, attn_kw: dict, norm_split_full: int,
-                  dtype, device, fp8_attn: Fp8AttnState | None = None) -> Tensor:
+                  dtype, device, fp8_attn: Fp8AttnState | None = None, out8=None) -> Tensor | None:
     """softmax(q k^T) v over the FULL joint sequence from this rank's [B*Lloc, 3*H*D] q|k|v rows: heads are scattered and
     the sequence gathered with one all-to-all (q, k, v travel together), attention runs on H/P heads, and the output comes
     back with the inverse exchange.  Without a group it is the plain local attention.  With `fp8_attn` the attention
-    itself runs on FP8 operands (it sees the whole sequence of its heads either way)."""
+    itself runs on FP8 operands (it sees the whole sequence of its heads either way).
+    With out8 = (codes, scales) the output is written there as e4m3 with 1 x 128 block scales (`_attention_e4m3`) and
+    None is returned; the inverse exchange then carries the codes (as bytes) and the per-(token, head) scales of the FP8
+    attention, or the bf16 rows that are quantized after it.  A (token, head) block is quantized alone either way, so
+    the codes equal the single-rank ones."""
     import torch.distributed as dist
 
     from opensora.acceleration.communications import all_to_all
@@ -250,6 +276,10 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
     g = _sp_group()
     P = dist.get_world_size(g) if g is not None else 1
     C = H * D
+    if P == 1 and out8 is not None:
+        _attention_e4m3(osb, fp8_attn, qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out8, B, Lloc, H, D, norm_split_full,
+                        attn_kw)
+        return None
     if P == 1:
         ao = torch.empty(B * Lloc, out_cols, dtype=dtype, device=device)
         _attention(osb, fp8_attn, qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ao[:, :C], B, Lloc, H, D,
@@ -260,10 +290,22 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
     Hp, L = H // P, Lloc * P
     full = all_to_all(qkv.view(B, Lloc, 3, H, D), g, scatter_dim=3, gather_dim=1).reshape(B * L, 3 * Hp * D)
     Cp = Hp * D
+    if out8 is not None and fp8_attn is not None:
+        c8 = torch.empty(B * L, Cp, dtype=torch.float8_e4m3fn, device=device)
+        s8 = torch.empty(B * L, Hp, dtype=torch.float32, device=device)
+        _attention(osb, fp8_attn, full[:, :Cp], full[:, Cp:2 * Cp], full[:, 2 * Cp:], c8, B, L, Hp, D, norm_split_full,
+                   attn_kw, out_scale=s8)
+        back8 = all_to_all(c8.view(torch.uint8).view(B, L, Hp, D), g, scatter_dim=1, gather_dim=2)
+        out8[0].copy_(back8.view(torch.float8_e4m3fn).reshape(B * Lloc, C))
+        out8[1].copy_(all_to_all(s8.view(B, L, Hp), g, scatter_dim=1, gather_dim=2).reshape(B * Lloc, H))
+        return None
     ao_full = torch.empty(B * L, Cp, dtype=dtype, device=device)
     _attention(osb, fp8_attn, full[:, :Cp], full[:, Cp:2 * Cp], full[:, 2 * Cp:], ao_full, B, L, Hp, D, norm_split_full,
                attn_kw)
     back = all_to_all(ao_full.view(B, L, Hp, D), g, scatter_dim=1, gather_dim=2).reshape(B * Lloc, C)
+    if out8 is not None:
+        osb.quant_blocks_fp8(back, out=out8[0], out_scale=out8[1])
+        return None
     if out_cols == C:
         return back
     ao = torch.empty(B * Lloc, out_cols, dtype=dtype, device=device)
@@ -272,11 +314,58 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
 
 
 class Fp8State:
-    """What the FP8 MLP path of one MMDiTModel keeps: e4m3 weights with per-output-channel scales, quantized once per
-    block and MLP (`weights`), and e4m3 / scale workspaces reused by every block, one per shape (`buf`)."""
+    """What the FP8 path of one MMDiTModel keeps: e4m3 weights with per-output-channel scales, quantized once per block
+    and MLP (`weights`) and, with `proj`, per block and stream for the q|k|v and attention-output projections
+    (`proj_weights`), and e4m3 / scale workspaces reused by every block, one per shape (`buf`)."""
 
-    def __init__(self):
+    def __init__(self, proj: bool = False):
+        self.proj = proj
         self._w, self._ws = {}, {}
+
+    @staticmethod
+    def proj_linears(blk: nn.Module, kind: str):
+        """The Linears holding the projections of the FP8 projection path: the q|k|v Linears and `proj` of one stream
+        (kind "img" / "txt"), or linear1 (q_proj, k_proj, v_mlp) of a single block, which hold its q|k|v rows."""
+        if kind != "single":
+            sa = blk.img_attn if kind == "img" else blk.txt_attn
+            qkv = (sa.qkv,) if getattr(sa, "fused_qkv", hasattr(sa, "qkv")) else (sa.q_proj, sa.k_proj, sa.v_proj)
+            return qkv + (sa.proj,)
+        if getattr(blk, "fused_qkv", hasattr(blk, "linear1")):
+            return (blk.linear1,)
+        return (blk.q_proj, blk.k_proj, blk.v_mlp)
+
+    def proj_weights(self, osb, blk: nn.Module, kind: str):
+        """(q|k|v e4m3 [3C, C], scales [3C], bias or None, proj e4m3 [C, C], scales [C], bias) of one stream of a double
+        block; the last three are None for a single block.  q|k|v rows in the order of the bf16 path's packing."""
+        key = (id(blk), kind, "proj")
+        hit = self._w.get(key)
+        if hit is None or hit[0] is not blk:
+            lins = self.proj_linears(blk, kind)
+            for lin in lins:
+                if adapter_of(lin) is not None:
+                    raise ValueError("FP8 projections: a LoRA / DoRA adapter on a projection Linear cannot run on the FP8 "
+                                     "path; unload_lora or disable_fp8 first")
+            if kind != "single":
+                qkv, proj = lins[:-1], lins[-1]
+                C = proj.out_features
+                w = qkv[0].weight if len(qkv) == 1 else torch.cat([lin.weight for lin in qkv], 0)
+                b = None if qkv[0].bias is None else (
+                    qkv[0].bias if len(qkv) == 1 else torch.cat([lin.bias for lin in qkv], 0).contiguous())
+            else:
+                C = blk.linear2.out_features
+                if len(lins) == 1:
+                    w, b = lins[0].weight[:3 * C], lins[0].bias[:3 * C]
+                else:
+                    w = torch.cat([lins[0].weight, lins[1].weight, lins[2].weight[:C]], 0)
+                    b = torch.cat([lins[0].bias, lins[1].bias, lins[2].bias[:C]], 0).contiguous()
+                proj = None
+            wq, sq = osb.quant_blocks_fp8(w, block=C)
+            pw = (None, None, None)
+            if proj is not None:
+                wp, sp = osb.quant_blocks_fp8(proj.weight, block=C)
+                pw = (wp, sp.view(-1), proj.bias)
+            hit = self._w[key] = (blk, (wq, sq.view(-1), b) + pw)
+        return hit[1]
 
     @staticmethod
     def mlp_linears(blk: nn.Module, kind: str):
@@ -325,6 +414,20 @@ def _mlp_fp8(osb, fp8: Fp8State, blk: nn.Module, kind: str, x: Tensor, mod, n: i
                                  out_scale=fp8.buf("hs", rows, hid // 128, device=dev))
     osb.gemm_fp8_blocks(h8, hs, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x, gate=mod.gate, group_rows=n,
                         out=x)
+
+
+def _qkv_fp8(osb, fp8: Fp8State, blk: nn.Module, kind: str, x: Tensor, mod, n: int, qkv: Tensor, L: int,
+             off: int) -> tuple[Tensor, Tensor]:
+    """q|k|v = W_qkv ((1 + scale) * LN(x) + shift) + b on FP8 operands: one ln_modulate_fp8 pass (codes + row scales,
+    returned) and, per sample of n rows, one row-scaled e4m3 GEMM into rows b*L + off .. of the joint buffer `qkv`."""
+    wq, sq, bq = fp8.proj_weights(osb, blk, kind)[:3]
+    rows, C = x.shape
+    dev, f8 = x.device, torch.float8_e4m3fn
+    x8, xs = osb.ln_modulate_fp8(x, mod.shift, mod.scale, group_rows=n, out=fp8.buf("x8", rows, C, dtype=f8, device=dev),
+                                 out_scale=fp8.buf("xs", rows, device=dev))
+    for b in range(rows // n):
+        osb.gemm_fp8_blocks(x8[b * n:(b + 1) * n], xs[b * n:(b + 1) * n], wq, sq, bq, out=qkv[b * L + off:b * L + off + n])
+    return x8, xs
 
 
 class _ProcessorBase:
@@ -395,6 +498,50 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
         img2, txt2 = img.reshape(B * Li, C).contiguous(), txt.reshape(B * Lt, C).contiguous()
         # q|k|v of both streams land in ONE joint [B*(Lt+Li), 3C] buffer in txt-then-img token order (layers.py:240-242)
         qkv = torch.empty(B * L, 3 * C, dtype=img.dtype, device=img.device)
+        fp8 = getattr(vec, "_osb_fp8", None)
+        proj8 = fp8 is not None and fp8.proj
+        if proj8:
+            for x2, mod, n, off, kind in ((img2, im1, Li, Lt, "img"), (txt2, tm1, Lt, 0, "txt")):
+                if n:
+                    _qkv_fp8(osb, fp8, attn, kind, x2, mod, n, qkv, L, off)
+        else:
+            self._qkv_bf16(osb, attn, img2, txt2, im1, tm1, qkv, B, Li, Lt)
+        cos, sin, half = _rope(pe)
+        kw = dict(q_norm_w=attn.txt_attn.norm.query_norm.scale, k_norm_w=attn.txt_attn.norm.key_norm.scale,
+                  q_norm_w2=attn.img_attn.norm.query_norm.scale, k_norm_w2=attn.img_attn.norm.key_norm.scale,
+                  rope_cos=cos, rope_sin=sin, rope_half=half)
+        # tokens at joint position >= the FULL text length take the image stream's QK-norm weights
+        split_full = getattr(vec, "_osb_txt_len", Lt)
+        img_o, txt_o = torch.empty_like(img2), torch.empty_like(txt2)
+        if proj8:   # attention output as e4m3 + 1 x 128 block scales -> x + gate * proj(attn) on FP8 operands
+            rows, f8, dev = B * L, torch.float8_e4m3fn, img.device
+            ao8 = (fp8.buf("ao8", rows, C, dtype=f8, device=dev), fp8.buf("aos", rows, C // 128, device=dev))
+            _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img.dtype, dev, getattr(vec, "_osb_fp8_attn", None),
+                          out8=ao8)
+            for x2, x_o, mod, n, off, kind in ((img2, img_o, im1, Li, Lt, "img"), (txt2, txt_o, tm1, Lt, 0, "txt")):
+                wp, sp, bp = fp8.proj_weights(osb, attn, kind)[3:]
+                for b in range(B if n else 0):
+                    r = slice(b * L + off, b * L + off + n)
+                    osb.gemm_fp8_blocks(ao8[0][r], ao8[1][r], wp, sp, bp, epilogue=osb.EPI_BIAS_GATE_RES,
+                                        residual=x2[b * n:(b + 1) * n], gate=mod.gate[b:b + 1], out=x_o[b * n:(b + 1) * n])
+        else:
+            self._proj_bf16(osb, attn, qkv, kw, split_full, img2, txt2, img_o, txt_o, im1, tm1, vec, B, L, Li, Lt, H, D)
+        # x + gate * MLP((1 + scale) * LN(x) + shift)   (layers.py:248, 252)
+        for x_o, mod, mlp, n, kind in ((img_o, im2, attn.img_mlp, Li, "img"), (txt_o, tm2, attn.txt_mlp, Lt, "txt")):
+            if n == 0:
+                continue
+            if fp8 is not None:
+                _mlp_fp8(osb, fp8, attn, kind, x_o, mod, n)
+                continue
+            xm = osb.ln_modulate(x_o, mod.shift, mod.scale, group_rows=n)
+            hid = _gemm(osb, xm, *linear_parts(mlp[0]), epilogue=osb.EPI_BIAS_GELU_TANH)
+            _gemm(osb, hid, *linear_parts(mlp[2]), epilogue=osb.EPI_BIAS_GATE_RES, residual=x_o, gate=mod.gate,
+                  group_rows=n, out=x_o)
+        return img_o.view(B, Li, C), txt_o.view(B, Lt, C)
+
+    def _qkv_bf16(self, osb, attn, img2, txt2, im1, tm1, qkv, B, Li, Lt):
+        """q|k|v of both streams on bf16 GEMMs (with their adapters) into the joint buffer."""
+        L = Lt + Li
         wi, bi = self._qkv(attn, attn.img_attn, "img_qkv")
         wt, bt = self._qkv(attn, attn.txt_attn, "txt_qkv")
         li, lt = self._qkv_lora(attn.img_attn), self._qkv_lora(attn.txt_attn)
@@ -412,15 +559,13 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
             if Li:
                 _gemm(osb, xi[b * Li:(b + 1) * Li], wi, bi, li, None if ui is None else ui[b * Li:(b + 1) * Li],
                       out=qkv[b * L + Lt:(b + 1) * L])
-        cos, sin, half = _rope(pe)
-        kw = dict(q_norm_w=attn.txt_attn.norm.query_norm.scale, k_norm_w=attn.txt_attn.norm.key_norm.scale,
-                  q_norm_w2=attn.img_attn.norm.query_norm.scale, k_norm_w2=attn.img_attn.norm.key_norm.scale,
-                  rope_cos=cos, rope_sin=sin, rope_half=half)
-        # tokens at joint position >= the FULL text length take the image stream's QK-norm weights
-        split_full = getattr(vec, "_osb_txt_len", Lt)
-        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img.dtype, img.device,
+
+    @staticmethod
+    def _proj_bf16(osb, attn, qkv, kw, split_full, img2, txt2, img_o, txt_o, im1, tm1, vec, B, L, Li, Lt, H, D):
+        """Attention in bf16 out and x + gate * proj(attn) of both streams on bf16 GEMMs (with their adapters)."""
+        C = img2.shape[1]
+        ao = _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img2.dtype, img2.device,
                            getattr(vec, "_osb_fp8_attn", None))
-        img_o, txt_o = torch.empty_like(img2), torch.empty_like(txt2)
         # both output projections read `ao`: one down projection for their adapters
         pi, pt = attn.img_attn.proj, attn.txt_attn.proj
         lp = lora_pack([[(pi, 0, pi.out_features)], [(pt, 0, pt.out_features)]])
@@ -436,19 +581,6 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
                 _gemm(osb, ao[b * L:b * L + Lt], pt.weight, pt.bias, lpt, None if up is None else up[b * L:b * L + Lt],
                       epilogue=osb.EPI_BIAS_GATE_RES, residual=txt2[b * Lt:(b + 1) * Lt], gate=tm1.gate[b:b + 1],
                       out=txt_o[b * Lt:(b + 1) * Lt])
-        # x + gate * MLP((1 + scale) * LN(x) + shift)   (layers.py:248, 252)
-        fp8 = getattr(vec, "_osb_fp8", None)
-        for x_o, mod, mlp, n, kind in ((img_o, im2, attn.img_mlp, Li, "img"), (txt_o, tm2, attn.txt_mlp, Lt, "txt")):
-            if n == 0:
-                continue
-            if fp8 is not None:
-                _mlp_fp8(osb, fp8, attn, kind, x_o, mod, n)
-                continue
-            xm = osb.ln_modulate(x_o, mod.shift, mod.scale, group_rows=n)
-            hid = _gemm(osb, xm, *linear_parts(mlp[0]), epilogue=osb.EPI_BIAS_GELU_TANH)
-            _gemm(osb, hid, *linear_parts(mlp[2]), epilogue=osb.EPI_BIAS_GATE_RES, residual=x_o, gate=mod.gate,
-                  group_rows=n, out=x_o)
-        return img_o.view(B, Li, C), txt_o.view(B, Lt, C)
 
 
 class DoubleStreamBlock(nn.Module):
@@ -514,6 +646,9 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         D, M4 = C // H, attn.linear2.in_features - C
         mod, _ = self._modulation(osb, attn.modulation, vec)
         x2 = x.reshape(B * L, C).contiguous()
+        fp8 = getattr(vec, "_osb_fp8", None)
+        if fp8 is not None and fp8.proj:
+            return self._fp8_proj(osb, fp8, attn, x2, mod, B, L, C, H, D, pe, vec).view(B, L, C)
         xm = osb.ln_modulate(x2, mod.shift, mod.scale, group_rows=L)
         wq, bq, wm, bm = self._split_weights(attn)
         lo = self._split_lora(attn, M4)
@@ -523,7 +658,6 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         cos, sin, half = _rope(pe)
         kw = dict(q_norm_w=attn.norm.query_norm.scale, k_norm_w=attn.norm.key_norm.scale, rope_cos=cos, rope_sin=sin,
                   rope_half=half)
-        fp8 = getattr(vec, "_osb_fp8", None)
         if fp8 is not None:
             return self._fp8_tail(osb, fp8, attn, x2, qkv, mod, B, L, C, H, D, kw, vec).view(B, L, C)
         # [attn | gelu(mlp)] side by side: the attention output and the GELU GEMM write one [rows, C + 4C] buffer
@@ -532,6 +666,30 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         out = _gemm(osb, cat, *linear_parts(attn.linear2), epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
                     group_rows=L)
         return out.view(B, L, C)
+
+    @staticmethod
+    def _fp8_proj(osb, fp8: Fp8State, attn: nn.Module, x2: Tensor, mod, B: int, L: int, C: int, H: int, D: int, pe,
+                  vec: Tensor) -> Tensor:
+        """x + gate * linear2(cat(attn, gelu(mlp))) with every Linear on FP8: ONE ln_modulate_fp8 pass feeds the qkv GEMM
+        (bf16 q|k|v for the attention) and the mlp GEMM (GELU codes into columns C.. of the e4m3 cat buffer), the
+        attention output fills columns 0..C-1 as e4m3 with its block scales, and linear2 is one block-scaled FP8 GEMM."""
+        wq, sq, bq = fp8.proj_weights(osb, attn, "single")[:3]
+        wm, sm, bm, w2, s2, b2 = fp8.weights(osb, attn, "single")
+        rows, M4, dev, f8 = B * L, wm.shape[0], x2.device, torch.float8_e4m3fn
+        x8, xs = osb.ln_modulate_fp8(x2, mod.shift, mod.scale, group_rows=L,
+                                     out=fp8.buf("x8", rows, C, dtype=f8, device=dev), out_scale=fp8.buf("xs", rows, device=dev))
+        qkv = osb.gemm_fp8_blocks(x8, xs, wq, sq, bq)
+        cat8 = fp8.buf("cat8", rows, C + M4, dtype=f8, device=dev)
+        cats = fp8.buf("cats", rows, (C + M4) // 128, device=dev)
+        cos, sin, half = _rope(pe)
+        kw = dict(q_norm_w=attn.norm.query_norm.scale, k_norm_w=attn.norm.key_norm.scale, rope_cos=cos, rope_sin=sin,
+                  rope_half=half)
+        _sp_attention(osb, qkv, C, B, L, H, D, kw, 0, x2.dtype, dev, getattr(vec, "_osb_fp8_attn", None),
+                      out8=(cat8[:, :C], cats[:, :C // 128]))
+        osb.gemm_fp8_blocks(x8, xs, wm, sm, bm, epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=cat8[:, C:],
+                            out_scale=cats[:, C // 128:])
+        return osb.gemm_fp8_blocks(cat8, cats, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
+                                   group_rows=L)
 
     @staticmethod
     def _fp8_tail(osb, fp8: Fp8State, attn: nn.Module, x2: Tensor, qkv: Tensor, mod, B: int, L: int, C: int, H: int,

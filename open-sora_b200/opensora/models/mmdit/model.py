@@ -85,6 +85,7 @@ class MMDiTModel(nn.Module):
         self._pe_cache = None
         self._sp_group = None
         self._fp8 = False
+        self._fp8_proj = False
         self._fp8_state = None
         self._fp8_attn = False
         self._fp8_attn_state = None
@@ -205,13 +206,28 @@ class MMDiTModel(nn.Module):
         names = {id(m): n for n, m in self.named_modules()}
         return [names[id(lin)] for blk, kind in self._mlps() for lin in Fp8State.mlp_linears(blk, kind)[::2]]
 
-    def enable_fp8(self) -> None:
+    def fp8_proj_linears(self) -> list[str]:
+        """Names of the Linears the FP8 projection path (`enable_fp8(projections=True)`) reads: the q|k|v Linears
+        (qkv, or q_proj / k_proj / v_proj) and `proj` of both streams of the double blocks, and linear1 (or q_proj /
+        k_proj / v_mlp) of the single blocks, which hold their q|k|v rows."""
+        names = {id(m): n for n, m in self.named_modules()}
+        blocks = [(b, k) for b in self.double_blocks for k in ("img", "txt")] + [(b, "single") for b in self.single_blocks]
+        return [names[id(lin)] for blk, kind in blocks for lin in Fp8State.proj_linears(blk, kind)]
+
+    def enable_fp8(self, projections: bool = False) -> None:
         """Run the MLPs of every double and single block on FP8 (e4m3) tensor cores.  The weights are quantized per output
         channel (s = amax / 448) into a per-model cache; the bf16 parameters and the state dict stay as they are.  The fc1
         input is the fp32 LN+modulate row, quantized per row; the fc2 / linear2 input is quantized per 1 x 128 block by
         the fc1 GELU epilogue (and, for the attention half of linear2's input, by osb_quant_blocks_fp8)
         (include/osb200.h, osb_gemm_fp8_blocks).  Needs a hidden size and an MLP width that are multiples of 128 and a
-        hidden size of at most 4096 (the FP8 LN+modulate); LoRA / DoRA adapters on the MLP Linears are refused."""
+        hidden size of at most 4096 (the FP8 LN+modulate); LoRA / DoRA adapters on the MLP Linears are refused.
+
+        `projections=True` also runs the q|k|v projections and the attention-output `proj` of the double blocks and the
+        qkv part of linear1 of the single blocks on FP8: weights per output channel, the q|k|v GEMM input the fp32
+        LN+modulate row quantized per row (in a single block the same codes feed its qkv and mlp GEMMs), the `proj` /
+        linear2 attention input per 1 x 128 block (by the FP8 attention kernel itself when `enable_fp8_attention()` is on,
+        else by osb_quant_blocks_fp8).  Every block Linear then runs on FP8; modulation, embedders and the final layer
+        stay bf16.  LoRA / DoRA adapters on those projection Linears (`fp8_proj_linears()`) are refused as well."""
         C, hid = self.hidden_size, int(self.hidden_size * self.config.mlp_ratio)
         if C % 128 or hid % 128:
             raise ValueError(f"FP8 MLPs need the hidden size ({C}) and the MLP width ({hid}) to be multiples of 128 "
@@ -223,18 +239,25 @@ class MMDiTModel(nn.Module):
         if adapted:
             raise ValueError(f"FP8 MLPs cannot run LoRA / DoRA adapters on MLP Linears ({adapted[0]} has one): "
                              "unload_lora first")
-        state = Fp8State()
+        if projections:
+            adapted = [n for n in self.fp8_proj_linears() if adapter_of(mods[n]) is not None]
+            if adapted:
+                raise ValueError(f"FP8 projections cannot run LoRA / DoRA adapters on projection Linears ({adapted[0]} "
+                                 "has one): unload_lora first")
+        state = Fp8State(projections)
         w = self.img_in.weight
         if w.is_cuda:   # quantized now; a model not yet on the GPU quantizes at its first forward
             import osb200
 
             for blk, kind in self._mlps():
                 state.weights(osb200, blk, kind)
-        self._fp8_state, self._fp8 = state, True
+                if projections:
+                    state.proj_weights(osb200, blk, kind)
+        self._fp8_state, self._fp8, self._fp8_proj = state, True, projections
 
     def disable_fp8(self) -> None:
-        """Back to the bf16 MLPs; the FP8 weight copies and workspaces are released."""
-        self._fp8, self._fp8_state = False, None
+        """Back to the bf16 MLPs and projections; the FP8 weight copies and workspaces are released."""
+        self._fp8, self._fp8_proj, self._fp8_state = False, False, None
 
     # ---- FP8 (e4m3) attention -------------------------------------------------------------------------------------
     def enable_fp8_attention(self) -> None:
@@ -286,7 +309,7 @@ class MMDiTModel(nn.Module):
         self._grouped_modulation(vec)
         if self._fp8:
             if self._fp8_state is None:
-                self._fp8_state = Fp8State()
+                self._fp8_state = Fp8State(self._fp8_proj)
             vec._osb_fp8 = self._fp8_state
         if self._fp8_attn:
             if self._fp8_attn_state is None:

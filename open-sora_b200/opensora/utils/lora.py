@@ -341,6 +341,11 @@ def load_lora(model: nn.Module, path: str, scale: float = 1.0) -> nn.Module:
         if on_mlp:
             raise ValueError(f"the model runs FP8 MLPs, which take no LoRA / DoRA adapter on an MLP Linear "
                              f"(target '{on_mlp[0]}'): disable_fp8 first")
+    if getattr(model, "_fp8_proj", False):
+        on_proj = sorted({p[0] for p in plan} & set(model.fp8_proj_linears()))
+        if on_proj:
+            raise ValueError(f"the model runs FP8 projections, which take no LoRA / DoRA adapter on a projection Linear "
+                             f"(target '{on_proj[0]}'): disable_fp8 first")
     extra = sorted(set(weights) - used)
     if extra:
         raise ValueError(f"adapter weights hold {len(extra)} tensors no target uses, e.g. {extra[:3]}")

@@ -42,6 +42,7 @@ EXPORTS = (
     "osb_gemm_fp8_blocks",
     "osb_quant_blocks_fp8",
     "osb_attn_fp8",
+    "osb_attn_fp8_blocks",
     "osb_head_tiles_fp8",
     "osb_attn_tiles_fp8",
     "osb_attn_frames",
@@ -88,6 +89,7 @@ def _load() -> C.CDLL:
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_attn_short_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     lib.osb_attn_fp8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.osb_attn_fp8_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_attn_frames.argtypes = [C.c_void_p, C.c_void_p]
     lib.osb_rms_norm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_void_p]
     lib.osb_conv3d_ndhwc.argtypes = [C.c_void_p, C.c_void_p]
@@ -832,6 +834,44 @@ def attn_fp8(q, k, v, out, *, workspace: AttnFp8Workspace, num_seqs: int, seqs_p
     with _Timed("attn_fp8", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):  # QK^T + PV FLOPs
         _check(_lib.osb_attn_fp8(C.byref(a), C.byref(workspace.args), _stream()), "osb_attn_fp8")
     return out
+
+
+class AttnFp8Out(C.Structure):
+    _fields_ = [("codes", C.c_void_p), ("scales", C.c_void_p), ("codes_ld", C.c_int64), ("scales_ld", C.c_int64)]
+
+
+def attn_fp8_blocks(q, k, v, out, out_scale, *, workspace: AttnFp8Workspace, num_seqs: int, seqs_per_batch: int,
+                    q_strides, k_strides, Lq: int, Lk: int, num_heads: int, head_dim: int, kv_lens=None, q_norm_w=None,
+                    k_norm_w=None, norm_eps: float = 1e-6, rope_cos=None, rope_sin=None,
+                    softmax_scale: float | None = None, q_norm_w2=None, k_norm_w2=None, norm_split: int = 0,
+                    impl: int = 0, rope_half: bool = False):
+    """`attn_fp8` whose output leaves as e4m3 codes with one scale per (row, head), the 1 x 128 block rule
+    (osb_attn_fp8_blocks): `out` e4m3 [rows, >= H * 128] and `out_scale` fp32 [rows, >= H], both with a free row stride
+    and unit column stride (column slices of the A operand of a block-mode `gemm_fp8_blocks`).  Rows as `attn_fp8`
+    writes them.  Returns (out, out_scale)."""
+    import torch
+
+    if not isinstance(workspace, AttnFp8Workspace):
+        raise OsbError("attn_fp8_blocks: workspace must come from attn_fp8_workspace()")
+    _need(out, torch.float8_e4m3fn, "out"); _need(out_scale, torch.float32, "out_scale")
+    for t, n, w in ((out, "out", num_heads * head_dim), (out_scale, "out_scale", num_heads)):
+        if t is None or t.dim() != 2 or t.stride(1) != 1 or t.shape[1] < w:
+            raise OsbError(f"attn_fp8_blocks: {n} must be a 2-D tensor of >= {w} unit-stride columns, got "
+                           f"{None if t is None else (tuple(t.shape), t.stride())}")
+    a = _attn_short_struct(q, k, v, q, num_seqs=num_seqs, seqs_per_batch=seqs_per_batch, q_strides=q_strides,
+                           k_strides=k_strides, Lq=Lq, Lk=Lk, num_heads=num_heads, head_dim=head_dim, kv_lens=kv_lens,
+                           q_norm_w=q_norm_w, k_norm_w=k_norm_w, norm_eps=norm_eps, rope_cos=rope_cos, rope_sin=rope_sin,
+                           softmax_scale=softmax_scale, q_norm_w2=q_norm_w2, k_norm_w2=k_norm_w2, norm_split=norm_split,
+                           impl=impl, rope_half=rope_half)
+    a.out, a.out_ld = None, 0   # not read: the output goes through `o`
+    if workspace.q8.device != q.device:
+        raise OsbError(f"attn_fp8_blocks: the workspace is on {workspace.q8.device}, q on {q.device}")
+    o = AttnFp8Out()
+    o.codes, o.scales, o.codes_ld, o.scales_ld = out.data_ptr(), out_scale.data_ptr(), out.stride(0), out_scale.stride(0)
+    with _Timed("attn_fp8", 4.0 * num_seqs * Lq * Lk * num_heads * head_dim):  # QK^T + PV FLOPs
+        _check(_lib.osb_attn_fp8_blocks(C.byref(a), C.byref(workspace.args), C.byref(o), _stream()),
+               "osb_attn_fp8_blocks")
+    return out, out_scale
 
 
 # ---- head tiles: projection GEMM -> attention without a layout pass (include/osb200.h) ------------------------------
