@@ -1,16 +1,20 @@
 // bf16 GEMM for sm_90a:  D[M,N] = epilogue(A[M,K] * W[N,K]^T + bias)
 //
-// Warp-specialised kernel, one 128 x BLOCK_N output tile per CTA.  Warpgroup 0 is the producer: one thread streams
-// the A and W tiles with TMA into 128-byte-swizzled shared memory (BLOCK_K = 64 bf16 = one swizzle row) through a
-// ring of mbarrier-guarded stages.  Warpgroups 1 and 2 each own 64 accumulator rows: wgmma.mma_async reads both
-// operands straight from the swizzled tiles (matrix descriptors), the fp32 accumulator lives in registers and the
-// epilogue runs on those registers, so the accumulator never goes through memory before its single rounding to bf16.
+// Warp-specialised persistent kernel over 128 x BLOCK_N output tiles: one CTA per SM (at most), CTA b computes tiles
+// b, b + gridDim.x, b + 2 gridDim.x, ...  Warpgroup 0 is the producer: one thread streams the A and W tiles with TMA
+// into 128-byte-swizzled shared memory (BLOCK_K = 64 bf16 = one swizzle row) through a ring of mbarrier-guarded
+// stages.  Warpgroups 1 and 2 each own 64 accumulator rows: wgmma.mma_async reads both operands straight from the
+// swizzled tiles (matrix descriptors), the fp32 accumulator lives in registers and the epilogue runs on those
+// registers, so the accumulator never goes through memory before its single rounding to bf16.
 // One wgmma group stays in flight while the next stage is waited for; a stage is handed back to the producer as soon
-// as the group that read it has retired.
+// as the group that read it has retired.  The ring's stage and phase run on across tiles, so the producer fills the
+// ring with the next tile's k-blocks while the consumers are still in the current tile's epilogue.
 // Every mode whose output is a bf16 [rows, N] tile (all but kHeadTiles, kText and the FP8-emitting GELU) stages its
-// epilogue through shared memory: the producer TMA-loads the residual tile into an epilogue buffer before the main loop,
+// epilogue through shared memory: the producer TMA-loads the residual tile into an epilogue buffer during the main loop,
 // the consumers round each result once into that buffer, over the residual, and one thread writes the tile with TMA
-// stores clipped to the output's extents.  No global load then waits behind a global store.
+// stores clipped to the output's extents.  No global load then waits behind a global store.  The buffer is reused by
+// every tile of the CTA: once the stores have read it, the store thread arrives on `epi_free`, and only then does the
+// next tile's residual (or, without a residual, the next tile's results) go into it.
 //
 // The same main loop serves five front ends (template kMode):
 //   kPlain      nn.Linear with fused bias / GELU(tanh) / gate * x + residual epilogues;
@@ -94,7 +98,7 @@ struct HeadTileParams {
 };
 
 // Implicit-GEMM view of a causal 3D convolution over a (replicate-)padded NDHWC activation tensor: one
-// CTA owns a Tt x Ht x Wt box of output positions (128 rows).  The K loop walks (kt, kh, kw) taps x 64-channel
+// output tile is a Tt x Ht x Wt box of output positions (128 rows).  The K loop walks (kt, kh, kw) taps x 64-channel
 // chunks; every k-block is ONE 5-D TMA box load at the tap's offset.
 struct ConvGeom {
   int32_t wt_log2, ht_log2;              // box: Wt = 1 << wt_log2, Ht = 1 << ht_log2, Tt = 128 / (Wt * Ht)
@@ -119,7 +123,7 @@ struct GemmCfg {
   static constexpr int RING_BUDGET = kStaged ? kSmemLimit - 1024 - 256 - EPI_BYTES : kStageBudget;
   static constexpr int STAGES_RAW = RING_BUDGET / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  static constexpr int NUM_BARS = 2 * STAGES + (kStaged ? 1 : 0);   // full / empty per stage (+ residual tile)
+  static constexpr int NUM_BARS = 2 * STAGES + (kStaged ? 2 : 0);   // full / empty per stage (+ residual, buffer free)
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 + 8 * NUM_BARS;  // +1024 alignment slack
   static_assert(STAGES >= 2, "pipeline needs at least two stages");
   static_assert(SMEM_BYTES <= kSmemLimit, "shared memory");
@@ -151,27 +155,38 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const uint32_t bar_base = epi_base + Cfg::EPI_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-  const uint32_t res_bar = bar_base + 8u * (2 * kStages);   // staged epilogue: the residual tile has landed
+  const uint32_t res_bar = bar_base + 8u * (2 * kStages);       // staged epilogue: the residual tile has landed
+  const uint32_t epi_free = bar_base + 8u * (2 * kStages + 1);  //   the previous tile's stores have read the buffer
   auto smem_a = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES; };
   auto smem_b = [&](int s) { return smem_base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
 
   const int wg = threadIdx.x >> 7;
   const int tid_wg = threadIdx.x & 127;
   const int64_t num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int64_t m_blk = blockIdx.x / num_n_blocks, n_blk = blockIdx.x % num_n_blocks;
+  const int64_t num_m_blocks =
+      kMode == kConv ? (int64_t)cg.nb * cg.tiles_t * cg.tiles_h * cg.tiles_w : (p.M + kBlockM - 1) / kBlockM;
+  const int64_t num_tiles = num_m_blocks * num_n_blocks;
   const int64_t num_k_blocks = (p.K + kBK - 1) / kBK;
   const int64_t total_k_blocks = kMode == kLora ? num_k_blocks + lora_k_blocks : num_k_blocks;
-  // conv: m_blk -> (batch, t-tile, h-tile, w-tile); the box origin in OUTPUT coordinates
-  int n_i = 0, t0 = 0, h0 = 0, w0 = 0;
-  if constexpr (kMode == kConv) {
-    const int tw = (int)(m_blk % cg.tiles_w);
-    const int th = (int)((m_blk / cg.tiles_w) % cg.tiles_h);
-    const int tt = (int)((m_blk / ((int64_t)cg.tiles_w * cg.tiles_h)) % cg.tiles_t);
-    n_i = (int)(m_blk / ((int64_t)cg.tiles_w * cg.tiles_h * cg.tiles_t));
-    w0 = tw << cg.wt_log2;
-    h0 = th << cg.ht_log2;
-    t0 = tt * (128 >> (cg.wt_log2 + cg.ht_log2));
-  }
+  // Tile t -> (m_blk, n_blk), in the order of the grid's CTAs: the tiles in flight at once share A panels and W.  conv:
+  // m_blk -> (batch, t-tile, h-tile, w-tile), the box origin in OUTPUT coordinates.
+  struct Tile {
+    int64_t m_blk, n_blk;
+    int n_i, t0, h0, w0;
+  };
+  auto tile_at = [&](int64_t t) {
+    Tile tl = {t / num_n_blocks, t % num_n_blocks, 0, 0, 0, 0};
+    if constexpr (kMode == kConv) {
+      const int tw = (int)(tl.m_blk % cg.tiles_w);
+      const int th = (int)((tl.m_blk / cg.tiles_w) % cg.tiles_h);
+      const int tt = (int)((tl.m_blk / ((int64_t)cg.tiles_w * cg.tiles_h)) % cg.tiles_t);
+      tl.n_i = (int)(tl.m_blk / ((int64_t)cg.tiles_w * cg.tiles_h * cg.tiles_t));
+      tl.w0 = tw << cg.wt_log2;
+      tl.h0 = th << cg.ht_log2;
+      tl.t0 = tt * (128 >> (cg.wt_log2 + cg.ht_log2));
+    }
+    return tl;
+  };
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
@@ -184,6 +199,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       if (p.R != nullptr) tma_prefetch_desc(&tmap_r);
       tma_prefetch_desc(&tmap_d);
       mbar_init(res_bar, 1);
+      mbar_init(epi_free, 1);
     }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
@@ -194,53 +210,63 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   __syncthreads();
   pdl_wait();  // everything above overlapped the previous kernel's tail; its outputs are visible from here on
 
+  // The producer needs few registers and the consumers hold up to 128 accumulators each plus the tile loop's state:
+  // 128 x 40 + 256 x 232 registers are what the 384 x 168 of one CTA per SM allow.
   if (wg == 0) {
     // ===================== TMA producer (A and W tiles) =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     if (tid_wg == 0) {
-      const int32_t a_row = (int32_t)(m_blk * kBlockM);
-      const int32_t w_row = (int32_t)(n_blk * BLOCK_N);
-      if constexpr (kStaged) {
-        // The residual tile goes first, into the epilogue buffer: its latency hides behind the whole main loop.  R may
-        // alias D (in-place update): only this CTA reads or writes this tile.  Boxes past N are not issued; the
-        // out-of-bounds part of a box is zero filled and counted.
-        if (p.R != nullptr) {
-          const int live = (int)min((int64_t)(BLOCK_N / 64), (p.N - w_row + 63) / 64);
-          mbar_expect_tx(res_bar, (uint32_t)live * kEpiBoxBytes);
-          for (int c = 0; c < live; ++c) {
-            if constexpr (kMode == kConv)
-              tma_load_5d(&tmap_r, res_bar, epi_base + c * kEpiBoxBytes, w_row + 64 * c, w0, h0, t0, n_i);
-            else
-              tma_load_2d(&tmap_r, res_bar, epi_base + c * kEpiBoxBytes, w_row + 64 * c, a_row);
-          }
-        }
-      }
       int stage = 0;
       uint32_t phase = 0;
-      for (int64_t kb = 0; kb < num_k_blocks; ++kb) {
-        mbar_wait_notrace(empty_bar(stage), phase ^ 1);
-        const int32_t k0 = (int32_t)(kb * kBK);
-        mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);   // out-of-bounds box elements are zero filled and counted
-        if constexpr (kMode == kConv) {   // tap offsets in the padded input, output origin scaled by the stride
-          const int tap = (int)(kb / cg.cin_chunks);
-          const int32_t ac = (int32_t)(kb - (int64_t)tap * cg.cin_chunks) * kBlockK;
-          const int32_t aw = w0 * cg.sw + tap % cg.kw_n;
-          const int32_t ah = h0 * cg.sh + (tap / cg.kw_n) % cg.kh_n;
-          const int32_t at = t0 * cg.st + tap / (cg.kw_n * cg.kh_n);
-          tma_load_5d(&tmap_a, full_bar(stage), smem_a(stage), ac, aw, ah, at, n_i);
-        } else {
-          tma_load_2d(&tmap_a, full_bar(stage), smem_a(stage), k0, a_row);
-        }
-        tma_load_2d(&tmap_w, full_bar(stage), smem_b(stage), k0, w_row);
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      if constexpr (kMode == kLora) {   // the rank tail beyond r is zero filled in both U and s B
-        for (int32_t lk = 0; lk < lora_k_blocks; ++lk) {
+      uint32_t it = 0;   // this CTA's tile count
+      for (int64_t t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
+        const Tile tl = tile_at(t);
+        const int32_t a_row = (int32_t)(tl.m_blk * kBlockM);
+        const int32_t w_row = (int32_t)(tl.n_blk * BLOCK_N);
+        auto load_k_block = [&](int64_t kb) {
           mbar_wait_notrace(empty_bar(stage), phase ^ 1);
-          mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-          tma_load_2d(&tmap_u, full_bar(stage), smem_a(stage), lk * kBlockK, a_row);
-          tma_load_2d(&tmap_lb, full_bar(stage), smem_b(stage), lk * kBlockK, w_row);
+          mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);   // out-of-bounds box elements are zero filled and counted
+          if (kMode == kLora && kb >= num_k_blocks) {   // the rank tail beyond r is zero filled in both U and s B
+            const int32_t lk0 = (int32_t)(kb - num_k_blocks) * kBlockK;
+            tma_load_2d(&tmap_u, full_bar(stage), smem_a(stage), lk0, a_row);
+            tma_load_2d(&tmap_lb, full_bar(stage), smem_b(stage), lk0, w_row);
+          } else {
+            const int32_t k0 = (int32_t)(kb * kBK);
+            if constexpr (kMode == kConv) {   // tap offsets in the padded input, output origin scaled by the stride
+              const int tap = (int)(kb / cg.cin_chunks);
+              const int32_t ac = (int32_t)(kb - (int64_t)tap * cg.cin_chunks) * kBlockK;
+              const int32_t aw = tl.w0 * cg.sw + tap % cg.kw_n;
+              const int32_t ah = tl.h0 * cg.sh + (tap / cg.kw_n) % cg.kh_n;
+              const int32_t at = tl.t0 * cg.st + tap / (cg.kw_n * cg.kh_n);
+              tma_load_5d(&tmap_a, full_bar(stage), smem_a(stage), ac, aw, ah, at, tl.n_i);
+            } else {
+              tma_load_2d(&tmap_a, full_bar(stage), smem_a(stage), k0, a_row);
+            }
+            tma_load_2d(&tmap_w, full_bar(stage), smem_b(stage), k0, w_row);
+          }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
+        };
+        int64_t kb = 0;
+        if constexpr (kStaged) {
+          // The residual tile goes into the epilogue buffer, which the previous tile's output stores may still be
+          // reading.  So the ring is filled first (those loads need only stages the previous tile has released, and
+          // overlap its epilogue), then the buffer is waited for and the residual issued: its latency hides behind the
+          // rest of the main loop.  R may alias D (in-place update): each tile has exactly one owner CTA, which reads
+          // and writes it.  Boxes past N are not issued; the out-of-bounds part of a box is zero filled and counted.
+          if (p.R != nullptr) {
+            for (; kb < min((int64_t)kStages, total_k_blocks); ++kb) load_k_block(kb);
+            if (it > 0) mbar_wait_notrace(epi_free, (it - 1) & 1u);
+            const int live = (int)min((int64_t)(BLOCK_N / 64), (p.N - w_row + 63) / 64);
+            mbar_expect_tx(res_bar, (uint32_t)live * kEpiBoxBytes);
+            for (int c = 0; c < live; ++c) {
+              if constexpr (kMode == kConv)
+                tma_load_5d(&tmap_r, res_bar, epi_base + c * kEpiBoxBytes, w_row + 64 * c, tl.w0, tl.h0, tl.t0, tl.n_i);
+              else
+                tma_load_2d(&tmap_r, res_bar, epi_base + c * kEpiBoxBytes, w_row + 64 * c, a_row);
+            }
+          }
         }
+        for (; kb < total_k_blocks; ++kb) load_k_block(kb);
       }
       pdl_launch_dependents();  // all loads issued: dependents may start filling SMs as they are vacated
     }
@@ -248,258 +274,34 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
 
   // ===================== consumers: wgmma main loop =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   const int cw = wg - 1;   // accumulator rows [64 cw, 64 cw + 64) of the tile
-  float acc[BLOCK_N / 2];
-#pragma unroll
-  for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-  if constexpr (kMode == kFp8 || kMode == kFp8Blk) {
-    // FP8 wgmma adds into its accumulator with fewer mantissa bits than an fp32 add, so a K-long sum in the wgmma
-    // accumulator loses precision with K.  Each k-block (128 e4m3 elements) is summed into `part` by the tensor core and
-    // promoted into the fp32 register accumulator `acc` before the next one: acc is an fp32 sum of 128-element partials.
-    // (Two accumulators per thread: BLOCK_N <= 128 fits the 168-register budget of a 384-thread CTA.)
-    float part[BLOCK_N / 2];
-#pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) part[i] = 0.f;
-    // kFp8Blk: the scale rows of this thread's two accumulator rows (clamped: rows >= M are computed but never stored)
-    const float* sa_row0 = a_scale;
-    const float* sa_row1 = a_scale;
-    if constexpr (kMode == kFp8Blk) {
-      const int64_t r0 = m_blk * kBlockM + cw * 64 + (tid_wg >> 5) * 16 + ((tid_wg & 31) >> 2);
-      sa_row0 = a_scale + min(r0, p.M - 1) * fb.a_ld;
-      sa_row1 = a_scale + min(r0 + 8, p.M - 1) * fb.a_ld;
-    }
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
-      float s0 = 1.f, s1 = 1.f;
-      if constexpr (kMode == kFp8Blk) {   // issued before the wait: the loads overlap the TMA and the tensor core
-        s0 = __ldg(sa_row0 + kb * fb.a_kstride);
-        s1 = __ldg(sa_row1 + kb * fb.a_kstride);
-      }
-      mbar_wait_notrace(full_bar(stage), phase);
-      const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
-      const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
-      wgmma_fence_regs(part);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < 4; ++k)   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
-        WgmmaFp8<BLOCK_N>::mma(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();   // this k-block's partial is complete and its stage has been read
-      wgmma_fence_regs(part);
-      if (tid_wg == 0) mbar_arrive(empty_bar(stage));
-      if constexpr (kMode == kFp8Blk) {   // acc[4 j + 2 h + e] belongs to row h of the fragment
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          acc[4 * j] = fmaf(part[4 * j], s0, acc[4 * j]);
-          acc[4 * j + 1] = fmaf(part[4 * j + 1], s0, acc[4 * j + 1]);
-          acc[4 * j + 2] = fmaf(part[4 * j + 2], s1, acc[4 * j + 2]);
-          acc[4 * j + 3] = fmaf(part[4 * j + 3], s1, acc[4 * j + 3]);
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
-      }
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-    }
-  } else {
-    int stage = 0, prev = 0;
-    uint32_t phase = 0;
-    for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
-      mbar_wait_notrace(full_bar(stage), phase);
-      const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
-      const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
-      wgmma_fence_regs(acc);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kBlockK / 16; ++k)   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
-        Wgmma<BLOCK_N>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();   // the group of the previous k-block has retired: its stage may be refilled
-      wgmma_fence_regs(acc);
-      if (kb > 0 && tid_wg == 0) mbar_arrive(empty_bar(prev));
-      prev = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-  }
-
-  // accumulator fragment: acc[4 j + 2 h + e] = (row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e)
-  const int warp_in = tid_wg >> 5, lane = tid_wg & 31;
-  const int r_frag = cw * 64 + warp_in * 16 + (lane >> 2);
-  const int c_frag = 2 * (lane & 3);
-
-  if constexpr (kMode == kLora) {
-    // DoRA: acc *= col_scale[n] (passed in the w_scale slot) before the epilogue adds the bias.  A thread's columns are
-    // the same for both of its rows, so each scale pair is loaded once per tile.  x * 1.0f is exact: an all-ones scale
-    // leaves the accumulator's bits as they are.  Columns >= N are never stored, so their index is clamped instead of
-    // branched around: the loads carry no control dependence and can all be in flight at once.
-    if (w_scale != nullptr) {
-#pragma unroll
-      for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);
-        const float2 cs = __ldg(reinterpret_cast<const float2*>(w_scale + n));
-        acc[4 * j] *= cs.x;
-        acc[4 * j + 1] *= cs.y;
-        acc[4 * j + 2] *= cs.x;
-        acc[4 * j + 3] *= cs.y;
+  int stage = 0;
+  uint32_t phase = 0;
+  uint32_t it = 0;   // this CTA's tile count
+  // The previous tile's output stores must have read the epilogue buffer before the buffer takes this tile's residual
+  // or results.  The store thread waits for that only once its warpgroup has issued this tile's first k-block, so the
+  // wait overlaps the tensor core, and then frees the buffer (epi_free completes phase it - 1).
+  auto release_epi_buffer = [&](int64_t kb) {
+    if constexpr (kStaged) {
+      if (kb == 0 && it > 0 && threadIdx.x == 128) {
+        bulk_wait_group_read_all();
+        mbar_arrive(epi_free);
       }
     }
-  }
-
-  if constexpr (kMode == kFp8Blk && BLOCK_N == 128) {
-    if (p.epilogue == OSB_EPI_BIAS_GELU_TANH_FP8) {
-      // ===================== epilogue: GELU-tanh -> e4m3 codes + one scale per (row, 128 columns) =====================
-      // N % 128 == 0 (host check): every column of the tile exists.  Rows >= M take part in the quad shuffles (all lanes
-      // must) and store nothing.
-      const int64_t n0 = n_blk * BLOCK_N + c_frag;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
-        float amax = 0.f;
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int64_t n = n0 + 8 * j;
-          const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
-          float v0 = acc[4 * j + 2 * h] * sw.x, v1 = acc[4 * j + 2 * h + 1] * sw.y;
-          if (p.bias) {
-            const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
-            v0 += b.x;
-            v1 += b.y;
-          }
-          v0 = gelu_tanh(v0);
-          v1 = gelu_tanh(v1);
-          acc[4 * j + 2 * h] = v0;
-          acc[4 * j + 2 * h + 1] = v1;
-          amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
-        }
-        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-        amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-        const float s = amax > 0.f ? amax / 448.0f : 1.0f;
-        if (row < p.M) {
-          uint8_t* drow = fb.d8 + row * fb.ldd8;
-#pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j)   // x / s, IEEE division as the contract states it
-            *reinterpret_cast<uint16_t*>(drow + n0 + 8 * j) =
-                (uint16_t)e4m3x2(acc[4 * j + 2 * h] / s, acc[4 * j + 2 * h + 1] / s);
-          if (c_frag == 0) fb.d_scale[row * fb.ld_dscale + n_blk] = s;
-        }
-      }
-      return;
-    }
-  }
-
-  if constexpr (kMode == kHeadTiles) {
-    // ===================== epilogue: head tiles =====================
-    // a row's D columns of one head are spread over the 4 lanes of a quad: RMSNorm reduces over the quad,
-    // RoPE pairs (2i, 2i+1) sit in one thread.
-    constexpr int D = BLOCK_N / 2;
-    using HT = HeadTileCfg<D>;
-    constexpr int JH = D / 8;   // 8-column fragments per head
-    const int C = ht.heads * D;
-    const uint32_t chunk_bytes = (uint32_t)ht.map.TR * 128u;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
-      const bool row_ok = row < p.M;
-      // token row -> (tile, position in its sequence, row in tile)  (the host checks M < 2^31)
-      uint32_t pos = 0, tile_i = 0;
-      int r = 0;
-      if (row_ok) tile_of_row(ht.map, (uint32_t)row, tile_i, pos, r);
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int64_t col0 = n_blk * BLOCK_N + hh * D;
-        if (col0 >= p.N) continue;   // uniform over the CTA
-        const int kidx = (int)((uint32_t)col0 / (uint32_t)C);
-        const int head = (int)((uint32_t)col0 - (uint32_t)kidx * (uint32_t)C) / D;
-        const int kind = kidx % ht.nkinds;
-        float x[JH][2];
-#pragma unroll
-        for (int j = 0; j < JH; ++j) {
-          x[j][0] = acc[4 * (hh * JH + j) + 2 * h];
-          x[j][1] = acc[4 * (hh * JH + j) + 2 * h + 1];
-          if (p.bias) {
-            const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + col0 + 8 * j + c_frag)));
-            x[j][0] += b.x;
-            x[j][1] += b.y;
-          }
-        }
-        if ((ht.norm_mask >> kind) & 1u) {
-          float ss = 0.f;
-#pragma unroll
-          for (int j = 0; j < JH; ++j) ss += x[j][0] * x[j][0] + x[j][1] * x[j][1];
-          ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-          ss += __shfl_xor_sync(0xffffffffu, ss, 2);
-          const float rs = rsqrtf(ss * (1.0f / D) + ht.eps);
-          // (a runtime index into the parameter struct would move the whole struct to local memory)
-          const __nv_bfloat16* w = kind == 0 ? ht.norm_w[0] : (kind == 1 ? ht.norm_w[1] : (kind == 2 ? ht.norm_w[2] : ht.norm_w[3]));
-#pragma unroll
-          for (int j = 0; j < JH; ++j) {
-            const float2 f = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(w + 8 * j + c_frag)));
-            x[j][0] *= rs * f.x;
-            x[j][1] *= rs * f.y;
-          }
-        }
-        if (!row_ok) continue;
-        if ((ht.rope_mask >> kind) & 1u) {
-#pragma unroll
-          for (int j = 0; j < JH; ++j) {
-            const int64_t i = (int64_t)pos * (D / 2) + (8 * j + c_frag) / 2;
-            const float cc = __ldg(ht.cos + i), sn = __ldg(ht.sin + i);
-            const float a = x[j][0], b = x[j][1];
-            x[j][0] = a * cc - b * sn;
-            x[j][1] = b * cc + a * sn;
-          }
-        }
-        uint8_t* dst = ht.base + (int64_t)kidx * ht.kind_stride + (int64_t)head * ht.head_stride + (int64_t)tile_i * ht.tile_bytes;
-#pragma unroll
-        for (int j = 0; j < JH; ++j)
-          *reinterpret_cast<uint32_t*>(dst + tile_unit_off<HT::MAIN>(r, j, chunk_bytes) + c_frag * 2) = pack_bf16x2(x[j][0], x[j][1]);
-        if constexpr (HT::UP > HT::U)   // head-dim padding columns stay zero
-          *reinterpret_cast<uint32_t*>(dst + tile_unit_off<HT::MAIN>(r, HT::U, chunk_bytes) + c_frag * 2) = 0u;
-      }
-    }
-  } else if constexpr (kMode == kText) {
-    // ===================== epilogue: gated GELU / bias + quick GELU =====================
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
-      if (row >= p.M) continue;
-      __nv_bfloat16* drow = p.D + row * p.ldd;
-#pragma unroll
-      for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int64_t n = n_blk * BLOCK_N + 8 * j + c_frag;
-        if (n >= p.N) continue;
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (p.bias) {
-          const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
-          v0 += b.x;
-          v1 += b.y;
-        }
-        if (p.epilogue == OSB_EPI_GATED_GELU) {   // columns (n, n + 1) = (wi_0, wi_1) of output column n / 2
-          drow[n >> 1] = __float2bfloat16_rn(gelu_tanh(v0) * v1);
-        } else {                                  // x * sigmoid(1.702 x)
-          v0 = v0 / (1.0f + __expf(-1.702f * v0));
-          v1 = v1 / (1.0f + __expf(-1.702f * v1));
-          *reinterpret_cast<uint32_t*>(drow + n) = pack_bf16x2(v0, v1);
-        }
-      }
-    }
-  } else {
-    // ===================== staged epilogue: bias / GELU / gate + residual =====================
-    // The tile is assembled in the epilogue buffer and leaves by TMA: the buffer row of tile row li is li (for kConv the
-    // 5-D output box orders its 128 positions exactly like the A box, so li is also its row there), column c of the tile
-    // sits in box c / 64 at 16-byte chunk (c % 64) / 8 XOR (li % 8) - the 128-byte swizzle.  A quad's four lanes cover
-    // one 16-byte chunk of a row and the eight rows of a warp's fragment land in eight different chunks: conflict free.
-    // Rows >= M and columns >= N are computed like the others and clipped by the tensor map on the store, so the only
-    // global reads left are the per-column bias / scale / gate vectors (clamped indices, no control dependence: they can
-    // all be in flight at once) and nothing is read after the first store.  The arithmetic per element is the register
-    // epilogue's, in its order and with its roundings (explicit _rn operations: no contraction into an FMA).
-    static_assert(kStaged, "every other mode has its own epilogue");
+  };
+  for (int64_t t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
+    const Tile tl = tile_at(t);
+    const int64_t m_blk = tl.m_blk, n_blk = tl.n_blk;
+    // accumulator fragment: acc[4 j + 2 h + e] = (row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e)
+    const int warp_in = tid_wg >> 5, lane = tid_wg & 31;
+    const int r_frag = cw * 64 + warp_in * 16 + (lane >> 2);
+    const int c_frag = 2 * (lane & 3);
+    // Staged epilogue: the per-row gate row (modulation group, then mod_index) and FP8 row scale depend on the tile
+    // only, so their loads are issued here and their latency hides behind the main loop.  Rows >= M are clamped.
     const float* gate_row[2] = {nullptr, nullptr};
     float sa[2] = {0.f, 0.f};
-    if constexpr (kMode != kConv) {
+    if constexpr (kStaged && kMode != kConv) {
       const uint32_t group_rows32 = (uint32_t)(p.group_rows > 0xffffffffll ? 0xffffffffu : p.group_rows);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -512,71 +314,342 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         if constexpr (kMode == kFp8) sa[h] = __ldg(a_scale + row);
       }
     }
-    uint8_t* const epi = smem_raw + (epi_base - smem_u32(smem_raw));
-    const bool gate_res = p.epilogue == OSB_EPI_BIAS_GATE_RES;
-    if (!gate_res) gate_row[0] = gate_row[1] = nullptr;
-    const bool has_res = gate_res && p.R != nullptr;
-    if (p.R != nullptr) mbar_wait_notrace(res_bar, 0);
-    // One straight-line body per activation, with the optional operands folded into identities that leave every bit of
-    // the value as it is (x + -0 = x, x * 1 = x): no branch splits the unrolled loop, so the loads are not held behind one.
-    auto body = [&](auto gelu) {
+    float acc[BLOCK_N / 2];
 #pragma unroll
-      for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);   // N % 8 == 0: n < N implies n + 1 < N
-        float2 sw = make_float2(1.f, 1.f), b = make_float2(-0.f, -0.f);
-        if constexpr (kMode == kFp8 || kMode == kFp8Blk) sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
-        if (p.bias) b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    if constexpr (kMode == kFp8 || kMode == kFp8Blk) {
+      // FP8 wgmma adds into its accumulator with fewer mantissa bits than an fp32 add, so a K-long sum in the wgmma
+      // accumulator loses precision with K.  Each k-block (128 e4m3 elements) is summed into `part` by the tensor core and
+      // promoted into the fp32 register accumulator `acc` before the next one: acc is an fp32 sum of 128-element partials.
+      // (Two accumulators per thread: BLOCK_N <= 128 fits the consumers' 232 registers with room to spare.)
+      float part[BLOCK_N / 2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int li = r_frag + 8 * h;
-          uint32_t* const cell = reinterpret_cast<uint32_t*>(epi + (j >> 3) * kEpiBoxBytes + li * 128 +
-                                                             (((j & 7) ^ (li & 7)) << 4) + c_frag * 2);
-          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-          if constexpr (kMode == kFp8) {
-            v0 = __fmul_rn(v0, __fmul_rn(sa[h], sw.x));
-            v1 = __fmul_rn(v1, __fmul_rn(sa[h], sw.y));
-          } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator
-            v0 = __fmul_rn(v0, sw.x);
-            v1 = __fmul_rn(v1, sw.y);
+      for (int i = 0; i < BLOCK_N / 2; ++i) part[i] = 0.f;
+      // kFp8Blk: the scale rows of this thread's two accumulator rows (clamped: rows >= M are computed but never stored)
+      const float* sa_row0 = a_scale;
+      const float* sa_row1 = a_scale;
+      if constexpr (kMode == kFp8Blk) {
+        const int64_t r0 = m_blk * kBlockM + cw * 64 + (tid_wg >> 5) * 16 + ((tid_wg & 31) >> 2);
+        sa_row0 = a_scale + min(r0, p.M - 1) * fb.a_ld;
+        sa_row1 = a_scale + min(r0 + 8, p.M - 1) * fb.a_ld;
+      }
+      for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
+        float s0 = 1.f, s1 = 1.f;
+        if constexpr (kMode == kFp8Blk) {   // issued before the wait: the loads overlap the TMA and the tensor core
+          s0 = __ldg(sa_row0 + kb * fb.a_kstride);
+          s1 = __ldg(sa_row1 + kb * fb.a_kstride);
+        }
+        mbar_wait_notrace(full_bar(stage), phase);
+        const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
+        const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
+        wgmma_fence_regs(part);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
+          WgmmaFp8<BLOCK_N>::mma(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        release_epi_buffer(kb);
+        wgmma_wait<0>();   // this k-block's partial is complete and its stage has been read
+        wgmma_fence_regs(part);
+        if (tid_wg == 0) mbar_arrive(empty_bar(stage));
+        if constexpr (kMode == kFp8Blk) {   // acc[4 j + 2 h + e] belongs to row h of the fragment
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            acc[4 * j] = fmaf(part[4 * j], s0, acc[4 * j]);
+            acc[4 * j + 1] = fmaf(part[4 * j + 1], s0, acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(part[4 * j + 2], s1, acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(part[4 * j + 3], s1, acc[4 * j + 3]);
           }
-          v0 = __fadd_rn(v0, b.x);
-          v1 = __fadd_rn(v1, b.y);
-          if constexpr (decltype(gelu)::value) {
-            v0 = gelu_tanh(v0);
-            v1 = gelu_tanh(v1);
-          } else {
-            // the residual element is read before this thread overwrites it with the result
-            const float2 g = gate_row[h] ? __ldg(reinterpret_cast<const float2*>(gate_row[h] + n)) : make_float2(1.f, 1.f);
-            const float2 rv = has_res ? unpack_bf16x2(*cell) : make_float2(-0.f, -0.f);
-            v0 = __fadd_rn(__fmul_rn(v0, g.x), rv.x);
-            v1 = __fadd_rn(__fmul_rn(v1, g.y), rv.y);
-          }
-          *cell = pack_bf16x2(v0, v1);
+        } else {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
+        }
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+    } else {
+      int prev = 0;
+      for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
+        mbar_wait_notrace(full_bar(stage), phase);
+        const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
+        const uint64_t db = make_sw128_kmajor_desc(smem_b(stage));
+        wgmma_fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k)   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
+          Wgmma<BLOCK_N>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        release_epi_buffer(kb);
+        wgmma_wait<1>();   // the group of the previous k-block has retired: its stage may be refilled
+        wgmma_fence_regs(acc);
+        if (kb > 0 && tid_wg == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (tid_wg == 0) mbar_arrive(empty_bar(prev));   // the tile's last stage: the next tile's k-blocks need it
+    }
+
+    if constexpr (kMode == kLora) {
+      // DoRA: acc *= col_scale[n] (passed in the w_scale slot) before the epilogue adds the bias.  A thread's columns are
+      // the same for both of its rows, so each scale pair is loaded once per tile.  x * 1.0f is exact: an all-ones scale
+      // leaves the accumulator's bits as they are.  Columns >= N are never stored, so their index is clamped instead of
+      // branched around: the loads carry no control dependence and can all be in flight at once.
+      if (w_scale != nullptr) {
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);
+          const float2 cs = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+          acc[4 * j] *= cs.x;
+          acc[4 * j + 1] *= cs.y;
+          acc[4 * j + 2] *= cs.x;
+          acc[4 * j + 3] *= cs.y;
         }
       }
-    };
-    if (p.epilogue == OSB_EPI_BIAS_GELU_TANH)
-      body(std::true_type{});
-    else
-      body(std::false_type{});
-    // Both consumer warpgroups' writes, made visible to the async proxy, then one thread stores the tile.  It waits only
-    // until the stores have READ the buffer, which is all the CTA needs before it exits and its shared memory is reused.
-    // The writes themselves belong to this grid's memory operations, which a dependent kernel's griddepcontrol.wait (PDL)
-    // or an ordinary stream-ordered launch waits for in full before it reads the output.
-    fence_proxy_async_smem();
-    named_barrier_sync(1, 256);
-    if (threadIdx.x == 128) {
-      const int32_t n0 = (int32_t)(n_blk * BLOCK_N);
-      const int live = (int)min((int64_t)(BLOCK_N / 64), (p.N - n0 + 63) / 64);
-      for (int c = 0; c < live; ++c) {
-        if constexpr (kMode == kConv)
-          tma_store_5d(&tmap_d, epi_base + c * kEpiBoxBytes, n0 + 64 * c, w0, h0, t0, n_i);
-        else
-          tma_store_2d(&tmap_d, epi_base + c * kEpiBoxBytes, n0 + 64 * c, (int32_t)(m_blk * kBlockM));
-      }
-      bulk_commit_group();
-      bulk_wait_group_read_all();
     }
+
+    if constexpr (kMode == kFp8Blk && BLOCK_N == 128) {
+      if (p.epilogue == OSB_EPI_BIAS_GELU_TANH_FP8) {
+        // ===================== epilogue: GELU-tanh -> e4m3 codes + one scale per (row, 128 columns) =====================
+        // N % 128 == 0 (host check): every column of the tile exists.  Rows >= M take part in the quad shuffles (all lanes
+        // must) and store nothing.
+        const int64_t n0 = n_blk * BLOCK_N + c_frag;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
+          float amax = 0.f;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int64_t n = n0 + 8 * j;
+            const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+            float v0 = acc[4 * j + 2 * h] * sw.x, v1 = acc[4 * j + 2 * h + 1] * sw.y;
+            if (p.bias) {
+              const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+              v0 += b.x;
+              v1 += b.y;
+            }
+            v0 = gelu_tanh(v0);
+            v1 = gelu_tanh(v1);
+            acc[4 * j + 2 * h] = v0;
+            acc[4 * j + 2 * h + 1] = v1;
+            amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+          }
+          amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+          amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+          const float s = amax > 0.f ? amax / 448.0f : 1.0f;
+          if (row < p.M) {
+            uint8_t* drow = fb.d8 + row * fb.ldd8;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j)   // x / s, IEEE division as the contract states it
+              *reinterpret_cast<uint16_t*>(drow + n0 + 8 * j) =
+                  (uint16_t)e4m3x2(acc[4 * j + 2 * h] / s, acc[4 * j + 2 * h + 1] / s);
+            if (c_frag == 0) fb.d_scale[row * fb.ld_dscale + n_blk] = s;
+          }
+        }
+        continue;
+      }
+    }
+
+    if constexpr (kMode == kHeadTiles) {
+      // ===================== epilogue: head tiles =====================
+      // a row's D columns of one head are spread over the 4 lanes of a quad: RMSNorm reduces over the quad,
+      // RoPE pairs (2i, 2i+1) sit in one thread.  The stores go out as whole 16-byte units (below), so every lane of a
+      // warp takes part in the quad exchanges and only the stores of rows >= M are skipped.
+      constexpr int D = BLOCK_N / 2;
+      using HT = HeadTileCfg<D>;
+      constexpr int JH = D / 8;   // 8-column fragments per head
+      const int C = ht.heads * D;
+      const uint32_t chunk_bytes = (uint32_t)ht.map.TR * 128u;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
+        const bool row_ok = row < p.M;
+        // token row -> (tile, position in its sequence, row in tile)  (the host checks M < 2^31)
+        uint32_t pos = 0, tile_i = 0;
+        int r = 0;
+        if (row_ok) tile_of_row(ht.map, (uint32_t)row, tile_i, pos, r);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int64_t col0 = n_blk * BLOCK_N + hh * D;
+          if (col0 >= p.N) continue;   // uniform over the CTA
+          const int kidx = (int)((uint32_t)col0 / (uint32_t)C);
+          const int head = (int)((uint32_t)col0 - (uint32_t)kidx * (uint32_t)C) / D;
+          const int kind = kidx % ht.nkinds;
+          float x[JH][2];
+#pragma unroll
+          for (int j = 0; j < JH; ++j) {
+            x[j][0] = acc[4 * (hh * JH + j) + 2 * h];
+            x[j][1] = acc[4 * (hh * JH + j) + 2 * h + 1];
+            if (p.bias) {
+              const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + col0 + 8 * j + c_frag)));
+              x[j][0] += b.x;
+              x[j][1] += b.y;
+            }
+          }
+          if ((ht.norm_mask >> kind) & 1u) {
+            float ss = 0.f;
+#pragma unroll
+            for (int j = 0; j < JH; ++j) ss += x[j][0] * x[j][0] + x[j][1] * x[j][1];
+            ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+            ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+            const float rs = rsqrtf(ss * (1.0f / D) + ht.eps);
+            // (a runtime index into the parameter struct would move the whole struct to local memory)
+            const __nv_bfloat16* w = kind == 0 ? ht.norm_w[0] : (kind == 1 ? ht.norm_w[1] : (kind == 2 ? ht.norm_w[2] : ht.norm_w[3]));
+#pragma unroll
+            for (int j = 0; j < JH; ++j) {
+              const float2 f = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(w + 8 * j + c_frag)));
+              x[j][0] *= rs * f.x;
+              x[j][1] *= rs * f.y;
+            }
+          }
+          if ((ht.rope_mask >> kind) & 1u) {   // rows >= M: position 0, never stored
+#pragma unroll
+            for (int j = 0; j < JH; ++j) {
+              const int64_t i = (int64_t)pos * (D / 2) + (8 * j + c_frag) / 2;
+              const float cc = __ldg(ht.cos + i), sn = __ldg(ht.sin + i);
+              const float a = x[j][0], b = x[j][1];
+              x[j][0] = a * cc - b * sn;
+              x[j][1] = b * cc + a * sn;
+            }
+          }
+          uint8_t* dst = ht.base + (int64_t)kidx * ht.kind_stride + (int64_t)head * ht.head_stride + (int64_t)tile_i * ht.tile_bytes;
+          // Swizzled units, four at a time: lane q of the quad holds columns (2q, 2q + 1) of each of units j0 .. j0 + 3;
+          // a 4 x 4 transpose over the quad (two exchange rounds) leaves it all 16 bytes of unit j0 + q.  A warp then
+          // writes 64 contiguous bytes of each of its 8 rows per store (four units of one 128-byte swizzle row), where
+          // 4-byte stores wrote 16 bytes per row and store.
+          const bool odd = (lane & 1) != 0, high = (lane & 2) != 0;
+#pragma unroll
+          for (int j0 = 0; j0 < HT::MAIN * 8; j0 += 4) {
+            uint32_t u0 = pack_bf16x2(x[j0][0], x[j0][1]), u1 = pack_bf16x2(x[j0 + 1][0], x[j0 + 1][1]);
+            uint32_t u2 = pack_bf16x2(x[j0 + 2][0], x[j0 + 2][1]), u3 = pack_bf16x2(x[j0 + 3][0], x[j0 + 3][1]);
+            uint32_t s0 = __shfl_xor_sync(0xffffffffu, odd ? u0 : u1, 1);   // lanes q, q ^ 1: 2 x 2 blocks
+            uint32_t s1 = __shfl_xor_sync(0xffffffffu, odd ? u2 : u3, 1);
+            if (odd) { u0 = s0; u2 = s1; } else { u1 = s0; u3 = s1; }
+            s0 = __shfl_xor_sync(0xffffffffu, high ? u0 : u2, 2);            // lanes q, q ^ 2: the blocks
+            s1 = __shfl_xor_sync(0xffffffffu, high ? u1 : u3, 2);
+            if (high) { u0 = s0; u1 = s1; } else { u2 = s0; u3 = s1; }
+            if (row_ok)
+              *reinterpret_cast<uint4*>(dst + tile_unit_off<HT::MAIN>(r, j0 + (lane & 3), chunk_bytes)) = make_uint4(u0, u1, u2, u3);
+          }
+          if (!row_ok) continue;
+#pragma unroll
+          for (int j = HT::MAIN * 8; j < JH; ++j)   // the head-dim tail (core-matrix layout)
+            *reinterpret_cast<uint32_t*>(dst + tile_unit_off<HT::MAIN>(r, j, chunk_bytes) + c_frag * 2) = pack_bf16x2(x[j][0], x[j][1]);
+          if constexpr (HT::UP > HT::U)   // head-dim padding columns stay zero
+            *reinterpret_cast<uint32_t*>(dst + tile_unit_off<HT::MAIN>(r, HT::U, chunk_bytes) + c_frag * 2) = 0u;
+        }
+      }
+    } else if constexpr (kMode == kText) {
+      // ===================== epilogue: gated GELU / bias + quick GELU =====================
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = m_blk * kBlockM + r_frag + 8 * h;
+        if (row >= p.M) continue;
+        __nv_bfloat16* drow = p.D + row * p.ldd;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int64_t n = n_blk * BLOCK_N + 8 * j + c_frag;
+          if (n >= p.N) continue;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (p.bias) {
+            const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+            v0 += b.x;
+            v1 += b.y;
+          }
+          if (p.epilogue == OSB_EPI_GATED_GELU) {   // columns (n, n + 1) = (wi_0, wi_1) of output column n / 2
+            drow[n >> 1] = __float2bfloat16_rn(gelu_tanh(v0) * v1);
+          } else {                                  // x * sigmoid(1.702 x)
+            v0 = v0 / (1.0f + __expf(-1.702f * v0));
+            v1 = v1 / (1.0f + __expf(-1.702f * v1));
+            *reinterpret_cast<uint32_t*>(drow + n) = pack_bf16x2(v0, v1);
+          }
+        }
+      }
+    } else {
+      // ===================== staged epilogue: bias / GELU / gate + residual =====================
+      // The tile is assembled in the epilogue buffer and leaves by TMA: the buffer row of tile row li is li (for kConv the
+      // 5-D output box orders its 128 positions exactly like the A box, so li is also its row there), column c of the tile
+      // sits in box c / 64 at 16-byte chunk (c % 64) / 8 XOR (li % 8) - the 128-byte swizzle.  A quad's four lanes cover
+      // one 16-byte chunk of a row and the eight rows of a warp's fragment land in eight different chunks: conflict free.
+      // Rows >= M and columns >= N are computed like the others and clipped by the tensor map on the store, so the only
+      // global reads left are the per-column bias / scale / gate vectors (clamped indices, no control dependence: they can
+      // all be in flight at once) and nothing is read after the first store.  The arithmetic per element is the register
+      // epilogue's, in its order and with its roundings (explicit _rn operations: no contraction into an FMA).
+      static_assert(kStaged, "every other mode has its own epilogue");
+      uint8_t* const epi = smem_raw + (epi_base - smem_u32(smem_raw));
+      const bool gate_res = p.epilogue == OSB_EPI_BIAS_GATE_RES;
+      if (!gate_res) gate_row[0] = gate_row[1] = nullptr;
+      const bool has_res = gate_res && p.R != nullptr;
+      // With a residual, the producer issued it only after the previous tile's stores had read the buffer; without one,
+      // the buffer is free once they have.
+      if (p.R != nullptr)
+        mbar_wait_notrace(res_bar, it & 1u);
+      else if (it > 0)
+        mbar_wait_notrace(epi_free, (it - 1) & 1u);
+      // One straight-line body per activation, with the optional operands folded into identities that leave every bit of
+      // the value as it is (x + -0 = x, x * 1 = x): no branch splits the unrolled loop, so the loads are not held behind one.
+      auto body = [&](auto gelu) {
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);   // N % 8 == 0: n < N implies n + 1 < N
+          float2 sw = make_float2(1.f, 1.f), b = make_float2(-0.f, -0.f);
+          if constexpr (kMode == kFp8 || kMode == kFp8Blk) sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+          if (p.bias) b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int li = r_frag + 8 * h;
+            uint32_t* const cell = reinterpret_cast<uint32_t*>(epi + (j >> 3) * kEpiBoxBytes + li * 128 +
+                                                               (((j & 7) ^ (li & 7)) << 4) + c_frag * 2);
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if constexpr (kMode == kFp8) {
+              v0 = __fmul_rn(v0, __fmul_rn(sa[h], sw.x));
+              v1 = __fmul_rn(v1, __fmul_rn(sa[h], sw.y));
+            } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator
+              v0 = __fmul_rn(v0, sw.x);
+              v1 = __fmul_rn(v1, sw.y);
+            }
+            v0 = __fadd_rn(v0, b.x);
+            v1 = __fadd_rn(v1, b.y);
+            if constexpr (decltype(gelu)::value) {
+              v0 = gelu_tanh(v0);
+              v1 = gelu_tanh(v1);
+            } else {
+              // the residual element is read before this thread overwrites it with the result
+              const float2 g = gate_row[h] ? __ldg(reinterpret_cast<const float2*>(gate_row[h] + n)) : make_float2(1.f, 1.f);
+              const float2 rv = has_res ? unpack_bf16x2(*cell) : make_float2(-0.f, -0.f);
+              v0 = __fadd_rn(__fmul_rn(v0, g.x), rv.x);
+              v1 = __fadd_rn(__fmul_rn(v1, g.y), rv.y);
+            }
+            *cell = pack_bf16x2(v0, v1);
+          }
+        }
+      };
+      if (p.epilogue == OSB_EPI_BIAS_GELU_TANH)
+        body(std::true_type{});
+      else
+        body(std::false_type{});
+      // Both consumer warpgroups' writes, made visible to the async proxy, then one thread stores the tile.  It waits only
+      // until the stores have READ the buffer (release_epi_buffer in the next tile, or before the CTA exits), which is all
+      // the next tile or the CTA's exit needs.  The writes themselves belong to this grid's memory operations, which a
+      // dependent kernel's griddepcontrol.wait (PDL) or an ordinary stream-ordered launch waits for in full before it
+      // reads the output.
+      fence_proxy_async_smem();
+      named_barrier_sync(1, 256);
+      if (threadIdx.x == 128) {
+        const int32_t n0 = (int32_t)(n_blk * BLOCK_N);
+        const int live = (int)min((int64_t)(BLOCK_N / 64), (p.N - n0 + 63) / 64);
+        for (int c = 0; c < live; ++c) {
+          if constexpr (kMode == kConv)
+            tma_store_5d(&tmap_d, epi_base + c * kEpiBoxBytes, n0 + 64 * c, tl.w0, tl.h0, tl.t0, tl.n_i);
+          else
+            tma_store_2d(&tmap_d, epi_base + c * kEpiBoxBytes, n0 + 64 * c, (int32_t)(m_blk * kBlockM));
+        }
+        bulk_commit_group();
+      }
+    }
+  }
+  if constexpr (kStaged) {
+    if (threadIdx.x == 128) bulk_wait_group_read_all();   // the last tile's stores have read the buffer: the CTA may exit
   }
 }
 
@@ -590,8 +663,9 @@ static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tw, const Gem
                          const float* w_scale = nullptr, const Fp8BlockParams& fb = Fp8BlockParams{},
                          const CUtensorMap* tr = nullptr, const CUtensorMap* td = nullptr) {
   if (tiles >= (1ll << 31)) { set_error("osb gemm: too many output tiles (%lld)", (long long)tiles); return OSB_ERR_UNSUPPORTED; }
+  const int64_t grid = tiles < sm_count() ? tiles : sm_count();   // one CTA per SM, each walks its tiles
   cudaLaunchAttribute attr[2];
-  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)tiles), dim3(kNumThreads),
+  cudaLaunchConfig_t cfg = launch_config(dim3((unsigned)grid), dim3(kNumThreads),
                                          GemmCfg<BLOCK_N, staged_epilogue(kMode)>::SMEM_BYTES, stream, attr);
   // the LoRA maps are read by kLora only, the residual / output maps by the staged epilogue only (the residual map only
   // when p.R is set); where a map is not read the main maps are passed as placeholders
@@ -699,8 +773,9 @@ int gemm_init() {
   return OSB_OK;
 }
 
-// Tile width: fewest (waves of tiles over the SMs) x (tile width), i.e. the least padded work once the last wave
-// is counted as full; ties go to the wider tile, which re-reads A less often.
+// Tile width: fewest (tiles per CTA, rounded up) x (tile width + 16), i.e. the least padded work once the last round of
+// tiles is counted as full, plus what every tile pays besides its main loop (the epilogue, which no main loop hides),
+// about 16 columns' worth on one H100 (DESIGN.md 5b); ties go to the wider tile, which re-reads A less often.
 static int pick_block_n(int64_t M, int64_t N) {
   if (N <= 64) return 64;
   const int cands[3] = {256, 192, 128};
@@ -710,7 +785,7 @@ static int pick_block_n(int64_t M, int64_t N) {
     const int bn = cands[i];
     const int64_t tiles = ((M + kBlockM - 1) / kBlockM) * ((N + bn - 1) / bn);
     const int64_t waves = (tiles + sm_count() - 1) / sm_count();
-    const int64_t cost = waves * bn;
+    const int64_t cost = waves * (bn + 16);
     if (cost < best_cost) { best_cost = cost; best = bn; }
   }
   return best;
