@@ -183,6 +183,24 @@ typedef struct osb_fp8_blocks_args {
  * mlp part of linear1 -> GELU) of the MMDiT blocks when FP8 is enabled; block mode replaces fc2 and linear2. */
 int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* gemm, const osb_fp8_blocks_args* blk, void* stream);
 
+/* osb_gemm_fp8_blocks plus an unmerged LoRA / DoRA update (osb_lora_args, as in osb_gemm_lora):
+ *     D = epilogue(col_scale[n] * (w_scale[n] * sum_kb a_scale[m, kb] * acc_kb + sum_j U[m, j] * B[n, j]) + bias)
+ * After the e4m3 k-blocks, ceil(r / 64) bf16 k-blocks of U [M, r] and B = scaling * lora_B [N, r] run through the same
+ * pipeline; their partials are promoted into the same fp32 register accumulator unscaled, after w_scale has been applied
+ * to the FP8 sum (w_scale never scales the update), and the one rounding is the epilogue's.  col_scale == NULL means 1;
+ * an all-ones col_scale gives the bits of NULL.  Every epilogue of osb_gemm_fp8_blocks works, per-row (a_scale_ld == 0)
+ * or block-scaled A: bias, GELU-tanh, gate + residual (group_rows / mod_index, R may alias D) and, with block_n 0 or
+ * 128, OSB_EPI_BIAS_GELU_TANH_FP8, where the update enters before the GELU and the block amax.
+ * The down projection U = x A_cat^T is osb_gemm_fp8_blocks with N = r on the same e4m3 input (A_cat quantized per row
+ * by osb_quant_blocks_fp8 with block = K) and a bf16 output.
+ * Requirements: those of osb_gemm_fp8_blocks, plus those of osb_gemm_lora: r > 0 and r % 8 == 0, U and B 16-byte
+ * aligned with ldu, ldb >= r and multiples of 8, col_scale 8-byte aligned.
+ * Returns OSB_ERR_INVALID for a null gemm, blk or lora argument, a null operand or scale, any shape, stride or alignment
+ * rule above, or an epilogue it does not build; OSB_ERR_UNSUPPORTED for block_n other than 0, 64 or 128;
+ * OSB_ERR_NOT_INIT before osb_init().  Runs the adapted block Linears of MMDiT when FP8 is enabled with lora=True. */
+int osb_gemm_fp8_lora(const osb_gemm_fp8_args* gemm, const osb_fp8_blocks_args* blk, const osb_lora_args* lora,
+                      void* stream);
+
 /* Block quantizer: bf16 x [rows, K] (row stride ldx) -> e4m3 y8 [rows, K] (row stride ldy) with the scale of (row r,
  * block b) at y_scale[r * lds + b].  block == 128: 1 x 128 block scales, one pass over x (the attention output of the
  * MMDiT single blocks).  block == K: one scale per row for rows of any length (the MLP weights, per output channel, up

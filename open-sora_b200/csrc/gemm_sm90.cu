@@ -36,6 +36,12 @@
 //               With BLOCK_N = 128 it also has the FP8-emitting GELU epilogue: one output tile row is exactly one
 //               128-column scale block, held by the 4 lanes of a quad, so the block amax is two shuffles; the codes and
 //               the scale go out instead of bf16.
+//   kFp8BlkLora kFp8Blk plus an unmerged low-rank update, as kLora adds one to kPlain: after the e4m3 k-blocks the
+//               producer streams ceil(r / 64) bf16 k-blocks of U = x A^T [M, r] and s B [N, r] through the same ring (64
+//               bf16 and 128 e4m3 elements are both one 128-byte swizzle row).  Before the first of them the accumulator
+//               is multiplied by w_scale[col], which scales the FP8 sum only; each bf16 k-block is summed into the partial
+//               accumulator by 4 wgmma k16 steps and promoted unscaled, then the optional DoRA column scale multiplies
+//               the total before the unchanged epilogue (the FP8-emitting GELU included).
 //
 // Replaces every nn.Linear on the denoiser block path of the reference
 // (opensora/models/mmdit/layers.py:209-214,247-252,277-281,314-334,401) and the fused epilogues
@@ -56,15 +62,17 @@ constexpr int kNumThreads = 384;            // producer warpgroup + two consumer
 constexpr int kStageBudget = 200 * 1024;    // operand ring of the register-epilogue modes (one CTA per SM)
 constexpr int kSmemLimit = 227 * 1024;      // sm_90 per-block dynamic shared memory limit
 
-enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4, kFp8 = 5, kFp8Blk = 6 };
+enum { kPlain = 0, kConv = 1, kHeadTiles = 2, kLora = 3, kText = 4, kFp8 = 5, kFp8Blk = 6, kFp8BlkLora = 7 };
 
-// kFp8Blk only: where the scale of (row m, k-block kb) of A is (a_scale + m * a_ld + kb * a_kstride; a_kstride = 0 for
-// per-row scales), and the e4m3 output of the FP8-emitting GELU epilogue (codes d8 [M, N], ldd8; scales [M, N / 128]).
+// kFp8Blk / kFp8BlkLora only: where the scale of (row m, k-block kb) of A is (a_scale + m * a_ld + kb * a_kstride;
+// a_kstride = 0 for per-row scales), the e4m3 output of the FP8-emitting GELU epilogue (codes d8 [M, N], ldd8; scales
+// [M, N / 128]) and, kFp8BlkLora only, the optional DoRA column scale (null: none).
 struct Fp8BlockParams {
   int64_t a_ld, a_kstride;
   uint8_t* d8;
   float* d_scale;
   int64_t ldd8, ld_dscale;
+  const float* col_scale;
 };
 
 struct GemmEpilogueParams {
@@ -111,7 +119,11 @@ struct ConvGeom {
 
 // Modes whose output is a bf16 [rows, N] tile go through the staged epilogue: the 128 x BLOCK_N tile is assembled in a
 // shared-memory buffer (the residual tile is TMA-loaded into it during the main loop) and leaves by TMA tile stores.
-__host__ __device__ constexpr bool staged_epilogue(int mode) { return mode == kPlain || mode == kConv || mode == kLora || mode == kFp8 || mode == kFp8Blk; }
+__host__ __device__ constexpr bool staged_epilogue(int mode) {
+  return mode == kPlain || mode == kConv || mode == kLora || mode == kFp8 || mode == kFp8Blk || mode == kFp8BlkLora;
+}
+__host__ __device__ constexpr bool fp8_mode(int mode) { return mode == kFp8 || mode == kFp8Blk || mode == kFp8BlkLora; }
+__host__ __device__ constexpr bool lora_mode(int mode) { return mode == kLora || mode == kFp8BlkLora; }
 
 template <int BLOCK_N, bool kStaged = false>
 struct GemmCfg {
@@ -137,16 +149,16 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                  const GemmEpilogueParams p, const ConvGeom cg, const HeadTileParams ht,
                  const __grid_constant__ CUtensorMap tmap_u, const __grid_constant__ CUtensorMap tmap_lb,
-                 const int32_t lora_k_blocks,     // kLora only: U / s B maps and ceil(r / 64)
+                 const int32_t lora_k_blocks,     // kLora / kFp8BlkLora: U / s B maps and ceil(r / 64)
                  const float* a_scale, const float* w_scale,     // kFp8: row scales of A and W; kLora: w_scale is the
                                                                  // optional per-column (DoRA) scale, may be null
-                 const Fp8BlockParams fb,                        // kFp8Blk only
+                 const Fp8BlockParams fb,                        // kFp8Blk / kFp8BlkLora only
                  const __grid_constant__ CUtensorMap tmap_r,     // staged epilogue: residual (read only when p.R)
                  const __grid_constant__ CUtensorMap tmap_d) {   //   and output, extents exactly those of the output
   constexpr bool kStaged = staged_epilogue(kMode);
   using Cfg = GemmCfg<BLOCK_N, kStaged>;
   constexpr int kStages = Cfg::STAGES;
-  constexpr int kBK = (kMode == kFp8 || kMode == kFp8Blk) ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
+  constexpr int kBK = fp8_mode(kMode) ? 2 * kBlockK : kBlockK;   // elements per k-block: always 128 bytes per row
   constexpr uint32_t kEpiBoxBytes = kBlockM * 128;   // one 128-row x 64-column box of the epilogue buffer
 
   extern __shared__ uint8_t smem_raw[];
@@ -167,7 +179,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       kMode == kConv ? (int64_t)cg.nb * cg.tiles_t * cg.tiles_h * cg.tiles_w : (p.M + kBlockM - 1) / kBlockM;
   const int64_t num_tiles = num_m_blocks * num_n_blocks;
   const int64_t num_k_blocks = (p.K + kBK - 1) / kBK;
-  const int64_t total_k_blocks = kMode == kLora ? num_k_blocks + lora_k_blocks : num_k_blocks;
+  const int64_t total_k_blocks = lora_mode(kMode) ? num_k_blocks + lora_k_blocks : num_k_blocks;
   // Tile t -> (m_blk, n_blk), in the order of the grid's CTAs: the tiles in flight at once share A panels and W.  conv:
   // m_blk -> (batch, t-tile, h-tile, w-tile), the box origin in OUTPUT coordinates.
   struct Tile {
@@ -191,7 +203,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w);
-    if constexpr (kMode == kLora) {
+    if constexpr (lora_mode(kMode)) {
       tma_prefetch_desc(&tmap_u);
       tma_prefetch_desc(&tmap_lb);
     }
@@ -226,7 +238,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         auto load_k_block = [&](int64_t kb) {
           mbar_wait_notrace(empty_bar(stage), phase ^ 1);
           mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);   // out-of-bounds box elements are zero filled and counted
-          if (kMode == kLora && kb >= num_k_blocks) {   // the rank tail beyond r is zero filled in both U and s B
+          if (lora_mode(kMode) && kb >= num_k_blocks) {   // the rank tail beyond r is zero filled in both U and s B
             const int32_t lk0 = (int32_t)(kb - num_k_blocks) * kBlockK;
             tma_load_2d(&tmap_u, full_bar(stage), smem_a(stage), lk0, a_row);
             tma_load_2d(&tmap_lb, full_bar(stage), smem_b(stage), lk0, w_row);
@@ -317,7 +329,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     float acc[BLOCK_N / 2];
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-    if constexpr (kMode == kFp8 || kMode == kFp8Blk) {
+    if constexpr (fp8_mode(kMode)) {
       // FP8 wgmma adds into its accumulator with fewer mantissa bits than an fp32 add, so a K-long sum in the wgmma
       // accumulator loses precision with K.  Each k-block (128 e4m3 elements) is summed into `part` by the tensor core and
       // promoted into the fp32 register accumulator `acc` before the next one: acc is an fp32 sum of 128-element partials.
@@ -328,16 +340,34 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       // kFp8Blk: the scale rows of this thread's two accumulator rows (clamped: rows >= M are computed but never stored)
       const float* sa_row0 = a_scale;
       const float* sa_row1 = a_scale;
-      if constexpr (kMode == kFp8Blk) {
+      if constexpr (kMode != kFp8) {
         const int64_t r0 = m_blk * kBlockM + cw * 64 + (tid_wg >> 5) * 16 + ((tid_wg & 31) >> 2);
         sa_row0 = a_scale + min(r0, p.M - 1) * fb.a_ld;
         sa_row1 = a_scale + min(r0 + 8, p.M - 1) * fb.a_ld;
       }
-      for (int64_t kb = 0; kb < total_k_blocks; ++kb) {
+      // One k-block: e4m3 (4 wgmma k32 steps, promoted with its A scales) or, is_tail (kFp8BlkLora's rank tail), bf16
+      // (4 wgmma k16 steps, promoted with scale 1: fmaf(p, 1, a) is p + a, one rounding).  Both step 32 bytes along K.
+      auto k_block = [&](int64_t kb, auto is_tail) {
+        constexpr bool tail = decltype(is_tail)::value;
         float s0 = 1.f, s1 = 1.f;
-        if constexpr (kMode == kFp8Blk) {   // issued before the wait: the loads overlap the TMA and the tensor core
+        if constexpr (kMode != kFp8 && !tail) {   // issued before the wait: the loads overlap the TMA and the tensor core
           s0 = __ldg(sa_row0 + kb * fb.a_kstride);
           s1 = __ldg(sa_row1 + kb * fb.a_kstride);
+        }
+        if constexpr (tail) {
+          // w_scale scales the FP8 sum only: applied once, before the tail's first k-block is promoted (a thread's
+          // columns are the same for both of its rows; columns >= N are clamped, never stored)
+          if (kb == num_k_blocks) {
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+              const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);
+              const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+              acc[4 * j] = __fmul_rn(acc[4 * j], sw.x);
+              acc[4 * j + 1] = __fmul_rn(acc[4 * j + 1], sw.y);
+              acc[4 * j + 2] = __fmul_rn(acc[4 * j + 2], sw.x);
+              acc[4 * j + 3] = __fmul_rn(acc[4 * j + 3], sw.y);
+            }
+          }
         }
         mbar_wait_notrace(full_bar(stage), phase);
         const uint64_t da = make_sw128_kmajor_desc(smem_a(stage) + (uint32_t)(cw * 64 * 128));
@@ -345,14 +375,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         wgmma_fence_regs(part);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
-          WgmmaFp8<BLOCK_N>::mma(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+        for (int k = 0; k < 4; ++k) {   // +32 bytes along K per step = +2 in the descriptor's 16-byte units
+          if constexpr (tail)
+            Wgmma<BLOCK_N>::mma(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+          else
+            WgmmaFp8<BLOCK_N>::mma(part, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+        }
         wgmma_commit();
         release_epi_buffer(kb);
         wgmma_wait<0>();   // this k-block's partial is complete and its stage has been read
         wgmma_fence_regs(part);
         if (tid_wg == 0) mbar_arrive(empty_bar(stage));
-        if constexpr (kMode == kFp8Blk) {   // acc[4 j + 2 h + e] belongs to row h of the fragment
+        if constexpr (kMode != kFp8) {   // acc[4 j + 2 h + e] belongs to row h of the fragment
 #pragma unroll
           for (int j = 0; j < BLOCK_N / 8; ++j) {
             acc[4 * j] = fmaf(part[4 * j], s0, acc[4 * j]);
@@ -365,6 +399,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] += part[i];
         }
         if (++stage == kStages) { stage = 0; phase ^= 1; }
+      };
+      for (int64_t kb = 0; kb < num_k_blocks; ++kb) k_block(kb, std::false_type{});
+      if constexpr (kMode == kFp8BlkLora) {
+        for (int64_t kb = num_k_blocks; kb < total_k_blocks; ++kb) k_block(kb, std::true_type{});
       }
     } else {
       int prev = 0;
@@ -390,16 +428,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       if (tid_wg == 0) mbar_arrive(empty_bar(prev));   // the tile's last stage: the next tile's k-blocks need it
     }
 
-    if constexpr (kMode == kLora) {
-      // DoRA: acc *= col_scale[n] (passed in the w_scale slot) before the epilogue adds the bias.  A thread's columns are
+    if constexpr (lora_mode(kMode)) {
+      // DoRA: acc *= col_scale[n] (kLora: passed in the w_scale slot) before the epilogue adds the bias.  A thread's columns are
       // the same for both of its rows, so each scale pair is loaded once per tile.  x * 1.0f is exact: an all-ones scale
       // leaves the accumulator's bits as they are.  Columns >= N are never stored, so their index is clamped instead of
       // branched around: the loads carry no control dependence and can all be in flight at once.
-      if (w_scale != nullptr) {
+      const float* col_scale = kMode == kLora ? w_scale : fb.col_scale;
+      if (col_scale != nullptr) {
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 8; ++j) {
           const int64_t n = min(n_blk * BLOCK_N + 8 * j + c_frag, p.N - 2);
-          const float2 cs = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+          const float2 cs = __ldg(reinterpret_cast<const float2*>(col_scale + n));
           acc[4 * j] *= cs.x;
           acc[4 * j + 1] *= cs.y;
           acc[4 * j + 2] *= cs.x;
@@ -408,7 +447,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
     }
 
-    if constexpr (kMode == kFp8Blk && BLOCK_N == 128) {
+    if constexpr ((kMode == kFp8Blk || kMode == kFp8BlkLora) && BLOCK_N == 128) {
       if (p.epilogue == OSB_EPI_BIAS_GELU_TANH_FP8) {
         // ===================== epilogue: GELU-tanh -> e4m3 codes + one scale per (row, 128 columns) =====================
         // N % 128 == 0 (host check): every column of the tile exists.  Rows >= M take part in the quad shuffles (all lanes
@@ -421,8 +460,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
           for (int j = 0; j < BLOCK_N / 8; ++j) {
             const int64_t n = n0 + 8 * j;
-            const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
-            float v0 = acc[4 * j + 2 * h] * sw.x, v1 = acc[4 * j + 2 * h + 1] * sw.y;
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if constexpr (kMode == kFp8Blk) {   // kFp8BlkLora: w_scale is already in the accumulator
+              const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n));
+              v0 *= sw.x;
+              v1 *= sw.y;
+            }
             if (p.bias) {
               const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
               v0 += b.x;
@@ -604,7 +647,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             if constexpr (kMode == kFp8) {
               v0 = __fmul_rn(v0, __fmul_rn(sa[h], sw.x));
               v1 = __fmul_rn(v1, __fmul_rn(sa[h], sw.y));
-            } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator
+            } else if constexpr (kMode == kFp8Blk) {   // the A scales are already in the accumulator (kFp8BlkLora: all scales)
               v0 = __fmul_rn(v0, sw.x);
               v1 = __fmul_rn(v1, sw.y);
             }
@@ -770,6 +813,8 @@ int gemm_init() {
   if ((rc = init_one<128, kFp8>())) return rc;
   if ((rc = init_one<64, kFp8Blk>())) return rc;
   if ((rc = init_one<128, kFp8Blk>())) return rc;
+  if ((rc = init_one<64, kFp8BlkLora>())) return rc;
+  if ((rc = init_one<128, kFp8BlkLora>())) return rc;
   return OSB_OK;
 }
 
@@ -792,7 +837,8 @@ static int pick_block_n(int64_t M, int64_t N) {
 }
 
 template <int BLOCK_N, int kMode = kFp8>
-static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream, const Fp8BlockParams& fb = Fp8BlockParams{}) {
+static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream, const Fp8BlockParams& fb = Fp8BlockParams{},
+                           const osb_lora_args* lora = nullptr) {
   CUtensorMap ta, tw;
   int rc = make_tmap_2d_e4m3(&ta, a.A, a.M, a.K, a.lda, kBlockM, 2 * kBlockK);
   if (rc) return rc;
@@ -815,6 +861,13 @@ static int launch_gemm_fp8(const osb_gemm_fp8_args& a, cudaStream_t stream, cons
   HeadTileParams ht = {};
   CUtensorMap tr = ta, td = ta;   // the FP8-emitting GELU epilogue writes no bf16 D (it may be null)
   if (a.epilogue != OSB_EPI_BIAS_GELU_TANH_FP8 && (rc = make_epilogue_maps(p, &tr, &td))) return rc;
+  if constexpr (kMode == kFp8BlkLora) {
+    CUtensorMap tu, tlb;
+    if ((rc = make_tmap_2d_bf16(&tu, lora->U, a.M, lora->r, lora->ldu, kBlockM, kBlockK))) return rc;
+    if ((rc = make_tmap_2d_bf16(&tlb, lora->B, a.N, lora->r, lora->ldb, BLOCK_N, kBlockK))) return rc;
+    return launch_kernel<BLOCK_N, kMode>(ta, tw, p, cg, ht, tiles, stream, &tu, &tlb, (lora->r + kBlockK - 1) / kBlockK,
+                                         a.a_scale, a.w_scale, fb, &tr, &td);
+  }
   return launch_kernel<BLOCK_N, kMode>(ta, tw, p, cg, ht, tiles, stream, nullptr, nullptr, 0, a.a_scale, a.w_scale, fb,
                                        &tr, &td);
 }
@@ -869,6 +922,18 @@ static int launch_conv(const osb_conv3d_args& a, const ConvGeom& cg, const uint3
 
 namespace osb {
 
+// The adapter operands of osb_gemm_lora and osb_gemm_fp8_lora (`fn` names the entry point in errors).
+static int check_lora_args(const char* fn, const osb_lora_args& l) {
+  OSB_REQUIRE(l.U && l.B, "%s: null U or B", fn);
+  OSB_REQUIRE(l.r > 0 && l.r % 8 == 0, "%s: rank r must be a positive multiple of 8 (zero-pad A and B), got %d", fn, l.r);
+  OSB_REQUIRE(l.ldu >= l.r && l.ldb >= l.r && l.ldu % 8 == 0 && l.ldb % 8 == 0 &&
+              ((reinterpret_cast<uintptr_t>(l.U) | reinterpret_cast<uintptr_t>(l.B)) & 15) == 0,
+              "%s: U and B must be 16-byte aligned with ldu, ldb >= r and multiples of 8 (r %d ldu %lld ldb %lld)", fn,
+              l.r, (long long)l.ldu, (long long)l.ldb);
+  OSB_REQUIRE((reinterpret_cast<uintptr_t>(l.col_scale) & 7) == 0, "%s: col_scale must be 8-byte aligned", fn);
+  return OSB_OK;
+}
+
 // Argument checks and tile-width dispatch shared by osb_gemm_bf16 and osb_gemm_lora (`fn` names the entry point in errors).
 static int gemm_dispatch(const char* fn, const osb_gemm_args* args, const osb_lora_args* lora, void* stream) {
   if (!initialised()) { set_error("osb_init() has not been called"); return OSB_ERR_NOT_INIT; }
@@ -895,14 +960,7 @@ static int gemm_dispatch(const char* fn, const osb_gemm_args* args, const osb_lo
               "%s: bias must be 16-byte aligned", fn);
   OSB_REQUIRE(a.cta_group >= 0 && a.cta_group <= 2, "%s: cta_group must be 0, 1 or 2", fn);
   if (lora != nullptr) {
-    const osb_lora_args& l = *lora;
-    OSB_REQUIRE(l.U && l.B, "%s: null U or B", fn);
-    OSB_REQUIRE(l.r > 0 && l.r % 8 == 0, "%s: rank r must be a positive multiple of 8 (zero-pad A and B), got %d", fn, l.r);
-    OSB_REQUIRE(l.ldu >= l.r && l.ldb >= l.r && l.ldu % 8 == 0 && l.ldb % 8 == 0 &&
-                ((reinterpret_cast<uintptr_t>(l.U) | reinterpret_cast<uintptr_t>(l.B)) & 15) == 0,
-                "%s: U and B must be 16-byte aligned with ldu, ldb >= r and multiples of 8 (r %d ldu %lld ldb %lld)", fn,
-                l.r, (long long)l.ldu, (long long)l.ldb);
-    OSB_REQUIRE((reinterpret_cast<uintptr_t>(l.col_scale) & 7) == 0, "%s: col_scale must be 8-byte aligned", fn);
+    if (int rc = check_lora_args(fn, *lora)) return rc;
   }
   const bool has_res = (a.epilogue == OSB_EPI_BIAS_GATE_RES) && a.R != nullptr;
   const int bn = a.block_n ? a.block_n : pick_block_n(a.M, a.N);
@@ -975,31 +1033,36 @@ extern "C" int osb_gemm_fp8(const osb_gemm_fp8_args* args, void* stream) {
   return OSB_ERR_UNSUPPORTED;
 }
 
-extern "C" int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* args, const osb_fp8_blocks_args* blk, void* stream) {
-  using namespace osb;
-  if (blk == nullptr) { set_error("osb_gemm_fp8_blocks: null block args"); return OSB_ERR_INVALID; }
+namespace osb {
+
+// osb_gemm_fp8_blocks, and with `lora` osb_gemm_fp8_lora (`fn` names the entry point in errors).
+static int fp8_blocks_dispatch(const char* fn, const osb_gemm_fp8_args* args, const osb_fp8_blocks_args* blk,
+                               const osb_lora_args* lora, void* stream) {
   const bool fp8_out = args != nullptr && args->epilogue == OSB_EPI_BIAS_GELU_TANH_FP8;
-  if (int rc = check_fp8_args("osb_gemm_fp8_blocks", args, fp8_out)) return rc;
+  if (int rc = check_fp8_args(fn, args, fp8_out)) return rc;
+  if (lora != nullptr) {
+    if (int rc = check_lora_args(fn, *lora)) return rc;
+  }
   const osb_gemm_fp8_args& a = *args;
   const osb_fp8_blocks_args& b = *blk;
   OSB_REQUIRE(b.a_scale_ld == 0 || b.a_scale_ld >= a.K / 128,
-              "osb_gemm_fp8_blocks: a_scale_ld must be 0 (per-row scales) or >= K / 128 (got %lld, K %lld)",
+              "%s: a_scale_ld must be 0 (per-row scales) or >= K / 128 (got %lld, K %lld)", fn,
               (long long)b.a_scale_ld, (long long)a.K);
   int bn = a.block_n ? a.block_n : (a.N <= 64 ? 64 : 128);
   if (fp8_out) {
     // one 128-column output tile = one scale block per row
-    OSB_REQUIRE(a.N % 128 == 0, "osb_gemm_fp8_blocks: the FP8 GELU epilogue needs N %% 128 == 0, got %lld", (long long)a.N);
-    OSB_REQUIRE(a.block_n == 0 || a.block_n == 128, "osb_gemm_fp8_blocks: the FP8 GELU epilogue needs block_n 128, got %d",
+    OSB_REQUIRE(a.N % 128 == 0, "%s: the FP8 GELU epilogue needs N %% 128 == 0, got %lld", fn, (long long)a.N);
+    OSB_REQUIRE(a.block_n == 0 || a.block_n == 128, "%s: the FP8 GELU epilogue needs block_n 128, got %d", fn,
                 a.block_n);
-    OSB_REQUIRE(b.D8 && b.d_scale, "osb_gemm_fp8_blocks: the FP8 GELU epilogue needs D8 and d_scale");
+    OSB_REQUIRE(b.D8 && b.d_scale, "%s: the FP8 GELU epilogue needs D8 and d_scale", fn);
     OSB_REQUIRE(b.ldd8 >= a.N && b.ldd8 % 2 == 0 && (reinterpret_cast<uintptr_t>(b.D8) & 1) == 0 &&
                 b.ld_dscale >= a.N / 128 && (reinterpret_cast<uintptr_t>(b.d_scale) & 3) == 0,
-                "osb_gemm_fp8_blocks: D8 must be 2-byte aligned with even ldd8 >= N, d_scale 4-byte aligned with "
-                "ld_dscale >= N / 128 (ldd8 %lld ld_dscale %lld)", (long long)b.ldd8, (long long)b.ld_dscale);
+                "%s: D8 must be 2-byte aligned with even ldd8 >= N, d_scale 4-byte aligned with "
+                "ld_dscale >= N / 128 (ldd8 %lld ld_dscale %lld)", fn, (long long)b.ldd8, (long long)b.ld_dscale);
     bn = 128;
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (b.a_scale_ld == 0 && !fp8_out) {   // per-row scales and a bf16 epilogue: exactly osb_gemm_fp8
+  if (lora == nullptr && b.a_scale_ld == 0 && !fp8_out) {   // per-row scales and a bf16 epilogue: exactly osb_gemm_fp8
     if (bn == 64) return launch_gemm_fp8<64>(a, s);
     if (bn == 128) return launch_gemm_fp8<128>(a, s);
   } else {
@@ -1010,11 +1073,30 @@ extern "C" int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* args, const osb_fp8_
     fb.d_scale = b.d_scale;
     fb.ldd8 = b.ldd8;
     fb.ld_dscale = b.ld_dscale;
-    if (bn == 64) return launch_gemm_fp8<64, kFp8Blk>(a, s, fb);
-    if (bn == 128) return launch_gemm_fp8<128, kFp8Blk>(a, s, fb);
+    if (lora != nullptr) {
+      fb.col_scale = lora->col_scale;
+      if (bn == 64) return launch_gemm_fp8<64, kFp8BlkLora>(a, s, fb, lora);
+      if (bn == 128) return launch_gemm_fp8<128, kFp8BlkLora>(a, s, fb, lora);
+    } else {
+      if (bn == 64) return launch_gemm_fp8<64, kFp8Blk>(a, s, fb);
+      if (bn == 128) return launch_gemm_fp8<128, kFp8Blk>(a, s, fb);
+    }
   }
-  set_error("osb_gemm_fp8_blocks: unsupported block_n %d (64 or 128)", bn);
+  set_error("%s: unsupported block_n %d (64 or 128)", fn, bn);
   return OSB_ERR_UNSUPPORTED;
+}
+
+}  // namespace osb
+
+extern "C" int osb_gemm_fp8_blocks(const osb_gemm_fp8_args* args, const osb_fp8_blocks_args* blk, void* stream) {
+  if (blk == nullptr) { osb::set_error("osb_gemm_fp8_blocks: null block args"); return OSB_ERR_INVALID; }
+  return osb::fp8_blocks_dispatch("osb_gemm_fp8_blocks", args, blk, nullptr, stream);
+}
+
+extern "C" int osb_gemm_fp8_lora(const osb_gemm_fp8_args* args, const osb_fp8_blocks_args* blk,
+                                 const osb_lora_args* lora, void* stream) {
+  if (blk == nullptr || lora == nullptr) { osb::set_error("osb_gemm_fp8_lora: null block or lora args"); return OSB_ERR_INVALID; }
+  return osb::fp8_blocks_dispatch("osb_gemm_fp8_lora", args, blk, lora, stream);
 }
 
 extern "C" int osb_conv3d_ndhwc(const osb_conv3d_args* args, void* stream) {

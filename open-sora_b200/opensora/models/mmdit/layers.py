@@ -33,7 +33,13 @@ blocks, per stream: ln_modulate_fp8 -> the q|k|v GEMM on per-row A (`osb_gemm_fp
 output leaves as e4m3 codes with 1 x 128 block scales (`osb_attn_fp8_blocks` with FP8 attention on, else the bf16
 attention and `osb_quant_blocks_fp8`) -> `proj` on block-scaled A (gate + residual).  Single blocks: ONE ln_modulate_fp8
 pass feeds the qkv GEMM and the mlp GEMM, the attention output fills columns 0..C-1 of the e4m3 cat buffer the same
-way, and no bf16 LN pass runs."""
+way, and no bf16 LN pass runs.
+
+LoRA on FP8 (MMDiTModel.enable_fp8(..., lora=True), `Fp8State.lora`): an adapter on a Linear that runs on e4m3 is applied by
+`osb_gemm_fp8_lora` (the FP8 GEMM with U (s B)^T, and DoRA's column scale, in the same fp32 accumulator).  Its down
+projection U = x A_cat^T reads the e4m3 codes the base GEMM reads (per-row codes of ln_modulate_fp8 for q|k|v, fc1 and
+linear1; block-scaled codes for proj, fc2 and linear2) on `osb_gemm_fp8_blocks` with A_cat quantized per row, one down
+GEMM per shared input as on the bf16 path."""
 from __future__ import annotations
 
 import math
@@ -112,6 +118,19 @@ def _gemm(osb, x2d: Tensor, w: Tensor, b, lora, u: Tensor | None = None, **kw) -
     if lora[2] is not None:
         kw["col_scale"] = lora[2]
     return osb.gemm_lora(x2d, w, b, u, lora[1], **kw)
+
+
+def _gemm8(osb, a8: Tensor, a_s: Tensor, w8: Tensor, w_s: Tensor, b, lora, u: Tensor | None, **kw):
+    """osb.gemm_fp8_blocks, or with lora = (A_cat, B, col_scale) and its down projection `u` the FP8 GEMM with the
+    unmerged update (osb.gemm_fp8_lora)."""
+    if lora is None or lora[1] is None:
+        return osb.gemm_fp8_blocks(a8, a_s, w8, w_s, b, **kw)
+    return osb.gemm_fp8_lora(a8, a_s, w8, w_s, b, u, lora[1], col_scale=lora[2], **kw)
+
+
+def _one(pack, i: int = 0):
+    """(A_cat, B, col_scale) of group i of a lora_pack result, or None."""
+    return None if pack is None else (pack[0], pack[1][i], pack[2][i])
 
 
 def _linear(x2d: Tensor, lin: nn.Linear, **kw) -> Tensor:
@@ -316,11 +335,12 @@ def _sp_attention(osb, qkv: Tensor, out_cols: int, B: int, Lloc: int, H: int, D:
 class Fp8State:
     """What the FP8 path of one MMDiTModel keeps: e4m3 weights with per-output-channel scales, quantized once per block
     and MLP (`weights`) and, with `proj`, per block and stream for the q|k|v and attention-output projections
-    (`proj_weights`), and e4m3 / scale workspaces reused by every block, one per shape (`buf`)."""
+    (`proj_weights`), and e4m3 / scale workspaces reused by every block, one per shape (`buf`).  With `lora`, adapters on
+    those Linears run on the FP8 path: the e4m3 copy of each pack's A_cat is cached per use (`down`)."""
 
-    def __init__(self, proj: bool = False):
-        self.proj = proj
-        self._w, self._ws = {}, {}
+    def __init__(self, proj: bool = False, lora: bool = False):
+        self.proj, self.lora = proj, lora
+        self._w, self._ws, self._la = {}, {}, {}
 
     @staticmethod
     def proj_linears(blk: nn.Module, kind: str):
@@ -342,7 +362,7 @@ class Fp8State:
         if hit is None or hit[0] is not blk:
             lins = self.proj_linears(blk, kind)
             for lin in lins:
-                if adapter_of(lin) is not None:
+                if adapter_of(lin) is not None and not self.lora:
                     raise ValueError("FP8 projections: a LoRA / DoRA adapter on a projection Linear cannot run on the FP8 "
                                      "path; unload_lora or disable_fp8 first")
             if kind != "single":
@@ -385,7 +405,7 @@ class Fp8State:
         if hit is None or hit[0] is not blk:
             l1, (lo, hi), l2 = self.mlp_linears(blk, kind)
             for lin in (l1, l2):
-                if adapter_of(lin) is not None:
+                if adapter_of(lin) is not None and not self.lora:
                     raise ValueError("FP8 MLPs: a LoRA / DoRA adapter on an MLP Linear cannot run on the FP8 path; "
                                      "unload_lora or disable_fp8 first")
             w1, s1 = osb.quant_blocks_fp8(l1.weight[lo:hi], block=l1.in_features)
@@ -393,6 +413,30 @@ class Fp8State:
             b1 = None if l1.bias is None else l1.bias[lo:hi]
             hit = self._w[key] = (blk, (w1, s1.view(-1), b1, w2, s2.view(-1), l2.bias))
         return hit[1]
+
+    def pack(self, groups):
+        """lora_pack(groups) when adapters run on the FP8 path, else None."""
+        return lora_pack(groups) if self.lora else None
+
+    def mlp_lora(self, blk: nn.Module, kind: str):
+        """(fc1 adapter, fc2 adapter) of one MLP as (A_cat, B, col_scale) or None each (see mlp_linears)."""
+        if not self.lora:
+            return None, None
+        l1, (lo, hi), l2 = self.mlp_linears(blk, kind)
+        return _one(lora_pack([[(l1, lo, hi)]])), _one(lora_pack([[(l2, 0, l2.out_features)]]))
+
+    def down(self, osb, key, lora, a8: Tensor, a_s: Tensor) -> Tensor | None:
+        """U = x A_cat^T (bf16 [rows, R]) of the adapters whose GEMMs read the e4m3 input (a8, a_s), on the block-scaled
+        FP8 GEMM; `lora` is a pack or one of its groups (A_cat first), None without adapters.  A_cat is quantized per row once per `key` and pack: lora_pack hands out a new
+        A_cat whenever the adapter state changes (reload, edited A / B, DoRA magnitude or base weight)."""
+        if lora is None:
+            return None
+        A = lora[0]
+        hit = self._la.get(key)
+        if hit is None or hit[0] is not A:
+            q, sc = osb.quant_blocks_fp8(A, block=A.shape[1])
+            hit = self._la[key] = (A, q, sc.view(-1))
+        return osb.gemm_fp8_blocks(a8, a_s, hit[1], hit[2])
 
     def buf(self, name: str, *shape, dtype=torch.float32, device=None) -> Tensor:
         key = (name, shape, dtype, device)
@@ -405,15 +449,16 @@ class Fp8State:
 def _mlp_fp8(osb, fp8: Fp8State, blk: nn.Module, kind: str, x: Tensor, mod, n: int) -> None:
     """x += gate * MLP((1 + scale) * LN(x) + shift) in place, on FP8 operands (x: [rows, C] bf16, group_rows = n)."""
     w1, s1, b1, w2, s2, b2 = fp8.weights(osb, blk, kind)
+    l1, l2 = fp8.mlp_lora(blk, kind)
     rows, C = x.shape
     hid, dev, f8 = w1.shape[0], x.device, torch.float8_e4m3fn
     x8, xs = osb.ln_modulate_fp8(x, mod.shift, mod.scale, group_rows=n, out=fp8.buf("x8", rows, C, dtype=f8, device=dev),
                                  out_scale=fp8.buf("xs", rows, device=dev))
-    h8, hs = osb.gemm_fp8_blocks(x8, xs, w1, s1, b1, epilogue=osb.EPI_BIAS_GELU_TANH_FP8,
-                                 out=fp8.buf("h8", rows, hid, dtype=f8, device=dev),
-                                 out_scale=fp8.buf("hs", rows, hid // 128, device=dev))
-    osb.gemm_fp8_blocks(h8, hs, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x, gate=mod.gate, group_rows=n,
-                        out=x)
+    h8, hs = _gemm8(osb, x8, xs, w1, s1, b1, l1, fp8.down(osb, (id(blk), kind, "fc1"), l1, x8, xs),
+                    epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=fp8.buf("h8", rows, hid, dtype=f8, device=dev),
+                    out_scale=fp8.buf("hs", rows, hid // 128, device=dev))
+    _gemm8(osb, h8, hs, w2, s2, b2, l2, fp8.down(osb, (id(blk), kind, "fc2"), l2, h8, hs), epilogue=osb.EPI_BIAS_GATE_RES,
+           residual=x, gate=mod.gate, group_rows=n, out=x)
 
 
 def _qkv_fp8(osb, fp8: Fp8State, blk: nn.Module, kind: str, x: Tensor, mod, n: int, qkv: Tensor, L: int,
@@ -421,12 +466,15 @@ def _qkv_fp8(osb, fp8: Fp8State, blk: nn.Module, kind: str, x: Tensor, mod, n: i
     """q|k|v = W_qkv ((1 + scale) * LN(x) + shift) + b on FP8 operands: one ln_modulate_fp8 pass (codes + row scales,
     returned) and, per sample of n rows, one row-scaled e4m3 GEMM into rows b*L + off .. of the joint buffer `qkv`."""
     wq, sq, bq = fp8.proj_weights(osb, blk, kind)[:3]
+    lq = _ProcessorBase._qkv_lora(blk.img_attn if kind == "img" else blk.txt_attn) if fp8.lora else None
     rows, C = x.shape
     dev, f8 = x.device, torch.float8_e4m3fn
     x8, xs = osb.ln_modulate_fp8(x, mod.shift, mod.scale, group_rows=n, out=fp8.buf("x8", rows, C, dtype=f8, device=dev),
                                  out_scale=fp8.buf("xs", rows, device=dev))
+    u = fp8.down(osb, (id(blk), kind, "qkv"), lq, x8, xs)   # one down projection over all rows of the stream
     for b in range(rows // n):
-        osb.gemm_fp8_blocks(x8[b * n:(b + 1) * n], xs[b * n:(b + 1) * n], wq, sq, bq, out=qkv[b * L + off:b * L + off + n])
+        r = slice(b * n, (b + 1) * n)
+        _gemm8(osb, x8[r], xs[r], wq, sq, bq, lq, None if u is None else u[r], out=qkv[b * L + off:b * L + off + n])
     return x8, xs
 
 
@@ -518,12 +566,17 @@ class DoubleStreamBlockProcessor(_ProcessorBase):
             ao8 = (fp8.buf("ao8", rows, C, dtype=f8, device=dev), fp8.buf("aos", rows, C // 128, device=dev))
             _sp_attention(osb, qkv, C, B, L, H, D, kw, split_full, img.dtype, dev, getattr(vec, "_osb_fp8_attn", None),
                           out8=ao8)
-            for x2, x_o, mod, n, off, kind in ((img2, img_o, im1, Li, Lt, "img"), (txt2, txt_o, tm1, Lt, 0, "txt")):
+            # both output projections read ao8: one down projection for their adapters
+            lp = fp8.pack([[(attn.img_attn.proj, 0, C)], [(attn.txt_attn.proj, 0, C)]])
+            up = fp8.down(osb, (id(attn), "proj"), lp, ao8[0], ao8[1])
+            for i, (x2, x_o, mod, n, off, kind) in enumerate(((img2, img_o, im1, Li, Lt, "img"),
+                                                              (txt2, txt_o, tm1, Lt, 0, "txt"))):
                 wp, sp, bp = fp8.proj_weights(osb, attn, kind)[3:]
                 for b in range(B if n else 0):
                     r = slice(b * L + off, b * L + off + n)
-                    osb.gemm_fp8_blocks(ao8[0][r], ao8[1][r], wp, sp, bp, epilogue=osb.EPI_BIAS_GATE_RES,
-                                        residual=x2[b * n:(b + 1) * n], gate=mod.gate[b:b + 1], out=x_o[b * n:(b + 1) * n])
+                    _gemm8(osb, ao8[0][r], ao8[1][r], wp, sp, bp, _one(lp, i), None if up is None else up[r],
+                           epilogue=osb.EPI_BIAS_GATE_RES, residual=x2[b * n:(b + 1) * n], gate=mod.gate[b:b + 1],
+                           out=x_o[b * n:(b + 1) * n])
         else:
             self._proj_bf16(osb, attn, qkv, kw, split_full, img2, txt2, img_o, txt_o, im1, tm1, vec, B, L, Li, Lt, H, D)
         # x + gate * MLP((1 + scale) * LN(x) + shift)   (layers.py:248, 252)
@@ -676,9 +729,13 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         wq, sq, bq = fp8.proj_weights(osb, attn, "single")[:3]
         wm, sm, bm, w2, s2, b2 = fp8.weights(osb, attn, "single")
         rows, M4, dev, f8 = B * L, wm.shape[0], x2.device, torch.float8_e4m3fn
+        lo = SingleStreamBlockProcessor._split_lora(attn, M4) if fp8.lora else None
+        lq, lm = (None, None) if lo is None else lo
+        l2 = fp8.mlp_lora(attn, "single")[1]
         x8, xs = osb.ln_modulate_fp8(x2, mod.shift, mod.scale, group_rows=L,
                                      out=fp8.buf("x8", rows, C, dtype=f8, device=dev), out_scale=fp8.buf("xs", rows, device=dev))
-        qkv = osb.gemm_fp8_blocks(x8, xs, wq, sq, bq)
+        u = fp8.down(osb, (id(attn), "linear1"), lq, x8, xs)   # one down projection for the qkv and mlp parts
+        qkv = _gemm8(osb, x8, xs, wq, sq, bq, lq, u)
         cat8 = fp8.buf("cat8", rows, C + M4, dtype=f8, device=dev)
         cats = fp8.buf("cats", rows, (C + M4) // 128, device=dev)
         cos, sin, half = _rope(pe)
@@ -686,10 +743,10 @@ class SingleStreamBlockProcessor(_ProcessorBase):
                   rope_half=half)
         _sp_attention(osb, qkv, C, B, L, H, D, kw, 0, x2.dtype, dev, getattr(vec, "_osb_fp8_attn", None),
                       out8=(cat8[:, :C], cats[:, :C // 128]))
-        osb.gemm_fp8_blocks(x8, xs, wm, sm, bm, epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=cat8[:, C:],
-                            out_scale=cats[:, C // 128:])
-        return osb.gemm_fp8_blocks(cat8, cats, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
-                                   group_rows=L)
+        _gemm8(osb, x8, xs, wm, sm, bm, lm, u, epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=cat8[:, C:],
+               out_scale=cats[:, C // 128:])
+        return _gemm8(osb, cat8, cats, w2, s2, b2, l2, fp8.down(osb, (id(attn), "linear2"), l2, cat8, cats),
+                      epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate, group_rows=L)
 
     @staticmethod
     def _fp8_tail(osb, fp8: Fp8State, attn: nn.Module, x2: Tensor, qkv: Tensor, mod, B: int, L: int, C: int, H: int,
@@ -698,6 +755,7 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         into columns 0..C-1, the mlp part of linear1 (on its own FP8 LN+modulate) emits its GELU codes into columns C..,
         and linear2 is one block-scaled FP8 GEMM."""
         wm, sm, bm, w2, s2, b2 = fp8.weights(osb, attn, "single")
+        l1, l2 = fp8.mlp_lora(attn, "single")
         rows, M4, dev, f8 = B * L, wm.shape[0], x2.device, torch.float8_e4m3fn
         cat8 = fp8.buf("cat8", rows, C + M4, dtype=f8, device=dev)
         cats = fp8.buf("cats", rows, (C + M4) // 128, device=dev)
@@ -705,10 +763,10 @@ class SingleStreamBlockProcessor(_ProcessorBase):
         osb.quant_blocks_fp8(ao, out=cat8[:, :C], out_scale=cats[:, :C // 128])
         x8, xs = osb.ln_modulate_fp8(x2, mod.shift, mod.scale, group_rows=L,
                                      out=fp8.buf("x8", rows, C, dtype=f8, device=dev), out_scale=fp8.buf("xs", rows, device=dev))
-        osb.gemm_fp8_blocks(x8, xs, wm, sm, bm, epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=cat8[:, C:],
-                            out_scale=cats[:, C // 128:])
-        return osb.gemm_fp8_blocks(cat8, cats, w2, s2, b2, epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate,
-                                   group_rows=L)
+        _gemm8(osb, x8, xs, wm, sm, bm, l1, fp8.down(osb, (id(attn), "single", "fc1"), l1, x8, xs),
+               epilogue=osb.EPI_BIAS_GELU_TANH_FP8, out=cat8[:, C:], out_scale=cats[:, C // 128:])
+        return _gemm8(osb, cat8, cats, w2, s2, b2, l2, fp8.down(osb, (id(attn), "linear2"), l2, cat8, cats),
+                      epilogue=osb.EPI_BIAS_GATE_RES, residual=x2, gate=mod.gate, group_rows=L)
 
 
 class SingleStreamBlock(nn.Module):

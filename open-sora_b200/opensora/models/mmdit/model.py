@@ -86,6 +86,7 @@ class MMDiTModel(nn.Module):
         self._sp_group = None
         self._fp8 = False
         self._fp8_proj = False
+        self._fp8_lora = False
         self._fp8_state = None
         self._fp8_attn = False
         self._fp8_attn_state = None
@@ -214,7 +215,7 @@ class MMDiTModel(nn.Module):
         blocks = [(b, k) for b in self.double_blocks for k in ("img", "txt")] + [(b, "single") for b in self.single_blocks]
         return [names[id(lin)] for blk, kind in blocks for lin in Fp8State.proj_linears(blk, kind)]
 
-    def enable_fp8(self, projections: bool = False) -> None:
+    def enable_fp8(self, projections: bool = False, lora: bool = False) -> None:
         """Run the MLPs of every double and single block on FP8 (e4m3) tensor cores.  The weights are quantized per output
         channel (s = amax / 448) into a per-model cache; the bf16 parameters and the state dict stay as they are.  The fc1
         input is the fp32 LN+modulate row, quantized per row; the fc2 / linear2 input is quantized per 1 x 128 block by
@@ -227,7 +228,15 @@ class MMDiTModel(nn.Module):
         LN+modulate row quantized per row (in a single block the same codes feed its qkv and mlp GEMMs), the `proj` /
         linear2 attention input per 1 x 128 block (by the FP8 attention kernel itself when `enable_fp8_attention()` is on,
         else by osb_quant_blocks_fp8).  Every block Linear then runs on FP8; modulation, embedders and the final layer
-        stay bf16.  LoRA / DoRA adapters on those projection Linears (`fp8_proj_linears()`) are refused as well."""
+        stay bf16.  LoRA / DoRA adapters on those projection Linears (`fp8_proj_linears()`) are refused as well.
+
+        `lora=True` runs LoRA / DoRA adapters on the FP8 Linears instead of refusing them, whether they are loaded
+        before or after this call: each adapted GEMM is osb_gemm_fp8_lora, the e4m3 GEMM with the bf16 update
+        U (s B)^T (and DoRA's column scale) in the same fp32 accumulator, and U = x A_cat^T is one block-scaled FP8 GEMM per
+        shared input that reads the same e4m3 codes as the base GEMM, with lora_A quantized per row (cached per adapter
+        state).  This is opt-in because the update then carries FP8 error that the bf16 adapter path does not (e4m3
+        activations times an e4m3 copy of lora_A): enabling FP8 never silently changes how a loaded adapter computes.
+        With no adapter loaded the output is that of `enable_fp8(projections)`."""
         C, hid = self.hidden_size, int(self.hidden_size * self.config.mlp_ratio)
         if C % 128 or hid % 128:
             raise ValueError(f"FP8 MLPs need the hidden size ({C}) and the MLP width ({hid}) to be multiples of 128 "
@@ -235,16 +244,16 @@ class MMDiTModel(nn.Module):
         if C > 4096:
             raise ValueError(f"FP8 MLPs need a hidden size <= 4096 (the FP8 LN+modulate holds one row), got {C}")
         mods = dict(self.named_modules())
-        adapted = [n for n in self.fp8_mlp_linears() if adapter_of(mods[n]) is not None]
+        adapted = [] if lora else [n for n in self.fp8_mlp_linears() if adapter_of(mods[n]) is not None]
         if adapted:
             raise ValueError(f"FP8 MLPs cannot run LoRA / DoRA adapters on MLP Linears ({adapted[0]} has one): "
                              "unload_lora first")
-        if projections:
+        if projections and not lora:
             adapted = [n for n in self.fp8_proj_linears() if adapter_of(mods[n]) is not None]
             if adapted:
                 raise ValueError(f"FP8 projections cannot run LoRA / DoRA adapters on projection Linears ({adapted[0]} "
                                  "has one): unload_lora first")
-        state = Fp8State(projections)
+        state = Fp8State(projections, lora)
         w = self.img_in.weight
         if w.is_cuda:   # quantized now; a model not yet on the GPU quantizes at its first forward
             import osb200
@@ -253,11 +262,12 @@ class MMDiTModel(nn.Module):
                 state.weights(osb200, blk, kind)
                 if projections:
                     state.proj_weights(osb200, blk, kind)
-        self._fp8_state, self._fp8, self._fp8_proj = state, True, projections
+        self._fp8_state, self._fp8, self._fp8_proj, self._fp8_lora = state, True, projections, lora
 
     def disable_fp8(self) -> None:
-        """Back to the bf16 MLPs and projections; the FP8 weight copies and workspaces are released."""
-        self._fp8, self._fp8_proj, self._fp8_state = False, False, None
+        """Back to the bf16 MLPs and projections (adapters on the bf16 LoRA path); the FP8 weight copies and workspaces
+        are released."""
+        self._fp8, self._fp8_proj, self._fp8_lora, self._fp8_state = False, False, False, None
 
     # ---- FP8 (e4m3) attention -------------------------------------------------------------------------------------
     def enable_fp8_attention(self) -> None:
@@ -309,7 +319,7 @@ class MMDiTModel(nn.Module):
         self._grouped_modulation(vec)
         if self._fp8:
             if self._fp8_state is None:
-                self._fp8_state = Fp8State(self._fp8_proj)
+                self._fp8_state = Fp8State(self._fp8_proj, self._fp8_lora)
             vec._osb_fp8 = self._fp8_state
         if self._fp8_attn:
             if self._fp8_attn_state is None:

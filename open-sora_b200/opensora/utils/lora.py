@@ -336,12 +336,12 @@ def load_lora(model: nn.Module, path: str, scale: float = 1.0) -> nn.Module:
             used.add(km)
             mag = weights[km]
         plan.append((name, lin, r, s, weights[ka], weights[kb], mag))
-    if getattr(model, "_fp8", False):
+    if getattr(model, "_fp8", False) and not getattr(model, "_fp8_lora", False):
         on_mlp = sorted({p[0] for p in plan} & set(model.fp8_mlp_linears()))
         if on_mlp:
             raise ValueError(f"the model runs FP8 MLPs, which take no LoRA / DoRA adapter on an MLP Linear "
                              f"(target '{on_mlp[0]}'): disable_fp8 first")
-    if getattr(model, "_fp8_proj", False):
+    if getattr(model, "_fp8_proj", False) and not getattr(model, "_fp8_lora", False):
         on_proj = sorted({p[0] for p in plan} & set(model.fp8_proj_linears()))
         if on_proj:
             raise ValueError(f"the model runs FP8 projections, which take no LoRA / DoRA adapter on a projection Linear "

@@ -46,6 +46,7 @@ EXPORTS = (
     "osb_head_tiles_fp8",
     "osb_attn_tiles_fp8",
     "osb_attn_frames",
+    "osb_gemm_fp8_lora",
 )
 
 EPI_BIAS, EPI_BIAS_GELU_TANH, EPI_BIAS_GATE_RES = 0, 1, 2
@@ -84,6 +85,7 @@ def _load() -> C.CDLL:
     lib.osb_quant_rows_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int,
                                        C.c_void_p]
     lib.osb_gemm_fp8_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.osb_gemm_fp8_lora.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.osb_quant_blocks_fp8.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64,
                                          C.c_int, C.c_int, C.c_void_p]
     lib.osb_attn_short.argtypes = [C.c_void_p, C.c_void_p]
@@ -575,26 +577,59 @@ def gemm_fp8_blocks(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_
     * acc_kb + bias).  EPI_BIAS, EPI_BIAS_GELU_TANH and EPI_BIAS_GATE_RES write bf16 `out` as in `gemm`.
     EPI_BIAS_GELU_TANH_FP8 writes e4m3 `out` [M, N] and fp32 `out_scale` [M, N / 128] (both row stride free, e.g. column
     slices of a wider buffer) and returns (out, out_scale); N % 128 == 0."""
+    return _gemm_fp8_blocks("gemm_fp8_blocks", a8, a_scale, w8, w_scale, bias, epilogue, residual, gate, group_rows,
+                            mod_index, out, out_scale, block_n, None)
+
+
+def gemm_fp8_lora(a8, a_scale, w8, w_scale, bias, u, b, *, epilogue: int = EPI_BIAS, residual=None, gate=None,
+                  group_rows: int = 0, mod_index=None, out=None, out_scale=None, block_n: int = 0, col_scale=None):
+    """`gemm_fp8_blocks` plus an unmerged LoRA update in the same fp32 accumulator (osb_gemm_fp8_lora):
+    out = epilogue(g * (w_scale[n] * sum_kb a_scale[m, kb] * acc_kb + u @ b.T) + bias), w_scale on the FP8 sum only.
+    u bf16 [M, r] = the down projection (row stride free), b bf16 [N, r] = scaling * lora_B, r a multiple of 8;
+    col_scale: None (g = 1) or a contiguous fp32 [N] tensor g on a8's device (DoRA).  Every epilogue of
+    `gemm_fp8_blocks`, EPI_BIAS_GELU_TANH_FP8 included (the update enters before the GELU)."""
+    import torch
+
+    _need(u, torch.bfloat16, "u"); _need(b, torch.bfloat16, "b")
+    if u is None or b is None or u.dim() != 2 or b.dim() != 2 or u.shape[0] != a8.shape[0] \
+            or b.shape[0] != w8.shape[0] or u.shape[1] != b.shape[1]:
+        raise OsbError(f"gemm_fp8_lora: u must be [M, r] and b [N, r] for a {tuple(a8.shape)} x {tuple(w8.shape)} GEMM, "
+                       f"got {None if u is None else tuple(u.shape)} and {None if b is None else tuple(b.shape)}")
+    if col_scale is not None:
+        if col_scale.dtype != torch.float32 or col_scale.shape != (w8.shape[0],) or not col_scale.is_contiguous() \
+                or col_scale.device != a8.device:
+            raise OsbError(f"gemm_fp8_lora: col_scale must be a contiguous float32 [{w8.shape[0]}] tensor on "
+                           f"{a8.device}, got {col_scale.dtype} {tuple(col_scale.shape)} on {col_scale.device}")
+    la = LoraArgs()
+    la.U, la.B, la.ldu, la.ldb, la.r = u.data_ptr(), b.data_ptr(), u.stride(0), b.stride(0), u.shape[1]
+    la.col_scale = None if col_scale is None else col_scale.data_ptr()
+    return _gemm_fp8_blocks("gemm_fp8_lora", a8, a_scale, w8, w_scale, bias, epilogue, residual, gate, group_rows,
+                            mod_index, out, out_scale, block_n, la)
+
+
+def _gemm_fp8_blocks(fn, a8, a_scale, w8, w_scale, bias, epilogue, residual, gate, group_rows, mod_index, out,
+                     out_scale, block_n, la):
+    """gemm_fp8_blocks, or with `la` (LoraArgs) gemm_fp8_lora; `fn` names the function in errors."""
     import torch
 
     _need(a8, torch.float8_e4m3fn, "a8"); _need(w8, torch.float8_e4m3fn, "w8"); _need(w_scale, torch.float32, "w_scale")
     _need(bias, torch.bfloat16, "bias"); _need(residual, torch.bfloat16, "residual"); _need(gate, torch.float32, "gate")
     _need(mod_index, torch.int32, "mod_index")
     if a8.dim() != 2 or w8.dim() != 2 or a8.shape[1] != w8.shape[1]:
-        raise OsbError(f"gemm_fp8_blocks: a8 [M, K] and w8 [N, K] expected, got {tuple(a8.shape)} and {tuple(w8.shape)}")
+        raise OsbError(f"{fn}: a8 [M, K] and w8 [N, K] expected, got {tuple(a8.shape)} and {tuple(w8.shape)}")
     M, K = a8.shape
     N = w8.shape[0]
     if w_scale is None or w_scale.shape != (N,):
-        raise OsbError(f"gemm_fp8_blocks: w_scale must be [{N}]")
+        raise OsbError(f"{fn}: w_scale must be [{N}]")
     b = Fp8BlocksArgs()
     if a_scale is not None and a_scale.dim() == 1:
         _need(a_scale, torch.float32, "a_scale")
         if a_scale.shape != (M,):
-            raise OsbError(f"gemm_fp8_blocks: a per-row a_scale must be [{M}], got {tuple(a_scale.shape)}")
+            raise OsbError(f"{fn}: a per-row a_scale must be [{M}], got {tuple(a_scale.shape)}")
     else:
         b.a_scale_ld = _scale_view(a_scale, M, K // 128, "a_scale")
     fp8_out = epilogue == EPI_BIAS_GELU_TANH_FP8
-    _epilogue_shapes("gemm_fp8_blocks", M, N, N, out, bias, residual, gate, group_rows, mod_index)
+    _epilogue_shapes(fn, M, N, N, out, bias, residual, gate, group_rows, mod_index)
     if fp8_out:
         if out is None:
             out = torch.empty((M, N), dtype=torch.float8_e4m3fn, device=a8.device)
@@ -602,7 +637,7 @@ def gemm_fp8_blocks(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_
             out_scale = torch.empty((M, N // 128), dtype=torch.float32, device=a8.device)
         _need(out, torch.float8_e4m3fn, "out")
         if out.shape != (M, N):
-            raise OsbError(f"gemm_fp8_blocks: out must be e4m3 [{M}, {N}], got {tuple(out.shape)}")
+            raise OsbError(f"{fn}: out must be e4m3 [{M}, {N}], got {tuple(out.shape)}")
         b.D8, b.ldd8 = out.data_ptr(), out.stride(0)
         b.d_scale, b.ld_dscale = out_scale.data_ptr(), _scale_view(out_scale, M, N // 128, "out_scale")
     else:
@@ -622,8 +657,12 @@ def gemm_fp8_blocks(a8, a_scale, w8, w_scale, bias=None, *, epilogue: int = EPI_
     g.group_rows = group_rows if group_rows > 0 else M
     g.gate_stride = gate.stride(0) if gate is not None else 0
     g.epilogue, g.block_n = epilogue, block_n
-    with _Timed("gemm_fp8", 2.0 * M * N * K):
-        _check(_lib.osb_gemm_fp8_blocks(C.byref(g), C.byref(b), _stream()), "osb_gemm_fp8_blocks")
+    if la is None:
+        with _Timed("gemm_fp8", 2.0 * M * N * K):
+            _check(_lib.osb_gemm_fp8_blocks(C.byref(g), C.byref(b), _stream()), "osb_gemm_fp8_blocks")
+    else:
+        with _Timed("gemm_fp8", 2.0 * M * N * (K + la.r)):
+            _check(_lib.osb_gemm_fp8_lora(C.byref(g), C.byref(b), C.byref(la), _stream()), "osb_gemm_fp8_lora")
     return (out, out_scale) if fp8_out else out
 
 
