@@ -12,8 +12,8 @@ from opensora.registry import MODELS
 
 from opensora.utils.lora import adapter_of, dora_magnitude, lora_pack
 
-from .layers import (DoubleStreamBlock, EmbedND, Fp8AttnState, Fp8State, LastLayer, LigerEmbedND, MLPEmbedder,
-                     SingleStreamBlock, _gemm, linear_parts, timestep_embedding)
+from .layers import (PROJ_GEMMS, DoubleStreamBlock, EmbedND, Fp8AttnState, Fp8State, LastLayer, LigerEmbedND,
+                     MLPEmbedder, SingleStreamBlock, _down, _gemm, block_gemms, linear_parts, timestep_embedding)
 
 
 @dataclass
@@ -170,7 +170,8 @@ class MMDiTModel(nn.Module):
             w = self._cond_w[1]
         import osb200
 
-        return _gemm(osb200, x2.contiguous(), w, bias, lora, **kw).view(B, L, -1)
+        x2 = x2.contiguous()
+        return _gemm(osb200, x2, w, bias, lora, _down(osb200, x2, lora), **kw).view(B, L, -1)
 
     def prepare_block_inputs(self, img: Tensor, img_ids: Tensor, txt: Tensor, txt_ids: Tensor, timesteps: Tensor,
                              y_vec: Tensor, cond: Tensor = None, guidance: Tensor | None = None):
@@ -197,23 +198,26 @@ class MMDiTModel(nn.Module):
         return img, txt, vec, pe
 
     # ---- FP8 (e4m3) MLPs -------------------------------------------------------------------------------------------
-    def _mlps(self):
-        """(block, kind) of every MLP: "img" / "txt" of the double blocks, "single" of the single blocks."""
+    def _streams(self):
+        """(block, kind) of every stream: "img" / "txt" of the double blocks, "single" of the single blocks."""
         return [(b, k) for b in self.double_blocks for k in ("img", "txt")] + [(b, "single") for b in self.single_blocks]
+
+    def _gemm_linears(self, proj: bool) -> list[str]:
+        """Names of the Linears that hold the block GEMMs of PROJ_GEMMS (proj) or the other block GEMMs."""
+        names = {id(m): n for n, m in self.named_modules()}
+        return [names[id(lin)] for blk, kind in self._streams() for gemm, slices in block_gemms(blk, kind).items()
+                if (gemm in PROJ_GEMMS) == proj for lin, _, _ in slices]
 
     def fp8_mlp_linears(self) -> list[str]:
         """Names of the Linears the FP8 path replaces: fc1 / fc2 of the double-block MLPs, and linear1 (or v_mlp) and
         linear2 of the single blocks, which hold their MLP's weights."""
-        names = {id(m): n for n, m in self.named_modules()}
-        return [names[id(lin)] for blk, kind in self._mlps() for lin in Fp8State.mlp_linears(blk, kind)[::2]]
+        return self._gemm_linears(False)
 
     def fp8_proj_linears(self) -> list[str]:
         """Names of the Linears the FP8 projection path (`enable_fp8(projections=True)`) reads: the q|k|v Linears
         (qkv, or q_proj / k_proj / v_proj) and `proj` of both streams of the double blocks, and linear1 (or q_proj /
         k_proj / v_mlp) of the single blocks, which hold their q|k|v rows."""
-        names = {id(m): n for n, m in self.named_modules()}
-        blocks = [(b, k) for b in self.double_blocks for k in ("img", "txt")] + [(b, "single") for b in self.single_blocks]
-        return [names[id(lin)] for blk, kind in blocks for lin in Fp8State.proj_linears(blk, kind)]
+        return self._gemm_linears(True)
 
     def enable_fp8(self, projections: bool = False, lora: bool = False) -> None:
         """Run the MLPs of every double and single block on FP8 (e4m3) tensor cores.  The weights are quantized per output
@@ -258,10 +262,10 @@ class MMDiTModel(nn.Module):
         if w.is_cuda:   # quantized now; a model not yet on the GPU quantizes at its first forward
             import osb200
 
-            for blk, kind in self._mlps():
-                state.weights(osb200, blk, kind)
-                if projections:
-                    state.proj_weights(osb200, blk, kind)
+            for blk, kind in self._streams():
+                for name, slices in block_gemms(blk, kind).items():
+                    if projections or name not in PROJ_GEMMS:
+                        state.weight(osb200, blk, kind, name, slices)
         self._fp8_state, self._fp8, self._fp8_proj, self._fp8_lora = state, True, projections, lora
 
     def disable_fp8(self) -> None:

@@ -79,11 +79,16 @@ def _case(model, inp, attn):
     return out, emu, floor, ref
 
 
-@pytest.mark.parametrize("fused,liger,attn", [(True, False, False), (False, True, False), (True, True, True),
-                                              (False, False, True)])
-def test_host_mmdit_fp8_projections_follow_the_emulation(osb8, fused, liger, attn):
+@pytest.mark.parametrize("fused,liger,attn,thw", [(True, False, False, (2, 4, 6)), (False, True, False, (2, 4, 6)),
+                                                  (True, True, True, (2, 4, 6)), (False, False, True, (2, 4, 6)),
+                                                  (False, True, True, (1, 4, 6))],
+                         ids=["True-False-False", "False-True-False", "True-True-True", "False-False-True",
+                              "False-True-True-txt_len_eq_img_len"])
+def test_host_mmdit_fp8_projections_follow_the_emulation(osb8, fused, liger, attn, thw):
     """C = 256 (2 heads of 128), 2 double + 2 single blocks, every block Linear on FP8 (and FP8 attention), against the
-    fp32 oracle.  Yardstick: the emulation reference measured in the same test."""
+    fp32 oracle.  Yardstick: the emulation reference measured in the same test.  With as many text as image tokens
+    (thw = (1, 4, 6)) both streams of a double block get workspaces of one shape: neither may overwrite the other's
+    LN+modulate codes before its q|k|v GEMMs have read them."""
     m = _rand_model(fused, liger)
     if attn and fused:   # the switches compose in either order
         m.enable_fp8_attention()
@@ -92,7 +97,7 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(osb8, fused, liger, att
         m.enable_fp8(projections=True)
         if attn:
             m.enable_fp8_attention()
-    inp = _inputs()
+    inp = _inputs(thw=thw)
     with torch.no_grad():
         m(**inp)             # weights are quantized at the first forward of a CPU model
     osb8.reset()
