@@ -298,7 +298,8 @@ typedef struct osb_attn_short_args {
 } osb_attn_short_args;
 
 /* softmax(q k^T * scale) v per (sequence, head), non-causal, optional per-head RMSNorm on q,k
- * and RoPE applied while staging operands into shared memory.  Replaces: mmdit/math.py:22-36
+ * and RoPE applied while staging operands into shared memory.  A row with no valid key (kv_lens
+ * 0) is written as zeros.  Replaces: mmdit/math.py:22-36
  * (`attention`), layers.py:126-135 (QKNorm), and upstream STDiT3 Attention / MultiHeadCrossAttention
  * (SURVEY.md §8a-S, Appendix A). */
 int osb_attn_short(const osb_attn_short_args* args, void* stream);
@@ -306,8 +307,9 @@ int osb_attn_short(const osb_attn_short_args* args, void* stream);
 /* osb_attn_short with an additive fp32 bias by relative position: the score of query token i and key token j is
  * q.k * softmax_scale + bias[h * bias_head_stride + j - i + Lq - 1] (bias: [heads][Lq + Lk - 1], or one shared vector
  * with bias_head_stride = 0), added before the running maximum.  -inf entries mask keys; key blocks that are -inf for
- * every query of a 128-row query tile are skipped, and a row never evaluates -inf - (-inf).  head_dim 64 only; kv_lens
- * and packed short sequences as in osb_attn_short; QK-norm and RoPE arguments keep their meaning.
+ * every query of a 128-row query tile are skipped, and a row never evaluates -inf - (-inf): a row whose every key is
+ * masked is written as zeros.  head_dim 64 only; kv_lens and packed short sequences as in osb_attn_short; QK-norm and
+ * RoPE arguments keep their meaning.
  * Replaces the self-attention of HF T5Attention (relative_attention_bias, unscaled scores: softmax_scale = 1) and
  * CLIPAttention (causal mask: bias 0 for j <= i, -inf for j > i) run by the reference's text_embedder
  * (opensora/models/text/conditioner.py:10-53). */
@@ -417,7 +419,7 @@ typedef struct osb_attn_tiles_args {
 } osb_attn_tiles_args;
 
 /* out = softmax(q k^T * scale) v per (sequence, head) over head tiles: one CTA per (query tile, head), bulk-copy loads
- * with the next key tile in flight (open-sora_b200/csrc/attn_sm90.cu).  Replaces mmdit/math.py:22-36. */
+ * with the next key tile in flight (open-sora_b200/csrc/attn_sm90.cu).  An empty key set (kv_lens 0) writes zeros.  Replaces mmdit/math.py:22-36. */
 int osb_attn_tiles(const osb_attn_tiles_args* args, void* stream);
 
 /* ---- FP8 (e4m3) head-tile attention: the opt-in attention path of STDiT3 ---------------------------------------------- */
