@@ -1,6 +1,5 @@
 """Test infrastructure for image / video conditioning (only tests import this module): the fp32 oracle loop of the
-conditioned rectified-flow sampler and the CPU stand-in of the binding's `rf_masked_step`, which the host-logic tests add
-to `tests/fake_osb200.py` for the duration of one test.
+conditioned rectified-flow sampler.
 
 Like STDiT3's v1.2 sampler (`oracle/sampling_oracle.py::rflow_sample`) the loop is a restatement of Open-Sora v1.2
 `schedulers/rf/__init__.py::RFLOW.sample` (mask branch) and `RFlowScheduler.add_noise`: PARITY UNPINNED, no reference
@@ -8,7 +7,6 @@ source or vector exists for it here."""
 import torch
 
 from oracle.sampling_oracle import rflow_timestep_transform
-from tests import fake_osb200 as _F
 
 
 def rflow_sample_masked(model, z, y, y_null, frame_mask, noises, mask=None, steps=30, cfg_scale=7.0, transform=None,
@@ -42,40 +40,3 @@ def rflow_sample_masked(model, z, y, y_null, frame_mask, noises, mask=None, step
         z = torch.where(frames(upper), z, x0)
     return z
 
-
-def rf_masked_step(vc, vu, z, frame_mask, t_cur, t_next, *, guidance: float, noise=None, update: bool = True,
-                   num_timesteps: int = 1000, out=None):
-    """Torch restatement of the documented contract of `osb200.rf_masked_step` (include/osb200.h osb_rf_masked_step),
-    with the kernel's rounding points: fp32 math, one rounding to bf16, frames left alone copied exactly."""
-    for t, n in ((vc, "vc"), (vu, "vu"), (z, "z"), (noise, "noise"), (out, "out")):
-        _F._need(t, torch.bfloat16, n)
-        if t is not None and t.shape != z.shape:
-            raise _F.OsbError(f"{n} must have the latent's shape")
-    for t, n in ((frame_mask, "frame_mask"), (t_cur, "t_cur"), (t_next, "t_next")):
-        _F._need(t, torch.float32, n)
-    if update and (vc is None or vu is None):
-        raise _F.OsbError("osb_rf_masked_step failed (-1): the update needs cond and uncond")
-    if not update and noise is None:
-        raise _F.OsbError("osb_rf_masked_step failed (-1): without the update there must be noise to add")
-    N = float(num_timesteps)   # dt and t/N multiply by fl(1/N), as the kernel (and torch's scalar division on CUDA) do
-    per_frame = lambda f: f[:, None, :, None, None]  # noqa: E731  [B, T] -> broadcast over [B, C, T, H, W]
-    per_sample = lambda v: v[:, None, None, None, None]  # noqa: E731
-    m = frame_mask * N
-    x = z.float()
-    if update:
-        upd = m >= t_cur[:, None]
-        c, u = vc.float(), vu.float()
-        x = torch.where(per_frame(upd), x + per_sample((t_cur - t_next) * (1.0 / N)) * (u + guidance * (c - u)), x)
-        prev = upd
-    else:
-        prev = frame_mask == 1
-    if noise is not None:
-        add = (m >= t_next[:, None]) & ~prev
-        a = per_sample(t_next * (1.0 / N))
-        x = torch.where(per_frame(add), (1.0 - a) * x + a * noise.float(), x)
-    y = x.to(torch.bfloat16)   # frames left alone round-trip bf16 -> fp32 -> bf16 exactly
-    _F._count("rf_masked_step", (tuple(z.shape), bool(update), noise is not None))
-    if out is None:
-        return y
-    out.copy_(y)
-    return out

@@ -8,8 +8,6 @@ import pytest
 import torch
 
 from tests import exact_attn as A
-from tests import (fake_osb200_attn_frames, fake_osb200_fp8_attn, fake_osb200_fp8_proj, fake_osb200_fp8_tiles,
-                   fake_osb200_text)
 
 # (id, builder, kwargs, leak): reduced sizes of the GPU matrix; `leak` is the off-by-one mask the case is built to catch
 CASES = [
@@ -122,18 +120,10 @@ def test_rejects_a_three_way_tie():
         A.check_budget(case)
 
 
-@pytest.fixture
-def doubles(fake_osb, monkeypatch):
-    for mod in (fake_osb200_fp8_attn, fake_osb200_fp8_tiles, fake_osb200_text, fake_osb200_attn_frames,
-                fake_osb200_fp8_proj):
-        mod.install(monkeypatch)
-    return fake_osb
-
-
 @pytest.mark.parametrize("i", range(len(CASES)), ids=IDS)
-def test_cpu_double_gives_the_expected_bits(doubles, i):
+def test_cpu_double_gives_the_expected_bits(fake_osb, i):
     case = _build(i)
-    got = case.run(doubles)
+    got = case.run(fake_osb)
     want = case.want()
     if isinstance(want, tuple):
         (codes, scales), (wc, ws) = got, want

@@ -2,8 +2,7 @@
 not a dependency) loaded by `opensora.utils.lora.load_lora`, the host-side MMDiT with a DoRA adapter on every Linear
 against the fp32 oracle on the merged weights g * (W + s B A), peft's unmerged DoRA formula restated on one layer, the
 modulation-group rule, launches, unloading, Ulysses sequence parallelism and the C ABI layout of osb_lora_args.  The
-binding stand-in gets the `gemm_lora` of tests/fake_osb200_dora.py (with `col_scale`); the kernel itself is checked on
-the GPU (tests/test_dora_gpu.py)."""
+kernel itself is checked on the GPU (tests/test_dora_gpu.py)."""
 import math
 import os
 
@@ -11,17 +10,9 @@ import pytest
 import torch
 from torch import nn
 
-from tests import fake_osb200_dora
 from tests.test_lora_cpu import _inputs, _rand_model, write_adapter
 from tests.test_mmdit_gpu import CFG
 from tests.util import rel_l2
-
-
-@pytest.fixture
-def fake_osb(fake_osb, monkeypatch):
-    """The binding stand-in of tests/conftest.py, with the DoRA-capable `gemm_lora` added for this test."""
-    fake_osb200_dora.install(monkeypatch)
-    return fake_osb
 
 
 # ---- adapter files ----------------------------------------------------------------------------------------------------
@@ -387,7 +378,6 @@ def _dora_sp_worker(rank, world, port, adapter_dirs, ret):
         from tests import fake_osb200
 
         sys.modules["osb200"] = fake_osb200
-        fake_osb200.gemm_lora = fake_osb200_dora.gemm_lora
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for (fused, liger, (B, Lt, thw)), d in zip(SP_CASES, adapter_dirs):

@@ -1,11 +1,11 @@
 """DoRA on the GPU: `osb_gemm_lora` with a per-output-channel `col_scale` (g * (x W^T + U B^T) + bias in one fp32
-accumulator) against the fp32 restatement of tests/fake_osb200_dora.py on identical bf16 operands, its bit-exactness
+accumulator) against the fp32 restatement of tests/fake_osb200.py on identical bf16 operands, its bit-exactness
 rules (NULL and all-ones scales), graph replay, and the MMDiT with a DoRA adapter on every Linear against the fp32 oracle
 (oracle/mmdit_oracle.py) on the fp32-merged weights g * (W + s B A)."""
 import pytest
 import torch
 
-from tests.fake_osb200_dora import gemm_dora_fp32
+from tests.fake_osb200 import gemm_lora_fp32
 from tests.util import BF16_ONE_ROUNDING_REL_L2, rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -47,18 +47,18 @@ CASES = [(1, 3072, 3072, 16, 0), (3, 200, 72, 8, 64), (200, 1000, 3072, 72, 128)
 def test_gemm_lora_col_scale_bias(osb, M, N, K, r, bn):
     a, w, bias, u, b, g = _operands(M, N, K, r)
     out = osb.gemm_lora(a, w, bias, u, b, block_n=bn, col_scale=g)
-    ref = gemm_dora_fp32(a, w, bias, u, b, col_scale=g)
+    ref = gemm_lora_fp32(a, w, bias, u, b, col_scale=g)
     r_, _ = report(f"gemm_lora col_scale M={M} N={N} K={K} r={r} bn={bn}", out, ref)
     assert r_ <= BF16_ONE_ROUNDING_REL_L2
     # g in [0.5, 1.5]: a kernel that dropped the scale (or applied it after the bias) would be far off
-    assert rel_l2(out, gemm_dora_fp32(a, w, bias, u, b)) > 0.1
+    assert rel_l2(out, gemm_lora_fp32(a, w, bias, u, b)) > 0.1
 
 
 @pytest.mark.parametrize("bn", [64, 128, 192, 256])
 def test_gemm_lora_col_scale_gelu(osb, bn):
     a, w, bias, u, b, g = _operands(777, 1032, 3072, 72, seed=10)
     out = osb.gemm_lora(a, w, bias, u, b, epilogue=osb.EPI_BIAS_GELU_TANH, block_n=bn, col_scale=g)
-    ref = gemm_dora_fp32(a, w, bias, u, b, col_scale=g, epilogue=osb.EPI_BIAS_GELU_TANH)
+    ref = gemm_lora_fp32(a, w, bias, u, b, col_scale=g, epilogue=osb.EPI_BIAS_GELU_TANH)
     r_, _ = report(f"gemm_lora col_scale gelu bn={bn}", out, ref)
     assert r_ <= BF16_ONE_ROUNDING_REL_L2
 
@@ -75,7 +75,7 @@ def test_gemm_lora_col_scale_gate_residual_in_place(osb, bn, mode):
     if mode == "no_gate":
         gate = None
     resid = _randn(M, N, seed=21)
-    ref = gemm_dora_fp32(a, w, bias, u, b, col_scale=cs, epilogue=osb.EPI_BIAS_GATE_RES, residual=resid, gate=gate,
+    ref = gemm_lora_fp32(a, w, bias, u, b, col_scale=cs, epilogue=osb.EPI_BIAS_GATE_RES, residual=resid, gate=gate,
                          group_rows=group_rows, mod_index=mod_index)
     d = resid.clone()
     osb.gemm_lora(a, w, bias, u, b, epilogue=osb.EPI_BIAS_GATE_RES, residual=d, gate=gate, group_rows=group_rows,
@@ -94,7 +94,7 @@ def test_gemm_lora_col_scale_strided_operands(osb):
     ga = torch.rand(3 * N, device="cuda") + 0.5
     a, u, b, g = xa[:, 64:], ua[:, r:2 * r], ba[N:, :r], ga[N:2 * N]
     out = osb.gemm_lora(a, w, None, u, b, col_scale=g)
-    r_, _ = report("gemm_lora col_scale strided", out, gemm_dora_fp32(a, w, None, u, b, col_scale=g))
+    r_, _ = report("gemm_lora col_scale strided", out, gemm_lora_fp32(a, w, None, u, b, col_scale=g))
     assert r_ <= BF16_ONE_ROUNDING_REL_L2
 
 

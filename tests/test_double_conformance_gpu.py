@@ -1,5 +1,4 @@
-"""Conformance of the CPU double of the binding (tests/fake_osb200.py, with tests/lora_ref.py::gemm_lora and
-tests/rf_conditioning_ref.py::rf_masked_step) with the osb200 kernels, element by element.
+"""Conformance of the CPU double of the binding (tests/fake_osb200.py) with the osb200 kernels, element by element.
 
 Most host-side evidence of this project runs on the CPU against the double, so the double is itself a reference: this
 module pins it to the kernels.  Every case builds its inputs on the CPU, runs the double there (ACC_DTYPE = fp32, as the
@@ -25,8 +24,6 @@ import torch
 import torch.nn.functional as TF
 
 from tests import fake_osb200 as F_
-from tests.lora_ref import gemm_lora as fake_gemm_lora
-from tests.rf_conditioning_ref import rf_masked_step as fake_rf_masked_step
 from tests.test_attn_tiles_gpu import read_tiles
 
 pytestmark = pytest.mark.gpu
@@ -485,7 +482,7 @@ def test_gemm_and_lora(case, rank):
     if rank:
         uc, bcl = _slice_to(u, dev), b.to(dev)
         out_k, out_d = _launches(osb, lambda: osb.gemm_lora(ac, wc, bc, uc, bcl, block_n=bn, **kc),
-                                 lambda: fake_gemm_lora(a, w, bias, u, b, block_n=bn, **kd))
+                                 lambda: F_.gemm_lora(a, w, bias, u, b, block_n=bn, **kd))
     else:
         out_k, out_d = _launches(osb, lambda: osb.gemm(ac, wc, bc, block_n=bn, **kc), lambda: F_.gemm(a, w, bias, block_n=bn, **kd))
     if res_mode == "alias":
@@ -833,7 +830,7 @@ def test_rf_masked_step(update, noise, HW, in_place):
     kwc = _to(kw, dev)
     args_k = (vc.to(dev), vu.to(dev), zk, fm.to(dev), tc.to(dev), tn.to(dev))
     got, want = _launches(osb, lambda: osb.rf_masked_step(*args_k, out=zk if in_place else None, **kwc),
-                          lambda: fake_rf_masked_step(vc, vu, zd, fm, tc, tn, out=zd if in_place else None, **kw))
+                          lambda: F_.rf_masked_step(vc, vu, zd, fm, tc, tn, out=zd if in_place else None, **kw))
     if in_place:
         assert got.data_ptr() == zk.data_ptr() and want.data_ptr() == zd.data_ptr()
     tag = f"rf_masked_step update={update} noise={noise} HW={HW} in_place={in_place}"
@@ -869,8 +866,7 @@ def _refusals():
                                                                     (osb_ht(m, d, 64, m.tile_map(0, 64), 5, 2, 64)), nkinds=5)),
         ("gemm K % 8", lambda m, d: m.gemm(b(16, 12).to(d), b(16, 12).to(d))),
         ("gemm N % 8", lambda m, d: m.gemm(b(16, 16).to(d), b(12, 16).to(d))),
-        ("gemm_lora r % 8", lambda m, d: (fake_gemm_lora if m is F_ else m.gemm_lora)(b(16, 16).to(d), b(16, 16).to(d), None,
-                                                                                     b(16, 4).to(d), b(16, 4).to(d))),
+        ("gemm_lora r % 8", lambda m, d: m.gemm_lora(b(16, 16).to(d), b(16, 16).to(d), None, b(16, 4).to(d), b(16, 4).to(d))),
         ("group_stats C/8 not dividing 256", lambda m, d: m.group_stats(b(1, 2, 4, 4, 24).to(d), 3)),
         ("cfg_euler n % 8", lambda m, d: m.cfg_euler(*(b(12).to(d) for _ in range(2)), None, b(12).to(d), g_txt=1.0, dt=0.1)),
         ("attn_tiles kv_lens with packed q map", lambda m, d: m.attn_tiles(osb_ht(m, d, 64, m.tile_map(0, 16), 3, 2, 64),
@@ -884,16 +880,10 @@ def _shape_refusals():
     """Wrong-shaped optional GEMM operands (out, bias, residual, gate, mod_index) and a K mismatch.  Each wrong-shaped
     tensor is a view into an allocation large enough for what a launch would touch, so a missing check shows as "did
     not raise", never as an out-of-bounds access."""
-    from tests import fake_osb200_dora, fake_osb200_fp8, fake_osb200_fp8_blocks
-
     b = lambda *s: torch.zeros(*s, dtype=torch.bfloat16)  # noqa: E731
     f = lambda *s: torch.zeros(*s, dtype=torch.float32)  # noqa: E731
     e = lambda *s: torch.zeros(*s, dtype=torch.float8_e4m3fn)  # noqa: E731
     gr = dict(epilogue=F_.EPI_BIAS_GATE_RES, group_rows=8)
-    lora = lambda m: fake_gemm_lora if m is F_ else m.gemm_lora  # noqa: E731
-    dora = lambda m: fake_osb200_dora.gemm_lora if m is F_ else m.gemm_lora  # noqa: E731
-    fp8 = lambda m: fake_osb200_fp8.gemm_fp8 if m is F_ else m.gemm_fp8  # noqa: E731
-    blk = lambda m: fake_osb200_fp8_blocks.gemm_fp8_blocks if m is F_ else m.gemm_fp8_blocks  # noqa: E731
     lo = lambda d: (b(16, 8).to(d), b(16, 8).to(d))  # noqa: E731   u [M, r], b [N, r]
     s8 = lambda d: (f(16).to(d) + 1, f(16).to(d) + 1)  # noqa: E731   a_scale [M], w_scale [N]
     return [
@@ -906,26 +896,26 @@ def _shape_refusals():
         ("gemm mod_index short", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 16).to(d), gate=f(2, 16).to(d),
                                                      mod_index=torch.zeros(2, dtype=torch.int32).to(d)[:1], **gr)),
         ("gemm K mismatch", lambda m, d: m.gemm(b(16, 16).to(d), b(16, 24).to(d))),
-        ("gemm_lora out [M-1, N]", lambda m, d: lora(m)(b(16, 16).to(d), b(16, 16).to(d), None, *lo(d),
-                                                        out=b(16, 16).to(d)[:15])),
-        ("gemm_lora gate [G, N-8]", lambda m, d: lora(m)(b(16, 16).to(d), b(16, 16).to(d), None, *lo(d),
-                                                         gate=f(2, 16).to(d)[:, :8], **gr)),
-        ("gemm_lora col_scale bias [N-8]", lambda m, d: dora(m)(b(16, 16).to(d), b(16, 16).to(d), b(16).to(d)[:8], *lo(d),
-                                                                col_scale=f(16).to(d) + 1)),
-        ("gemm_fp8 out [M, N-8]", lambda m, d: fp8(m)(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
-                                                      out=b(16, 16).to(d)[:, :8])),
-        ("gemm_fp8 residual [M, N-8]", lambda m, d: fp8(m)(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
-                                                           residual=b(16, 16).to(d)[:, :8], epilogue=F_.EPI_BIAS_GATE_RES)),
-        ("gemm_fp8 gate rows < groups", lambda m, d: fp8(m)(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
-                                                            gate=f(2, 16).to(d)[:1], **gr)),
-        ("gemm_fp8_blocks out [M-1, N]", lambda m, d: blk(m)(e(16, 128).to(d), f(16, 1).to(d) + 1, e(16, 128).to(d),
-                                                             s8(d)[1], out=b(16, 16).to(d)[:15])),
-        ("gemm_fp8_blocks FP8 GELU bias [N-8]", lambda m, d: blk(m)(e(16, 128).to(d), f(16, 1).to(d) + 1, e(128, 128).to(d),
-                                                                    f(128).to(d) + 1, b(128).to(d)[:120],
-                                                                    epilogue=fake_osb200_fp8_blocks.EPI_BIAS_GELU_TANH_FP8)),
-        ("gemm_fp8_blocks mod_index short", lambda m, d: blk(m)(e(16, 128).to(d), f(16, 1).to(d) + 1, e(16, 128).to(d),
-                                                                s8(d)[1], gate=f(2, 16).to(d),
-                                                                mod_index=torch.zeros(2, dtype=torch.int32).to(d)[:1], **gr)),
+        ("gemm_lora out [M-1, N]", lambda m, d: m.gemm_lora(b(16, 16).to(d), b(16, 16).to(d), None, *lo(d),
+                                                            out=b(16, 16).to(d)[:15])),
+        ("gemm_lora gate [G, N-8]", lambda m, d: m.gemm_lora(b(16, 16).to(d), b(16, 16).to(d), None, *lo(d),
+                                                             gate=f(2, 16).to(d)[:, :8], **gr)),
+        ("gemm_lora col_scale bias [N-8]", lambda m, d: m.gemm_lora(b(16, 16).to(d), b(16, 16).to(d), b(16).to(d)[:8], *lo(d),
+                                                                    col_scale=f(16).to(d) + 1)),
+        ("gemm_fp8 out [M, N-8]", lambda m, d: m.gemm_fp8(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
+                                                          out=b(16, 16).to(d)[:, :8])),
+        ("gemm_fp8 residual [M, N-8]", lambda m, d: m.gemm_fp8(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
+                                                               residual=b(16, 16).to(d)[:, :8], epilogue=F_.EPI_BIAS_GATE_RES)),
+        ("gemm_fp8 gate rows < groups", lambda m, d: m.gemm_fp8(e(16, 128).to(d), s8(d)[0], e(16, 128).to(d), s8(d)[1],
+                                                                gate=f(2, 16).to(d)[:1], **gr)),
+        ("gemm_fp8_blocks out [M-1, N]", lambda m, d: m.gemm_fp8_blocks(e(16, 128).to(d), f(16, 1).to(d) + 1, e(16, 128).to(d),
+                                                                        s8(d)[1], out=b(16, 16).to(d)[:15])),
+        ("gemm_fp8_blocks FP8 GELU bias [N-8]", lambda m, d: m.gemm_fp8_blocks(e(16, 128).to(d), f(16, 1).to(d) + 1, e(128, 128).to(d),
+                                                                               f(128).to(d) + 1, b(128).to(d)[:120],
+                                                                               epilogue=F_.EPI_BIAS_GELU_TANH_FP8)),
+        ("gemm_fp8_blocks mod_index short", lambda m, d: m.gemm_fp8_blocks(e(16, 128).to(d), f(16, 1).to(d) + 1, e(16, 128).to(d),
+                                                                           s8(d)[1], gate=f(2, 16).to(d),
+                                                                           mod_index=torch.zeros(2, dtype=torch.int32).to(d)[:1], **gr)),
     ]
 
 
@@ -1030,7 +1020,7 @@ def _replay_one(name, args, kw, result):
     if name == "gemm_lora":
         a, w, bias, u, b = args
         e = err_gemm(a, w, bias, u=u, b=b, **kw)
-        return [("", result, fake_gemm_lora(*args, **kw), e)]
+        return [("", result, F_.gemm_lora(*args, **kw), e)]
     if name == "ln_modulate":
         e = err_ln(*args, **kw)
         return [("", result, F_.ln_modulate(*args, **kw), e)]
@@ -1042,7 +1032,7 @@ def _replay_one(name, args, kw, result):
         return [("", result, F_.cfg_euler(*args, **kw), e)]
     if name == "rf_masked_step":
         e = err_rf_masked_step(*args, **kw)
-        return [("", result, fake_rf_masked_step(*args, **kw), e)]
+        return [("", result, F_.rf_masked_step(*args, **kw), e)]
     if name == "conv3d":
         e = err_conv(*args, **kw)
         return [("", result, F_.conv3d(*args, **kw), e)]

@@ -1,4 +1,4 @@
-"""The FP8 (e4m3) MLP path on the CPU: the stand-in entries of tests/fake_osb200_fp8.py against the contract arithmetic
+"""The FP8 (e4m3) MLP path on the CPU: the stand-in entries of tests/fake_osb200.py against the contract arithmetic
 of tests/fp8_ref.py on its edge cases, the host-side STDiT3 with `enable_fp8()` against the FP8-emulating oracle,
 `disable_fp8()`, the K % 128 refusal and the ctypes mirror of `osb_gemm_fp8_args`."""
 import ctypes
@@ -8,18 +8,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import fake_osb200_fp8 as F8
 from tests import fp8_ref as R
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4M3 = torch.float8_e4m3fn
-
-
-@pytest.fixture
-def osb8(fake_osb, monkeypatch):
-    F8.install(monkeypatch)
-    return fake_osb
 
 
 def _rows(seed=0, rows=12, K=256):
@@ -31,9 +24,9 @@ def _rows(seed=0, rows=12, K=256):
     return x
 
 
-def test_quant_rows_matches_the_contract(osb8):
+def test_quant_rows_matches_the_contract(fake_osb):
     x = _rows().to(torch.bfloat16)
-    q, s = osb8.quant_rows_fp8(x)
+    q, s = fake_osb.quant_rows_fp8(x)
     rq, rs = R.quantize(x.float())
     assert q.dtype == E4M3 and s.dtype == torch.float32
     assert torch.equal(s, rs) and torch.equal(q.double(), rq)
@@ -41,14 +34,14 @@ def test_quant_rows_matches_the_contract(osb8):
     assert q[5, 7].float() == -448.0 and torch.all(q[6].float() == 448.0)
     # a strided view (row stride > K) quantizes its K columns only
     wide = torch.randn(12, 384).to(torch.bfloat16)
-    q2, s2 = osb8.quant_rows_fp8(wide[:, :256])
+    q2, s2 = fake_osb.quant_rows_fp8(wide[:, :256])
     rq2, rs2 = R.quantize(wide[:, :256].float())
     assert torch.equal(s2, rs2) and torch.equal(q2.double(), rq2)
-    with pytest.raises(osb8.OsbError):
-        osb8.quant_rows_fp8(torch.zeros(4, 12, dtype=torch.bfloat16))   # K % 8
+    with pytest.raises(fake_osb.OsbError):
+        fake_osb.quant_rows_fp8(torch.zeros(4, 12, dtype=torch.bfloat16))   # K % 8
 
 
-def test_ln_modulate_fp8_quantizes_the_fp32_value(osb8):
+def test_ln_modulate_fp8_quantizes_the_fp32_value(fake_osb):
     """The fc1 input is the fp32 LN+modulate row, quantized without a bf16 rounding first; mod_index selects the table."""
     g = torch.Generator().manual_seed(1)
     rows, C = 16, 256
@@ -56,7 +49,7 @@ def test_ln_modulate_fp8_quantizes_the_fp32_value(osb8):
     x[4] = 0.0                                    # LN of a constant row is 0: modulate leaves the shift only
     mod = torch.randn(3, 2, C, generator=g)
     mod_index = torch.tensor([2, 0, 1, 2], dtype=torch.int32)
-    q, s = osb8.ln_modulate_fp8(x, mod[:, 0], mod[:, 1], group_rows=4, mod_index=mod_index)
+    q, s = fake_osb.ln_modulate_fp8(x, mod[:, 0], mod[:, 1], group_rows=4, mod_index=mod_index)
     xf = x.float()
     gi = mod_index.long()[torch.arange(rows) // 4]
     y = F.layer_norm(xf, (C,), eps=1e-6) * (1 + mod[gi, 1]) + mod[gi, 0]
@@ -68,13 +61,13 @@ def test_ln_modulate_fp8_quantizes_the_fp32_value(osb8):
     # quantizing the bf16-rounded row instead would differ on a visible share of the codes
     qb, _ = R.quantize(y.to(torch.bfloat16).float())
     assert not torch.equal(qb, rq)
-    with pytest.raises(osb8.OsbError):
-        osb8.ln_modulate_fp8(torch.zeros(2, 8192, dtype=torch.bfloat16), mod[:1, 0].repeat(1, 32)[:, :8192],
+    with pytest.raises(fake_osb.OsbError):
+        fake_osb.ln_modulate_fp8(torch.zeros(2, 8192, dtype=torch.bfloat16), mod[:1, 0].repeat(1, 32)[:, :8192],
                              mod[:1, 1].repeat(1, 32)[:, :8192], group_rows=2)
 
 
 @pytest.mark.parametrize("epilogue", [0, 1, 2])
-def test_gemm_fp8_matches_dequantized_fp32(osb8, epilogue):
+def test_gemm_fp8_matches_dequantized_fp32(fake_osb, epilogue):
     g = torch.Generator().manual_seed(2)
     M, N, K = 70, 48, 384
     a = _rows(3, M, K)
@@ -88,7 +81,7 @@ def test_gemm_fp8_matches_dequantized_fp32(osb8, epilogue):
     kw = dict(residual=res, gate=gate, group_rows=16, mod_index=mod_index) if epilogue == 2 else {}
     a_view = torch.zeros(M, K + 128, dtype=E4M3)
     a_view[:, :K] = a8.float().to(E4M3)
-    got = osb8.gemm_fp8(a_view[:, :K], sa, w8.float().to(E4M3), sw, bias, epilogue=epilogue, **kw)
+    got = fake_osb.gemm_fp8(a_view[:, :K], sa, w8.float().to(E4M3), sw, bias, epilogue=epilogue, **kw)
     ref = R.dequantize(a8, sa).double() @ R.dequantize(w8, sw).double().t() + bias.double()
     if epilogue == 1:
         ref = F.gelu(ref, approximate="tanh")
@@ -99,8 +92,8 @@ def test_gemm_fp8_matches_dequantized_fp32(osb8, epilogue):
     assert rel_l2(got, ref) < 3e-3
     for bad in (dict(K=288), dict(epilogue=3)):
         Kb = bad.get("K", K)
-        with pytest.raises(osb8.OsbError):
-            osb8.gemm_fp8(torch.zeros(8, Kb, dtype=E4M3), torch.ones(8), torch.zeros(8, Kb, dtype=E4M3), torch.ones(8),
+        with pytest.raises(fake_osb.OsbError):
+            fake_osb.gemm_fp8(torch.zeros(8, Kb, dtype=E4M3), torch.ones(8), torch.zeros(8, Kb, dtype=E4M3), torch.ones(8),
                           epilogue=bad.get("epilogue", 0))
 
 
@@ -111,7 +104,7 @@ def _inputs(cfg, B, T, H, W, lens=None):
     return {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v) for k, v in inp.items()}
 
 
-def test_host_stdit3_fp8_follows_the_emulation(osb8):
+def test_host_stdit3_fp8_follows_the_emulation(fake_osb):
     """XS/2 at hidden 256 with FP8 MLPs on the stand-in, against the fp32 oracle.  The yardstick is the FP8-emulation
     reference: the oracle in bf16 with its block MLPs at the FP8 rounding points (tests/fp8_ref.py), measured in the same
     test.  The product may not be more than 1.1x further from the fp32 oracle than that reference, plain and with an
@@ -123,7 +116,7 @@ def test_host_stdit3_fp8_follows_the_emulation(osb8):
     xm[1, 1:3] = False
     ob = R.build_pair("xs", device="cpu")[1].to(torch.bfloat16)
     for kw in ({}, {"x_mask": xm}):
-        osb8.reset()
+        fake_osb.reset()
         with torch.no_grad():
             ref = oracle(**inp, **kw)
             out = prod(**inp, **kw)
@@ -134,7 +127,7 @@ def test_host_stdit3_fp8_follows_the_emulation(osb8):
         print(f"[fp8 host] {'x_mask' if kw else 'plain'}: product {r_out:.3e}, FP8 emulation {r_emu:.3e}, "
               f"bf16 oracle {r_bf:.3e} (rel-L2 against the fp32 oracle)")
         assert r_out < 1.1 * r_emu and r_emu > r_bf, (r_out, r_emu, r_bf)
-        names = [c[0] for c in osb8.calls]
+        names = [c[0] for c in fake_osb.calls]
         nb = 2 * cfg.depth
         assert names.count("gemm_fp8") == 2 * nb and names.count("ln_modulate_fp8") == nb
         # the fc2 input once per block; on the CPU the weights (2 per block) are quantized by the first forward
@@ -142,7 +135,7 @@ def test_host_stdit3_fp8_follows_the_emulation(osb8):
         assert names.count("ln_modulate") == nb + 1
 
 
-def test_disable_fp8_restores_the_bf16_path(osb8):
+def test_disable_fp8_restores_the_bf16_path(fake_osb):
     prod, _, cfg = R.build_pair("xs", device="cpu")
     inp = _inputs(cfg, 1, 4, 8, 8)
     with torch.no_grad():
@@ -150,15 +143,15 @@ def test_disable_fp8_restores_the_bf16_path(osb8):
         prod.enable_fp8()
         fp8 = prod(**inp)
         prod.disable_fp8()
-        osb8.reset()
+        fake_osb.reset()
         after = prod(**inp)
     assert not torch.equal(before, fp8)
     assert torch.equal(before, after)
     assert not any(k[0] == "fp8" for k in prod._cache)
-    assert not any(c[0].endswith("fp8") for c in osb8.calls)
+    assert not any(c[0].endswith("fp8") for c in fake_osb.calls)
 
 
-def test_fp8_refuses_hidden_sizes_off_the_k_block(osb8):
+def test_fp8_refuses_hidden_sizes_off_the_k_block(fake_osb):
     """XS/2 as shipped has hidden size 288, not a multiple of the 128-element e4m3 k-block."""
     from opensora.models.stdit.stdit3 import STDiT3_XS_2
 

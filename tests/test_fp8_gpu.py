@@ -1,12 +1,12 @@
 """The FP8 (e4m3) MLP path on the H100: `osb_gemm_fp8` against an fp32 matmul of the dequantized operands, the two
-quantizers against their CPU stand-in (tests/fake_osb200_fp8.py), STDiT3-XL/2 at the benchmark shape with FP8 MLPs
+quantizers against their CPU stand-in (tests/fake_osb200.py), STDiT3-XL/2 at the benchmark shape with FP8 MLPs
 against the fp32 oracle (yardstick: the FP8-emulation reference of tests/fp8_ref.py, measured in the same test), graph
 replay, and `disable_fp8()`."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import fake_osb200_fp8 as F8
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests.util import rel_l2, report
 
@@ -22,7 +22,7 @@ def _cuda():
 
 def _q(x):
     """quantize on the CPU stand-in's rule, return device tensors (codes as e4m3, scales fp32)"""
-    q, s = F8._quant(x.float().cpu())
+    q, s = F_._quant(x.float().cpu())
     return q.cuda(), s.cuda()
 
 
@@ -86,7 +86,7 @@ def test_quant_rows_fp8_matches_the_stand_in(rows, K, ld):
     x[2, 5] = 3e4
     xs = x.cuda()[:, :K]
     q, s = osb200.quant_rows_fp8(xs)
-    rq, rs = F8.quant_rows_fp8(x[:, :K])
+    rq, rs = F_.quant_rows_fp8(x[:, :K])
     assert torch.equal(s.cpu(), rs)                    # amax is exact and amax / 448 is one IEEE division
     qc, rc = q.cpu().float(), rq.float()
     assert ((qc - rc).abs() <= _step(rc)).all()
@@ -107,7 +107,7 @@ def test_ln_modulate_fp8_matches_the_stand_in(rows, C, x_mask):
     mod_index = torch.tensor([1, 0, 3, 2, 2, 3, 0, 1], dtype=torch.int32) if x_mask else None
     q, s = osb200.ln_modulate_fp8(x.cuda(), mod[:, 0].cuda(), mod[:, 1].cuda(), group_rows=group_rows,
                                   mod_index=None if mod_index is None else mod_index.cuda())
-    rq, rs = F8.ln_modulate_fp8(x, mod[:, 0], mod[:, 1], group_rows=group_rows, mod_index=mod_index)
+    rq, rs = F_.ln_modulate_fp8(x, mod[:, 0], mod[:, 1], group_rows=group_rows, mod_index=mod_index)
     sc = s.cpu()
     assert ((sc - rs).abs() <= 1e-6 * rs).all()
     qc, rc = q.cpu().float(), rq.float()

@@ -6,10 +6,6 @@ import torch
 
 from tests import exact_gemm as X
 from tests import fake_osb200 as F_
-from tests import fake_osb200_dora as dora
-from tests import fake_osb200_fp8 as f8
-from tests import fake_osb200_fp8_blocks as fb
-from tests import lora_ref
 from tests.exact_gemm import quant_edge_rows, quant_expected
 
 E4M3 = torch.float8_e4m3fn
@@ -18,11 +14,7 @@ CASES = X.matrix(max_m=CPU_M)
 
 
 def _standin(case):
-    if case.fn == "gemm":
-        return F_.gemm
-    if case.fn == "gemm_lora":
-        return dora.gemm_lora if case.col_scale is not None else lora_ref.gemm_lora
-    return f8.gemm_fp8 if case.fn == "gemm_fp8" else fb.gemm_fp8_blocks
+    return getattr(F_, case.fn)
 
 
 def test_budget_holds_for_every_case():
@@ -105,9 +97,9 @@ def test_quantizer_tie_table(which):
     x = quant_edge_rows()
     K = x.shape[1]
     if which == "rows":
-        q, s = f8.quant_rows_fp8(x)
+        q, s = F_.quant_rows_fp8(x)
     else:
-        q, s = fb.quant_blocks_fp8(x, block=128 if which == "blocks128" else K)
+        q, s = F_.quant_blocks_fp8(x, block=128 if which == "blocks128" else K)
     codes = q.view(torch.uint8)
     assert [int(c) for c in codes[0, :len(TIE_CODES)]] == [c for _, c in TIE_CODES]
     assert [float(v) for v in x[0, :len(TIE_CODES)]] == [v for v, _ in TIE_CODES]
@@ -150,10 +142,10 @@ def test_standin_refuses_wrong_shapes(fn, what):
     w = b(N, Kw) if bf else b(N, Kw).to(E4M3)
     call = {
         "gemm": lambda: F_.gemm(a, w, bias, **kw),
-        "gemm_lora": lambda: lora_ref.gemm_lora(a, w, bias, b(M, 8), b(N, 8), **kw),
-        "dora": lambda: dora.gemm_lora(a, w, bias, b(M, 8), b(N, 8), col_scale=torch.ones(N), **kw),
-        "gemm_fp8": lambda: f8.gemm_fp8(a, torch.ones(M), w, torch.ones(N), bias, **kw),
-        "gemm_fp8_blocks": lambda: fb.gemm_fp8_blocks(a, torch.ones(M, K // 128), w, torch.ones(N), bias, **kw),
+        "gemm_lora": lambda: F_.gemm_lora(a, w, bias, b(M, 8), b(N, 8), **kw),
+        "dora": lambda: F_.gemm_lora(a, w, bias, b(M, 8), b(N, 8), col_scale=torch.ones(N), **kw),
+        "gemm_fp8": lambda: F_.gemm_fp8(a, torch.ones(M), w, torch.ones(N), bias, **kw),
+        "gemm_fp8_blocks": lambda: F_.gemm_fp8_blocks(a, torch.ones(M, K // 128), w, torch.ones(N), bias, **kw),
     }[fn]
     n0 = F_.launch_count()
     with pytest.raises(F_.OsbError):

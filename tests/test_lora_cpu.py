@@ -1,7 +1,6 @@
 """LoRA adapters on the CPU: PEFT adapter directories written by the tests (peft itself is not a dependency) loaded by
 `opensora.utils.lora.load_lora` - config semantics and every refusal -, the host-side MMDiT with an adapter on every Linear
-against the fp32 oracle on the merged weights W + s B A (through the binding stand-in, with the fp32 restatement of
-`gemm_lora` from tests/lora_ref.py added), Ulysses sequence parallelism, unloading, the guards of the models that take no
+against the fp32 oracle on the merged weights W + s B A (through the binding stand-in), Ulysses sequence parallelism, unloading, the guards of the models that take no
 adapter, and the C ABI layout of osb_lora_args.  The kernel itself is checked on the GPU (tests/test_lora_gpu.py)."""
 import json
 import math
@@ -11,16 +10,8 @@ import pytest
 import torch
 from torch import nn
 
-from tests import lora_ref
 from tests.test_mmdit_gpu import CFG, _ids
 from tests.util import rel_l2
-
-
-@pytest.fixture
-def fake_osb(fake_osb, monkeypatch):
-    """The binding stand-in of tests/conftest.py, with the fp32 restatement of `gemm_lora` added for this test."""
-    monkeypatch.setattr(fake_osb, "gemm_lora", lora_ref.gemm_lora, raising=False)
-    return fake_osb
 
 
 # ---- adapter files ----------------------------------------------------------------------------------------------------
@@ -327,7 +318,6 @@ def _lora_sp_worker(rank, world, port, adapter_dirs, ret):
         from tests import fake_osb200
 
         sys.modules["osb200"] = fake_osb200
-        fake_osb200.gemm_lora = lora_ref.gemm_lora
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for (fused, liger, (B, Lt, thw)), d in zip(SP_CASES, adapter_dirs):

@@ -1,10 +1,10 @@
 """LoRA on the GPU: `osb_gemm_lora` (base GEMM + unmerged low-rank update in one fp32 accumulator) against the fp32
-restatement of tests/lora_ref.py on identical bf16 operands, and the MMDiT with an adapter on every Linear against the
+restatement of tests/fake_osb200.py on identical bf16 operands, and the MMDiT with an adapter on every Linear against the
 fp32 oracle (oracle/mmdit_oracle.py) on the fp32-merged weights W + s B A."""
 import pytest
 import torch
 
-from tests.lora_ref import gemm_lora_fp32
+from tests.fake_osb200 import gemm_lora_fp32
 from tests.util import BF16_ONE_ROUNDING_REL_L2, rel_l2, report
 
 pytestmark = pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""The FP8 (e4m3) attention path of MMDiT on the CPU: the stand-in of tests/fake_osb200_fp8_attn.py against the written
+"""The FP8 (e4m3) attention path of MMDiT on the CPU: the stand-in of tests/fake_osb200.py against the written
 contract and workspace layout, the host-side MMDiTModel with `enable_fp8_attention()` against the FP8-emulation reference
 of tests/mmdit_fp8_attn_ref.py (both QKV and both RoPE layouts, alone and with the FP8 MLPs), `disable_fp8_attention()`,
 LoRA, the refusals, Ulysses sequence parallelism on two gloo ranks, and the ctypes mirror of `osb_attn_fp8_workspace`."""
@@ -8,8 +8,7 @@ import os
 import pytest
 import torch
 
-from tests import fake_osb200_fp8_attn as FA
-from tests import fake_osb200_fp8_blocks as FB
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_ref as MR
@@ -20,13 +19,6 @@ from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4M3 = torch.float8_e4m3fn
-
-
-@pytest.fixture
-def osb8(fake_osb, monkeypatch):
-    FA.install(monkeypatch)
-    FB.install(monkeypatch)
-    return fake_osb
 
 
 def _operands(B, L, H, seed=0, split=None, liger=True):
@@ -60,21 +52,21 @@ def _accumulator_order():
 def test_vt8_permutation_is_the_accumulator_order():
     want = _accumulator_order()
     assert sorted(want) == list(range(32))
-    got = FA.vt8_key(torch.arange(96))
+    got = F_.vt8_key(torch.arange(96))
     assert got[:32].tolist() == want and got[32:64].tolist() == [32 + k for k in want]
 
 
 @pytest.mark.parametrize("liger,split", [(True, 50), (False, None)])
-def test_stand_in_matches_the_contract(osb8, liger, split):
+def test_stand_in_matches_the_contract(fake_osb, liger, split):
     B, L, H = 2, 200, 2
     qkv, kw = _operands(B, L, H, split=split, liger=liger)
     C = H * 128
-    ws = osb8.attn_fp8_workspace(B, L, H, "cpu")
+    ws = fake_osb.attn_fp8_workspace(B, L, H, "cpu")
     out = torch.zeros(B * L, C, dtype=torch.bfloat16)
-    osb8.attn_fp8(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out, workspace=ws, **kw)
-    assert ws.Lpad == 256 and osb8.calls[-1][0] == "attn_fp8"
+    fake_osb.attn_fp8(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], out, workspace=ws, **kw)
+    assert ws.Lpad == 256 and fake_osb.calls[-1][0] == "attn_fp8"
     skip = ("seqs_per_batch", "Lq", "Lk", "num_heads", "head_dim")
-    qf, kf, vf, _ = FA.stage(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], L=L, H=H, norm_eps=1e-6,
+    qf, kf, vf, _ = F_.stage(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], L=L, H=H, norm_eps=1e-6,
                              **{k: v for k, v in kw.items() if k not in skip})
     # q / k: per (token, head) rows, codes = the grid rounding of x / s (tests/fp8_ref.py builds it from the e4m3 grid)
     for x, q8, s in ((qf, ws.q8, ws.s_q), (kf, ws.k8, ws.s_k)):
@@ -91,7 +83,7 @@ def test_stand_in_matches_the_contract(osb8, liger, split):
     amax = ws.vt8.float().abs().amax(-1)
     assert ((amax == 448) | (amax == 0)).all() and int((amax == 0).sum()) == B   # every nonzero channel reaches +-448
     # the output: fp64 softmax attention on the dequantized workspace operands, within the P quantization
-    q8, sq, k8, sk, v8k, sv = FA.workspace_operands(ws, B * H, L)
+    q8, sq, k8, sk, v8k, sv = F_.workspace_operands(ws, B * H, L)
     qd, kd = q8[:, :L].double() * sq[:, :L, None], k8[:, :L].double() * sk[:, :L, None]
     vd = v8k[:, :L].double() * sv[:, None, :]
     ref = torch.softmax(qd @ kd.transpose(1, 2) / 128 ** 0.5, -1) @ vd
@@ -100,17 +92,17 @@ def test_stand_in_matches_the_contract(osb8, liger, split):
     assert rel_l2(got, ref) < 1.1 * rel_l2(emu, ref) + 4e-3   # + the bf16 rounding of the output
 
 
-def test_stand_in_refusals(osb8):
+def test_stand_in_refusals(fake_osb):
     qkv, kw = _operands(1, 64, 2)
     q, k, v = qkv[:, :256], qkv[:, 256:512], qkv[:, 512:]
     out = torch.empty(64, 256, dtype=torch.bfloat16)
-    ws = osb8.attn_fp8_workspace(1, 64, 2, "cpu")
+    ws = fake_osb.attn_fp8_workspace(1, 64, 2, "cpu")
     for bad in (dict(head_dim=64), dict(Lk=32), dict(kv_lens=torch.tensor([3], dtype=torch.int32)),
                 dict(seqs_per_batch=2)):
-        with pytest.raises(osb8.OsbError):
-            osb8.attn_fp8(q, k, v, out, workspace=ws, **dict(kw, **bad))
-    with pytest.raises(osb8.OsbError):   # a workspace for fewer heads
-        osb8.attn_fp8(q, k, v, out, workspace=osb8.attn_fp8_workspace(1, 64, 1, "cpu"), **kw)
+        with pytest.raises(fake_osb.OsbError):
+            fake_osb.attn_fp8(q, k, v, out, workspace=ws, **dict(kw, **bad))
+    with pytest.raises(fake_osb.OsbError):   # a workspace for fewer heads
+        fake_osb.attn_fp8(q, k, v, out, workspace=fake_osb.attn_fp8_workspace(1, 64, 1, "cpu"), **kw)
 
 
 def _case(model, inp, mlps=False):
@@ -136,7 +128,7 @@ def _case(model, inp, mlps=False):
 
 @pytest.mark.parametrize("fused,liger,mlps", [(True, False, False), (False, False, False), (False, True, False),
                                               (True, True, False), (False, True, True), (True, False, True)])
-def test_host_mmdit_fp8_attention_follows_the_emulation(osb8, fused, liger, mlps):
+def test_host_mmdit_fp8_attention_follows_the_emulation(fake_osb, fused, liger, mlps):
     """C = 256 (2 heads of 128), 2 double + 2 single blocks, FP8 attention (and FP8 MLPs) on the stand-in, against the
     fp32 oracle.  Yardstick: the emulation reference measured in the same test."""
     m = _rand_model(fused, liger)
@@ -153,49 +145,44 @@ def test_host_mmdit_fp8_attention_follows_the_emulation(osb8, fused, liger, mlps
     print(f"[mmdit fp8 attn host] fused={fused} liger={liger} mlps={mlps}: product {r_out:.3e}, FP8 emulation "
           f"{r_emu:.3e}, bf16 oracle {r_bf:.3e} (rel-L2 against the fp32 oracle)")
     assert r_out < 1.1 * r_emu, (r_out, r_emu, r_bf)
-    names = [c[0] for c in osb8.calls]
+    names = [c[0] for c in fake_osb.calls]
     nd, ns = CFG["depth"], CFG["depth_single_blocks"]
     assert names.count("attn_fp8") == nd + ns and "attn_short" not in names
     assert (names.count("gemm_fp8_blocks") > 0) == mlps
 
 
-def test_disable_fp8_attention_restores_the_bf16_bits(osb8):
+def test_disable_fp8_attention_restores_the_bf16_bits(fake_osb):
     m, plain = _rand_model(False, True), _rand_model(False, True)
     inp = _inputs(B=1)
     with torch.no_grad():
         want = plain(**inp)
-        plain_calls = list(osb8.calls)
-        osb8.reset()
+        plain_calls = list(fake_osb.calls)
+        fake_osb.reset()
         m.enable_fp8_attention()
         fp8 = m(**inp)
         m.disable_fp8_attention()
-        osb8.reset()
+        fake_osb.reset()
         back = m(**inp)
     assert not torch.equal(fp8, want)
     assert torch.equal(back, want)
-    assert m._fp8_attn_state is None and osb8.calls == plain_calls
+    assert m._fp8_attn_state is None and fake_osb.calls == plain_calls
 
 
-def test_lora_adapter_applies_with_fp8_attention(osb8, fake_osb, tmp_path):
+def test_lora_adapter_applies_with_fp8_attention(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora
-    from tests import lora_ref
 
-    fake_osb.gemm_lora = lora_ref.gemm_lora
-    try:
-        m = _rand_model(True)
-        m.enable_fp8_attention()
-        inp = _inputs(B=1)
-        with torch.no_grad():
-            base = m(**inp)
-            load_lora(m, write_adapter(str(tmp_path / "a"), m, targets=["double_blocks.0.img_attn.qkv",
-                                                                         "single_blocks.1.linear2"]))
-            osb8.reset()
-            adapted = m(**inp)
-        names = [c[0] for c in osb8.calls]
-        assert "gemm_lora" in names and names.count("attn_fp8") == 4
-        assert not torch.equal(adapted, base) and torch.isfinite(adapted.float()).all()
-    finally:
-        del fake_osb.gemm_lora
+    m = _rand_model(True)
+    m.enable_fp8_attention()
+    inp = _inputs(B=1)
+    with torch.no_grad():
+        base = m(**inp)
+        load_lora(m, write_adapter(str(tmp_path / "a"), m, targets=["double_blocks.0.img_attn.qkv",
+                                                                     "single_blocks.1.linear2"]))
+        fake_osb.reset()
+        adapted = m(**inp)
+    names = [c[0] for c in fake_osb.calls]
+    assert "gemm_lora" in names and names.count("attn_fp8") == 4
+    assert not torch.equal(adapted, base) and torch.isfinite(adapted.float()).all()
 
 
 def test_fp8_attention_refuses_other_head_sizes():
@@ -219,13 +206,6 @@ def _sp_worker(rank, world, port, ret):
     try:
         from tests import fake_osb200
 
-        class _MP:   # monkeypatch stand-in for a process without pytest fixtures
-            @staticmethod
-            def setattr(obj, name, value, raising=True):
-                setattr(obj, name, value)
-
-        FA.install(_MP)
-        FB.install(_MP)
         sys.modules["osb200"] = fake_osb200
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []

@@ -1,10 +1,10 @@
-"""The FP8 (e4m3) attention of MMDiT on the GPU: the prep kernels against the stand-in (tests/fake_osb200_fp8_attn.py),
+"""The FP8 (e4m3) attention of MMDiT on the GPU: the prep kernels against the stand-in (tests/fake_osb200.py),
 the attention kernel against fp32 softmax attention on the dequantized workspace operands, the refusals, and MMDiT with
 FP8 attention (alone and with the FP8 MLPs) against the fp32 oracle, with the emulation references as yardsticks."""
 import pytest
 import torch
 
-from tests import fake_osb200_fp8_attn as FA
+from tests import fake_osb200 as F_
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_ref as MR
 from tests.test_mmdit_fp8_gpu import _inputs, _wide_model
@@ -52,10 +52,10 @@ def test_prep_matches_the_stand_in(B, L, H, liger, split):
     ws, _ = _run(qkv, kw)
     C = H * 128
     skip = ("seqs_per_batch", "Lq", "Lk", "num_heads", "head_dim")
-    qf, kf, vf, _ = FA.stage(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], L=L, H=H, norm_eps=1e-6,
+    qf, kf, vf, _ = F_.stage(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], L=L, H=H, norm_eps=1e-6,
                              **{k: v for k, v in kw.items() if k not in skip})
-    ref = FA.AttnFp8Workspace(B, L, H, "cuda")
-    FA.fill_workspace(ref, qf, kf, vf)
+    ref = F_.AttnFp8Workspace(B, L, H, "cuda")
+    F_.fill_workspace(ref, qf, kf, vf)
     u8 = lambda t: t.view(torch.uint8)   # noqa: E731
     assert torch.equal(u8(ws.vt8), u8(ref.vt8)) and torch.equal(ws.s_v, ref.s_v)
     assert not ws.v_amax.any()   # left zero for the next call
@@ -77,7 +77,7 @@ def _check_kernel(qkv, kw, heads=6, bar=None):
     ws, out = _run(qkv, kw)
     B, L, H = kw["num_seqs"], kw["Lq"], kw["num_heads"]
     assert torch.isfinite(out.float()).all()
-    q8, sq, k8, sk, v8, sv = FA.workspace_operands(ws, B * H, L)
+    q8, sq, k8, sk, v8, sv = F_.workspace_operands(ws, B * H, L)
     got = out.view(B, L, H, 128).transpose(1, 2).reshape(B * H, L, 128)
     sel = torch.linspace(0, B * H - 1, min(heads, B * H)).round().long().tolist()
     errs = []

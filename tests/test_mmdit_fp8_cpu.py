@@ -1,4 +1,4 @@
-"""The block-scaled FP8 (e4m3) MLP path of MMDiT on the CPU: the stand-in entries of tests/fake_osb200_fp8_blocks.py
+"""The block-scaled FP8 (e4m3) MLP path of MMDiT on the CPU: the stand-in entries of tests/fake_osb200.py
 against the contract arithmetic, the host-side MMDiTModel with `enable_fp8()` against the FP8-emulation reference of
 tests/mmdit_fp8_ref.py (both QKV and both RoPE layouts), `disable_fp8()`, the refusals, Ulysses sequence parallelism on
 two gloo ranks, and the ctypes mirror of `osb_fp8_blocks_args`."""
@@ -9,7 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import fake_osb200_fp8_blocks as FB
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests import mmdit_fp8_ref as MR
 from tests.test_host_mmdit_cpu import _rand_model
@@ -21,12 +21,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4M3 = torch.float8_e4m3fn
 
 
-@pytest.fixture
-def osb8(fake_osb, monkeypatch):
-    FB.install(monkeypatch)
-    return fake_osb
-
-
 def _blocky(seed=0, rows=6, K=512):
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(rows, K, generator=g) * torch.logspace(-3, 2, K // 128).repeat_interleave(128)
@@ -36,9 +30,9 @@ def _blocky(seed=0, rows=6, K=512):
     return x
 
 
-def test_quant_blocks_matches_the_contract(osb8):
+def test_quant_blocks_matches_the_contract(fake_osb):
     x = _blocky().to(torch.bfloat16)
-    q, s = osb8.quant_blocks_fp8(x)
+    q, s = fake_osb.quant_blocks_fp8(x)
     rq, rs = R.quantize(x.float().view(6, 4, 128))
     assert q.dtype == E4M3 and s.shape == (6, 4)
     assert torch.equal(s, rs) and torch.equal(q.double().view(6, 4, 128), rq)
@@ -46,32 +40,32 @@ def test_quant_blocks_matches_the_contract(osb8):
     assert q[2, 300].float() == -448.0 and torch.all(q[3, :128].float() == 448.0)
     # block = K: one scale per row, any K (the weights: K = 5 x 3072 is beyond the row quantizer's 8192)
     w = torch.randn(8, 15360).to(torch.bfloat16)
-    qw, sw = osb8.quant_blocks_fp8(w, block=15360)
+    qw, sw = fake_osb.quant_blocks_fp8(w, block=15360)
     rqw, rsw = R.quantize(w.float())
     assert sw.shape == (8, 1) and torch.equal(sw[:, 0], rsw) and torch.equal(qw.double(), rqw)
     # column views of a wider buffer on both sides
     cat, cats = torch.zeros(6, 640, dtype=E4M3), torch.zeros(6, 5)
-    osb8.quant_blocks_fp8(x[:, :256], out=cat[:, :256], out_scale=cats[:, :2])
+    fake_osb.quant_blocks_fp8(x[:, :256], out=cat[:, :256], out_scale=cats[:, :2])
     assert torch.equal(cat[:, :256].float(), q[:, :256].float()) and torch.equal(cats[:, :2], s[:, :2])
-    with pytest.raises(osb8.OsbError):
-        osb8.quant_blocks_fp8(torch.zeros(4, 200, dtype=torch.bfloat16))
+    with pytest.raises(fake_osb.OsbError):
+        fake_osb.quant_blocks_fp8(torch.zeros(4, 200, dtype=torch.bfloat16))
 
 
 @pytest.mark.parametrize("epilogue", [0, 1, 2, 5])
-def test_gemm_fp8_blocks_matches_dequantized_fp32(osb8, epilogue):
+def test_gemm_fp8_blocks_matches_dequantized_fp32(fake_osb, epilogue):
     g = torch.Generator().manual_seed(4)
     M, N, K = 70, 256, 512
     a = _blocky(5, M, K)
     w = torch.randn(N, K, generator=g) / K ** 0.5
-    a8, sa = osb8.quant_blocks_fp8(a.to(torch.bfloat16))
-    w8, sw = osb8.quant_blocks_fp8(w.to(torch.bfloat16), block=K)
+    a8, sa = fake_osb.quant_blocks_fp8(a.to(torch.bfloat16))
+    w8, sw = fake_osb.quant_blocks_fp8(w.to(torch.bfloat16), block=K)
     sw = sw.view(-1)
     bias = torch.randn(N, generator=g).to(torch.bfloat16)
     res = torch.randn(M, N, generator=g).to(torch.bfloat16)
     gate = torch.randn(4, N, generator=g)
     mod_index = torch.tensor([3, 1, 0, 2, 1], dtype=torch.int32)
     kw = dict(residual=res, gate=gate, group_rows=16, mod_index=mod_index) if epilogue == 2 else {}
-    got = osb8.gemm_fp8_blocks(a8, sa, w8, sw, bias, epilogue=epilogue, **kw)
+    got = fake_osb.gemm_fp8_blocks(a8, sa, w8, sw, bias, epilogue=epilogue, **kw)
     deq_a = (a8.double().view(M, 4, 128) * sa.double()[..., None]).view(M, K)
     ref = deq_a @ (w8.double() * sw.double()[:, None]).t() + bias.double()
     if epilogue in (1, 5):
@@ -92,11 +86,11 @@ def test_gemm_fp8_blocks_matches_dequantized_fp32(osb8, epilogue):
         return
     assert rel_l2(got, ref) < 3e-3
     if epilogue != 5:   # per-row A scales: the same value as block scales that repeat along the row
-        row = osb8.gemm_fp8_blocks(a8, sa[:, 0].contiguous(), w8, sw, bias, epilogue=epilogue, **kw)
-        rep = osb8.gemm_fp8_blocks(a8, sa[:, :1].expand(M, 4).contiguous(), w8, sw, bias, epilogue=epilogue, **kw)
+        row = fake_osb.gemm_fp8_blocks(a8, sa[:, 0].contiguous(), w8, sw, bias, epilogue=epilogue, **kw)
+        rep = fake_osb.gemm_fp8_blocks(a8, sa[:, :1].expand(M, 4).contiguous(), w8, sw, bias, epilogue=epilogue, **kw)
         assert torch.equal(row, rep)
-    with pytest.raises(osb8.OsbError):   # the FP8 GELU epilogue needs whole 128-column scale blocks
-        osb8.gemm_fp8_blocks(a8, sa, w8[:200], sw[:200], epilogue=5)
+    with pytest.raises(fake_osb.OsbError):   # the FP8 GELU epilogue needs whole 128-column scale blocks
+        fake_osb.gemm_fp8_blocks(a8, sa, w8[:200], sw[:200], epilogue=5)
 
 
 def _fp8_case(model, inp):
@@ -119,7 +113,7 @@ def _fp8_case(model, inp):
 
 
 @pytest.mark.parametrize("fused,liger", [(True, False), (False, False), (False, True), (True, True)])
-def test_host_mmdit_fp8_follows_the_emulation(osb8, fused, liger):
+def test_host_mmdit_fp8_follows_the_emulation(fake_osb, fused, liger):
     """C = 256 (2 heads), 2 double + 2 single blocks, FP8 MLPs on the stand-in, against the fp32 oracle.  Yardstick: the
     FP8-emulation reference (the oracle in bf16 with its MLPs at the FP8 rounding points), measured in the same test."""
     m = _rand_model(fused, liger)
@@ -130,26 +124,26 @@ def test_host_mmdit_fp8_follows_the_emulation(osb8, fused, liger):
     print(f"[mmdit fp8 host] fused={fused} liger={liger}: product {r_out:.3e}, FP8 emulation {r_emu:.3e}, "
           f"bf16 oracle {r_bf:.3e} (rel-L2 against the fp32 oracle)")
     assert r_out < 1.1 * r_emu and r_emu > r_bf, (r_out, r_emu, r_bf)
-    names = [c[0] for c in osb8.calls]
+    names = [c[0] for c in fake_osb.calls]
     nd, ns = CFG["depth"], CFG["depth_single_blocks"]
     assert names.count("ln_modulate_fp8") == 2 * nd + ns
     assert names.count("gemm_fp8_blocks") == 2 * (2 * nd + ns)
     # the attention output of every single block, and (first forward on the CPU) the 2 weights of every MLP
     assert names.count("quant_blocks_fp8") == ns + 2 * (2 * nd + ns)
     assert "gemm_fp8" not in names and "quant_rows_fp8" not in names
-    blocks = [c[1] for c in osb8.calls if c[0] == "gemm_fp8_blocks"]
-    assert all(d[3] == FB.EPI_BIAS_GELU_TANH_FP8 and d[4] == 1 for d in blocks[0::2])   # fc1: per-row A, FP8 out
+    blocks = [c[1] for c in fake_osb.calls if c[0] == "gemm_fp8_blocks"]
+    assert all(d[3] == F_.EPI_BIAS_GELU_TANH_FP8 and d[4] == 1 for d in blocks[0::2])   # fc1: per-row A, FP8 out
     assert all(d[3] == 2 and d[4] == 2 for d in blocks[1::2])                          # fc2: block A, gate + residual
     assert sorted({d[2] for d in blocks[1::2]}) == [4 * 256, 5 * 256]                  # K = 4C (fc2), 5C (linear2)
-    osb8.reset()
+    fake_osb.reset()
     with torch.no_grad():
         again = m(**inp)
     assert torch.equal(again, out)
-    assert "quant_blocks_fp8" in [c[0] for c in osb8.calls] and \
-        [c[0] for c in osb8.calls].count("quant_blocks_fp8") == ns   # weights stay quantized
+    assert "quant_blocks_fp8" in [c[0] for c in fake_osb.calls] and \
+        [c[0] for c in fake_osb.calls].count("quant_blocks_fp8") == ns   # weights stay quantized
 
 
-def test_disable_fp8_restores_the_bf16_bits(osb8):
+def test_disable_fp8_restores_the_bf16_bits(fake_osb):
     m, plain = _rand_model(False, True), _rand_model(False, True)
     inp = _inputs(B=1)
     with torch.no_grad():
@@ -157,11 +151,11 @@ def test_disable_fp8_restores_the_bf16_bits(osb8):
         m.enable_fp8()
         fp8 = m(**inp)
         m.disable_fp8()
-        osb8.reset()
+        fake_osb.reset()
         back = m(**inp)
     assert not torch.equal(fp8, want)
     assert torch.equal(back, want)
-    assert m._fp8_state is None and not any("fp8" in c[0] for c in osb8.calls)
+    assert m._fp8_state is None and not any("fp8" in c[0] for c in fake_osb.calls)
 
 
 def test_fp8_refuses_sizes_beyond_the_kernels():
@@ -181,7 +175,7 @@ def test_fp8_refuses_sizes_beyond_the_kernels():
 
 
 @pytest.mark.parametrize("fused", [True, False])
-def test_fp8_and_mlp_adapters_refuse_each_other(osb8, fake_osb, tmp_path, fused):
+def test_fp8_and_mlp_adapters_refuse_each_other(fake_osb, tmp_path, fused):
     """LoRA / DoRA on an MLP Linear cannot run on the FP8 path: enable_fp8 on an adapted model and load_lora on an FP8
     model both refuse it.  Adapters on other Linears keep working with FP8 on."""
     from opensora.utils.lora import load_lora, unload_lora
@@ -210,15 +204,11 @@ def test_fp8_and_mlp_adapters_refuse_each_other(osb8, fake_osb, tmp_path, fused)
             load_lora(m, d)
         m.disable_fp8()
     # an adapter on the attention projections runs with FP8 MLPs
-    from tests import lora_ref
-
-    fake_osb.gemm_lora = lora_ref.gemm_lora
     load_lora(m, write_adapter(str(tmp_path / "proj"), m, targets=["double_blocks.0.img_attn.proj"]))
     m.enable_fp8()
     with torch.no_grad():
         out = m(**_inputs(B=1))
     assert torch.isfinite(out.float()).all()
-    del fake_osb.gemm_lora
 
 
 def _sp_worker(rank, world, port, ret):
@@ -231,12 +221,6 @@ def _sp_worker(rank, world, port, ret):
     try:
         from tests import fake_osb200
 
-        class _MP:   # monkeypatch stand-in for a process without pytest fixtures
-            @staticmethod
-            def setattr(obj, name, value, raising=True):
-                setattr(obj, name, value)
-
-        FB.install(_MP)
         sys.modules["osb200"] = fake_osb200
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []

@@ -7,7 +7,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import fake_osb200_fp8_blocks as FB
+from tests import fake_osb200 as F_
 from tests import mmdit_fp8_ref as MR
 from tests.test_mmdit_gpu import CFG, _ids, _rand_model
 from tests.util import rel_l2, report
@@ -27,8 +27,8 @@ def _operands(M, N, K, seed):
     a = torch.randn(M, K, generator=g) * torch.logspace(-2, 1, K // 128).repeat_interleave(128)
     a = a * torch.logspace(-1, 1, M)[:, None]
     w = torch.randn(N, K, generator=g) / K ** 0.5
-    a8, sa = FB.quant_blocks(a)
-    w8, sw = FB.quant_blocks(w, K)
+    a8, sa = F_.quant_blocks(a)
+    w8, sw = F_.quant_blocks(w, K)
     return g, a8.cuda(), sa.cuda(), w8.cuda(), sw.view(-1).cuda()
 
 
@@ -74,8 +74,8 @@ def test_per_row_mode_is_gemm_fp8(epilogue):
 
     M, N, K = 1000, 640, 3072
     g = torch.Generator().manual_seed(9)
-    a8, sa = (t.cuda() for t in FB.f8._quant(torch.randn(M, K, generator=g)))
-    w8, sw = (t.cuda() for t in FB.f8._quant(torch.randn(N, K, generator=g) / K ** 0.5))
+    a8, sa = (t.cuda() for t in F_._quant(torch.randn(M, K, generator=g)))
+    w8, sw = (t.cuda() for t in F_._quant(torch.randn(N, K, generator=g) / K ** 0.5))
     bias = torch.randn(N, generator=g).to(torch.bfloat16).cuda()
     res = torch.randn(M, N, generator=g).to(torch.bfloat16).cuda()
     gate = torch.randn(2, N, generator=g).cuda()
@@ -134,7 +134,7 @@ def test_quant_blocks_fp8_matches_the_stand_in(rows, K, block, ld):
     x[1] = 0
     x[2, 5] = 3e4
     q, s = osb200.quant_blocks_fp8(x.cuda()[:, :K], block=block)
-    rq, rs = FB.quant_blocks_fp8(x[:, :K], block=block)
+    rq, rs = F_.quant_blocks_fp8(x[:, :K], block=block)
     assert torch.equal(s.cpu(), rs)
     assert torch.equal(q.cpu().view(torch.uint8), rq.view(torch.uint8))
 

@@ -1,5 +1,5 @@
 """LoRA / DoRA adapters on the MMDiT FP8 GEMMs on the CPU (`enable_fp8(..., lora=True)`): the stand-in of
-`gemm_fp8_lora` (tests/fake_osb200_fp8_lora.py) against its formula, the host-side model against the FP8-emulation
+`gemm_fp8_lora` (tests/fake_osb200.py) against its formula, the host-side model against the FP8-emulation
 reference with the adapters (tests/mmdit_fp8_lora_ref.py) for LoRA and DoRA on MLP and projection targets in both QKV
 and RoPE layouts, with and without FP8 projections and attention, the order of load / enable calls, unload and disable,
 the e4m3 A_cat cache, the bits without an adapter, the default refusal and Ulysses sequence parallelism on two gloo ranks."""
@@ -9,8 +9,7 @@ import os
 import pytest
 import torch
 
-from tests import fake_osb200_fp8_blocks as FB
-from tests import fake_osb200_fp8_lora as FL
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_lora_ref as LR
@@ -22,15 +21,6 @@ from tests.test_mmdit_gpu import CFG
 from tests.util import rel_l2
 
 E4M3 = torch.float8_e4m3fn
-
-
-@pytest.fixture
-def osb8(fake_osb, monkeypatch):
-    FL.install_fp8_proj(monkeypatch)
-    from tests import fake_osb200_dora
-
-    fake_osb200_dora.install(monkeypatch)   # adapters on bf16 Linears (modulation, embedders, final layer)
-    return fake_osb
 
 
 def _mlp_targets(m):
@@ -48,28 +38,28 @@ def _adapter(tmp_path, m, targets, dora, name="a", **kw):
 
 
 # ---- the stand-in ------------------------------------------------------------------------------------------------------
-def test_stand_in_formula_and_col_scale(osb8):
+def test_stand_in_formula_and_col_scale(fake_osb):
     g = torch.Generator().manual_seed(0)
     M, N, K, r = 70, 256, 384, 72
-    a8, sa = FB.quant_blocks(torch.randn(M, K, generator=g))
-    w8, sw = FB.quant_blocks(torch.randn(N, K, generator=g), K)
+    a8, sa = F_.quant_blocks(torch.randn(M, K, generator=g))
+    w8, sw = F_.quant_blocks(torch.randn(N, K, generator=g), K)
     u = torch.randn(M, r, generator=g).to(torch.bfloat16)
     b = (0.1 * torch.randn(N, r, generator=g)).to(torch.bfloat16)
     bias = torch.randn(N, generator=g).to(torch.bfloat16)
     cs = 0.5 + torch.rand(N, generator=g)
-    out = osb8.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u, b, col_scale=cs)
+    out = fake_osb.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u, b, col_scale=cs)
     want = cs * ((a8.float() * sa.repeat_interleave(128, 1)) @ (w8.float() * sw).t() + u.float() @ b.float().t()) + bias.float()
     assert rel_l2(out, want) < 4e-3
-    ones = osb8.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u, b, col_scale=torch.ones(N))
-    assert torch.equal(ones, osb8.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u, b))
-    codes, scales = osb8.gemm_fp8_lora(a8, sa[:, 0].contiguous(), w8, sw.view(-1), bias, u, b,
-                                       epilogue=FB.EPI_BIAS_GELU_TANH_FP8)
-    acc = FL.gemm_fp8_lora_acc(a8, sa[:, 0].contiguous(), w8, sw.view(-1), u, b) + bias.float()
-    q, s = FB.quant_blocks(torch.nn.functional.gelu(acc, approximate="tanh"))
+    ones = fake_osb.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u, b, col_scale=torch.ones(N))
+    assert torch.equal(ones, fake_osb.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u, b))
+    codes, scales = fake_osb.gemm_fp8_lora(a8, sa[:, 0].contiguous(), w8, sw.view(-1), bias, u, b,
+                                       epilogue=F_.EPI_BIAS_GELU_TANH_FP8)
+    acc = F_.gemm_fp8_lora_acc(a8, sa[:, 0].contiguous(), w8, sw.view(-1), u, b) + bias.float()
+    q, s = F_.quant_blocks(torch.nn.functional.gelu(acc, approximate="tanh"))
     assert torch.equal(codes.float(), q.float()) and torch.equal(scales, s)
-    with pytest.raises(osb8.OsbError):
-        osb8.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u[:, :12], b[:, :12])   # r % 8
-    assert osb8.calls[-1][0] == "gemm_fp8_lora"
+    with pytest.raises(fake_osb.OsbError):
+        fake_osb.gemm_fp8_lora(a8, sa, w8, sw.view(-1), bias, u[:, :12], b[:, :12])   # r % 8
+    assert fake_osb.calls[-1][0] == "gemm_fp8_lora"
 
 
 # ---- the host model ----------------------------------------------------------------------------------------------------
@@ -95,7 +85,7 @@ def _case(model, inp, proj, attn):
 @pytest.mark.parametrize("fused,liger,proj,attn,dora", [(True, False, True, False, False), (False, True, True, True, True),
                                                         (True, True, False, False, True), (False, False, False, True, False),
                                                         (True, False, True, True, True)])
-def test_host_mmdit_fp8_lora_follows_the_emulation(osb8, tmp_path, fused, liger, proj, attn, dora):
+def test_host_mmdit_fp8_lora_follows_the_emulation(fake_osb, tmp_path, fused, liger, proj, attn, dora):
     """C = 256, 2 double + 2 single blocks, an adapter (update 30% of |W|) on every FP8 Linear, against the fp32 oracle on
     the merged weights.  Yardstick: the FP8-emulation reference with the adapters, measured in the same test."""
     m = _rand_model(fused, liger)
@@ -107,21 +97,21 @@ def test_host_mmdit_fp8_lora_follows_the_emulation(osb8, tmp_path, fused, liger,
         if attn:
             m.enable_fp8_attention()
         load_lora(m, _adapter(tmp_path, m, _block_targets(m) if proj else _mlp_targets(m), dora, rel=0.3))
-        osb8.reset()
+        fake_osb.reset()
         out, emu, ref = _case(m, inp, proj, attn)
     r_out, r_emu = rel_l2(out, ref), rel_l2(emu, ref)
     print(f"[mmdit fp8 lora host] fused={fused} liger={liger} proj={proj} attn={attn} dora={dora}: product {r_out:.3e}, "
           f"FP8 emulation {r_emu:.3e} (rel-L2 against the fp32 oracle on merged weights)")
     assert r_out < 1.1 * r_emu, (r_out, r_emu)
     assert rel_l2(out, base.float()) > 2 * r_out, "the adapter must move the output well beyond the error"
-    names = [c[0] for c in osb8.calls]
+    names = [c[0] for c in fake_osb.calls]
     nd, ns, B = CFG["depth"], CFG["depth_single_blocks"], inp["img"].shape[0]
     # without FP8 projections the q|k|v rows of linear1 / v_mlp (an MLP Linear) run on the bf16 LoRA GEMM
     assert names.count("gemm_lora") == (0 if proj else ns)
     if proj:   # per double block: 2 x B qkv, 2 x B proj, 2 x 2 MLP; per single block: qkv, mlp, linear2
         assert names.count("gemm_fp8_lora") == nd * (4 * B + 4) + 3 * ns
         # down GEMMs: per double block 2 qkv + 1 proj + 2 x 2 MLP; per single block linear1 (shared) + linear2
-        downs = [c for c in osb8.calls if c[0] == "gemm_fp8_blocks" and c[1][1] % 128 != 0]
+        downs = [c for c in fake_osb.calls if c[0] == "gemm_fp8_blocks" and c[1][1] % 128 != 0]
         assert len(downs) == 7 * nd + 2 * ns
     else:
         assert names.count("gemm_fp8_lora") == 4 * nd + 2 * ns
@@ -138,7 +128,7 @@ def _forward(m, inp):
         return m(**inp)
 
 
-def test_call_order_unload_and_disable(osb8, tmp_path):
+def test_call_order_unload_and_disable(fake_osb, tmp_path):
     from opensora.utils.lora import unload_lora
 
     inp = _inputs(B=1)
@@ -154,8 +144,8 @@ def test_call_order_unload_and_disable(osb8, tmp_path):
     plain.enable_fp8(projections=True)
     want = _forward(plain, inp)
     unload_lora(a)
-    osb8.reset()
-    assert torch.equal(_forward(a, inp), want) and "gemm_fp8_lora" not in [c[0] for c in osb8.calls]
+    fake_osb.reset()
+    assert torch.equal(_forward(a, inp), want) and "gemm_fp8_lora" not in [c[0] for c in fake_osb.calls]
     b.disable_fp8()
     bf = _rand_model(True, False)
     load_lora(bf, path)
@@ -163,18 +153,18 @@ def test_call_order_unload_and_disable(osb8, tmp_path):
 
 
 @pytest.mark.parametrize("proj", [False, True])
-def test_lora_keyword_without_adapter_gives_the_fp8_bits(osb8, proj):
+def test_lora_keyword_without_adapter_gives_the_fp8_bits(fake_osb, proj):
     inp = _inputs(B=1)
     a, b = _rand_model(False, True), _rand_model(False, True)
     a.enable_fp8(projections=proj)
     b.enable_fp8(projections=proj, lora=True)
     want = _forward(a, inp)
-    calls = list(osb8.calls)
-    osb8.reset()
-    assert torch.equal(_forward(b, inp), want) and osb8.calls == calls
+    calls = list(fake_osb.calls)
+    fake_osb.reset()
+    assert torch.equal(_forward(b, inp), want) and fake_osb.calls == calls
 
 
-def test_cached_a_cat_follows_the_adapter_state(osb8, tmp_path):
+def test_cached_a_cat_follows_the_adapter_state(fake_osb, tmp_path):
     """An edited lora_A, lora_B or DoRA magnitude, or a reloaded adapter, reaches the FP8 path: the output equals a fresh
     model's with the same adapter state."""
     from opensora.utils.lora import unload_lora
@@ -204,7 +194,7 @@ def test_cached_a_cat_follows_the_adapter_state(osb8, tmp_path):
     assert torch.equal(_forward(m, inp), _forward(other, inp))
 
 
-def test_default_enable_fp8_still_refuses(osb8, tmp_path):
+def test_default_enable_fp8_still_refuses(fake_osb, tmp_path):
     m = _rand_model(True, False)
     load_lora(m, _adapter(tmp_path, m, ["double_blocks.0.img_mlp.0"], False))
     with pytest.raises(ValueError, match="FP8 MLPs cannot run LoRA / DoRA adapters"):
@@ -218,7 +208,7 @@ def test_default_enable_fp8_still_refuses(osb8, tmp_path):
     assert torch.isfinite(_forward(n, _inputs(B=1)).float()).all()
 
 
-def test_down_projection_reads_the_fp8_codes(osb8, tmp_path):
+def test_down_projection_reads_the_fp8_codes(fake_osb, tmp_path):
     """U = bf16(qdq(x) qdq_rows(A_cat)^T): the down GEMM of fc1 reads the LN+modulate codes and an A_cat quantized per
     row, whatever its rank padding."""
     m = _rand_model(True, False)
@@ -239,15 +229,8 @@ def _sp_worker(rank, world, port, adapter_dir, ret):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        from tests import fake_osb200, fake_osb200_dora
+        from tests import fake_osb200
 
-        class _MP:   # monkeypatch stand-in for a process without pytest fixtures
-            @staticmethod
-            def setattr(obj, name, value, raising=True):
-                setattr(obj, name, value)
-
-        FL.install_fp8_proj(_MP)
-        fake_osb200_dora.install(_MP)
         sys.modules["osb200"] = fake_osb200
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []

@@ -1,5 +1,5 @@
 """LoRA / DoRA on the FP8 GEMM (osb_gemm_fp8_lora) on the GPU: the kernel against the arithmetic of its CPU stand-in
-(tests/fake_osb200_fp8_lora.py) for every epilogue, block_n, per-row and block-scaled A, ranks of one and two tail
+(tests/fake_osb200.py) for every epilogue, block_n, per-row and block-scaled A, ranks of one and two tail
 k-blocks and a zero-padded tail, M off the tile grid, strided U / B and gate + residual in place; exact operands (bit
 for bit); NULL against all-ones col_scale; CUDA-graph replay; argument errors; and MMDiT with an adapter on every block
 Linear against the fp32 oracle on the merged weights g (W + s B A), with the FP8-emulation reference as the yardstick."""
@@ -7,8 +7,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import fake_osb200_fp8_blocks as FB
-from tests import fake_osb200_fp8_lora as FL
+from tests import fake_osb200 as F_
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_lora_ref as LR
 from tests import mmdit_fp8_proj_ref as PR
@@ -20,7 +19,7 @@ from tests.util import rel_l2, report
 pytestmark = pytest.mark.gpu
 
 GATE_RES, GELU, BIAS = 2, 1, 0
-GELU_FP8 = FB.EPI_BIAS_GELU_TANH_FP8
+GELU_FP8 = F_.EPI_BIAS_GELU_TANH_FP8
 
 
 @pytest.fixture(autouse=True)
@@ -33,8 +32,8 @@ def _operands(M, N, K, r, seed, block_a=True, ldu=None, ldb=None):
     g = torch.Generator().manual_seed(seed)
     a = torch.randn(M, K, generator=g) * torch.logspace(-1, 1, K // 128).repeat_interleave(128)
     w = torch.randn(N, K, generator=g) / K ** 0.5
-    a8, sa = FB.quant_blocks(a, 128 if block_a else K)
-    w8, sw = FB.quant_blocks(w, K)
+    a8, sa = F_.quant_blocks(a, 128 if block_a else K)
+    w8, sw = F_.quant_blocks(w, K)
     ub = torch.zeros(M, ldu or r)
     ub[:, :r] = torch.randn(M, r, generator=g)
     bb = torch.zeros(N, ldb or r)
@@ -46,7 +45,7 @@ def _operands(M, N, K, r, seed, block_a=True, ldu=None, ldb=None):
 
 def _reference(a8, sa, w8, sw, u, b, bias, col_scale, epilogue, res, gate, group_rows):
     """The stand-in's arithmetic in fp64, up to (not including) the rounding."""
-    acc = FL.gemm_fp8_lora_acc(a8, sa, w8, sw, u, b, col_scale, torch.float64)
+    acc = F_.gemm_fp8_lora_acc(a8, sa, w8, sw, u, b, col_scale, torch.float64)
     if bias is not None:
         acc = acc + bias.double()
     if epilogue in (GELU, GELU_FP8):
@@ -85,7 +84,7 @@ def test_kernel_against_the_stand_in(M, N, K, r, block_n, epilogue, block_a, dor
         torch.cuda.synchronize()
         c, s = codes[:, 128:128 + N].float(), scales[:, 1:1 + N // 128]
         deq = (c.view(M, N // 128, 128) * s[..., None]).view(M, N)
-        q, sq = FB.quant_blocks(want.float())
+        q, sq = F_.quant_blocks(want.float())
         err = rel_l2(deq, want.float())
         print(f"[fp8 lora gelu fp8] M={M} N={N} K={K} r={r}: rel-L2 {err:.3e}, code mismatches "
               f"{float((c != q.float()).float().mean()):.2e}")

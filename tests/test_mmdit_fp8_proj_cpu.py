@@ -1,5 +1,5 @@
 """The FP8 (e4m3) projection path of MMDiT on the CPU (`enable_fp8(projections=True)`): the block-scaled output of the FP8
-attention stand-in (tests/fake_osb200_fp8_proj.py) against the block rule, the host-side model against the
+attention stand-in (tests/fake_osb200.py) against the block rule, the host-side model against the
 FP8-emulation reference of tests/mmdit_fp8_proj_ref.py (both QKV and both RoPE layouts, with and without FP8 attention),
 the launches it makes, `enable_fp8()` without the keyword, `disable_fp8()`, the adapter refusals, Ulysses sequence
 parallelism on two gloo ranks and the ctypes mirror of `osb_attn_fp8_out`."""
@@ -10,9 +10,7 @@ import os
 import pytest
 import torch
 
-from tests import fake_osb200_fp8_attn as FA
-from tests import fake_osb200_fp8_blocks as FB
-from tests import fake_osb200_fp8_proj as FP
+from tests import fake_osb200 as F_
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_proj_ref as PR
 from tests.test_host_mmdit_cpu import _rand_model
@@ -25,39 +23,33 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4M3 = torch.float8_e4m3fn
 
 
-@pytest.fixture
-def osb8(fake_osb, monkeypatch):
-    FP.install(monkeypatch)
-    return fake_osb
-
-
-def test_stand_in_block_output_follows_the_block_rule(osb8):
+def test_stand_in_block_output_follows_the_block_rule(fake_osb):
     """Codes and scales land in column slices of wider buffers; each (row, head) block is the block rule applied to the
     fp32 attention value, which the bf16 output of `attn_fp8` rounds."""
     B, L, H = 2, 200, 2
     qkv, kw = _operands(B, L, H, split=50)
     C = H * 128
     q, k, v = qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:]
-    ws = osb8.attn_fp8_workspace(B, L, H, "cpu")
+    ws = fake_osb.attn_fp8_workspace(B, L, H, "cpu")
     codes = torch.zeros(B * L, 5 * C, dtype=E4M3)
     scales = torch.full((B * L, 5 * H), -1.0)
-    osb8.attn_fp8_blocks(q, k, v, codes[:, :C], scales[:, :H], workspace=ws, **kw)
-    assert osb8.calls[-1][0] == "attn_fp8_blocks"
+    fake_osb.attn_fp8_blocks(q, k, v, codes[:, :C], scales[:, :H], workspace=ws, **kw)
+    assert fake_osb.calls[-1][0] == "attn_fp8_blocks"
     assert not codes[:, C:].float().any() and torch.all(scales[:, H:] == -1.0)
-    o = FA.attention_from_workspace(ws, B * H, L, 128 ** -0.5)
+    o = F_.attention_from_workspace(ws, B * H, L, 128 ** -0.5)
     o = o.view(B, H, L, 128).transpose(1, 2).reshape(B * L, C)
-    want_codes, want_s = FB.quant_blocks(o)
+    want_codes, want_s = F_.quant_blocks(o)
     assert torch.equal(codes[:, :C].float(), want_codes.float()) and torch.equal(scales[:, :H], want_s)
     deq = (codes[:, :C].float().view(B * L, H, 128) * scales[:, :H, None]).view(B * L, C)
     amax = codes[:, :C].float().view(B * L, H, 128).abs().amax(-1)
     assert torch.all(amax == 448)                                          # every nonzero block reaches +-448
     bf = torch.zeros(B * L, C, dtype=torch.bfloat16)
-    osb8.attn_fp8(q, k, v, bf, workspace=osb8.attn_fp8_workspace(B, L, H, "cpu"), **kw)
+    fake_osb.attn_fp8(q, k, v, bf, workspace=fake_osb.attn_fp8_workspace(B, L, H, "cpu"), **kw)
     assert rel_l2(deq, bf.float()) < 0.05                                  # within the e4m3 rounding of the bf16 output
-    with pytest.raises(osb8.OsbError):                                     # the refusals of attn_fp8
-        osb8.attn_fp8_blocks(q, k, v, codes[:, :C], scales[:, :H], workspace=ws, **dict(kw, Lk=100))
-    with pytest.raises(osb8.OsbError):                                     # a scale view narrower than the heads
-        osb8.attn_fp8_blocks(q, k, v, codes[:, :C], scales[:, :1], workspace=ws, **kw)
+    with pytest.raises(fake_osb.OsbError):                                     # the refusals of attn_fp8
+        fake_osb.attn_fp8_blocks(q, k, v, codes[:, :C], scales[:, :H], workspace=ws, **dict(kw, Lk=100))
+    with pytest.raises(fake_osb.OsbError):                                     # a scale view narrower than the heads
+        fake_osb.attn_fp8_blocks(q, k, v, codes[:, :C], scales[:, :1], workspace=ws, **kw)
 
 
 def _case(model, inp, attn):
@@ -84,7 +76,7 @@ def _case(model, inp, attn):
                                                   (False, True, True, (1, 4, 6))],
                          ids=["True-False-False", "False-True-False", "True-True-True", "False-False-True",
                               "False-True-True-txt_len_eq_img_len"])
-def test_host_mmdit_fp8_projections_follow_the_emulation(osb8, fused, liger, attn, thw):
+def test_host_mmdit_fp8_projections_follow_the_emulation(fake_osb, fused, liger, attn, thw):
     """C = 256 (2 heads of 128), 2 double + 2 single blocks, every block Linear on FP8 (and FP8 attention), against the
     fp32 oracle.  Yardstick: the emulation reference measured in the same test.  With as many text as image tokens
     (thw = (1, 4, 6)) both streams of a double block get workspaces of one shape: neither may overwrite the other's
@@ -100,13 +92,13 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(osb8, fused, liger, att
     inp = _inputs(thw=thw)
     with torch.no_grad():
         m(**inp)             # weights are quantized at the first forward of a CPU model
-    osb8.reset()
+    fake_osb.reset()
     out, emu, floor, ref = _case(m, inp, attn)
     r_out, r_emu, r_bf = rel_l2(out, ref), rel_l2(emu, ref), rel_l2(floor, ref)
     print(f"[mmdit fp8 proj host] fused={fused} liger={liger} attn={attn}: product {r_out:.3e}, FP8 emulation "
           f"{r_emu:.3e}, bf16 oracle {r_bf:.3e} (rel-L2 against the fp32 oracle)")
     assert r_out < 1.1 * r_emu, (r_out, r_emu, r_bf)
-    calls = list(osb8.calls)
+    calls = list(fake_osb.calls)
     names = [c[0] for c in calls]
     nd, ns = CFG["depth"], CFG["depth_single_blocks"]
     assert names.count("ln_modulate") == 1                     # the final layer only: no bf16 LN pass in any block
@@ -119,46 +111,46 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(osb8, fused, liger, att
     assert names.count("gemm") == 12 and "gemm_lora" not in names   # 9 + 1 + 2
 
 
-def test_enable_fp8_without_keyword_keeps_the_mlp_path(osb8):
+def test_enable_fp8_without_keyword_keeps_the_mlp_path(fake_osb):
     m = _rand_model(True, False)
     inp = _inputs(B=1)
     m.enable_fp8()
     with torch.no_grad():
         m(**inp)
-        osb8.reset()
+        fake_osb.reset()
         mlp = m(**inp)
-        mlp_calls = list(osb8.calls)
+        mlp_calls = list(fake_osb.calls)
         m.enable_fp8(projections=True)
         m(**inp)
-        osb8.reset()
+        fake_osb.reset()
         proj = m(**inp)
         m.enable_fp8()
         m(**inp)
-        osb8.reset()
+        fake_osb.reset()
         again = m(**inp)
     names = [c[0] for c in mlp_calls]
     nd, ns = CFG["depth"], CFG["depth_single_blocks"]
     assert names.count("ln_modulate") == 2 * nd + ns + 1 and names.count("quant_blocks_fp8") == ns
     assert "attn_fp8_blocks" not in names
-    assert torch.equal(again, mlp) and osb8.calls == mlp_calls
+    assert torch.equal(again, mlp) and fake_osb.calls == mlp_calls
     assert not torch.equal(proj, mlp)
 
 
-def test_disable_fp8_restores_the_bf16_bits(osb8):
+def test_disable_fp8_restores_the_bf16_bits(fake_osb):
     m, plain = _rand_model(False, True), _rand_model(False, True)
     inp = _inputs(B=1)
     with torch.no_grad():
         want = plain(**inp)
-        plain_calls = list(osb8.calls)
+        plain_calls = list(fake_osb.calls)
         m.enable_fp8_attention()
         m.enable_fp8(projections=True)
         fp8 = m(**inp)
         m.disable_fp8()
         m.disable_fp8_attention()
-        osb8.reset()
+        fake_osb.reset()
         back = m(**inp)
     assert not torch.equal(fp8, want)
-    assert torch.equal(back, want) and osb8.calls == plain_calls
+    assert torch.equal(back, want) and fake_osb.calls == plain_calls
     assert m._fp8_state is None and m._fp8_proj is False
 
 
@@ -172,33 +164,28 @@ def test_fp8_proj_linears_lists_the_projections():
                                                                 "double_blocks.0.img_attn.proj"]
 
 
-def test_adapter_refusals(osb8, fake_osb, tmp_path):
+def test_adapter_refusals(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora, unload_lora
-    from tests import lora_ref
 
-    fake_osb.gemm_lora = lora_ref.gemm_lora
-    try:
-        m = _rand_model(True)
-        load_lora(m, write_adapter(str(tmp_path / "a"), m, targets=["double_blocks.0.txt_attn.proj"]))
-        with pytest.raises(ValueError, match="FP8 projections cannot run LoRA / DoRA adapters"):
-            m.enable_fp8(projections=True)
-        assert m._fp8 is False
-        m.enable_fp8()            # the MLP path takes an adapter on a projection Linear
-        m.disable_fp8()
-        unload_lora(m)
+    m = _rand_model(True)
+    load_lora(m, write_adapter(str(tmp_path / "a"), m, targets=["double_blocks.0.txt_attn.proj"]))
+    with pytest.raises(ValueError, match="FP8 projections cannot run LoRA / DoRA adapters"):
         m.enable_fp8(projections=True)
-        with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
-            load_lora(m, write_adapter(str(tmp_path / "b"), m, targets=["double_blocks.0.img_attn.proj"]))
-        with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
-            load_lora(m, write_adapter(str(tmp_path / "c"), m, targets=["double_blocks.1.img_attn.qkv"]))
-        load_lora(m, write_adapter(str(tmp_path / "d"), m, targets=["double_blocks.0.img_mod.lin", "final_layer.linear"]))
-        inp = _inputs(B=1)
-        osb8.reset()
-        with torch.no_grad():
-            out = m(**inp)
-        assert "gemm_lora" in [c[0] for c in osb8.calls] and torch.isfinite(out.float()).all()
-    finally:
-        del fake_osb.gemm_lora
+    assert m._fp8 is False
+    m.enable_fp8()            # the MLP path takes an adapter on a projection Linear
+    m.disable_fp8()
+    unload_lora(m)
+    m.enable_fp8(projections=True)
+    with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
+        load_lora(m, write_adapter(str(tmp_path / "b"), m, targets=["double_blocks.0.img_attn.proj"]))
+    with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
+        load_lora(m, write_adapter(str(tmp_path / "c"), m, targets=["double_blocks.1.img_attn.qkv"]))
+    load_lora(m, write_adapter(str(tmp_path / "d"), m, targets=["double_blocks.0.img_mod.lin", "final_layer.linear"]))
+    inp = _inputs(B=1)
+    fake_osb.reset()
+    with torch.no_grad():
+        out = m(**inp)
+    assert "gemm_lora" in [c[0] for c in fake_osb.calls] and torch.isfinite(out.float()).all()
 
 
 def _sp_worker(rank, world, port, ret):
@@ -211,12 +198,6 @@ def _sp_worker(rank, world, port, ret):
     try:
         from tests import fake_osb200
 
-        class _MP:   # monkeypatch stand-in for a process without pytest fixtures
-            @staticmethod
-            def setattr(obj, name, value, raising=True):
-                setattr(obj, name, value)
-
-        FP.install(_MP)
         sys.modules["osb200"] = fake_osb200
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []

@@ -10,13 +10,6 @@ from tests import rf_conditioning_ref as R
 from tests.util import rel_l2
 
 
-@pytest.fixture
-def fake_osb(fake_osb, monkeypatch):
-    """The binding stand-in of tests/conftest.py, with the CPU restatement of `rf_masked_step` added for this test."""
-    monkeypatch.setattr(fake_osb, "rf_masked_step", R.rf_masked_step, raising=False)
-    return fake_osb
-
-
 def _toy(x, timestep, y, mask=None, fps=None, x_mask=None, **kw):
     """[2B, C, T, H, W] -> [2B, 2C, T, H, W] fp32 (velocity | sigma halves); ignores x_mask."""
     f = x.float()

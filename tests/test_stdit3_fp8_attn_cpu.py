@@ -1,4 +1,4 @@
-"""The FP8 (e4m3) head-tile attention of STDiT3 on the CPU: the stand-in entries of tests/fake_osb200_fp8_tiles.py against
+"""The FP8 (e4m3) head-tile attention of STDiT3 on the CPU: the stand-in entries of tests/fake_osb200.py against
 the written contract (conversion codes and scales, attention against fp32 softmax on the dequantized tiles) on every set
 shape the model uses, the host-side STDiT3 with `enable_fp8_attention()` against the FP8-emulation reference
 (tests/stdit3_fp8_attn_ref.py), `disable_fp8_attention()`, the refusals, sequence parallelism on two gloo ranks and the
@@ -11,20 +11,12 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from tests import fake_osb200_fp8 as F8
-from tests import fake_osb200_fp8_tiles as FT
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests.mmdit_fp8_attn_ref import attention_from_operands
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture
-def osb8(fake_osb, monkeypatch):
-    F8.install(monkeypatch)
-    FT.install(monkeypatch)
-    return fake_osb
 
 
 def _tiles(osb, rows, tmap, kinds, H, D, seed, spread=True):
@@ -40,10 +32,10 @@ def _tiles(osb, rows, tmap, kinds, H, D, seed, spread=True):
 
 def _dequantized(t8, kind, rows, is_v):
     """fp64 [rows, H, D] values of one kind read back from the e4m3 tiles through the tile map."""
-    ti, r = FT.tile_index(t8.map, rows, t8.codes.device)
+    ti, r = F_.tile_index(t8.map, rows, t8.codes.device)
     codes = t8.codes[kind].double()
     if is_v:
-        codes = FT.v_in_key_order(t8.codes[kind]).double()
+        codes = F_.v_in_key_order(t8.codes[kind]).double()
         x = codes[:, ti, r, : t8.head_dim] * t8.scales[kind][:, ti, : t8.head_dim].double()
     else:
         x = codes[:, ti, r, : t8.head_dim] * t8.scales[kind][:, ti, r, None].double()
@@ -51,13 +43,13 @@ def _dequantized(t8, kind, rows, is_v):
 
 
 @pytest.mark.parametrize("L,D", [(300, 72), (16, 64)])
-def test_conversion_follows_the_contract(osb8, L, D):
+def test_conversion_follows_the_contract(fake_osb, L, D):
     """q / k per row, v per (tile, channel) over the tile's rows, transposed in the vt8 key order; zero rows give scale 1."""
-    tm = osb8.tile_map(0, L)
+    tm = fake_osb.tile_map(0, L)
     rows, H = 4 * L, 2
-    t = _tiles(osb8, rows, tm, 3, H, D, 0)
-    t8 = osb8.head_tiles_fp8(t, osb8.HeadTilesFp8(t), v_period=3, v_slot=2)
-    ti, r = FT.tile_index(tm, rows, "cpu")
+    t = _tiles(fake_osb, rows, tm, 3, H, D, 0)
+    t8 = fake_osb.head_tiles_fp8(t, fake_osb.HeadTilesFp8(t), v_period=3, v_slot=2)
+    ti, r = F_.tile_index(tm, rows, "cpu")
     for kind in (0, 1):
         x = t.dense[kind].float().view(rows, H, D)
         q, s = R.quantize(x)
@@ -106,36 +98,36 @@ CASES = {
 
 
 @pytest.mark.parametrize("name", list(CASES))
-def test_attention_follows_dequantized_softmax(osb8, name):
+def test_attention_follows_dequantized_softmax(fake_osb, name):
     c = CASES[name]
     L, nseq, D, H = c["L"], c["nseq"], c["D"], 2
     rows = L * nseq
     out_map = None
     if "Lk" in c:   # cross: queries unpacked, keys of the text tiles
-        qt = _tiles(osb8, rows, osb8.tile_map(0, L, pack=False), 1, H, D, 1)
-        kv = _tiles(osb8, c["Lk"] * nseq, osb8.tile_map(0, c["Lk"], keys_only=True), 2, H, D, 2)
-        q8 = osb8.head_tiles_fp8(qt, osb8.HeadTilesFp8(qt))
-        kv8 = osb8.head_tiles_fp8(kv, osb8.HeadTilesFp8(kv), v_period=2, v_slot=1)
+        qt = _tiles(fake_osb, rows, fake_osb.tile_map(0, L, pack=False), 1, H, D, 1)
+        kv = _tiles(fake_osb, c["Lk"] * nseq, fake_osb.tile_map(0, c["Lk"], keys_only=True), 2, H, D, 2)
+        q8 = fake_osb.head_tiles_fp8(qt, fake_osb.HeadTilesFp8(qt))
+        kv8 = fake_osb.head_tiles_fp8(kv, fake_osb.HeadTilesFp8(kv), v_period=2, v_slot=1)
         kv_lens = torch.tensor(c["kv_lens"], dtype=torch.int32)
         kw = dict(q_kind=0, k_kind=0, v_kind=1, Lk=c["Lk"], num_seqs=nseq, kv_lens=kv_lens)
         kv_rows, Lk = c["Lk"] * nseq, c["Lk"]
     else:
-        qt = _tiles(osb8, rows, osb8.tile_map(0, L), 3, H, D, 3)
-        q8 = kv8 = osb8.head_tiles_fp8(qt, osb8.HeadTilesFp8(qt), v_period=3, v_slot=2)
+        qt = _tiles(fake_osb, rows, fake_osb.tile_map(0, L), 3, H, D, 3)
+        q8 = kv8 = fake_osb.head_tiles_fp8(qt, fake_osb.HeadTilesFp8(qt), v_period=3, v_slot=2)
         kw = dict(Lk=L, num_seqs=nseq)
         kv_rows, Lk, kv_lens = rows, L, None
         if c.get("transposed"):   # tiles from the [B, S, T] stream, output rows frame-major [B, T, S]
             S = nseq // 2
-            out_map = osb8.tile_map(1, L, S, L)
+            out_map = fake_osb.tile_map(1, L, S, L)
             kw["out_map"] = out_map
     out = torch.full((rows, H * D), float("nan"), dtype=torch.bfloat16)
-    osb8.attn_tiles_fp8(q8, kv8, out, **kw)
-    qseq, _ = osb8._seq_pos(q8.map, rows, "cpu")
-    kseq, kpos = osb8._seq_pos(kv8.map, kv_rows, "cpu")
+    fake_osb.attn_tiles_fp8(q8, kv8, out, **kw)
+    qseq, _ = fake_osb._seq_pos(q8.map, rows, "cpu")
+    kseq, kpos = fake_osb._seq_pos(kv8.map, kv_rows, "cpu")
     exact, emu = _reference(q8, kv8, rows, kv_rows, qseq, kseq, kpos, nseq, Lk, kv_lens, kw.get("q_kind", 0),
                             kw.get("k_kind", 1), kw.get("v_kind", 2))
     if out_map is not None:   # row (seq, pos) of the tiles' stream lives at the frame-major row of `out`
-        so, po = osb8._seq_pos(out_map, rows, "cpu")
+        so, po = fake_osb._seq_pos(out_map, rows, "cpu")
         inv = torch.empty(rows, dtype=torch.long)
         inv[so * L + po] = torch.arange(rows)
         got = out[inv[qseq * L + torch.arange(rows) % L]].float().view(rows, H, D)
@@ -165,7 +157,7 @@ def _pair(which):
 
 
 @pytest.mark.parametrize("which,mlps", [("xs72", False), ("xs64", False), ("xs64", True)])
-def test_host_stdit3_fp8_attention_follows_the_emulation(osb8, which, mlps):
+def test_host_stdit3_fp8_attention_follows_the_emulation(fake_osb, which, mlps):
     """The product with FP8 attention (and FP8 MLPs) on the stand-in, against the fp32 oracle: at most 1.1x further away
     than the emulation reference (the bf16 oracle with its attentions, and MLPs, at the FP8 rounding points), plain and
     with an x_mask and ragged text."""
@@ -180,7 +172,7 @@ def test_host_stdit3_fp8_attention_follows_the_emulation(osb8, which, mlps):
     xm[1, 1:3] = False
     ob = _pair(which)[1].to(torch.bfloat16)
     for kw in ({}, {"x_mask": xm}):
-        osb8.reset()
+        fake_osb.reset()
         with torch.no_grad():
             ref = oracle(**inp, **kw)
             out = prod(**inp, **kw)
@@ -195,33 +187,33 @@ def test_host_stdit3_fp8_attention_follows_the_emulation(osb8, which, mlps):
         print(f"[fp8 attn host {which} mlps={mlps}] {'x_mask' if kw else 'plain'}: product {r_out:.3e}, "
               f"emulation {r_emu:.3e}, bf16 oracle {r_bf:.3e}")
         assert r_out < 1.1 * r_emu and r_emu > r_bf, (r_out, r_emu, r_bf)
-        names = [c[0] for c in osb8.calls]
+        names = [c[0] for c in fake_osb.calls]
         nb = 2 * cfg.depth
         assert names.count("attn_tiles_fp8") == 2 * nb and names.count("attn_tiles") == 0
         # per block: the q | k | v conversion and the cross-attention q; once per forward: all blocks' text k | v
         assert names.count("head_tiles_fp8") == 2 * nb + 1
 
 
-def test_disable_fp8_attention_restores_the_bf16_path(osb8):
+def test_disable_fp8_attention_restores_the_bf16_path(fake_osb):
     prod, _, cfg = _pair("xs72")
     inp = _inputs(cfg, 1, 4, 8, 8)
     with torch.no_grad():
-        osb8.reset()
+        fake_osb.reset()
         before = prod(**inp)
-        calls_before = list(osb8.calls)
+        calls_before = list(fake_osb.calls)
         prod.enable_fp8_attention()
         fp8 = prod(**inp)
         assert any(k[0] == "fp8attn" for k in prod._cache)
         prod.disable_fp8_attention()
-        osb8.reset()
+        fake_osb.reset()
         after = prod(**inp)
     assert not torch.equal(before, fp8)
     assert torch.equal(before, after)
-    assert osb8.calls == calls_before
+    assert fake_osb.calls == calls_before
     assert not any(k[0] == "fp8attn" for k in prod._cache)
 
 
-def test_fp8_attention_refusals(osb8, monkeypatch):
+def test_fp8_attention_refusals(fake_osb, monkeypatch):
     from opensora.models.stdit.stdit3 import STDiT3, STDiT3Config
 
     with torch.device("meta"):
@@ -251,8 +243,6 @@ def _sp_worker(rank, world, port, ret):
     try:
         from tests import fake_osb200
 
-        for name in ("HeadTilesFp8", "head_tiles_fp8", "attn_tiles_fp8"):
-            setattr(fake_osb200, name, getattr(FT, name))
         sys.modules["osb200"] = fake_osb200
         torch.manual_seed(0)
         prod, _, cfg = _pair("xs72")

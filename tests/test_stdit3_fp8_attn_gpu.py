@@ -1,5 +1,5 @@
 """The FP8 (e4m3) head-tile attention of STDiT3 on the H100: `osb_head_tiles_fp8` bit for bit against its CPU stand-in
-(tests/fake_osb200_fp8_tiles.py) on the bf16 tiles the projection GEMM wrote, `osb_attn_tiles_fp8` against fp32 softmax
+(tests/fake_osb200.py) on the bf16 tiles the projection GEMM wrote, `osb_attn_tiles_fp8` against fp32 softmax
 on the dequantized e4m3 tiles (bar: 1.1x the error of the P-emulation on the same operands) for every set shape of the
 model, the peer-scatter routing, repeatability, STDiT3-XL/2 at the benchmark shape against the fp32 oracle (yardstick:
 tests/stdit3_fp8_attn_ref.py), graph replay and `disable_fp8_attention()`."""
@@ -8,7 +8,7 @@ import types
 import pytest
 import torch
 
-from tests import fake_osb200_fp8_tiles as FT
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests.test_stdit3_fp8_attn_cpu import _reference
 from tests.util import rel_l2, report
@@ -82,7 +82,7 @@ def test_conversion_is_bit_equal_to_the_stand_in(L, D, kinds, vp):
     lg = logical(t8)
     for k in range(kinds):
         x = bf16_tiles(t, k)
-        codes, scales = FT.convert_v(x) if k % vp == vp - 1 else FT.convert_qk(x)
+        codes, scales = F_.convert_v(x) if k % vp == vp - 1 else F_.convert_qk(x)
         assert torch.equal(lg.codes[k].view(torch.uint8), codes.view(torch.uint8)), k
         assert torch.equal(lg.scales[k], scales), k
 
@@ -127,8 +127,8 @@ def test_attention_against_dequantized_softmax(name):
     torch.cuda.synchronize()
     assert torch.equal(out.view(torch.int16), again.view(torch.int16)), "a second call gives other bits"
     lq, lkv = logical(q8), logical(kv8)
-    qseq, _ = FT.base._seq_pos(q8.map, rows, "cuda")
-    kseq, kpos = FT.base._seq_pos(kv8.map, kv_rows, "cuda")
+    qseq, _ = F_._seq_pos(q8.map, rows, "cuda")
+    kseq, kpos = F_._seq_pos(kv8.map, kv_rows, "cuda")
     exact, emu = _reference(lq, lkv, rows, kv_rows, qseq, kseq, kpos, kw["num_seqs"], Lk,
                             None if kv_lens is None else kv_lens.cpu(), kw.get("q_kind", 0), kw.get("k_kind", 1),
                             kw.get("v_kind", 2))

@@ -16,15 +16,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "text_encoders.npz")
 
 
-@pytest.fixture
-def fake_osb(fake_osb, monkeypatch):
-    """The binding stand-in of tests/conftest.py with the text-encoder entries of tests/fake_osb200_text.py added."""
-    from tests import fake_osb200_text
-
-    fake_osb200_text.install(monkeypatch)
-    return fake_osb
-
-
 def _golden():
     return np.load(GOLDEN)
 
@@ -295,8 +286,8 @@ def test_enum_values_match_header(tmp_path):
                  'OSB_EPI_BIAS_QUICK_GELU);return 0;}\n')
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), src, "-o", exe])
     vals = [int(v) for v in subprocess.check_output([exe], text=True).split()]
-    from tests import fake_osb200_text
+    from tests import fake_osb200
 
-    assert vals == [3, 4] == [fake_osb200_text.EPI_GATED_GELU, fake_osb200_text.EPI_BIAS_QUICK_GELU]
+    assert vals == [3, 4] == [fake_osb200.EPI_GATED_GELU, fake_osb200.EPI_BIAS_QUICK_GELU]
     text = open(os.path.join(ROOT, "open-sora_b200", "osb200", "__init__.py")).read()
     assert "EPI_GATED_GELU, EPI_BIAS_QUICK_GELU = 3, 4" in text

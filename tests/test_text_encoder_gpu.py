@@ -1,6 +1,6 @@
 """text_embedder kernels and encoders on the H100: osb_attn_short_bias (T5 relative bias and the -inf causal mask),
 osb_rms_norm and the gated-GELU / quick-GELU GEMM epilogues against fp32 restatements, with the CPU stand-in's entries
-(tests/fake_osb200_text.py) held to the same element-wise bounds; whole-encoder parity against the oracle at the golden
+(tests/fake_osb200.py) held to the same element-wise bounds; whole-encoder parity against the oracle at the golden
 configs, full T5-XXL and full CLIP-L; CUDA-graph replay.  Each case prints max |delta| / bound."""
 import json
 import math
@@ -79,7 +79,7 @@ ATTN_CASES = [(L, kind) for L in (1, 7, 77, 128, 300, 512, 513) for kind in ("t5
 @pytest.mark.parametrize("kv_lens", [False, True])
 def test_attn_short_bias(L, kind, kv_lens):
     osb = _osb()
-    from tests import fake_osb200_text as fake
+    from tests import fake_osb200 as fake
 
     H, B = 4, 3
     qkv, bias, scale, lens = _attn_case(L, H, kind, B, kv_lens, seed=L)
@@ -102,7 +102,7 @@ def test_attn_short_bias(L, kind, kv_lens):
 def test_attn_short_bias_packed_sequences():
     """Lq < 64: 128 // L sequences share a query tile (block-diagonal keys), with the relative bias per sequence."""
     osb = _osb()
-    from tests import fake_osb200_text as fake
+    from tests import fake_osb200 as fake
 
     for L, kind in ((7, "t5"), (16, "causal"), (33, "t5")):
         H, B = 2, 11
@@ -121,7 +121,7 @@ def test_attn_short_bias_packed_sequences():
 
 def test_attn_short_bias_refusals():
     osb = _osb()
-    from tests import fake_osb200_text as fake
+    from tests import fake_osb200 as fake
 
     q = torch.zeros(8, 3 * 72, dtype=torch.bfloat16, device="cuda")
     bias = torch.zeros(15, device="cuda")
@@ -142,7 +142,7 @@ def test_attn_short_bias_refusals():
 @pytest.mark.parametrize("C", [8, 64, 128, 760, 4096])
 def test_rms_norm(C):
     osb = _osb()
-    from tests import fake_osb200_text as fake
+    from tests import fake_osb200 as fake
 
     g = torch.Generator(device="cuda").manual_seed(C)
     x = (torch.randn(333, C, generator=g, device="cuda") * 3).bfloat16()
@@ -159,7 +159,7 @@ def test_rms_norm(C):
 
 def test_rms_norm_refusals():
     osb = _osb()
-    from tests import fake_osb200_text as fake
+    from tests import fake_osb200 as fake
 
     for impl in (osb, fake):
         n0 = impl.launch_count()
@@ -175,7 +175,7 @@ def test_rms_norm_refusals():
 @pytest.mark.parametrize("epi", ["gated", "quick"])
 def test_text_epilogues(block_n, N, epi):
     osb = _osb()
-    from tests import fake_osb200_text as fake
+    from tests import fake_osb200 as fake
 
     g = torch.Generator(device="cuda").manual_seed(N + block_n)
     M, K = 300, 392

@@ -8,17 +8,10 @@ import os
 import pytest
 import torch
 
-from tests import fake_osb200_attn_frames as FA
 from tests.util import rel_l2
 
 BAR = 4e-3          # the bf16 attention bar of the GPU tests
 VAE_BAR = 1.5e-2    # the bar of the other whole-model VAE comparisons in bf16
-
-
-@pytest.fixture
-def fake_frames(fake_osb, monkeypatch):
-    FA.install(monkeypatch)
-    return fake_osb
 
 
 def masked_softmax_reference(q, k, v, hw, q_frame0=0):
@@ -34,40 +27,40 @@ def masked_softmax_reference(q, k, v, hw, q_frame0=0):
 
 @pytest.mark.parametrize("hw", [1, 4, 100])
 @pytest.mark.parametrize("T", [1, 3, 5])
-def test_stand_in_matches_the_explicit_mask(fake_frames, hw, T):
+def test_stand_in_matches_the_explicit_mask(fake_osb, hw, T):
     torch.manual_seed(hw * 10 + T)
     q, k, v = (torch.randn(2, T * hw, 512).to(torch.bfloat16) for _ in range(3))
-    out = fake_frames.attn_frames(q, k, v, frame_tokens=hw)
+    out = fake_osb.attn_frames(q, k, v, frame_tokens=hw)
     assert out.shape == q.shape and out.dtype == torch.bfloat16
     assert rel_l2(out, masked_softmax_reference(q, k, v, hw)) < BAR
-    assert [c[0] for c in fake_frames.calls] == ["attn_frames"] and fake_frames.launch_count() == 1
+    assert [c[0] for c in fake_osb.calls] == ["attn_frames"] and fake_osb.launch_count() == 1
 
 
-def test_stand_in_with_a_frame_offset_and_column_slices(fake_frames):
+def test_stand_in_with_a_frame_offset_and_column_slices(fake_osb):
     """Frame-sharded shape: 2 local frames starting at global frame 2, keys of 5 frames; q | k | v as column slices of
     one buffer (ld 1536) and a batch of 2."""
     torch.manual_seed(5)
     hw, Tq, Tk, first = 4, 2, 5, 2
     buf = torch.randn(2, Tk * hw, 1536).to(torch.bfloat16)
     q, k, v = buf[:, first * hw:(first + Tq) * hw, :512], buf[:, :, 512:1024], buf[:, :, 1024:]
-    out = fake_frames.attn_frames(q, k, v, frame_tokens=hw, q_frame0=first)
+    out = fake_osb.attn_frames(q, k, v, frame_tokens=hw, q_frame0=first)
     assert rel_l2(out, masked_softmax_reference(q, k, v, hw, first)) < BAR
     # local frames are global frames 2 and 3: changing the keys of frame 3 leaves the first local frame alone
     k2, v2 = k.clone(), v.clone()
     k2[:, 3 * hw:4 * hw] += 1
     v2[:, 3 * hw:4 * hw] += 1
-    out2 = fake_frames.attn_frames(q, k2, v2, frame_tokens=hw, q_frame0=first)
+    out2 = fake_osb.attn_frames(q, k2, v2, frame_tokens=hw, q_frame0=first)
     assert torch.equal(out2[:, :hw], out[:, :hw]) and not torch.equal(out2[:, hw:], out[:, hw:])
 
 
-def test_stand_in_refusals_count_no_launch(fake_frames):
+def test_stand_in_refusals_count_no_launch(fake_osb):
     q = torch.zeros(1, 8, 512, dtype=torch.bfloat16)
     for kw, args in ((dict(frame_tokens=0), (q, q, q)), (dict(frame_tokens=4, q_frame0=-1), (q, q, q)),
                      (dict(frame_tokens=4), (q[..., :256], q[..., :256], q[..., :256])),
                      (dict(frame_tokens=4), (q, q, q[:, :4]))):
-        with pytest.raises(fake_frames.OsbError):
-            fake_frames.attn_frames(*args, **kw)
-    assert fake_frames.launch_count() == 0
+        with pytest.raises(fake_osb.OsbError):
+            fake_osb.attn_frames(*args, **kw)
+    assert fake_osb.launch_count() == 0
 
 
 # ---- the host switch on a small VAE with a 512-wide mid block ----------------------------------------------------------
@@ -94,7 +87,7 @@ def _count_sdpa(monkeypatch):
 
 
 @pytest.mark.parametrize("tiled", [False, True])
-def test_native_attention_matches_the_sdpa_path(fake_frames, monkeypatch, tiled):
+def test_native_attention_matches_the_sdpa_path(fake_osb, monkeypatch, tiled):
     m = _vae512(sample_size=16, sample_tsize=64, use_spatial_tiling=tiled)
     sdpa = _count_sdpa(monkeypatch)
     torch.manual_seed(2)
@@ -102,12 +95,12 @@ def test_native_attention_matches_the_sdpa_path(fake_frames, monkeypatch, tiled)
     z = torch.randn(1, 4, 3, 4, 4)
     with torch.no_grad():
         ze0, yd0 = m.encode(x, sample_posterior=False), m.decode(z)
-        off_sdpa, off_frames = sdpa[0], sum(c[0] == "attn_frames" for c in fake_frames.calls)
+        off_sdpa, off_frames = sdpa[0], sum(c[0] == "attn_frames" for c in fake_osb.calls)
         m.enable_native_attention()
-        fake_frames.reset()
+        fake_osb.reset()
         sdpa[0] = 0
         ze1, yd1 = m.encode(x, sample_posterior=False), m.decode(z)
-        on_sdpa, on_frames = sdpa[0], sum(c[0] == "attn_frames" for c in fake_frames.calls)
+        on_sdpa, on_frames = sdpa[0], sum(c[0] == "attn_frames" for c in fake_osb.calls)
         m.disable_native_attention()
         ze2, yd2 = m.encode(x, sample_posterior=False), m.decode(z)
         # the floor: how far the SDPA path itself moves when its attention is computed in fp32 and rounded once
@@ -119,12 +112,12 @@ def test_native_attention_matches_the_sdpa_path(fake_frames, monkeypatch, tiled)
     assert rel_l2(ze1, ze0) < max(VAE_BAR, 1.5 * rel_l2(ze3, ze0)) and rel_l2(yd1, yd0) < max(VAE_BAR, 1.5 * rel_l2(yd3, yd0))
     # T = 3 SDPA calls per mid block become one attn_frames launch
     assert off_frames == 0 and on_sdpa == 0 and off_sdpa == 3 * on_frames and on_frames >= 2
-    hw = {c[1][4] for c in fake_frames.calls if c[0] == "attn_frames"}                  # frame_tokens = H * W of the (tile's) latent
-    assert (max(hw) <= 4 if tiled else hw == {16}) and all(c[1][5] == 0 for c in fake_frames.calls if c[0] == "attn_frames")
+    hw = {c[1][4] for c in fake_osb.calls if c[0] == "attn_frames"}                  # frame_tokens = H * W of the (tile's) latent
+    assert (max(hw) <= 4 if tiled else hw == {16}) and all(c[1][5] == 0 for c in fake_osb.calls if c[0] == "attn_frames")
     assert torch.equal(ze2, ze0) and torch.equal(yd2, yd0), "disable_native_attention() restores the default path's bits"
 
 
-def test_native_attention_refuses_another_width(fake_frames):
+def test_native_attention_refuses_another_width(fake_osb):
     from opensora.registry import MODELS, build_module
 
     m = build_module(dict(type="hunyuan_vae", block_out_channels=(16, 32, 32, 32), layers_per_block=1, norm_num_groups=4,
@@ -145,7 +138,6 @@ def _shard_worker(rank, world, port, ret):
         from tests import fake_osb200
 
         sys.modules["osb200"] = fake_osb200
-        fake_osb200.attn_frames = FA.attn_frames
         m = _vae512()
         m.enable_native_attention()
         torch.manual_seed(3)

@@ -6,7 +6,7 @@ against the fp32 oracle."""
 import pytest
 import torch
 
-from tests import fake_osb200_attn_frames as FA
+from tests import fake_osb200 as F_
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -89,12 +89,12 @@ def test_causality_determinism_and_range(osb):
 
 
 def test_stand_in_matches_the_kernel(osb):
-    """Pins tests/fake_osb200_attn_frames.py, which the CPU tests of the host switch rely on."""
+    """Pins the stand-in's attn_frames (tests/fake_osb200.py), which the CPU tests of the host switch rely on."""
     hw, Tq, Tk, first = 36, 3, 6, 1
     q, k, v = _rand(2, Tq * hw, 512, seed=40), _rand(2, Tk * hw, 512, seed=41), _rand(2, Tk * hw, 512, seed=42)
     out = osb.attn_frames(q, k, v, frame_tokens=hw, q_frame0=first)
     torch.cuda.synchronize()
-    assert report("kernel vs stand-in", out, FA.attn_frames(q, k, v, frame_tokens=hw, q_frame0=first))[0] < BAR
+    assert report("kernel vs stand-in", out, F_.attn_frames(q, k, v, frame_tokens=hw, q_frame0=first))[0] < BAR
 
 
 def test_refusals_do_not_launch(osb):
