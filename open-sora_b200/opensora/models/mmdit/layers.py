@@ -48,7 +48,7 @@ from dataclasses import dataclass
 import torch
 from torch import Tensor, nn
 
-from opensora.utils.lora import adapter_of, lora_pack
+from opensora.utils.lora import adapters_of, lora_pack
 
 from .math import liger_rope, rope, rope_tables
 
@@ -100,9 +100,9 @@ def timestep_embedding(t: Tensor, dim, max_period=10000, time_factor: float = 10
 
 
 def linear_parts(lin: nn.Module, k_pad: int = 0):
-    """(weight, bias, lora) of a Linear the forward sends to osb200: lora is None, or (A [r, K + k_pad], scaling * B,
-    DoRA column scale or None) of its adapter (lora_pack)."""
-    if adapter_of(lin) is None:
+    """(weight, bias, lora) of a Linear the forward sends to osb200: lora is None, or (A_cat [R, K + k_pad], B_cat,
+    DoRA column scale or None) of its active adapters (lora_pack)."""
+    if not adapters_of(lin):
         return lin.weight, lin.bias, None
     A, (B,), (S,) = lora_pack([[(lin, 0, lin.out_features)]], k_pad)
     return lin.weight, lin.bias, (A, B, S)
@@ -357,7 +357,7 @@ class Fp8State:
         key = (id(blk), kind, name)
         hit = self._w.get(key)
         if hit is None or hit[0] is not blk:
-            if not self.lora and any(adapter_of(lin) is not None for lin, _, _ in slices):
+            if not self.lora and any(adapters_of(lin) for lin, _, _ in slices):
                 what, lin = ("FP8 projections", "a projection") if name in PROJ_GEMMS else ("FP8 MLPs", "an MLP")
                 raise ValueError(f"{what}: a LoRA / DoRA adapter on {lin} Linear cannot run on the FP8 path; "
                                  "unload_lora or disable_fp8 first")

@@ -10,7 +10,7 @@ from torch import Tensor, nn
 
 from opensora.registry import MODELS
 
-from opensora.utils.lora import adapter_of, dora_magnitude, lora_pack
+from opensora.utils.lora import adapters_of, lora_pack
 
 from .layers import (PROJ_GEMMS, DoubleStreamBlock, EmbedND, Fp8AttnState, Fp8State, LastLayer, LigerEmbedND,
                      MLPEmbedder, SingleStreamBlock, _down, _gemm, block_gemms, linear_parts, timestep_embedding)
@@ -105,16 +105,16 @@ class MMDiTModel(nn.Module):
     def _grouped_modulation(self, vec: Tensor) -> None:
         """All 2*19 + 38 `Modulation.lin` projections of `vec` as ONE GEMM (the reference launches 76 tiny ones per step,
         layers.py:179-192).  The fp32 result and the column range of every layer ride on `vec`; the processors pick their
-        slice (a processor installed on a block this model does not own simply does its own projection).  A layer with a
-        DoRA adapter stays out of the group: its magnitude factor scales its base product too, which one grouped launch
-        cannot do per layer, so the block projects it itself (osb_gemm_lora with col_scale)."""
+        slice (a processor installed on a block this model does not own simply does its own projection).  A layer whose
+        active adapters include a DoRA adapter stays out of the group: its magnitude factor scales its base product too,
+        which one grouped launch cannot do per layer, so the block projects it itself (osb_gemm_lora with col_scale)."""
         import osb200
 
         lins = [m.lin for b in self.double_blocks for m in (b.img_mod, b.txt_mod)] + [b.modulation.lin for b in self.single_blocks]
-        lins = [lin for lin in lins if dora_magnitude(lin) is None]
+        lins = [lin for lin in lins if all(ad.magnitude is None for ad in adapters_of(lin))]
         if not lins:
             return
-        adapted = [lin for lin in lins if adapter_of(lin) is not None]
+        adapted = [lin for lin in lins if adapters_of(lin)]
         key = tuple((id(l), l.weight.data_ptr(), l.weight._version) for l in lins)
         if self._mod_pack is None or self._mod_pack[0] != key:
             cols, off = {}, 0
@@ -130,7 +130,7 @@ class MMDiTModel(nn.Module):
             # The base projection keeps its one launch.  Each adapted layer's update is then added into its slice of the
             # bf16 output (R = D, no gate): peft's own two roundings, without a block-diagonal B over every layer and
             # without reading the modulation weights again.  One down projection serves all layers (same input).
-            parts = [lora_pack([[(lin, 0, lin.out_features)]]) for lin in adapted]   # per layer (A, [s B]), cached
+            parts = [lora_pack([[(lin, 0, lin.out_features)]]) for lin in adapted]   # per layer (A_cat, [B_cat]), cached
             ml = self._mod_lora
             if ml is None or len(ml[0]) != len(parts) or any(a is not b for a, b in zip(ml[0], parts)):
                 self._mod_lora = ml = (parts, torch.cat([p[0] for p in parts], 0).contiguous())
@@ -248,12 +248,12 @@ class MMDiTModel(nn.Module):
         if C > 4096:
             raise ValueError(f"FP8 MLPs need a hidden size <= 4096 (the FP8 LN+modulate holds one row), got {C}")
         mods = dict(self.named_modules())
-        adapted = [] if lora else [n for n in self.fp8_mlp_linears() if adapter_of(mods[n]) is not None]
+        adapted = [] if lora else [n for n in self.fp8_mlp_linears() if adapters_of(mods[n])]
         if adapted:
             raise ValueError(f"FP8 MLPs cannot run LoRA / DoRA adapters on MLP Linears ({adapted[0]} has one): "
                              "unload_lora first")
         if projections and not lora:
-            adapted = [n for n in self.fp8_proj_linears() if adapter_of(mods[n]) is not None]
+            adapted = [n for n in self.fp8_proj_linears() if adapters_of(mods[n])]
             if adapted:
                 raise ValueError(f"FP8 projections cannot run LoRA / DoRA adapters on projection Linears ({adapted[0]} "
                                  "has one): unload_lora first")

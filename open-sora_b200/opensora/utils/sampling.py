@@ -232,8 +232,9 @@ def prepare_ids(img: Tensor, t5_embedding: Tensor, clip_embedding: Tensor) -> di
 def prepare_models(cfg, device, dtype, offload_model: bool = False):
     """:511-559.  Builds (model, model_ae, model_t5, model_clip, optional_models) from the config's `model`, `ae`, `t5` and
     `clip` dicts through the registry, with `device_map` / `torch_dtype` as the reference passes them;
-    `pretrained_lora_path` goes through `load_lora`.  The text-to-image-to-video models (`img_flux`, `img_flux_ae`) need
-    the Flux image autoencoder, which is not registered here."""
+    `pretrained_lora_path` goes through `load_lora`: one path, or a list of paths and (path, weight) pairs stacked in that
+    order (adapters "default", "adapter_1", ...; `set_adapters`).  The text-to-image-to-video models (`img_flux`,
+    `img_flux_ae`) need the Flux image autoencoder, which is not registered here."""
     from opensora.registry import MODELS, build_module
 
     if cfg.get("img_flux", None) is not None and "autoencoder_2d" not in MODELS:
@@ -244,10 +245,20 @@ def prepare_models(cfg, device, dtype, offload_model: bool = False):
     model_ae = build_module(cfg.get("ae"), MODELS, device_map=model_device, torch_dtype=dtype).eval()
     model_t5 = build_module(cfg.get("t5"), MODELS, device_map=device, torch_dtype=dtype).eval()
     model_clip = build_module(cfg.get("clip"), MODELS, device_map=device, torch_dtype=dtype).eval()
-    if cfg.get("pretrained_lora_path", None) is not None:
-        from opensora.utils.lora import load_lora
+    lora = cfg.get("pretrained_lora_path", None)
+    if lora is not None:
+        from opensora.utils.lora import load_lora, set_adapters
 
-        model = load_lora(model, cfg.get("pretrained_lora_path"))
+        if isinstance(lora, (str, os.PathLike)):
+            model = load_lora(model, lora)
+        else:
+            names, weights = [], []
+            for i, entry in enumerate(lora):
+                path, weight = (entry, 1.0) if isinstance(entry, (str, os.PathLike)) else entry
+                names.append("default" if i == 0 else f"adapter_{i}")
+                weights.append(weight)
+                model = load_lora(model, path, adapter_name=names[-1])
+            model = set_adapters(model, names, weights)
     optional_models = {}
     if cfg.get("img_flux", None) is not None:
         optional_models["img_flux"] = build_module(cfg.get("img_flux"), MODELS, device_map=device, torch_dtype=dtype).eval()
