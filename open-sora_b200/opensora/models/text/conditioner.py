@@ -15,6 +15,8 @@ key names, and `config.json` is read as JSON.  Only tokenization imports transfo
 
 The token-embedding gather and CLIP's position-embedding add are torch ops.  The forward after tokenization
 (`encode`) is CUDA-graph capturable once the bias vector of its length is cached (the first eager call caches it).
+`encode(ids, mask)` runs T5 with a right-padded attention mask, as Open-Sora v1.2's T5 wrapper
+(`opensora/models/text_encoder/t5.py`) needs: the pad keys are excluded in every layer through per-sequence key counts.
 `shardformer=True` is accepted for T5 and changes no arithmetic: the ColossalAI policy of the reference only jit-fuses
 the dropout-add and the feed-forward forward (opensora/acceleration/shardformer/policy/t5_encoder.py)."""
 from __future__ import annotations
@@ -305,29 +307,52 @@ class HFEmbedder(nn.Module):
             self._bias[L] = b
         return b
 
-    def encode(self, ids: torch.Tensor) -> torch.Tensor:
-        """Token ids [B, L] on the model's device -> T5 last_hidden_state [B, L, d_model] or CLIP pooler_output [B, d]."""
+    def encode(self, ids: torch.Tensor, mask: torch.Tensor | None = None) -> torch.Tensor:
+        """Token ids [B, L] on the model's device -> T5 last_hidden_state [B, L, d_model] or CLIP pooler_output [B, d].
+
+        `mask` [B, L] (T5 only): the tokenizer's attention mask, 1 for a real token and 0 for a pad, right-padded.  As
+        transformers' T5Attention does with it, every layer excludes the pad keys from the softmax; the query rows at
+        pad positions are still computed, over the real keys.  Its row sums become the attention's per-sequence key
+        counts.  A mask that is not of the form 1..1 0..0 in every row, or a row without a real token, is refused.
+        Checking the mask reads it on the host, so a masked encode is not CUDA-graph capturable."""
         osb = _osb()
         osb.require_cuda_bf16(self._weight(), "text_embedder")
         if ids.device != self._weight().device:
             raise osb.OsbError(f"text_embedder: input_ids on {ids.device}, model on {self._weight().device}")
-        return self._clip(ids) if self.is_clip else self._t5(ids)
+        if self.is_clip:
+            if mask is not None:
+                raise ValueError("text_embedder: an attention mask is supported for T5 only")
+            return self._clip(ids)
+        return self._t5(ids, None if mask is None else self._kv_lens(mask, ids.shape))
 
-    def _attention(self, qkv: torch.Tensor, B: int, L: int, scale: float) -> torch.Tensor:
+    def _kv_lens(self, mask: torch.Tensor, shape) -> torch.Tensor:
+        """Right-padded attention mask [B, L] -> int32 number of real tokens per row, on the model's device."""
+        if tuple(mask.shape) != tuple(shape):
+            raise ValueError(f"text_embedder: attention mask of shape {tuple(mask.shape)} for input_ids of shape {tuple(shape)}")
+        m = mask.detach().to("cpu", torch.long)
+        lens = (m != 0).sum(dim=1)
+        if not torch.equal(m, (torch.arange(m.shape[1])[None, :] < lens[:, None]).long()):
+            raise ValueError("text_embedder: the attention mask must be right-padded, 1..1 0..0 in every row")
+        if bool((lens == 0).any()):
+            raise ValueError(f"text_embedder: attention mask rows {(lens == 0).nonzero().flatten().tolist()} have no "
+                             "real token (the tokenizer always emits eos)")
+        return lens.to(device=self._weight().device, dtype=torch.int32)
+
+    def _attention(self, qkv: torch.Tensor, B: int, L: int, scale: float, kv_lens: torch.Tensor | None = None) -> torch.Tensor:
         osb = _osb()
         inner = self.num_heads * HEAD_DIM
         out = torch.empty(B * L, inner, dtype=qkv.dtype, device=qkv.device)
         return osb.attn_short_bias(qkv[:, :inner], qkv[:, inner:2 * inner], qkv[:, 2 * inner:], out, self.attn_bias(L),
                                    num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L,
-                                   num_heads=self.num_heads, head_dim=HEAD_DIM, softmax_scale=scale)
+                                   num_heads=self.num_heads, head_dim=HEAD_DIM, kv_lens=kv_lens, softmax_scale=scale)
 
-    def _t5(self, ids: torch.Tensor) -> torch.Tensor:
+    def _t5(self, ids: torch.Tensor, kv_lens: torch.Tensor | None = None) -> torch.Tensor:
         osb = _osb()
         B, L = ids.shape
         x = F.embedding(ids, self.shared).reshape(B * L, -1).contiguous()
         for lay in self.layers:
             h = osb.rms_norm(x, lay.ln0, eps=self.eps)
-            a = self._attention(osb.gemm(h, lay.qkv_w), B, L, 1.0)   # T5 does not scale its scores
+            a = self._attention(osb.gemm(h, lay.qkv_w), B, L, 1.0, kv_lens)   # T5 does not scale its scores
             x = osb.gemm(a, lay.o_w, epilogue=osb.EPI_BIAS_GATE_RES, residual=x, out=x)
             h = osb.rms_norm(x, lay.ln1, eps=self.eps)
             f = osb.gemm(h, lay.wi, epilogue=osb.EPI_GATED_GELU)
