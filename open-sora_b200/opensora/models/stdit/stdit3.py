@@ -19,8 +19,8 @@ With `enable_fp8()` the MLP runs on e4m3 operands with per-row scales instead (1
 With `enable_fp8_attention()` each attention reads e4m3 copies of its head tiles: head_tiles_fp8 -> attn_tiles_fp8 in
 place of attn_tiles (12 launches per block; the text keys / values of all blocks convert once per forward).
 q / k / v never exist in token layout: the projection epilogue writes "head tiles" (include/osb200.h) that the
-attention kernel loads with one bulk copy per tile.  Head sizes the tile path is not built for (anything but
-64 / 72 / 128, or an odd head count) use the register-path kernel `osb_attn_short` on token-layout q / k / v.
+attention kernel loads with one bulk copy per tile.  The head tiles are built for an even number of heads of 64, 72 or
+128; the forward raises for any other head layout.
 """
 from __future__ import annotations
 
@@ -245,7 +245,7 @@ class STDiT3(nn.Module):
 
     def _peer_exchange(self, dev):
         """The PeerExchange of this model (created collectively on first use), or None when the exchange is NCCL's."""
-        if self._sp_group is None or self._sp_exchange != "peer" or dev.type != "cuda" or not self._use_tiles():
+        if self._sp_group is None or self._sp_exchange != "peer" or dev.type != "cuda":
             return None
         if self._peer is None:
             try:
@@ -287,8 +287,7 @@ class STDiT3(nn.Module):
         """Run every self-attention (spatial and temporal) and every cross-attention on FP8 (e4m3) tensor cores: the bf16
         head tiles of each attention are converted to e4m3 tiles (q / k per row, v per key tile and channel) and
         osb_attn_tiles_fp8 replaces osb_attn_tiles (include/osb200.h).  The text keys / values of all blocks convert once per
-        forward.  Composes with enable_fp8().  Head sizes 72 and 64 only; the forward raises if the head-tile attention
-        path is off (OSB_ATTN_TILES=0, or an odd head count)."""
+        forward.  Composes with enable_fp8().  Head sizes 72 and 64 only."""
         if self.head_dim not in (64, 72):
             raise ValueError(f"FP8 attention is built for head sizes 72 and 64, not {self.head_dim}")
         self._fp8_attn = True
@@ -409,9 +408,12 @@ class STDiT3(nn.Module):
         w0 = self.x_embedder.proj.weight
         osb.require_cuda_bf16(w0, "STDiT3")
         refuse_adapters(self, "STDiT3")   # its head-tile GEMMs have no LoRA path: never silently run the base model
+        if self.num_heads % 2 or self.head_dim not in (64, 72, 128):
+            raise ValueError(f"STDiT3 attention runs on head tiles, built for an even number of heads of 64, 72 or 128; "
+                             f"this model has {self.num_heads} heads of {self.head_dim}")
         dev = w0.device
         bf = torch.bfloat16
-        C, Hh, D = self.hidden_size, self.num_heads, self.head_dim
+        C = self.hidden_size
         cst = self._const(dev)
         B = x.size(0)
         x = x.to(dev, bf)
@@ -474,19 +476,13 @@ class STDiT3(nn.Module):
         yp = self.y_embedder.y_proj
         yh = osb.gemm(yt, yp.fc1.weight, yp.fc1.bias, epilogue=osb.EPI_BIAS_GELU_TANH)
         ye = osb.gemm(yh, yp.fc2.weight, yp.fc2.bias)                                    # [B*Ly, C]
-        use_tiles = self._use_tiles()
         fp8_attn = self._fp8_attn
-        if fp8_attn and not use_tiles:
-            raise RuntimeError("FP8 attention runs on the head-tile attention path, which is off here (OSB_ATTN_TILES=0 "
-                               f"or an odd head count, {self.num_heads}); disable_fp8_attention() for the bf16 path")
         kv8 = None
-        if use_tiles:   # keys / values of all 2*depth blocks as attention operand tiles: [block][k|v][head][tile]
-            kv_all = self._tiles(osb, ("kv", B, Ly), B * Ly, osb.tile_map(0, Ly, keys_only=True), 2 * nb, dev)
-            osb.gemm_head_tiles(ye, cst["kv_w"], cst["kv_b"], kv_all, nkinds=2)
-            if fp8_attn:   # every block's text k | v pair in one conversion launch
-                kv8 = osb.head_tiles_fp8(kv_all, self._tiles_fp8(osb, kv_all), v_period=2, v_slot=1)
-        else:
-            kv_all = osb.gemm(ye, cst["kv_w"], cst["kv_b"])                              # [B*Ly, nb*2C]
+        # keys / values of all 2*depth blocks as attention operand tiles: [block][k|v][head][tile]
+        kv_all = self._tiles(osb, ("kv", B, Ly), B * Ly, osb.tile_map(0, Ly, keys_only=True), 2 * nb, dev)
+        osb.gemm_head_tiles(ye, cst["kv_w"], cst["kv_b"], kv_all, nkinds=2)
+        if fp8_attn:   # every block's text k | v pair in one conversion launch
+            kv8 = osb.head_tiles_fp8(kv_all, self._tiles_fp8(osb, kv_all), v_period=2, v_slot=1)
         if mask is not None:
             m2 = mask.to(dev)
             if m2.shape[0] != B:
@@ -519,26 +515,22 @@ class STDiT3(nn.Module):
         ao = wsbuf("ao", R, C)
         hid = wsbuf("hid", R, int(C * self.config.mlp_ratio))
         cos, sin = self._rope(T, dev)
-        ws = dict(xm=xm_buf, ao=ao, hid=hid, cos=cos, sin=sin, kv=kv_all, kv_lens=kv_lens, tiles=use_tiles,
-                  fp8_attn=fp8_attn, kv8=kv8, peer=self._peer_exchange(dev) if P > 1 else None)
+        ws = dict(xm=xm_buf, ao=ao, hid=hid, cos=cos, sin=sin, kv=kv_all, kv_lens=kv_lens, fp8_attn=fp8_attn, kv8=kv8,
+                  peer=self._peer_exchange(dev) if P > 1 else None)
         if self._fp8:   # e4m3 codes + row scales of the fc1 input (C wide) and the fc2 input (hid wide)
             f8 = torch.float8_e4m3fn
             ws.update(fp8=self._fp8_weights(dev), xm8=wsbuf("xm8", R, C, dtype=f8), xm8_s=wsbuf("xm8_s", R, dtype=torch.float32),
                       hid8=wsbuf("hid8", *hid.shape, dtype=f8), hid8_s=wsbuf("hid8_s", R, dtype=torch.float32))
-        if use_tiles:
-            Sl = S // P   # temporal attention runs on this rank's S/P columns of every frame
-            ws["sp_t"] = self._tiles(osb, ("spatial", B, Tl, S), R, osb.tile_map(0, S), 3, dev)
-            # temporal attention tiles.  Default: LN+modulate writes its rows transposed to [B, S, T] (a free row
-            # permutation of its stores), so a temporal sequence is a contiguous row block for the QKV GEMM (tile map mode 0)
-            # and only the attention OUTPUT is addressed frame-major (`tm_out`, mode 1).  When the rows arrive frame-major
-            # (NCCL all-to-all exchange) the GEMM reads them through a strided TMA view instead (mode 1 map).
-            ws["tm_out"] = osb.tile_map(1, T, Sl, T)
-            ws["tm_t"] = self._tiles(osb, ("temporal", B, T, Sl), B * T * Sl, osb.tile_map(0, T), 3, dev)
-            ws["xm_t"] = wsbuf("xm_t", R, C) if P == 1 else None
-            ws["q_t"] = self._tiles(osb, ("crossq", B, N), R, osb.tile_map(0, N, pack=False), 1, dev)
-        else:
-            ws["qkv"] = wsbuf("qkv", R, 3 * C)
-            ws["qc"] = wsbuf("qc", R, C)
+        Sl = S // P   # temporal attention runs on this rank's S/P columns of every frame
+        ws["sp_t"] = self._tiles(osb, ("spatial", B, Tl, S), R, osb.tile_map(0, S), 3, dev)
+        # temporal attention tiles.  Default: LN+modulate writes its rows transposed to [B, S, T] (a free row
+        # permutation of its stores), so a temporal sequence is a contiguous row block for the QKV GEMM (tile map mode 0)
+        # and only the attention OUTPUT is addressed frame-major (`tm_out`, mode 1).  When the rows arrive frame-major
+        # (NCCL all-to-all exchange) the GEMM reads them through a strided TMA view instead (mode 1 map).
+        ws["tm_out"] = osb.tile_map(1, T, Sl, T)
+        ws["tm_t"] = self._tiles(osb, ("temporal", B, T, Sl), B * T * Sl, osb.tile_map(0, T), 3, dev)
+        ws["xm_t"] = wsbuf("xm_t", R, C) if P == 1 else None
+        ws["q_t"] = self._tiles(osb, ("crossq", B, N), R, osb.tile_map(0, N, pack=False), 1, dev)
 
         bi = 0
         for sb, tb in zip(self.spatial_blocks, self.temporal_blocks):
@@ -562,12 +554,6 @@ class STDiT3(nn.Module):
         o = o.view(B, T, H, W, pt, ph, pw, self.out_channels).permute(0, 7, 1, 4, 2, 5, 3, 6)
         o = o.reshape(B, self.out_channels, T * pt, H * ph, W * pw)[:, :, :Tx, :Hx, :Wx]
         return o.to(torch.float32)
-
-    def _use_tiles(self) -> bool:
-        """The head-tile attention path (osb_gemm_head_tiles + osb_attn_tiles) is built for head sizes 64 / 72 / 128 and an
-        even head count; OSB_ATTN_TILES=0 forces the register-path kernel (A/B measurements)."""
-        return (self.head_dim in (64, 72, 128) and self.num_heads % 2 == 0
-                and os.environ.get("OSB_ATTN_TILES", "1") != "0")
 
     def _tiles(self, osb, key, rows, tmap, kinds, dev):
         """Tile workspaces are cached per shape: they are zero-filled once (rows no token maps to must stay finite)."""
@@ -593,12 +579,12 @@ class STDiT3(nn.Module):
         return osb.attn_tiles(tiles, tiles, out, **kw)
 
     def _block(self, osb, blk, bi, xs, m, mod_index, group_rows, Ly, B, T, Tl, S, ws, sp):
-        C, Hh, D = self.hidden_size, self.num_heads, self.head_dim
+        C = self.hidden_size
         N = Tl * S
         a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
         qn = a.q_norm.weight if isinstance(a.q_norm, _Norm) else None
         kn = a.k_norm.weight if isinstance(a.k_norm, _Norm) else None
-        xm_buf, ao, hid, cos, sin, tiles = ws["xm"], ws["ao"], ws["hid"], ws["cos"], ws["sin"], ws["tiles"]
+        xm_buf, ao, hid, cos, sin = ws["xm"], ws["ao"], ws["hid"], ws["cos"], ws["sin"]
         # 1. self attention (spatial: sequences over S; temporal: sequences over T with RoPE)
         peer = ws.get("peer") if (blk.temporal and sp is not None) else None
         if peer is not None:
@@ -618,7 +604,7 @@ class STDiT3(nn.Module):
                             out_scatter=peer.scatter(2, T, Sl, ar_ptrs), out_ld=C)
             peer.barrier()
             ao = ar
-        elif blk.temporal and tiles and sp is None:
+        elif blk.temporal and sp is None:
             # single GPU: LN+modulate stores its rows transposed ([B, T, S] -> [B, S, T]) so temporal sequences are
             # contiguous row blocks; the attention output comes back frame-major
             xm_t, tt = ws["xm_t"], ws["tm_t"]
@@ -628,66 +614,38 @@ class STDiT3(nn.Module):
                                 rope_kinds=0b011)
             self._self_attn(osb, tt, ao, ws, Lk=T, num_seqs=B * S, out_map=ws["tm_out"])
         elif blk.temporal:
-            osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
-            if sp is not None:
-                # T-sharded -> S-sharded transposition (all-to-all over NVLink), attention over the full T
-                # for this rank's S/P columns, and back.  Rows stay B*T*S/P on both sides.
-                from opensora.acceleration.communications import all_to_all
+            # sequence parallel, NCCL exchange: T-sharded -> S-sharded transposition (all-to-all over NVLink), attention
+            # over the full T for this rank's S/P columns, and back.  Rows stay B*T*S/P on both sides.
+            from opensora.acceleration.communications import all_to_all
 
-                Sl = S // (T // Tl)
-                xt = all_to_all(xm_buf.view(B, Tl, S, C), sp, scatter_dim=2, gather_dim=1).view(B * T * Sl, C)
-            else:
-                Sl, xt = S, xm_buf
-            ao_t = ao if sp is None else torch.empty_like(ao)
-            if tiles:
-                # (looked up here, not through a closure stored in `ws`: a ws -> lambda -> ws cycle would keep every
-                # forward's workspaces alive until the cyclic GC runs, and the allocator would cudaMalloc new ones each step)
-                tt = self._tiles(osb, ("temporal-fm", B, T, Sl), B * T * Sl, ws["tm_out"], 3, xs.device)
-                osb.gemm_head_tiles(xt, a.qkv.weight, a.qkv.bias, tt, nkinds=3, norm_w=(qn, kn, None), rope=(cos, sin),
-                                    rope_kinds=0b011)
-                self._self_attn(osb, tt, ao_t, ws, Lk=T, num_seqs=B * Sl)
-            else:
-                qkv = ws["qkv"]
-                osb.gemm(xt, a.qkv.weight, a.qkv.bias, out=qkv)
-                strides = (T * Sl, 1, Sl)
-                osb.attn_short(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ao_t, num_seqs=B * Sl, seqs_per_batch=Sl,
-                               q_strides=strides, k_strides=strides, Lq=T, Lk=T, num_heads=Hh, head_dim=D,
-                               q_norm_w=qn, k_norm_w=kn, rope_cos=cos, rope_sin=sin)
-            if sp is not None:
-                ao = all_to_all(ao_t.view(B, T, Sl, C), sp, scatter_dim=1, gather_dim=2).view(B * N, C)
-        elif tiles:
+            osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
+            Sl = S // (T // Tl)
+            xt = all_to_all(xm_buf.view(B, Tl, S, C), sp, scatter_dim=2, gather_dim=1).view(B * T * Sl, C)
+            ao_t = torch.empty_like(ao)
+            # (looked up here, not through a closure stored in `ws`: a ws -> lambda -> ws cycle would keep every
+            # forward's workspaces alive until the cyclic GC runs, and the allocator would cudaMalloc new ones each step)
+            tt = self._tiles(osb, ("temporal-fm", B, T, Sl), B * T * Sl, ws["tm_out"], 3, xs.device)
+            osb.gemm_head_tiles(xt, a.qkv.weight, a.qkv.bias, tt, nkinds=3, norm_w=(qn, kn, None), rope=(cos, sin),
+                                rope_kinds=0b011)
+            self._self_attn(osb, tt, ao_t, ws, Lk=T, num_seqs=B * Sl)
+            ao = all_to_all(ao_t.view(B, T, Sl, C), sp, scatter_dim=1, gather_dim=2).view(B * N, C)
+        else:
             osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
             st = ws["sp_t"]
             osb.gemm_head_tiles(xm_buf, a.qkv.weight, a.qkv.bias, st, nkinds=3, norm_w=(qn, kn, None))
             self._self_attn(osb, st, ao, ws, Lk=S, num_seqs=B * Tl)
-        else:
-            osb.ln_modulate(xs, m[:, 0], m[:, 1], group_rows=group_rows, mod_index=mod_index, out=xm_buf)
-            qkv = ws["qkv"]
-            osb.gemm(xm_buf, a.qkv.weight, a.qkv.bias, out=qkv)
-            strides = (N, S, 1)
-            osb.attn_short(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ao, num_seqs=B * Tl, seqs_per_batch=Tl,
-                           q_strides=strides, k_strides=strides, Lq=S, Lk=S, num_heads=Hh, head_dim=D,
-                           q_norm_w=qn, k_norm_w=kn)
         osb.gemm(ao, a.proj.weight, a.proj.bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=xs, gate=m[:, 2],
                  group_rows=group_rows, mod_index=mod_index, out=xs)
         # 2. cross attention over the T5 tokens (plain residual)
-        ao = ws["ao"]
-        if tiles:
-            qt = ws["q_t"]
-            osb.gemm_head_tiles(xs, ca.q_linear.weight, ca.q_linear.bias, qt, nkinds=1)
-            if ws["fp8_attn"]:   # q per block; the text keys / values were converted once per forward
-                q8 = osb.head_tiles_fp8(qt, self._tiles_fp8(osb, qt))
-                osb.attn_tiles_fp8(q8, ws["kv8"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
-                                   kv_lens=ws["kv_lens"])
-            else:
-                osb.attn_tiles(qt, ws["kv"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
+        ao, qt = ws["ao"], ws["q_t"]
+        osb.gemm_head_tiles(xs, ca.q_linear.weight, ca.q_linear.bias, qt, nkinds=1)
+        if ws["fp8_attn"]:   # q per block; the text keys / values were converted once per forward
+            q8 = osb.head_tiles_fp8(qt, self._tiles_fp8(osb, qt))
+            osb.attn_tiles_fp8(q8, ws["kv8"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
                                kv_lens=ws["kv_lens"])
         else:
-            qc = ws["qc"]
-            kv = ws["kv"][:, bi * 2 * C:(bi + 1) * 2 * C]
-            osb.gemm(xs, ca.q_linear.weight, ca.q_linear.bias, out=qc)
-            osb.attn_short(qc, kv[:, :C], kv[:, C:], ao, num_seqs=B, seqs_per_batch=1, q_strides=(N, 0, 1),
-                           k_strides=(Ly, 0, 1), Lq=N, Lk=Ly, num_heads=Hh, head_dim=D, kv_lens=ws["kv_lens"])
+            osb.attn_tiles(qt, ws["kv"], ao, q_kind=0, k_kind=2 * bi, v_kind=2 * bi + 1, Lk=Ly, num_seqs=B,
+                           kv_lens=ws["kv_lens"])
         osb.gemm(ao, ca.proj.weight, ca.proj.bias, epilogue=osb.EPI_BIAS_GATE_RES, residual=xs, gate=None, out=xs)
         # 3. MLP
         if "fp8" in ws:

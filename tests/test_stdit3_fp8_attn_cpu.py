@@ -213,7 +213,9 @@ def test_disable_fp8_attention_restores_the_bf16_path(fake_osb):
     assert not any(k[0] == "fp8attn" for k in prod._cache)
 
 
-def test_fp8_attention_refusals(fake_osb, monkeypatch):
+def test_head_layout_refusals(fake_osb):
+    """FP8 attention refuses head sizes it is not built for; the forward refuses, with or without FP8 attention, any
+    head layout the head tiles are not built for, before its first launch."""
     from opensora.models.stdit.stdit3 import STDiT3, STDiT3Config
 
     with torch.device("meta"):
@@ -221,18 +223,19 @@ def test_fp8_attention_refusals(fake_osb, monkeypatch):
     with pytest.raises(ValueError, match="head sizes 72 and 64"):
         m.enable_fp8_attention()                    # 2 heads of 128
     assert m._fp8_attn is False
-    prod, _, cfg = _pair("xs72")
-    prod.enable_fp8_attention()
+    _, _, cfg = _pair("xs72")
     inp = _inputs(cfg, 1, 2, 4, 4)
-    monkeypatch.setenv("OSB_ATTN_TILES", "0")
-    with pytest.raises(RuntimeError, match="head-tile attention path"), torch.no_grad():
-        prod(**inp)
-    monkeypatch.delenv("OSB_ATTN_TILES")
-    odd = STDiT3(STDiT3Config(depth=1, hidden_size=216, num_heads=3, caption_channels=cfg.caption_channels,
-                              model_max_length=cfg.model_max_length)).to(torch.bfloat16)
-    odd.enable_fp8_attention()                      # 3 heads of 72: the tile path needs an even head count
-    with pytest.raises(RuntimeError, match="odd head count"), torch.no_grad():
-        odd(**inp)
+    # head tiles need an even head count (3 heads of 72, with and without FP8 attention) and a head size they are built
+    # for (4 heads of 96): the forward refuses both before its first launch
+    for heads, hidden, fp8 in ((3, 216, False), (3, 216, True), (4, 384, False)):
+        bad = STDiT3(STDiT3Config(depth=1, hidden_size=hidden, num_heads=heads, caption_channels=cfg.caption_channels,
+                                  model_max_length=cfg.model_max_length)).to(torch.bfloat16)
+        if fp8:
+            bad.enable_fp8_attention()
+        fake_osb.reset()
+        with pytest.raises(ValueError, match=f"{heads} heads of {hidden // heads}"), torch.no_grad():
+            bad(**inp)
+        assert fake_osb.launch_count() == 0
 
 
 def _sp_worker(rank, world, port, ret):
