@@ -22,20 +22,8 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.lora_bench import M_ROWS, SHAPES, _card, _ms  # noqa: E402
-
-
-def _alternate(fns: dict, reps: int, iters: int) -> dict:
-    """Median of `reps` windows per function; the order of the functions is reversed every other window, so a drift of
-    the clock over a round does not favour whichever runs first."""
-    for f in fns.values():   # warm-up: descriptor cache, module load
-        _ms(f, 2)
-    t = {k: [] for k in fns}
-    for i in range(reps):
-        for k in (list(fns) if i % 2 == 0 else list(fns)[::-1]):
-            t[k].append(_ms(fns[k], iters))
-    return {k: round(statistics.median(v), 4) for k, v in t.items()} | {
-        f"{k}_spread": round(max(v) - min(v), 4) for k, v in t.items()}
+from tests.models import GEMMS_256PX as SHAPES, ROWS_256PX as M_ROWS, mmdit_256px  # noqa: E402
+from tests.timing import alternate, card, window_ms  # noqa: E402
 
 
 def _peft_dora(x, w, b, A, B, s, m):
@@ -61,7 +49,7 @@ def gemms(reps, iters):
             m = (w.float().norm(dim=1) * 1.1).to(torch.bfloat16)
             cs = torch.rand(N, device="cuda", generator=g) + 0.5
             u = osb200.gemm(x, A)
-            t = _alternate({
+            t = alternate({
                 "fused_lora": lambda: osb200.gemm_lora(x, w, b, u, Bm, out=out),
                 "fused_dora": lambda: osb200.gemm_lora(x, w, b, u, Bm, out=out, col_scale=cs),
                 "dora_pair": lambda: osb200.gemm_lora(x, w, b, osb200.gemm(x, A), Bm, out=out, col_scale=cs),
@@ -75,30 +63,9 @@ def gemms(reps, iters):
 
 def model(reps):
     import osb200
-    from bench import MMDIT_256PX
-    from opensora.models.mmdit.model import MMDiTConfig, MMDiTModel
     from opensora.utils.lora import LoraLinear
 
-    cfg = MMDIT_256PX
-    B, T, H, W, Lt = 3, 33, 12, 21, 512
-    Li = T * H * W
-    torch.manual_seed(0)
-    prev = torch.get_default_dtype()
-    torch.set_default_dtype(torch.bfloat16)
-    try:
-        with torch.device("cuda"):
-            net = MMDiTModel(MMDiTConfig(from_pretrained=None, cache_dir=None, **cfg)).eval()
-    finally:
-        torch.set_default_dtype(prev)
-    with torch.no_grad():
-        torch.nn.init.normal_(net.cond_in.weight, std=0.02)
-    g = torch.Generator(device="cuda").manual_seed(5)
-    rb = lambda *s: torch.randn(*s, device="cuda", generator=g).to(torch.bfloat16)   # noqa: E731
-    ids = torch.stack(torch.meshgrid(torch.arange(T), torch.arange(H), torch.arange(W), indexing="ij"), -1).reshape(1, Li, 3)
-    inp = dict(img=rb(B, Li, 64), img_ids=ids.float().repeat(B, 1, 1).cuda().to(torch.bfloat16), txt=rb(B, Lt, 4096),
-               txt_ids=torch.zeros(B, Lt, 3, device="cuda", dtype=torch.bfloat16),
-               timesteps=torch.full((B,), 0.7, device="cuda", dtype=torch.bfloat16), y_vec=rb(B, 768), cond=rb(B, Li, 68),
-               guidance=None)
+    net, inp = mmdit_256px()
     res = {}
     with torch.no_grad():
         # r = 64 on every Linear of every block, as LoRA and as DoRA with the same A and B (magnitudes 1.1 x the row
@@ -135,7 +102,7 @@ def model(reps):
             for k in t:
                 put(k)
                 net(**inp)   # re-reads the cached packs after the swap (off the clock)
-                t[k].append(_ms(lambda: net(**inp), 1))
+                t[k].append(window_ms(lambda: net(**inp), 1))
         put("plain")
     res.update({f"{k}_ms": round(statistics.median(v), 2) for k, v in t.items()})
     res.update({f"{k}_spread_ms": round(max(v) - min(v), 2) for k, v in t.items()})
@@ -156,7 +123,7 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "rows": M_ROWS, "gemm_ms": gemms(a.reps, a.iters)}
     if not a.no_model:
         res["mmdit_256px_forward"] = model(a.reps)

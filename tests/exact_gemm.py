@@ -471,3 +471,15 @@ def first_mismatch(got, want, *, signed_zero=False):
 def assert_bits(what, got, want, **kw):
     msg = first_mismatch(got, want, **kw)
     assert msg is None, f"{what}: {msg}"
+
+
+def conv_box(t_out, h_out, w_out):
+    """(Tt, Ht, Wt) of the CTA box osb_conv3d_ndhwc picks: least padded work, wide W first."""
+    best, box = 1e30, None
+    for wl in range(7, 2, -1):
+        for hl in range(0, 8 - wl):
+            Wt, Ht, Tt = 1 << wl, 1 << hl, 128 >> (wl + hl)
+            work = (-(-w_out // Wt) * Wt) * (-(-h_out // Ht) * Ht) * (-(-t_out // Tt) * Tt)
+            if work < best * 0.999:
+                best, box = work, (Tt, Ht, Wt)
+    return box

@@ -10,7 +10,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -18,21 +17,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "open-sora_b200")]
 
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-
-
-def window_ms(fn, iters):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
+from tests.timing import card, window_ms  # noqa: E402
 
 
 def alternate(fns: dict, min_iters: int, windows: int = 5, window_ms_min: float = 200.0):
@@ -85,14 +70,12 @@ def gemms():
 
 
 def step(steps: int):
-    from oracle import stdit3_oracle as O
-    from tests.fp8_ref import build_pair
+    from tests.models import stdit3_inputs, stdit3_pair
 
-    bf, _, cfg = build_pair("xl")
-    f8, _, _ = build_pair("xl")
+    bf, _, cfg = stdit3_pair("xl")
+    f8, _, _ = stdit3_pair("xl")
     f8.enable_fp8()
-    inp = O.synthetic_inputs(cfg, B=1, T=64, H=32, W=32, lens=[260])
-    inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
+    inp = stdit3_inputs(cfg, 1, 64, 32, 32, lens=[260], device="cuda")
     with torch.no_grad():
         fns = {"step_bf16_eager": lambda: bf(**inp), "step_fp8_eager": lambda: f8(**inp)}
         t = alternate(fns, steps)
@@ -113,7 +96,7 @@ def main():
     import osb200
 
     osb200.init()
-    out = {"card": card(), "mlp_gemms_m16384": gemms(), "xl_step_64x32x32": step(a.steps)}
+    out = {"card": ", ".join(card()), "mlp_gemms_m16384": gemms(), "xl_step_64x32x32": step(a.steps)}
     print(json.dumps(out))
 
 

@@ -71,20 +71,3 @@ def fp8_mlps(oracle):
         for b in blocks:
             del b.mlp.forward
 
-
-def build_pair(cfg_name: str = "xs", device="cuda", seed=1234):
-    """tests/smoke_impl.build_pair for the FP8 tests: "xl" is STDiT3-XL/2; "xs" is the XS/2 plumbing size at hidden size
-    256 (4 heads of 64), since FP8 needs hidden sizes that are multiples of 128 and XS/2's 288 is not."""
-    from opensora.models.stdit.stdit3 import STDiT3 as Product, STDiT3Config as PCfg
-    from oracle import stdit3_oracle as O
-
-    ocfg = (O.STDiT3_XL_2_config() if cfg_name == "xl"
-            else O.STDiT3Config(depth=2, hidden_size=256, patch_size=(1, 2, 2), num_heads=4))
-    oracle = O.STDiT3(ocfg).eval()
-    O.init_synthetic_weights(oracle, seed)
-    sd = {k: v.to(torch.bfloat16) for k, v in oracle.state_dict().items()}
-    oracle.load_state_dict({k: v.float() for k, v in sd.items()})
-    prod = Product(PCfg(depth=ocfg.depth, hidden_size=ocfg.hidden_size, num_heads=ocfg.num_heads,
-                        patch_size=ocfg.patch_size)).eval()
-    prod.load_state_dict(sd)
-    return prod.to(device=device, dtype=torch.bfloat16), oracle, ocfg

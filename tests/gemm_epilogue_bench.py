@@ -16,8 +16,6 @@ The card's name and power limit are read in the same run."""
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 
 import torch
@@ -27,40 +25,12 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
+from tests.timing import alternate, card  # noqa: E402
+
 M_ROWS, C, HEADS, HEAD_DIM, S = 16384, 1152, 16, 72, 256
 BLOCKS = 56
 SHAPES = {"qkv": (C, 3 * C), "proj": (C, C), "cross_q": (C, C), "cross_proj": (C, C), "fc1": (C, 4 * C),
           "fc2": (4 * C, C)}
-
-
-def _card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except (OSError, IndexError, subprocess.SubprocessError):
-        q = "unknown"
-    return torch.cuda.get_device_name(0), q
-
-
-def _ms(fn, n):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / n
-
-
-def _alternate(fns: dict, reps: int, iters: int) -> dict:
-    for f in fns.values():   # warm-up: descriptor cache, module load
-        _ms(f, 3)
-    t = {k: [] for k in fns}
-    for _ in range(reps):
-        for k, f in fns.items():
-            t[k].append(_ms(f, iters))
-    return {k: round(statistics.median(v), 4) for k, v in t.items()} | {
-        f"{k}_spread": round(max(v) - min(v), 4) for k, v in t.items()}
 
 
 def epilogue_calls():
@@ -105,11 +75,11 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "rows": M_ROWS, "gemm_ms": {}}
     total_epi = total_cost = 0.0
     for k, (prod, bias_only, K, N) in epilogue_calls().items():
-        t = _alternate({"epi": prod, "bias": bias_only}, a.reps, a.iters)
+        t = alternate({"epi": prod, "bias": bias_only}, a.reps, a.iters, warmup=3)
         t["epi_cost"] = round(t["epi"] - t["bias"], 4)
         flop = 2.0 * M_ROWS * N * K
         t["epi_tflops"] = round(flop / (t["epi"] * 1e-3) / 1e12, 1)

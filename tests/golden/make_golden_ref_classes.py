@@ -20,8 +20,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "open-sora_b200"))
 
 from oracle import ref_loader  # noqa: E402
-from tests.test_host_mmdit_cpu import TOKEN_STRIDE, mmdit_block_case  # noqa: E402
-from tests.test_host_vae_cpu import posterior_inputs  # noqa: E402
+from tests.models import TOKEN_STRIDE, mmdit_block_case, posterior_inputs  # noqa: E402
 from tests.util import rel_l2  # noqa: E402
 
 

@@ -13,7 +13,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -23,39 +22,8 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-M_ROWS = 3 * (33 * 12 * 21 + 512)
-SHAPES = {"qkv": (3072, 9216), "proj": (3072, 3072), "mlp_up": (3072, 12288), "mlp_down": (12288, 3072),
-          "linear1": (3072, 21504), "linear2": (15360, 3072)}
-
-
-def _card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except (OSError, IndexError, subprocess.SubprocessError):
-        q = "unknown"
-    return torch.cuda.get_device_name(0), q
-
-
-def _ms(fn, n):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / n
-
-
-def _alternate(fns: dict, reps: int, iters: int) -> dict:
-    for f in fns.values():   # warm-up: descriptor cache, module load
-        _ms(f, 2)
-    t = {k: [] for k in fns}
-    for _ in range(reps):
-        for k, f in fns.items():
-            t[k].append(_ms(f, iters))
-    return {k: round(statistics.median(v), 4) for k, v in t.items()} | {
-        f"{k}_spread": round(max(v) - min(v), 4) for k, v in t.items()}
+from tests.models import GEMMS_256PX as SHAPES, ROWS_256PX as M_ROWS, mmdit_256px  # noqa: E402
+from tests.timing import alternate, card, window_ms  # noqa: E402
 
 
 def gemms(reps, iters):
@@ -70,7 +38,7 @@ def gemms(reps, iters):
         for r in (16, 64, 128):
             A, Bm = rn(r, K, sc=K ** -0.5), rn(N, r, sc=0.01)
             u = osb200.gemm(x, A)
-            t = _alternate({
+            t = alternate({
                 "base": lambda: osb200.gemm(x, w, b, out=out),
                 "adapted": lambda: osb200.gemm_lora(x, w, b, osb200.gemm(x, A), Bm, out=out),
                 "down": lambda: osb200.gemm(x, A, out=u),
@@ -84,30 +52,9 @@ def gemms(reps, iters):
 
 def model(reps):
     import osb200
-    from bench import MMDIT_256PX
-    from opensora.models.mmdit.model import MMDiTConfig, MMDiTModel
     from opensora.utils.lora import LoraLinear
 
-    cfg = MMDIT_256PX
-    B, T, H, W, Lt = 3, 33, 12, 21, 512
-    Li = T * H * W
-    torch.manual_seed(0)
-    prev = torch.get_default_dtype()
-    torch.set_default_dtype(torch.bfloat16)
-    try:
-        with torch.device("cuda"):
-            plain = MMDiTModel(MMDiTConfig(from_pretrained=None, cache_dir=None, **cfg)).eval()
-    finally:
-        torch.set_default_dtype(prev)
-    with torch.no_grad():
-        torch.nn.init.normal_(plain.cond_in.weight, std=0.02)
-    g = torch.Generator(device="cuda").manual_seed(5)
-    rb = lambda *s: torch.randn(*s, device="cuda", generator=g).to(torch.bfloat16)   # noqa: E731
-    ids = torch.stack(torch.meshgrid(torch.arange(T), torch.arange(H), torch.arange(W), indexing="ij"), -1).reshape(1, Li, 3)
-    inp = dict(img=rb(B, Li, 64), img_ids=ids.float().repeat(B, 1, 1).cuda().to(torch.bfloat16), txt=rb(B, Lt, 4096),
-               txt_ids=torch.zeros(B, Lt, 3, device="cuda", dtype=torch.bfloat16),
-               timesteps=torch.full((B,), 0.7, device="cuda", dtype=torch.bfloat16), y_vec=rb(B, 768), cond=rb(B, Li, 68),
-               guidance=None)
+    plain, inp = mmdit_256px()
     res = {}
     with torch.no_grad():
         out_plain = plain(**inp).clone()
@@ -143,7 +90,7 @@ def model(reps):
             for k in ("plain", "lora"):
                 put(k == "lora")
                 plain(**inp)   # repacks after the swap (off the clock)
-                t[k].append(_ms(lambda: plain(**inp), 1))
+                t[k].append(window_ms(lambda: plain(**inp), 1))
         put(False)
     res.update({f"{k}_ms": round(statistics.median(v), 2) for k, v in t.items()})
     res.update({f"{k}_spread_ms": round(max(v) - min(v), 2) for k, v in t.items()})
@@ -162,7 +109,7 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "rows": M_ROWS, "gemm_ms": gemms(a.reps, a.iters)}
     if not a.no_model:
         res["mmdit_256px_forward"] = model(a.reps)

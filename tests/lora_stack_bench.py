@@ -25,7 +25,8 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.lora_bench import _card, _ms  # noqa: E402
+from tests.models import mmdit_256px  # noqa: E402
+from tests.timing import card, window_ms  # noqa: E402
 
 # state -> [(rank, DoRA)] in the order the forward applies them
 STATES = {"plain": [], "one_r64": [(64, False)], "two_r32": [(32, False), (32, False)],
@@ -52,28 +53,8 @@ def _wrap(lin, spec):
 
 def model(reps):
     import osb200
-    from bench import MMDIT_256PX
-    from opensora.models.mmdit.model import MMDiTConfig, MMDiTModel
 
-    B, T, H, W, Lt = 3, 33, 12, 21, 512
-    Li = T * H * W
-    torch.manual_seed(0)
-    prev = torch.get_default_dtype()
-    torch.set_default_dtype(torch.bfloat16)
-    try:
-        with torch.device("cuda"):
-            net = MMDiTModel(MMDiTConfig(from_pretrained=None, cache_dir=None, **MMDIT_256PX)).eval()
-    finally:
-        torch.set_default_dtype(prev)
-    with torch.no_grad():
-        torch.nn.init.normal_(net.cond_in.weight, std=0.02)
-    g = torch.Generator(device="cuda").manual_seed(5)
-    rb = lambda *s: torch.randn(*s, device="cuda", generator=g).to(torch.bfloat16)   # noqa: E731
-    ids = torch.stack(torch.meshgrid(torch.arange(T), torch.arange(H), torch.arange(W), indexing="ij"), -1).reshape(1, Li, 3)
-    inp = dict(img=rb(B, Li, 64), img_ids=ids.float().repeat(B, 1, 1).cuda().to(torch.bfloat16), txt=rb(B, Lt, 4096),
-               txt_ids=torch.zeros(B, Lt, 3, device="cuda", dtype=torch.bfloat16),
-               timesteps=torch.full((B,), 0.7, device="cuda", dtype=torch.bfloat16), y_vec=rb(B, 768), cond=rb(B, Li, 68),
-               guidance=None)
+    net, inp = mmdit_256px()
     res = {}
     with torch.no_grad():
         sites = []
@@ -102,7 +83,7 @@ def model(reps):
             for k in (list(STATES) if i % 2 == 0 else list(STATES)[::-1]):
                 put(k)
                 net(**inp)   # re-reads the cached packs after the swap (off the clock)
-                t[k].append(_ms(lambda: net(**inp), 1))
+                t[k].append(window_ms(lambda: net(**inp), 1))
         put("plain")
     res.update({f"{k}_ms": round(statistics.median(v), 2) for k, v in t.items()})
     res.update({f"{k}_spread_ms": round(max(v) - min(v), 2) for k, v in t.items()})
@@ -120,7 +101,7 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "mmdit_256px_forward": model(a.reps)}
     print(json.dumps(res), flush=True)
 

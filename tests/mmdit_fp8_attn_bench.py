@@ -24,10 +24,10 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.dora_bench import _alternate  # noqa: E402
-from tests.lora_bench import _card, _ms  # noqa: E402
+from tests.models import B_256PX as B, L_256PX as L, LT_256PX as LT, mmdit_256px  # noqa: E402
+from tests.timing import alternate, card, window_ms  # noqa: E402
 
-B, L, H, D, LT = 3, 33 * 12 * 21 + 512, 24, 128, 512
+H, D = 24, 128
 
 
 def profile(net, inp):
@@ -36,13 +36,9 @@ def profile(net, inp):
     with torch.no_grad():
         net(**inp)
         torch.cuda.synchronize()
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         osb200.start_profile()
-        s.record()
-        net(**inp)
-        e.record()
+        total = window_ms(lambda: net(**inp), 1)
         rec = osb200.stop_profile()
-    total = s.elapsed_time(e)
     fam = collections.defaultdict(lambda: [0.0, 0.0, 0])
     for name, work, ms in rec:
         f = fam[name]
@@ -72,7 +68,7 @@ def attention(reps, iters):
     ws = osb200.attn_fp8_workspace(B, L, H, "cuda")
     fns = {"bf16": lambda: osb200.attn_short(q, k, v, out_bf, **kw),
            "fp8": lambda: osb200.attn_fp8(q, k, v, out_f8, workspace=ws, **kw)}
-    t = _alternate(fns, reps, iters)
+    t = alternate(fns, reps, iters)
     flops = 4.0 * B * L * L * H * D
     res = dict(t)
     for name in ("bf16", "fp8"):
@@ -104,7 +100,7 @@ def model(net, inp, reps):
             for m in (list(modes) if i % 2 == 0 else list(modes)[::-1]):
                 setmode(m)
                 net(**inp)   # quantizes the weights / warms the workspaces off the clock
-                t[m].append(_ms(lambda: net(**inp), 1))
+                t[m].append(window_ms(lambda: net(**inp), 1))
         setmode("bf16")
     res.update({f"{m}_ms": round(statistics.median(v), 2) for m, v in t.items()})
     res.update({f"{m}_spread_ms": round(max(v) - min(v), 2) for m, v in t.items()})
@@ -122,12 +118,10 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power}
     net = inp = None
     if not a.no_model:
-        from tests.mmdit_fp8_gpu_common import mmdit_256px
-
         net, inp = mmdit_256px()
         res["bf16_forward_profile"] = profile(net, inp)
     res["attention_B3_L8828_H24"] = attention(a.reps, a.iters)

@@ -49,3 +49,33 @@ def fp8_attention():
         yield M
     finally:
         M.attention = saved
+
+
+def operands_cpu(B, L, H, seed=0, split=None, liger=True):
+    g = torch.Generator().manual_seed(seed)
+    C = H * 128
+    qkv = (torch.randn(B * L, 3 * C, generator=g) * 2).to(torch.bfloat16)
+    qkv[3, 2 * C:2 * C + 5] = 40.0                      # a v column with one large entry
+    qkv[:, 2 * C + 7] = 0.0                             # an all-zero v column: scale 1, codes 0
+    w = [(1 + 0.3 * torch.randn(128, generator=g)).to(torch.bfloat16) for _ in range(4)]
+    ang = torch.randn(L, 64, generator=g)
+    kw = dict(num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H,
+              head_dim=128, q_norm_w=w[0], k_norm_w=w[1], rope_cos=torch.cos(ang), rope_sin=torch.sin(ang),
+              rope_half=liger, q_norm_w2=None, k_norm_w2=None, norm_split=0)
+    if split is not None:
+        kw.update(q_norm_w2=w[2], k_norm_w2=w[3], norm_split=split)
+    return qkv, kw
+
+
+def operands_cuda(B, L, H, liger, split, seed=0, wscale=0.3, wmean=1.0):
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    C = H * 128
+    qkv = (torch.randn(B * L, 3 * C, device="cuda", generator=g) * 2).to(torch.bfloat16)
+    w = [(wmean + wscale * torch.randn(128, device="cuda", generator=g)).to(torch.bfloat16) for _ in range(4)]
+    ang = torch.rand(L, 64, device="cuda", generator=g) * 6.28
+    kw = dict(num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H,
+              head_dim=128, q_norm_w=w[0], k_norm_w=w[1], rope_cos=torch.cos(ang), rope_sin=torch.sin(ang),
+              rope_half=liger, q_norm_w2=None, k_norm_w2=None, norm_split=0)
+    if split is not None:
+        kw.update(q_norm_w2=w[2], k_norm_w2=w[3], norm_split=split)
+    return qkv, kw

@@ -25,8 +25,8 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.dora_bench import _alternate  # noqa: E402
-from tests.lora_bench import M_ROWS, _card, _ms  # noqa: E402
+from tests.models import ROWS_256PX as M_ROWS, mmdit_256px  # noqa: E402
+from tests.timing import alternate, card, window_ms  # noqa: E402
 
 
 def gemms(reps, iters):
@@ -79,7 +79,7 @@ def gemms(reps, iters):
     }
     r = {}
     for name, fns in cases.items():
-        t = _alternate(fns, reps, iters)
+        t = alternate(fns, reps, iters)
         if "bf16" in t:
             t["fp8_over_bf16"] = round(t["fp8"] / t["bf16"], 3)
         r[name] = t
@@ -87,8 +87,6 @@ def gemms(reps, iters):
 
 
 def model(reps):
-    from tests.mmdit_fp8_gpu_common import mmdit_256px
-
     net, inp = mmdit_256px()
     res = {}
     with torch.no_grad():
@@ -105,7 +103,7 @@ def model(reps):
                 else:
                     net.disable_fp8()
                 net(**inp)   # quantizes the weights / warms the workspaces off the clock
-                t[k].append(_ms(lambda: net(**inp), 1))
+                t[k].append(window_ms(lambda: net(**inp), 1))
         net.disable_fp8()
     res.update({f"{k}_ms": round(statistics.median(v), 2) for k, v in t.items()})
     res.update({f"{k}_spread_ms": round(max(v) - min(v), 2) for k, v in t.items()})
@@ -124,7 +122,7 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "rows": M_ROWS, "gemm_ms": gemms(a.reps, a.iters)}
     if not a.no_model:
         res["mmdit_256px_forward"] = model(a.reps)

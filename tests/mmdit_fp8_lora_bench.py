@@ -25,9 +25,8 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.dora_bench import _alternate  # noqa: E402
-from tests.lora_bench import _card, _ms  # noqa: E402
-from tests.mmdit_fp8_attn_bench import B, L  # noqa: E402
+from tests.models import B_256PX as B, L_256PX as L, mmdit_256px  # noqa: E402
+from tests.timing import alternate, card, window_ms  # noqa: E402
 
 C = 3072
 
@@ -78,7 +77,7 @@ def ops(reps, iters):
                 for (N, w, bias, w8, ws, kw16, kw8), Bm in zip(ps, Bs):
                     osb200.gemm_lora(x, w, bias, u, Bm, **kw16)
 
-            t = _alternate({"fp8": fp8, "fp8_down_plus_fp8_lora": fp8_lora, "bf16_down_plus_bf16_lora": bf16_lora},
+            t = alternate({"fp8": fp8, "fp8_down_plus_fp8_lora": fp8_lora, "bf16_down_plus_bf16_lora": bf16_lora},
                            reps, iters)
             t["fp8_lora_over_fp8"] = round(t["fp8_down_plus_fp8_lora"] / t["fp8"], 3)
             t["fp8_lora_speedup_over_bf16_lora"] = round(t["bf16_down_plus_bf16_lora"] / t["fp8_down_plus_fp8_lora"], 3)
@@ -88,7 +87,7 @@ def ops(reps, iters):
 
 def model(net, inp, reps):
     from opensora.utils.lora import load_lora, unload_lora
-    from tests.test_lora_cpu import write_adapter
+    from tests.adapters import write_adapter
 
     targets = net.fp8_mlp_linears() + net.fp8_proj_linears()
     tmp = tempfile.mkdtemp()
@@ -121,7 +120,7 @@ def model(net, inp, reps):
             for m in (list(modes) if i % 2 == 0 else list(modes)[::-1]):
                 setmode(m)
                 net(**inp)   # quantizes the weights / warms the workspaces off the clock
-                t[m].append(_ms(lambda: net(**inp), 1))
+                t[m].append(window_ms(lambda: net(**inp), 1))
     res.update({f"{m}_ms": round(statistics.median(v), 2) for m, v in t.items()})
     res.update({f"{m}_spread_ms": round(max(v) - min(v), 2) for m, v in t.items()})
     return res
@@ -138,11 +137,9 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "ops": ops(a.reps, a.iters)}
     if not a.no_model:
-        from tests.mmdit_fp8_gpu_common import mmdit_256px
-
         net, inp = mmdit_256px()
         res["mmdit_256px_forward"] = model(net, inp, a.reps)
     print(json.dumps(res), flush=True)

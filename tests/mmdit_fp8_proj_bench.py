@@ -22,11 +22,10 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.dora_bench import _alternate  # noqa: E402
-from tests.lora_bench import _card, _ms  # noqa: E402
-from tests.mmdit_fp8_attn_bench import B, H, L, LT  # noqa: E402
+from tests.models import B_256PX as B, L_256PX as L, LT_256PX as LT, mmdit_256px  # noqa: E402
+from tests.timing import alternate, card, window_ms  # noqa: E402
 
-C = 3072
+C, H = 3072, 24
 
 
 def ops(reps, iters):
@@ -43,7 +42,7 @@ def ops(reps, iters):
     wq8, sq = osb200.quant_blocks_fp8(wq, block=C)
     sq = sq.view(-1)
     out = torch.empty(M, 3 * C, dtype=torch.bfloat16, device="cuda")
-    t = _alternate({"bf16": lambda: osb200.gemm(x, wq, bq, out=out),
+    t = alternate({"bf16": lambda: osb200.gemm(x, wq, bq, out=out),
                     "fp8": lambda: osb200.gemm_fp8_blocks(x8, xs, wq8, sq, bq, out=out)}, reps, iters)
     t.update(TF_per_s_bf16=round(2.0 * M * 3 * C * C / t["bf16"] / 1e9, 1),
              TF_per_s_fp8=round(2.0 * M * 3 * C * C / t["fp8"] / 1e9, 1), speedup=round(t["bf16"] / t["fp8"], 3))
@@ -56,7 +55,7 @@ def ops(reps, iters):
     sp = sp.view(-1)
     out = torch.empty(M, C, dtype=torch.bfloat16, device="cuda")
     kw = dict(epilogue=osb200.EPI_BIAS_GATE_RES, residual=res_x, gate=gate, out=out)
-    t = _alternate({"bf16": lambda: osb200.gemm(x, wp, bp, **kw),
+    t = alternate({"bf16": lambda: osb200.gemm(x, wp, bp, **kw),
                     "fp8": lambda: osb200.gemm_fp8_blocks(a8, as_, wp8, sp, bp, **kw)}, reps, iters)
     t.update(TF_per_s_bf16=round(2.0 * M * C * C / t["bf16"] / 1e9, 1),
              TF_per_s_fp8=round(2.0 * M * C * C / t["fp8"] / 1e9, 1), speedup=round(t["bf16"] / t["fp8"], 3))
@@ -74,7 +73,7 @@ def ops(reps, iters):
     out_bf = torch.empty(M, C, dtype=torch.bfloat16, device="cuda")
     cat8 = torch.empty(M, 5 * C, dtype=torch.float8_e4m3fn, device="cuda")
     cats = torch.empty(M, 5 * C // 128, device="cuda")
-    t = _alternate({"bf16_out": lambda: osb200.attn_fp8(q, k, v, out_bf, workspace=ws, **akw),
+    t = alternate({"bf16_out": lambda: osb200.attn_fp8(q, k, v, out_bf, workspace=ws, **akw),
                     "fp8_out": lambda: osb200.attn_fp8_blocks(q, k, v, cat8[:, :C], cats[:, :H], workspace=ws, **akw),
                     "bf16_out_then_quant_blocks": lambda: (osb200.attn_fp8(q, k, v, out_bf, workspace=ws, **akw),
                                                            osb200.quant_blocks_fp8(out_bf, out=cat8[:, :C],
@@ -109,7 +108,7 @@ def model(net, inp, reps):
             for m in (list(modes) if i % 2 == 0 else list(modes)[::-1]):
                 setmode(m)
                 net(**inp)   # quantizes the weights / warms the workspaces off the clock
-                t[m].append(_ms(lambda: net(**inp), 1))
+                t[m].append(window_ms(lambda: net(**inp), 1))
         setmode("bf16")
     res.update({f"{m}_ms": round(statistics.median(v), 2) for m, v in t.items()})
     res.update({f"{m}_spread_ms": round(max(v) - min(v), 2) for m, v in t.items()})
@@ -127,11 +126,9 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, power = _card()
+    name, power = card()
     res = {"card": name, "power_limit,max_sm_clock": power, "ops": ops(a.reps, a.iters)}
     if not a.no_model:
-        from tests.mmdit_fp8_gpu_common import mmdit_256px
-
         net, inp = mmdit_256px()
         res["mmdit_256px_forward"] = model(net, inp, a.reps)
     print(json.dumps(res), flush=True)

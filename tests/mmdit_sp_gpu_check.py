@@ -22,19 +22,19 @@ def main():
     local = int(os.environ.get("LOCAL_RANK", rank))
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    from tests.test_mmdit_gpu import _ids, _rand_model
+    from tests.models import mmdit_ids, mmdit_model
     from tests.util import rel_l2
 
     ok = True
     for fused, liger, (B, Lt, T, H, W) in ((True, False, (2, 40, 3, 6, 8)), (False, True, (1, 64, 5, 12, 16))):
-        m = _rand_model(fused, liger)          # seeded: the same model on every rank; num_heads = 2 -> world 2 only
+        m = mmdit_model(fused, liger, device="cuda")          # seeded: the same model on every rank; num_heads = 2 -> world 2 only
         if m.config.num_heads % world:
             if rank == 0:
                 print(f"[mmdit-sp{world}] {m.config.num_heads} heads do not divide over {world} ranks: skipped")
             continue
         g = torch.Generator().manual_seed(3)
         rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-        txt_ids, img_ids = _ids(B, Lt, T, H, W)
+        txt_ids, img_ids = mmdit_ids(B, Lt, T, H, W)
         inp = dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids, timesteps=torch.rand(B, generator=g),
                    y_vec=rb(B, 96), cond=rb(B, T * H * W, 68), guidance=torch.full((B,), 4.0))
         inp = {k: v.cuda() for k, v in inp.items()}

@@ -14,7 +14,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -24,24 +23,7 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-
-def _card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except (OSError, IndexError, subprocess.SubprocessError):
-        q = "unknown"
-    return torch.cuda.get_device_name(0), q
-
-
-def _events(fn, n):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / n
+from tests.timing import card, window_ms  # noqa: E402
 
 
 def kernel(shape, iters=200):
@@ -68,8 +50,8 @@ def kernel(shape, iters=200):
         graphs[k].replay()
     ms_m, ms_c = [], []
     for _ in range(5):
-        ms_m.append(_events(graphs["masked"].replay, 1) / iters)
-        ms_c.append(_events(graphs["t2v"].replay, 1) / iters)
+        ms_m.append(window_ms(graphs["masked"].replay, 1) / iters)
+        ms_c.append(window_ms(graphs["t2v"].replay, 1) / iters)
     n = z.numel()
     bytes_m, bytes_c = 8.0 * n * (T - 1) / T, 8.0 * n
     m, c = statistics.median(ms_m), statistics.median(ms_c)
@@ -79,15 +61,13 @@ def kernel(shape, iters=200):
 
 
 def model_legs(steps, reps):
-    from oracle import stdit3_oracle as O
     from opensora.schedulers import RFLOW
     from opensora.utils.inference_utils import apply_mask_strategy
-    from tests.smoke_impl import build_pair
+    from tests.models import stdit3_inputs, stdit3_pair
 
-    prod, _, cfg = build_pair("xl")
+    prod, _, cfg = stdit3_pair("xl")
     B = 1
-    inp = O.synthetic_inputs(cfg, B=B, T=64, H=32, W=32, lens=[260])
-    inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
+    inp = stdit3_inputs(cfg, B, 64, 32, 32, lens=[260], device="cuda")
     z = inp["x"].to(torch.bfloat16)
     ref = [[torch.randn(cfg.in_channels, 1, 32, 32, device="cuda")]]
     zc = z.clone()
@@ -115,7 +95,7 @@ def model_legs(steps, reps):
             times = {k: [] for k in legs}
             for _ in range(reps):
                 for k, f in legs.items():
-                    times[k].append(_events(f, n) / per)
+                    times[k].append(window_ms(f, n) / per)
             for k, v in times.items():
                 res[k + "_ms"] = round(statistics.median(v), 2)
                 res[k + "_ms_spread"] = [round(min(v), 2), round(max(v), 2)]
@@ -129,7 +109,7 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("rf_cond_bench needs a CUDA device")
-    name, power = _card()
+    name, power = card()
     out = {"gpu": name, "power_limit_and_max_sm_clock": power,
            "kernel": [kernel((1, 4, 64, 32, 32)), kernel((2, 4, 128, 90, 160))],
            "stdit3_xl_64x32x32": dict(model_legs(a.steps, a.reps), steps_per_run=a.steps, cfg_batch=2)}

@@ -88,3 +88,9 @@ SCENARIOS = [
     ("distilled_image", dict(height=32, width=48, num_frames=1, num_steps=4, guidance=3.5, method="distill", seed=8),
      dict(cond_type="t2v", text=["a tree", "a hill"])),
 ]
+
+
+def toy_model(x, timestep, y, mask=None, x_mask=None, **kw):
+    v = torch.tanh(0.8 * x.float() + y.float().mean(dim=(1, 2, 3))[:, None, None, None, None])
+    v = v * (0.5 + timestep.float()[:, None, None, None, None] / 1000.0)
+    return torch.cat((v, 0.1 * x.float()), dim=1)

@@ -3,35 +3,17 @@ place outside tests/ and bench.py's cpu_baseline that touches oracle/, as the ch
 import torch
 
 
-def build_pair(cfg_name: str = "xs", device="cuda", seed=1234):
-    """(product model in bf16 on `device`, fp32 oracle holding the SAME bf16-rounded weights)."""
-    from opensora.models.stdit.stdit3 import STDiT3 as Product, STDiT3Config as PCfg
-    from oracle import stdit3_oracle as O
-
-    ocfg = O.STDiT3_XS_2_config() if cfg_name == "xs" else O.STDiT3_XL_2_config()
-    oracle = O.STDiT3(ocfg).eval()
-    O.init_synthetic_weights(oracle, seed)
-    sd = {k: v.to(torch.bfloat16) for k, v in oracle.state_dict().items()}
-    oracle.load_state_dict({k: v.float() for k, v in sd.items()})
-    prod = Product(PCfg(depth=ocfg.depth, hidden_size=ocfg.hidden_size, num_heads=ocfg.num_heads,
-                        patch_size=ocfg.patch_size)).eval()
-    prod.load_state_dict(sd)
-    prod = prod.to(device=device, dtype=torch.bfloat16)
-    return prod, oracle, ocfg
-
-
 def run_smoke():
-    from oracle import stdit3_oracle as O
+    from tests.models import stdit3_inputs, stdit3_pair
     from tests.util import report
 
     assert torch.cuda.is_available(), "smoke() needs cuda:0"
     torch.cuda.set_device(0)
-    prod, oracle, cfg = build_pair("xs")
-    inp = O.synthetic_inputs(cfg, B=1, T=8, H=16, W=16)
-    inp = {k: v.to(torch.bfloat16).float() if v.is_floating_point() else v for k, v in inp.items()}
+    prod, oracle, cfg = stdit3_pair("xs")
+    inp = stdit3_inputs(cfg, 1, 8, 16, 16, device="cuda")
     with torch.no_grad():
-        ref = oracle.cuda()(**{k: v.cuda() for k, v in inp.items()})
-        out = prod(**{k: v.cuda() for k, v in inp.items()})
+        ref = oracle.cuda()(**inp)
+        out = prod(**inp)
     torch.cuda.synchronize()
     r, _ = report("smoke STDiT3-XS/2 1x8x16x16", out, ref)
     assert out.shape == ref.shape and torch.isfinite(out).all()

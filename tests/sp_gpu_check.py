@@ -20,15 +20,13 @@ def main():
     local = int(os.environ.get("LOCAL_RANK", rank))
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    from oracle import stdit3_oracle as O
-    from tests.smoke_impl import build_pair
+    from tests.models import stdit3_inputs, stdit3_pair
     from tests.util import rel_l2
 
     ok = True
     for cfg_name, (B, T, H, W) in (("xs", (2, 8, 16, 16)), ("xs", (1, 16, 8, 16))):
-        prod, oracle, cfg = build_pair(cfg_name, device=torch.device("cuda", local))
-        inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=[300, 40][:B])
-        inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
+        prod, oracle, cfg = stdit3_pair(cfg_name, device=torch.device("cuda", local))
+        inp = stdit3_inputs(cfg, B, T, H, W, lens=[300, 40][:B], device="cuda")
         xm = torch.ones(B, T, dtype=torch.bool, device="cuda")
         xm[0, 1] = False
         for x_mask in (None, xm):

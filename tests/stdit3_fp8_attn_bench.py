@@ -22,8 +22,7 @@ for p in (ROOT, os.path.join(ROOT, "open-sora_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
-from tests.dora_bench import _alternate  # noqa: E402
-from tests.lora_bench import _card  # noqa: E402
+from tests.timing import alternate, card  # noqa: E402
 
 H, D, LY = 16, 72, 300
 
@@ -66,7 +65,7 @@ def kinds(T, S, reps, iters):
                   lambda: osb.attn_tiles_fp8(qt8, kv8, out, q_kind=0, k_kind=0, v_kind=1, Lk=LY, num_seqs=1)),
     }
     for name, (work, bf, conv, att) in calls.items():
-        t = _alternate({"bf16": bf, "fp8": lambda conv=conv, att=att: (conv(), att()), "convert": conv}, reps, iters)
+        t = alternate({"bf16": bf, "fp8": lambda conv=conv, att=att: (conv(), att()), "convert": conv}, reps, iters)
         t["bf16_TF_per_s"] = round(work / t["bf16"] / 1e9, 1)
         t["fp8_TF_per_s"] = round(work / t["fp8"] / 1e9, 1)
         t["speedup"] = round(t["bf16"] / t["fp8"], 3)
@@ -117,13 +116,13 @@ def model(T, Hx, Wx, reps, iters, graphs):
                 net(**inp)
         return f
 
-    res["eager_ms"] = _alternate({k: eager(*v) for k, v in modes.items()}, reps, iters)
+    res["eager_ms"] = alternate({k: eager(*v) for k, v in modes.items()}, reps, iters)
     if graphs:
         replays = {}
         for k, (a, m) in modes.items():
             net._fp8_attn, net._fp8 = a, m
             replays[k] = net.capture(**inp)
-        res["graph_ms"] = _alternate({k: (lambda r=r: r.graph.replay()) for k, r in replays.items()}, reps, iters)
+        res["graph_ms"] = alternate({k: (lambda r=r: r.graph.replay()) for k, r in replays.items()}, reps, iters)
         del replays
     setmode(False, False)
     return res
@@ -140,7 +139,7 @@ def main():
     import osb200
 
     osb200.init(0)
-    name, q = _card()
+    name, q = card()
     out = {"card": name, "power_limit_and_max_sm_clock": q}
     for shape in a.shapes.split(","):
         T, Hx, Wx = (int(v) for v in shape.split("x"))

@@ -15,6 +15,7 @@ import contextlib
 
 import torch
 
+from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests.mmdit_fp8_attn_ref import attention_from_operands
 
@@ -86,3 +87,38 @@ def fp8_attention(oracle):
         for b in blocks:
             del b.attn.forward
             del b.cross_attn.forward
+
+
+def dequantized(t8, kind, rows, is_v):
+    """fp64 [rows, H, D] values of one kind read back from the e4m3 tiles through the tile map."""
+    ti, r = F_.tile_index(t8.map, rows, t8.codes.device)
+    codes = t8.codes[kind].double()
+    if is_v:
+        codes = F_.v_in_key_order(t8.codes[kind]).double()
+        x = codes[:, ti, r, : t8.head_dim] * t8.scales[kind][:, ti, : t8.head_dim].double()
+    else:
+        x = codes[:, ti, r, : t8.head_dim] * t8.scales[kind][:, ti, r, None].double()
+    return x.transpose(0, 1)
+
+
+def tiles_reference(t8, kv8, q_rows, kv_rows, qseq, kseq, kpos, num_seqs, Lk, kv_lens, q_kind, k_kind, v_kind):
+    """(exact fp32 softmax, the P-emulation) on the dequantized e4m3 operands, per output token row [rows, H, D]."""
+    q = dequantized(t8, q_kind, q_rows, False).float()
+    k = dequantized(kv8, k_kind, kv_rows, False).float()
+    v = dequantized(kv8, v_kind, kv_rows, True).float()
+    H, D = t8.heads, t8.head_dim
+    exact = torch.zeros(q_rows, H, D, device=q.device)
+    emu = torch.zeros(q_rows, H, D, device=q.device)
+    for s_ in range(num_seqs):
+        rq = (qseq == s_).nonzero().flatten()
+        rk = (kseq == s_).nonzero().flatten()
+        rk = rk[kpos[rk].argsort()]
+        n = Lk if kv_lens is None else min(int(kv_lens[s_]), Lk)
+        if n <= 0:
+            continue
+        rk = rk[:n]
+        qq, kk, vv = q[rq].transpose(0, 1), k[rk].transpose(0, 1), v[rk].transpose(0, 1)
+        sc = qq @ kk.transpose(-1, -2) * D ** -0.5
+        exact[rq] = (torch.softmax(sc.double(), -1).float() @ vv).transpose(0, 1)
+        emu[rq] = attention_from_operands(qq, kk, vv, D ** -0.5).transpose(0, 1)
+    return exact, emu

@@ -8,7 +8,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import tempfile
 
@@ -17,20 +16,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "open-sora_b200")]
 
+from tests.timing import card, window_ms  # noqa: E402
+
 # prompt lengths in tokens, eos included: one typical prompt, and a batch from the eos-only prompt to a full one
 BATCHES = ([40], [1, 17, 40, 60, 77, 120, 200, 300])
-
-
-def _window(fn, iters):
-    """Mean ms per call over `iters` calls, timed by device events."""
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
 
 
 def main():
@@ -44,9 +33,7 @@ def main():
 
     osb200.init()
     torch.set_grad_enabled(False)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"gpu": q[0] if q else "unknown", "windows": args.windows, "iters_per_window": args.iters}
+    res = {"gpu": ", ".join(card()), "windows": args.windows, "iters_per_window": args.iters}
     cfg = tf.T5_XXL
     with tempfile.TemporaryDirectory() as tmp:
         w = G.device_weights(_t5_shapes(cfg), False, 1, cfg["d_model"])
@@ -58,11 +45,11 @@ def main():
             ids[mask == 0] = 0
             legs = {"masked": lambda: emb.encode(ids, mask), "unmasked": lambda: emb.encode(ids)}
             for fn in legs.values():
-                _window(fn, 3)
+                window_ms(fn, 3)
             times = {k: [] for k in legs}
             for r in range(args.windows):
                 for k in (list(legs) if r % 2 == 0 else list(legs)[::-1]):
-                    times[k].append(_window(legs[k], args.iters))
+                    times[k].append(window_ms(legs[k], args.iters))
             res[f"batch_{B}"] = {"prompt_tokens": lens, **{
                 k: {"median_ms": round(statistics.median(v), 3), "min_ms": round(min(v), 3), "max_ms": round(max(v), 3)}
                 for k, v in times.items()}}

@@ -8,8 +8,7 @@ import math
 import pytest
 import torch
 
-from tests.test_attn_tiles_gpu import _self_case
-from tests.util import rel_l2
+from tests.util import rel_l2, self_case
 
 pytestmark = pytest.mark.gpu
 
@@ -37,7 +36,7 @@ def test_self_attention_runs(mode, B, T, S, H, D):
     L = S if mode == 0 else T
     items = H * (nseq * -(-L // 128) if mode == 0 else -(-nseq // (128 // L)))
     assert items > _sms(), "the case must give every CTA several items"
-    _self_case(mode, B, T, S, H, D, seed=7)
+    self_case(mode, B, T, S, H, D, seed=7)
 
 
 def _cross(B, N, Ly, lens, H, D, seed=13):

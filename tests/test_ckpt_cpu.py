@@ -85,7 +85,7 @@ def test_model_factories_load_reference_keyed_checkpoints(tmp_path):
     import numpy as np
 
     from opensora.registry import MODELS, build_module
-    from tests.test_mmdit_gpu import CFG
+    from tests.models import MMDIT_CFG
 
     G = load_golden("vae_blocks.npz")
     kw = dict(type="hunyuan_vae", block_out_channels=(16, 32, 32, 32), layers_per_block=1, norm_num_groups=4, latent_channels=4)
@@ -100,9 +100,9 @@ def test_model_factories_load_reference_keyed_checkpoints(tmp_path):
     with pytest.raises(RuntimeError):   # the VAE factory loads strictly (autoencoder_kl_causal_3d.py:636)
         build_module(dict(kw, from_pretrained=str(tmp_path / "vae_bad.safetensors")), MODELS, device_map="cpu")
 
-    flux = build_module(dict(type="flux", **CFG), MODELS, device_map="cpu", torch_dtype=torch.float32)
+    flux = build_module(dict(type="flux", **MMDIT_CFG), MODELS, device_map="cpu", torch_dtype=torch.float32)
     sd = {k: torch.randn_like(v) for k, v in flux.state_dict().items()}
     save_file(sd, str(tmp_path / "flux.safetensors"))
-    again = build_module(dict(type="flux", from_pretrained=str(tmp_path / "flux.safetensors"), **CFG), MODELS, device_map="cpu",
+    again = build_module(dict(type="flux", from_pretrained=str(tmp_path / "flux.safetensors"), **MMDIT_CFG), MODELS, device_map="cpu",
                          torch_dtype=torch.float32)
     assert all(torch.equal(v, sd[k]) for k, v in again.state_dict().items())

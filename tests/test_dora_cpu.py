@@ -3,80 +3,15 @@ not a dependency) loaded by `opensora.utils.lora.load_lora`, the host-side MMDiT
 against the fp32 oracle on the merged weights g * (W + s B A), peft's unmerged DoRA formula restated on one layer, the
 modulation-group rule, launches, unloading, Ulysses sequence parallelism and the C ABI layout of osb_lora_args.  The
 kernel itself is checked on the GPU (tests/test_dora_gpu.py)."""
-import math
 import os
 
 import pytest
 import torch
 from torch import nn
 
-from tests.test_lora_cpu import _inputs, _rand_model, write_adapter
-from tests.test_mmdit_gpu import CFG
+from tests.adapters import dora_g, merged_state_dora, write_adapter, write_dora_adapter
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
-
-
-# ---- adapter files ----------------------------------------------------------------------------------------------------
-def write_dora_adapter(path, model, *, spread=0.3, mag_seed=1, fmt="safetensors", **kw):
-    """A PEFT DoRA adapter directory for `model`: write_adapter's A / B plus, per target, the magnitude vector peft saves
-    as `base_model.model.<name>.lora_magnitude_vector`, set to the row norms of W + s B A times a factor in
-    [1 - spread, 1 + spread] so that g = m / ||W + s B A|| is well away from 1."""
-    import json
-
-    write_adapter(path, model, fmt=fmt, use_dora=True, **kw)
-    cfg = json.load(open(os.path.join(path, "adapter_config.json")))
-    f = os.path.join(path, "adapter_model.safetensors" if fmt == "safetensors" else "adapter_model.bin")
-    if fmt == "safetensors":
-        from safetensors.torch import load_file, save_file
-
-        sd = {k: v.clone() for k, v in load_file(f).items()}
-    else:
-        sd = torch.load(f, weights_only=True)
-    from opensora.utils.lora import _pattern_value
-
-    g = torch.Generator().manual_seed(mag_seed)
-    mods = dict(model.named_modules())
-    for k in [k for k in sd if k.endswith(".lora_A.weight")]:
-        name = k[len("base_model.model."):-len(".lora_A.weight")]
-        lin = mods[name]
-        r = int(_pattern_value(cfg["rank_pattern"], name, cfg["r"]))
-        a = float(_pattern_value(cfg["alpha_pattern"], name, cfg["lora_alpha"]))
-        s = a / math.sqrt(r) if cfg["use_rslora"] else a / r
-        W = lin.weight.detach().float().cpu() + s * sd[f"base_model.model.{name}.lora_B.weight"] @ sd[k]
-        fac = 1 + spread * (2 * torch.rand(lin.out_features, generator=g) - 1)
-        sd[f"base_model.model.{name}.lora_magnitude_vector"] = (W.norm(dim=1) * fac).contiguous()
-    if fmt == "safetensors":
-        save_file(sd, f)
-    else:
-        torch.save(sd, f)
-    return path
-
-
-def dora_g(lin):
-    """g = m / ||W + s B A||_2 per output row, fp32, from the layer's own (bf16) tensors."""
-    from opensora.utils.lora import adapter_of, dora_magnitude
-
-    A, B, s = adapter_of(lin)
-    with torch.no_grad():
-        W = lin.weight.float() + s * (B.float() @ A.float())
-        return dora_magnitude(lin).float() / W.norm(dim=1)
-
-
-def merged_state_dora(model):
-    """fp32 state dict of the plain model with every adapter merged: g * (W + s B A) for DoRA layers (bias untouched),
-    W + s B A for plain LoRA layers."""
-    from opensora.utils.lora import adapter_of, dora_magnitude, is_wrapped
-
-    W = {k.replace(".base_layer.", "."): v.float() for k, v in model.state_dict().items()
-         if ".lora_" not in k}
-    with torch.no_grad():
-        for name, m in model.named_modules():
-            if is_wrapped(m):
-                A, B, s = adapter_of(m)
-                w = W[f"{name}.weight"] + s * (B.float() @ A.float())
-                if dora_magnitude(m) is not None:
-                    w = dora_g(m)[:, None] * w
-                W[f"{name}.weight"] = w
-    return W
 
 
 def _mod_names(model):
@@ -88,7 +23,7 @@ def _mod_names(model):
 def test_dora_directory_loads_magnitudes(tmp_path, fmt):
     from opensora.utils.lora import DoraMagnitude, LoraLinear, adapter_of, dora_magnitude, load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     d = write_dora_adapter(tmp_path / fmt, m, targets=["qkv", "linear1", "img_in"], fmt=fmt)
     f = d / ("adapter_model.safetensors" if fmt == "safetensors" else "adapter_model.bin")
     if fmt == "safetensors":
@@ -113,7 +48,7 @@ def test_dora_missing_or_misshaped_magnitude_is_refused(tmp_path):
 
     from opensora.utils.lora import load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     d = write_dora_adapter(tmp_path, m, targets=["proj"])
     f = str(d / "adapter_model.safetensors")
     sd = {k: v.clone() for k, v in load_file(f).items()}
@@ -142,7 +77,7 @@ def test_dora_rank_alpha_patterns_and_rslora(fake_osb, tmp_path):
     from opensora.models.mmdit.layers import linear_parts
     from opensora.utils.lora import load_lora, unload_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     write_dora_adapter(tmp_path / "a", m, r=8, alpha=16, targets=["qkv", "proj", "linear2"], rank_pattern={"proj": 16},
                        alpha_pattern={r"single_blocks\.1\.linear2": 4})
     load_lora(m, str(tmp_path / "a"), scale=0.5)
@@ -168,7 +103,7 @@ def test_peft_unmerged_formula_equals_merged_form(fake_osb, tmp_path):
     form g * x (W + s B A)^T + b that the kernel computes; the layer's forward on the stand-in is that up to bf16."""
     from opensora.utils.lora import adapter_of, dora_magnitude, load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     load_lora(m, str(write_dora_adapter(tmp_path, m, targets=["linear2"], rel=0.2)))
     lin = m.single_blocks[0].linear2
     A, B, s = (t.detach().float() if torch.is_tensor(t) else t for t in adapter_of(lin))
@@ -194,7 +129,7 @@ def test_peft_style_dora_layer_takes_the_same_path(fake_osb, tmp_path):
     from opensora.models.mmdit.layers import _linear, linear_parts
     from opensora.utils.lora import dora_magnitude, load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     load_lora(m, str(write_dora_adapter(tmp_path, m, targets=["img_in"])))
     own = m.img_in
 
@@ -243,13 +178,13 @@ def test_mmdit_dora_on_every_linear_vs_oracle_on_merged_weights(fake_osb, tmp_pa
     from oracle import mmdit_oracle as M
     from opensora.utils.lora import load_lora
 
-    m = _rand_model(fused, liger)
-    inp = _inputs()
+    m = mmdit_model(fused, liger)
+    inp = mmdit_inputs()
     with torch.no_grad():
         base = m(**inp)
         load_lora(m, str(write_dora_adapter(tmp_path, m, r=12, alpha=24, rel=0.1, seed=9)))
         out = m(**inp)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
     W32 = merged_state_dora(m)
     finp = {k: (v.float() if v.is_floating_point() else v) for k, v in inp.items()}
     ref = M.model_forward(W32, cfg, finp["img"], finp["img_ids"], finp["txt"], finp["txt_ids"], finp["timesteps"],
@@ -280,9 +215,9 @@ def test_modulation_group_keeps_only_layers_without_dora(fake_osb, tmp_path):
     modulation layer there is no grouped GEMM at all."""
     from opensora.utils.lora import load_lora, unload_lora
 
-    m = _rand_model()
-    inp = _inputs(B=1)
-    C, nd, ns = CFG["hidden_size"], CFG["depth"], CFG["depth_single_blocks"]
+    m = mmdit_model()
+    inp = mmdit_inputs(B=1)
+    C, nd, ns = MMDIT_CFG["hidden_size"], MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
     load_lora(m, str(write_dora_adapter(tmp_path / "img", m, targets=r".*img_mod\.lin", r=8, rel=0.5)))
     with torch.no_grad():
         fake_osb.reset()
@@ -306,10 +241,10 @@ def test_dora_launches_equal_plain_lora(fake_osb, tmp_path):
     launch list (only the column scale differs)."""
     from opensora.utils.lora import load_lora, unload_lora
 
-    m = _rand_model(False, True)
+    m = mmdit_model(False, True)
     mods = set(_mod_names(m))
     targets = [n for n, x in m.named_modules() if type(x) is nn.Linear and n not in mods]
-    inp = _inputs()
+    inp = mmdit_inputs()
     with torch.no_grad():
         load_lora(m, str(write_adapter(tmp_path / "lora", m, targets=targets, seed=2)))
         fake_osb.reset()
@@ -326,8 +261,8 @@ def test_dora_launches_equal_plain_lora(fake_osb, tmp_path):
 def test_unload_dora_restores_outputs_and_launches(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora, unload_lora
 
-    plain, m = _rand_model(True, False), _rand_model(True, False)
-    inp = _inputs()
+    plain, m = mmdit_model(True, False), mmdit_model(True, False)
+    inp = mmdit_inputs()
     with torch.no_grad():
         fake_osb.reset()
         want = plain(**inp)
@@ -347,7 +282,7 @@ def test_pack_is_rebuilt_when_magnitude_or_base_weight_changes(fake_osb, tmp_pat
     from opensora.models.mmdit.layers import linear_parts
     from opensora.utils.lora import dora_magnitude, load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     load_lora(m, str(write_dora_adapter(tmp_path, m, targets=["img_in"])))
     lin = m.img_in
     s0 = linear_parts(lin)[2][2]
@@ -381,9 +316,9 @@ def _dora_sp_worker(rank, world, port, adapter_dirs, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for (fused, liger, (B, Lt, thw)), d in zip(SP_CASES, adapter_dirs):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             load_lora(m, d)
-            inp = _inputs(B, Lt, thw)
+            inp = mmdit_inputs(B, Lt, thw)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)
@@ -404,7 +339,7 @@ def test_mmdit_ulysses_with_dora_world2(tmp_path):
 
     dirs = []
     for i, (fused, liger, _) in enumerate(SP_CASES):
-        dirs.append(str(write_dora_adapter(tmp_path / f"a{i}", _rand_model(fused, liger), seed=i)))
+        dirs.append(str(write_dora_adapter(tmp_path / f"a{i}", mmdit_model(fused, liger), seed=i)))
     port = 29500 + (os.getpid() + 23) % 2000
     mgr = mp.Manager()
     ret = mgr.dict()

@@ -24,7 +24,9 @@ import torch
 import torch.nn.functional as TF
 
 from tests import fake_osb200 as F_
-from tests.test_attn_tiles_gpu import read_tiles
+from tests.models import mmdit_ids, mmdit_model, stdit3_inputs, stdit3_pair, tiny_vae
+from tests.sampling_toys import toy_model
+from tests.util import load_golden, read_tiles
 
 pytestmark = pytest.mark.gpu
 
@@ -1068,45 +1070,36 @@ def _workload(name):
     """One forward of a product path on the GPU (the binding is recorded while it runs)."""
     dev = _dev()
     if name == "stdit3-xs":
-        from oracle import stdit3_oracle as O
-        from tests.smoke_impl import build_pair
-
-        prod, _, cfg = build_pair("xs")
-        inp = O.synthetic_inputs(cfg, B=1, T=4, H=16, W=16)
-        inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).to(dev) for k, v in inp.items()}
+        prod, _, cfg = stdit3_pair("xs")
+        inp = stdit3_inputs(cfg, 1, 4, 16, 16, device=dev)
         with torch.no_grad():
             prod(**inp)
     elif name.startswith("mmdit"):
-        from tests.test_mmdit_gpu import _ids, _rand_model
-
         fused, liger = name == "mmdit-fused-flux", name == "mmdit-split-liger"
-        m = _rand_model(fused, liger)
+        m = mmdit_model(fused, liger, device="cuda")
         B, Lt, T, H, W = 2, 40, 3, 6, 8
         g = _gen(3)
         rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-        txt_ids, img_ids = _ids(B, Lt, T, H, W)
+        txt_ids, img_ids = mmdit_ids(B, Lt, T, H, W)
         inp = dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids,
                    timesteps=torch.tensor([0.3, 0.8]), y_vec=rb(B, 96), cond=rb(B, T * H * W, 68),
                    guidance=torch.tensor([4.0, 7.5]))
         with torch.no_grad():
             m(**{k: v.to(dev) for k, v in inp.items()})
     elif name == "vae":
-        from tests.test_host_vae_cpu import _golden, _model
-
-        G = _golden("vae_blocks.npz")
-        m = _model(G).to(torch.bfloat16).to(dev)
+        G = load_golden("vae_blocks.npz")
+        m = tiny_vae(G).to(torch.bfloat16).to(dev)
         with torch.no_grad():
             m.encoder(m._to_ndhwc(G["enc_x"].to(torch.bfloat16).to(dev), cpad=8))
             m.decoder(m._to_ndhwc(G["enc_y"][:, :4].to(torch.bfloat16).to(dev)))
     else:
         from opensora.schedulers import RFLOW
-        from tests.test_rf_conditioning_gpu import _toy_model
 
         g = torch.Generator(device="cuda").manual_seed(1)
         z = torch.randn(2, 4, 6, 8, 8, device=dev, generator=g).to(torch.bfloat16)
         y = torch.randn(2, 1, 5, 8, device=dev, generator=g)
         fm = torch.tensor([[0.0, 0.5, 1.0, 1.0, 0.3, 1.0], [1.0, 1.0, 0.0, 0.7, 1.0, 1.0]], device=dev)
-        RFLOW(num_sampling_steps=2, cfg_scale=6.0).sample(_toy_model, z, y, y, frame_mask=fm, generator=g)
+        RFLOW(num_sampling_steps=2, cfg_scale=6.0).sample(toy_model, z, y, y, frame_mask=fm, generator=g)
 
 
 @pytest.mark.parametrize("workload", ["stdit3-xs", "mmdit-fused-flux", "mmdit-split-liger", "vae", "rf-masked-loop"])

@@ -9,6 +9,7 @@ import torch
 import torch.nn.functional as F
 
 from tests import fp8_ref as R
+from tests.models import stdit3_inputs, stdit3_pair
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -97,24 +98,17 @@ def test_gemm_fp8_matches_dequantized_fp32(fake_osb, epilogue):
                           epilogue=bad.get("epilogue", 0))
 
 
-def _inputs(cfg, B, T, H, W, lens=None):
-    from oracle import stdit3_oracle as O
-
-    inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=lens)
-    return {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v) for k, v in inp.items()}
-
-
 def test_host_stdit3_fp8_follows_the_emulation(fake_osb):
     """XS/2 at hidden 256 with FP8 MLPs on the stand-in, against the fp32 oracle.  The yardstick is the FP8-emulation
     reference: the oracle in bf16 with its block MLPs at the FP8 rounding points (tests/fp8_ref.py), measured in the same
     test.  The product may not be more than 1.1x further from the fp32 oracle than that reference, plain and with an
     x_mask (the mod_index route)."""
-    prod, oracle, cfg = R.build_pair("xs", device="cpu")
+    prod, oracle, cfg = stdit3_pair("xs64", device="cpu")
     prod.enable_fp8()
-    inp = _inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 9])
+    inp = stdit3_inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 9])
     xm = torch.ones(2, 4, dtype=torch.bool)
     xm[1, 1:3] = False
-    ob = R.build_pair("xs", device="cpu")[1].to(torch.bfloat16)
+    ob = stdit3_pair("xs64", device="cpu")[1].to(torch.bfloat16)
     for kw in ({}, {"x_mask": xm}):
         fake_osb.reset()
         with torch.no_grad():
@@ -136,8 +130,8 @@ def test_host_stdit3_fp8_follows_the_emulation(fake_osb):
 
 
 def test_disable_fp8_restores_the_bf16_path(fake_osb):
-    prod, _, cfg = R.build_pair("xs", device="cpu")
-    inp = _inputs(cfg, 1, 4, 8, 8)
+    prod, _, cfg = stdit3_pair("xs64", device="cpu")
+    inp = stdit3_inputs(cfg, 1, 4, 8, 8)
     with torch.no_grad():
         before = prod(**inp)
         prod.enable_fp8()

@@ -8,6 +8,7 @@ import torch.nn.functional as F
 
 from tests import fake_osb200 as F_
 from tests import fp8_ref as R
+from tests.models import stdit3_inputs, stdit3_pair
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -117,20 +118,13 @@ def test_ln_modulate_fp8_matches_the_stand_in(rows, C, x_mask):
     assert mism < 1e-3
 
 
-def _inputs(cfg, B, T, H, W, lens=None):
-    from oracle import stdit3_oracle as O
-
-    inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=lens)
-    return {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
-
-
 def test_xl_fp8_at_the_benchmark_shape():
     """STDiT3-XL/2, full depth, 1x4x64x32x32 (16 384 tokens), FP8 MLPs, against the fp32 oracle holding the same bf16
     weights.  Bars: the error is at most 1.1x that of the FP8-emulation reference (the oracle in bf16 with its block
     MLPs at the FP8 rounding points), and the residual stream never jumps by more than 3x between consecutive blocks."""
-    prod, oracle, cfg = R.build_pair("xl")
+    prod, oracle, cfg = stdit3_pair("xl")
     prod.enable_fp8()
-    inp = _inputs(cfg, 1, 64, 32, 32, lens=[260])
+    inp = stdit3_inputs(cfg, 1, 64, 32, 32, lens=[260], device="cuda")
     oracle = oracle.cuda()
     ref_x, got_x = [], []
     hooks = [b.register_forward_hook(lambda m, a, out: ref_x.append(out.detach().float()))
@@ -172,7 +166,7 @@ def test_enable_fp8_stays_off_when_quantization_fails():
     """fp32 weights on the GPU: the weight quantizer refuses them, and the model keeps running its bf16 MLPs."""
     import osb200
 
-    prod = R.build_pair("xs")[0].float()
+    prod = stdit3_pair("xs64")[0].float()
     with pytest.raises(osb200.OsbError):
         prod.enable_fp8()
     assert prod._fp8 is False and not any(k[0] == "fp8" for k in prod._cache)
@@ -181,9 +175,9 @@ def test_enable_fp8_stays_off_when_quantization_fails():
 def test_fp8_graph_replay_and_disable():
     """XS/2 at hidden 256 with an x_mask: the captured FP8 step replays to the eager bits; disable_fp8() gives the bits
     of a model that never enabled FP8."""
-    prod, oracle, cfg = R.build_pair("xs")
-    plain = R.build_pair("xs")[0]
-    inp = _inputs(cfg, 2, 8, 16, 16, lens=[300, 21])
+    prod, oracle, cfg = stdit3_pair("xs64")
+    plain = stdit3_pair("xs64")[0]
+    inp = stdit3_inputs(cfg, 2, 8, 16, 16, lens=[300, 21], device="cuda")
     xm = torch.ones(2, 8, dtype=torch.bool, device="cuda")
     xm[1, :3] = False
     with torch.no_grad():

@@ -79,18 +79,6 @@ def test_output_view_in_sentinel_buffer(fn, bn, epi, gm):
     assert bad.numel() == 0, f"{case}: wrote {bad.shape[0]} elements outside the output view, first at {tuple(bad[0].tolist())}"
 
 
-def _conv_box(t_out, h_out, w_out):
-    """(Tt, Ht, Wt) of the CTA box osb_conv3d_ndhwc picks: least padded work, wide W first."""
-    best, box = 1e30, None
-    for wl in range(7, 2, -1):
-        for hl in range(0, 8 - wl):
-            Wt, Ht, Tt = 1 << wl, 1 << hl, 128 >> (wl + hl)
-            work = (-(-w_out // Wt) * Wt) * (-(-h_out // Ht) * Ht) * (-(-t_out // Tt) * Tt)
-            if work < best * 0.999:
-                best, box = work, (Tt, Ht, Wt)
-    return box
-
-
 @pytest.mark.parametrize("block_n", [128, 64])
 def test_conv3d_residual_ragged_box(block_n):
     """3x3x3 convolution + bias + residual on exact operands (x in {0, +-1}, w in {0, +-1} x 2^e per output channel, bias
@@ -102,7 +90,7 @@ def test_conv3d_residual_ragged_box(block_n):
 
     dev = _dev()
     nb, (t, h, w), cin, cout = 2, (3, 3, 12), 64, 136
-    Tt, Ht, Wt = _conv_box(t, h, w)
+    Tt, Ht, Wt = X.conv_box(t, h, w)
     assert t % Tt and h % Ht and w % Wt, f"box {Tt}x{Ht}x{Wt} is not ragged in every dimension of {t}x{h}x{w}"
     g = torch.Generator(device=dev).manual_seed(11)
     ints = lambda lo, hi, *s: torch.randint(lo, hi + 1, s, generator=g, device=dev).double()   # noqa: E731

@@ -9,8 +9,7 @@ import pytest
 import torch
 
 from tests import exact_gemm as X
-from tests.test_attn_tiles_gpu import read_tiles
-from tests.test_gemm_epilogue_gpu import _conv_box
+from tests.util import read_tiles
 
 pytestmark = pytest.mark.gpu
 
@@ -159,7 +158,7 @@ def test_conv3d_residual_many_tiles(block_n):
 
     _dev()
     nb, (t, h, w), cout = CONV["nb"], CONV["thw"], CONV["cout"]
-    Tt, Ht, Wt = _conv_box(t, h, w)
+    Tt, Ht, Wt = X.conv_box(t, h, w)
     assert t % Tt and h % Ht and w % Wt, f"box {Tt}x{Ht}x{Wt} is not ragged in every dimension of {t}x{h}x{w}"
     assert cout % block_n and nb * -(-t // Tt) * -(-h // Ht) * -(-w // Wt) * -(-cout // block_n) > 2 * _sms()
     x, wt, bias, res, ref = _conv_operands()

@@ -7,40 +7,24 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_mmdit_gpu import CFG, _ids
+from tests.models import MMDIT_CFG, TOKEN_STRIDE, mmdit_block_case, mmdit_ids, mmdit_model
 from tests.util import rel_l2
-
-
-def _rand_model(fused, liger=False):
-    from opensora.registry import MODELS, build_module
-
-    torch.manual_seed(7)
-    m = build_module(dict(type="flux", fused_qkv=fused, use_liger_rope=liger, **CFG), MODELS, device_map="cpu",
-                     torch_dtype=torch.float32)
-    g = torch.Generator().manual_seed(11)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if n.endswith("scale"):
-                p.copy_(1 + 0.2 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 or "cond_in" in n:
-                p.copy_(0.05 * torch.randn(p.shape, generator=g))
-    return m.to(torch.bfloat16)
 
 
 @pytest.mark.parametrize("fused,liger", [(True, False), (False, False), (False, True)])
 def test_mmdit_model_host_logic(fake_osb, fused, liger):
     from oracle import mmdit_oracle as M
 
-    m = _rand_model(fused, liger)
+    m = mmdit_model(fused, liger)
     B, Lt, (T, H, W) = 2, 24, (2, 4, 6)
     g = torch.Generator().manual_seed(3)
     rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-    txt_ids, img_ids = _ids(B, Lt, T, H, W)
+    txt_ids, img_ids = mmdit_ids(B, Lt, T, H, W)
     inp = dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids,
                timesteps=torch.tensor([0.3, 0.8]), y_vec=rb(B, 96), cond=rb(B, T * H * W, 68), guidance=torch.tensor([4.0, 7.5]))
     with torch.no_grad():
         out = m(**inp)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
     W32 = {k: v.float() for k, v in m.state_dict().items()}
     finp = {k: (v.float() if v.is_floating_point() else v) for k, v in inp.items()}
     ref = M.model_forward(W32, cfg, finp["img"], finp["img_ids"], finp["txt"], finp["txt_ids"], finp["timesteps"],
@@ -53,14 +37,14 @@ def test_mmdit_model_host_logic(fake_osb, fused, liger):
     assert r < 2e-2 and r < max(1.5 * rn, 5e-3), (r, rn)
     # one attention call per block over the joint txt|img sequence, with the second norm-weight pair for the img part
     attn = [c for c in fake_osb.calls if c[0] == "attn_short"]
-    assert len(attn) == CFG["depth"] + CFG["depth_single_blocks"]
+    assert len(attn) == MMDIT_CFG["depth"] + MMDIT_CFG["depth_single_blocks"]
     assert all(c[1][1] == Lt + T * H * W for c in attn)
 
 
 def test_processor_hook_is_the_plugin_point(fake_osb):
     from opensora.models.mmdit.layers import DoubleStreamBlockProcessor
 
-    m = _rand_model(True)
+    m = mmdit_model(True)
     seen = []
 
     class Spy(DoubleStreamBlockProcessor):
@@ -71,37 +55,13 @@ def test_processor_hook_is_the_plugin_point(fake_osb):
     for b in m.double_blocks:
         assert isinstance(b.get_processor(), DoubleStreamBlockProcessor)
         b.set_processor(Spy())
-    txt_ids, img_ids = _ids(1, 8, 1, 4, 4)
+    txt_ids, img_ids = mmdit_ids(1, 8, 1, 4, 4)
     bf = torch.bfloat16
     with torch.no_grad():
         out = m(img=torch.randn(1, 16, 64).to(bf), img_ids=img_ids, txt=torch.randn(1, 8, 128).to(bf), txt_ids=txt_ids,
                 timesteps=torch.tensor([0.5]), y_vec=torch.randn(1, 96).to(bf), cond=torch.randn(1, 16, 68).to(bf),
                 guidance=torch.tensor([4.0]))
-    assert len(seen) == CFG["depth"] and out.shape == (1, 16, 64) and torch.isfinite(out.float()).all()
-
-
-TOKEN_STRIDE = 3   # tests/golden/ref_classes.npz keeps every third token of the reference outputs (float16)
-
-
-def mmdit_block_case(L, fused):
-    """Seeded DoubleStreamBlock / SingleStreamBlock (C = 256, 2 heads) built from the layers module `L` (the reference's
-    mmdit/layers.py executed by path, or the in-tree mirror, which draws identical parameters) and their inputs."""
-    torch.manual_seed(5)
-    C, H, B, Lt, Li = 256, 2, 2, 24, 48
-    dbl = L.DoubleStreamBlock(C, H, mlp_ratio=4.0, qkv_bias=True, fused_qkv=fused).eval()
-    sgl = L.SingleStreamBlock(C, H, mlp_ratio=4.0, fused_qkv=fused).eval()
-    with torch.no_grad():
-        for blk in (dbl, sgl):
-            for n, p in blk.named_parameters():
-                p.copy_(torch.randn_like(p) * (0.2 if n.endswith("scale") else 0.05) + (1.0 if n.endswith("scale") else 0.0))
-    ids = torch.zeros(B, Lt + Li, 3)
-    ids[:, Lt:, 0] = torch.arange(Li) // 16
-    ids[:, Lt:, 1] = (torch.arange(Li) // 4) % 4
-    ids[:, Lt:, 2] = torch.arange(Li) % 4
-    pe = L.EmbedND(dim=C // H, theta=10000, axes_dim=[16, 56, 56])(ids)
-    bf = torch.bfloat16
-    img, txt, vec = torch.randn(B, Li, C).to(bf), torch.randn(B, Lt, C).to(bf), torch.randn(B, C).to(bf)
-    return dbl, sgl, pe, img, txt, vec
+    assert len(seen) == MMDIT_CFG["depth"] and out.shape == (1, 16, 64) and torch.isfinite(out.float()).all()
 
 
 @pytest.mark.parametrize("fused", [True, False])
@@ -140,9 +100,9 @@ def test_processors_run_on_the_reference_own_blocks(fake_osb, fused):
 def test_per_step_constants_are_hoisted(fake_osb):
     """SURVEY.md 8f-2: ONE grouped GEMM projects `vec` through every block's modulation layer (the reference launches
     2*depth + depth_single tiny ones), and `pe` is computed once for id tensors that do not change between steps."""
-    m = _rand_model(True)
-    C, nd, ns = CFG["hidden_size"], CFG["depth"], CFG["depth_single_blocks"]
-    txt_ids, img_ids = _ids(1, 8, 1, 4, 4)
+    m = mmdit_model(True)
+    C, nd, ns = MMDIT_CFG["hidden_size"], MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
+    txt_ids, img_ids = mmdit_ids(1, 8, 1, 4, 4)
     bf = torch.bfloat16
     inp = dict(img=torch.randn(1, 16, 64).to(bf), img_ids=img_ids, txt=torch.randn(1, 8, 128).to(bf), txt_ids=txt_ids,
                timesteps=torch.tensor([0.5]), y_vec=torch.randn(1, 96).to(bf), cond=torch.randn(1, 16, 68).to(bf),
@@ -179,10 +139,10 @@ def _mmdit_sp_worker(rank, world, port, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for fused, liger, (B, Lt, T, H, W) in ((True, False, (2, 24, 2, 4, 6)), (False, True, (1, 8, 1, 4, 6)), (True, False, (1, 40, 1, 2, 4))):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             g = torch.Generator().manual_seed(3)
             rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-            txt_ids, img_ids = _ids(B, Lt, T, H, W)
+            txt_ids, img_ids = mmdit_ids(B, Lt, T, H, W)
             inp = dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids, timesteps=torch.rand(B, generator=g),
                        y_vec=rb(B, 96), cond=rb(B, T * H * W, 68), guidance=torch.full((B,), 4.0))
             with torch.no_grad():

@@ -10,26 +10,14 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from tests.models import stdit3_inputs, stdit3_pair
 from tests.util import rel_l2
-
-
-def _pair(seed=1234):
-    from tests.smoke_impl import build_pair
-
-    return build_pair("xs", device="cpu", seed=seed)
-
-
-def _inputs(cfg, B, T, H, W, lens=None):
-    from oracle import stdit3_oracle as O
-
-    inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=lens)
-    return {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v) for k, v in inp.items()}
 
 
 @pytest.mark.parametrize("B,T,H,W", [(1, 4, 8, 8), (2, 3, 6, 10)])
 def test_forward_matches_oracle(fake_osb, B, T, H, W):
-    prod, oracle, cfg = _pair()
-    inp = _inputs(cfg, B, T, H, W)
+    prod, oracle, cfg = stdit3_pair("xs", device="cpu")
+    inp = stdit3_inputs(cfg, B, T, H, W)
     with torch.no_grad():
         ref = oracle(**inp)
         out = prod(**inp)
@@ -47,8 +35,8 @@ def test_forward_matches_oracle(fake_osb, B, T, H, W):
 
 
 def test_x_mask_and_ragged_text(fake_osb):
-    prod, oracle, cfg = _pair()
-    inp = _inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 7])
+    prod, oracle, cfg = stdit3_pair("xs", device="cpu")
+    inp = stdit3_inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 7])
     xm = torch.ones(2, 4, dtype=torch.bool)
     xm[0, 1:] = False
     xm[1, 0] = False
@@ -61,8 +49,8 @@ def test_x_mask_and_ragged_text(fake_osb):
 
 
 def test_non_multiple_sizes_are_padded_and_cropped(fake_osb):
-    prod, oracle, cfg = _pair()
-    inp = _inputs(cfg, 1, 3, 7, 9)      # H, W not multiples of the (1,2,2) patch
+    prod, oracle, cfg = stdit3_pair("xs", device="cpu")
+    inp = stdit3_inputs(cfg, 1, 3, 7, 9)      # H, W not multiples of the (1,2,2) patch
     with torch.no_grad():
         ref = oracle(**inp)
         out = prod(**inp)
@@ -71,9 +59,9 @@ def test_non_multiple_sizes_are_padded_and_cropped(fake_osb):
 
 
 def test_dtype_contract_is_enforced(fake_osb):
-    prod, _, cfg = _pair()
+    prod, _, cfg = stdit3_pair("xs", device="cpu")
     with pytest.raises(fake_osb.OsbError):
-        prod.float()(**_inputs(cfg, 1, 2, 4, 4))
+        prod.float()(**stdit3_inputs(cfg, 1, 2, 4, 4))
 
 
 def _sp_worker(rank, world, port, ret):
@@ -86,8 +74,8 @@ def _sp_worker(rank, world, port, ret):
 
         sys.modules["osb200"] = fake_osb200
         torch.manual_seed(0)
-        prod, _, cfg = _pair()
-        inp = _inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 9])
+        prod, _, cfg = stdit3_pair("xs", device="cpu")
+        inp = stdit3_inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 9])
         xm = torch.ones(2, 4, dtype=torch.bool)
         xm[1, 2:] = False
         with torch.no_grad():
@@ -124,8 +112,8 @@ def test_rflow_sampler_drives_the_model(fake_osb):
     from opensora.schedulers import RFLOW
     from oracle import sampling_oracle as S
 
-    prod, oracle, cfg = _pair()
-    inp = _inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 11])
+    prod, oracle, cfg = stdit3_pair("xs", device="cpu")
+    inp = stdit3_inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 11])
     B = 2
     y_null = prod.y_embedder.y_embedding.detach()[None, None].repeat(B, 1, 1, 1)
     extra = dict(fps=inp["fps"], height=inp["height"], width=inp["width"])

@@ -8,30 +8,14 @@ import numpy as np
 import pytest
 import torch
 
+from tests.models import posterior_inputs, tiny_vae
 from tests.util import load_golden, rel_l2
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _golden(name):
-    return load_golden(name)
-
-
-def _model(G, **kw):
-    from opensora.registry import MODELS, build_module
-
-    m = build_module(dict(type="hunyuan_vae", block_out_channels=(16, 32, 32, 32), layers_per_block=1, norm_num_groups=4,
-                          latent_channels=4, **kw), MODELS, device_map="cpu")
-    m.encoder.load_state_dict({k[4:]: v for k, v in G.items() if k.startswith("enc.")})
-    m.decoder.load_state_dict({k[4:]: v for k, v in G.items() if k.startswith("dec.")})
-    return m
-
 
 def test_encoder_decoder_against_reference_goldens(fake_osb):
     from oracle import vae_oracle as V
 
-    G = _golden("vae_blocks.npz")
-    m = _model(G).to(torch.bfloat16)
+    G = load_golden("vae_blocks.npz")
+    m = tiny_vae(G).to(torch.bfloat16)
     down, up = V.stage_plan(4, 4, 8)
     Wb = {k: v.to(torch.bfloat16) for k, v in G.items()}
     ze_bf = V.encoder({k[4:]: v for k, v in Wb.items() if k.startswith("enc.")}, Wb["enc_x"], groups=4, strides=down)
@@ -51,8 +35,8 @@ def test_encoder_decoder_against_reference_goldens(fake_osb):
 def test_tiled_modes_against_reference_goldens(fake_osb, tag, sp, tp):
     from oracle import vae_oracle as V
 
-    G, GT = _golden("vae_blocks.npz"), _golden("vae_tiled.npz")
-    m = _model(G, sample_size=32, sample_tsize=8, use_spatial_tiling=sp, use_temporal_tiling=tp)
+    G, GT = load_golden("vae_blocks.npz"), load_golden("vae_tiled.npz")
+    m = tiny_vae(G, sample_size=32, sample_tsize=8, use_spatial_tiling=sp, use_temporal_tiling=tp)
     with torch.no_grad():
         m.quant_conv.weight.copy_(GT["quant_w"]); m.quant_conv.bias.copy_(GT["quant_b"])
         m.post_quant_conv.weight.copy_(GT["post_w"]); m.post_quant_conv.bias.copy_(GT["post_b"])
@@ -92,17 +76,6 @@ def test_causal_conv_is_causal_and_latent_size_api(fake_osb):
         z = m.encode(v, sample_posterior=False)
         rec, _, z2 = m(v, sample_posterior=False)
     assert list(z.shape) == [1, 4] + m.get_latent_size([9, 32, 32]) and rec.shape == v.shape and torch.equal(z, z2)
-
-
-def posterior_inputs():
-    """Seeded (parameters, second parameters) pairs: 5-D latent, 4-D image and token-shaped distributions."""
-    g = torch.Generator().manual_seed(5)
-    out = []
-    for shape in ((2, 8, 3, 4, 5), (2, 8, 6, 7), (2, 9, 8)):
-        par = torch.randn(*shape, generator=g) * 3.0
-        par2 = torch.randn(*shape, generator=g)
-        out.append((par, par2))
-    return out
 
 
 def test_posterior_distribution_matches_the_reference_class():
@@ -145,8 +118,8 @@ def _tp_worker(rank, world, port, ret):
         from opensora.acceleration.communications import gather_forward_split_backward_var_len
 
         torch.manual_seed(11)   # the same model on every rank (quant / post_quant convolutions are not in the golden file)
-        G = _golden("vae_blocks.npz")
-        m = _model(G, sample_size=32, sample_tsize=8).to(torch.bfloat16)
+        G = load_golden("vae_blocks.npz")
+        m = tiny_vae(G, sample_size=32, sample_tsize=8).to(torch.bfloat16)
         real_stats, real_combine = fake_osb200.group_stats, U._combine_group_stats
 
         def whole_video_stats(x, groups, eps=1e-6):

@@ -3,98 +3,26 @@
 against the fp32 oracle on the merged weights W + s B A (through the binding stand-in), Ulysses sequence parallelism, unloading, the guards of the models that take no
 adapter, and the C ABI layout of osb_lora_args.  The kernel itself is checked on the GPU (tests/test_lora_gpu.py)."""
 import json
-import math
 import os
 
 import pytest
 import torch
 from torch import nn
 
-from tests.test_mmdit_gpu import CFG, _ids
+from tests.adapters import merged_state, write_adapter
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
-
-
-# ---- adapter files ----------------------------------------------------------------------------------------------------
-def linear_names(model):
-    return [n for n, m in model.named_modules() if type(m) is nn.Linear]
-
-
-def write_adapter(path, model, *, r=8, alpha=16, rel=0.1, seed=0, targets=None, fmt="safetensors", rank_pattern=None,
-                  alpha_pattern=None, **cfg_extra):
-    """A PEFT LoRA adapter directory for `model`: every targeted Linear gets A [r, in], B [out, r] with
-    |scaling B A| = rel |W| (Frobenius), scaling as load_lora computes it for scale 1."""
-    os.makedirs(path, exist_ok=True)
-    targets = linear_names(model) if targets is None else targets
-    cfg = dict(peft_type="LORA", r=r, lora_alpha=alpha, target_modules=targets, lora_dropout=0.05, bias="none",
-               rank_pattern=rank_pattern or {}, alpha_pattern=alpha_pattern or {}, use_rslora=False, use_dora=False,
-               modules_to_save=None, layers_to_transform=None, layers_pattern=None, fan_in_fan_out=False,
-               task_type=None, base_model_name_or_path=None)
-    cfg.update(cfg_extra)
-    from opensora.utils.lora import _pattern_value, _targets
-
-    g = torch.Generator().manual_seed(seed)
-    sd = {}
-    mods = dict(model.named_modules())
-    for name in _targets(model, targets):
-        lin = mods[name]
-        rr = int(_pattern_value(cfg["rank_pattern"], name, r))
-        aa = float(_pattern_value(cfg["alpha_pattern"], name, alpha))
-        s = aa / math.sqrt(rr) if cfg["use_rslora"] else aa / rr
-        A = torch.randn(rr, lin.in_features, generator=g) / math.sqrt(lin.in_features)
-        B = torch.randn(lin.out_features, rr, generator=g)
-        upd = s * B @ A
-        B = B * (rel * lin.weight.detach().float().cpu().norm() / upd.norm().clamp_min(1e-30))
-        sd[f"base_model.model.{name}.lora_A.weight"] = A.contiguous()
-        sd[f"base_model.model.{name}.lora_B.weight"] = B.contiguous()
-    with open(os.path.join(path, "adapter_config.json"), "w") as f:
-        json.dump(cfg, f)
-    if fmt == "safetensors":
-        from safetensors.torch import save_file
-
-        save_file(sd, os.path.join(path, "adapter_model.safetensors"))
-    else:
-        torch.save(sd, os.path.join(path, "adapter_model.bin"))
-    return path
-
-
-def merged_state(model):
-    """fp32 state dict of the plain model with every adapter merged: W + scaling * B A."""
-    from opensora.utils.lora import adapter_of, is_wrapped
-
-    W = {k.replace(".base_layer.", "."): v.float() for k, v in model.state_dict().items() if ".lora_" not in k}
-    with torch.no_grad():
-        for name, m in model.named_modules():
-            if is_wrapped(m):
-                A, B, s = adapter_of(m)
-                W[f"{name}.weight"] = W[f"{name}.weight"] + s * (B.float() @ A.float())
-    return W
-
-
-def _rand_model(fused=True, liger=False):
-    from tests.test_host_mmdit_cpu import _rand_model as rm
-
-    return rm(fused, liger)
-
-
-def _inputs(B=2, Lt=24, thw=(2, 4, 6), seed=3):
-    T, H, W = thw
-    g = torch.Generator().manual_seed(seed)
-    rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-    txt_ids, img_ids = _ids(B, Lt, T, H, W)
-    return dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids,
-                timesteps=torch.linspace(0.3, 0.8, B), y_vec=rb(B, 96), cond=rb(B, T * H * W, 68),
-                guidance=torch.full((B,), 4.0))
 
 
 # ---- config and format -----------------------------------------------------------------------------------------------
 def test_target_modules_list_and_regex(tmp_path):
     from opensora.utils.lora import LoraLinear, load_lora, unload_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     write_adapter(tmp_path / "list", m, targets=["qkv", "img_in", "adaLN_modulation.1"])
     load_lora(m, str(tmp_path / "list"))
     wrapped = sorted(n for n, x in m.named_modules() if isinstance(x, LoraLinear))
-    want = sorted([f"double_blocks.{i}.{s}_attn.qkv" for i in range(CFG["depth"]) for s in ("img", "txt")]
+    want = sorted([f"double_blocks.{i}.{s}_attn.qkv" for i in range(MMDIT_CFG["depth"]) for s in ("img", "txt")]
                   + ["img_in", "final_layer.adaLN_modulation.1"])
     assert wrapped == want
     unload_lora(m)
@@ -111,7 +39,7 @@ def test_target_modules_list_and_regex(tmp_path):
 def test_rank_alpha_patterns_rslora_and_scale(tmp_path):
     from opensora.utils.lora import load_lora, unload_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     write_adapter(tmp_path / "a", m, r=8, alpha=16, targets=["qkv", "proj", "linear2"], rank_pattern={"proj": 16},
                   alpha_pattern={r"single_blocks\.1\.linear2": 4})
     load_lora(m, str(tmp_path / "a"), scale=0.5)
@@ -129,7 +57,7 @@ def test_rank_alpha_patterns_rslora_and_scale(tmp_path):
 def test_bin_format_loads_like_safetensors(tmp_path):
     from opensora.utils.lora import adapter_of, load_lora
 
-    m1, m2 = _rand_model(), _rand_model()
+    m1, m2 = mmdit_model(), mmdit_model()
     write_adapter(tmp_path / "st", m1, targets=["linear1"], seed=4)
     write_adapter(tmp_path / "bin", m2, targets=["linear1"], seed=4, fmt="bin")
     load_lora(m1, str(tmp_path / "st"))
@@ -146,7 +74,7 @@ def test_bin_format_loads_like_safetensors(tmp_path):
 def test_config_refusals(tmp_path, change, match):
     from opensora.utils.lora import load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     write_adapter(tmp_path, m, targets=["qkv"], **change)
     with pytest.raises(ValueError, match=match):
         load_lora(m, str(tmp_path))
@@ -157,7 +85,7 @@ def test_target_and_tensor_refusals(tmp_path):
 
     from opensora.utils.lora import load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     # targets: an entry that matches nothing, a regex that matches nothing, a module that is not an nn.Linear
     for i, (tgt, match) in enumerate(((["qkv", "nope"], "'nope' matches no module"), ("nope.*", "matches no module"),
                                       (["img_norm1"], "not an nn.Linear"))):
@@ -187,7 +115,7 @@ def test_one_adapter_at_a_time_and_mmdit_only(tmp_path):
     from opensora.models.stdit.stdit3 import STDiT3_XS_2
     from opensora.utils.lora import load_lora
 
-    m = _rand_model()
+    m = mmdit_model()
     write_adapter(tmp_path, m, targets=["qkv"])
     load_lora(m, str(tmp_path))
     with pytest.raises(ValueError, match="already carries"):
@@ -204,14 +132,14 @@ def test_mmdit_adapter_on_every_linear_vs_oracle_on_merged_weights(fake_osb, tmp
     from oracle import mmdit_oracle as M
     from opensora.utils.lora import load_lora
 
-    m = _rand_model(fused, liger)
-    inp = _inputs()
+    m = mmdit_model(fused, liger)
+    inp = mmdit_inputs()
     with torch.no_grad():
         base = m(**inp)
         load_lora(m, str(write_adapter(tmp_path, m, r=12, alpha=24, rel=0.1, seed=9)))
         fake_osb.reset()
         out = m(**inp)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
     W32 = merged_state(m)
     finp = {k: (v.float() if v.is_floating_point() else v) for k, v in inp.items()}
     ref = M.model_forward(W32, cfg, finp["img"], finp["img_ids"], finp["txt"], finp["txt_ids"], finp["timesteps"],
@@ -225,8 +153,8 @@ def test_mmdit_adapter_on_every_linear_vs_oracle_on_merged_weights(fake_osb, tmp
     assert rel_l2(out, base) > 10 * r, "the adapter must move the output well beyond the error"
     # every token-row Linear runs on the fused kernel; the modulation stays one grouped GEMM plus one down GEMM
     names = [c[0] for c in fake_osb.calls]
-    nd, ns = CFG["depth"], CFG["depth_single_blocks"]
-    C = CFG["hidden_size"]
+    nd, ns = MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
+    C = MMDIT_CFG["hidden_size"]
     mod_width = (2 * nd * 6 + ns * 3) * C
     assert sum(1 for c in fake_osb.calls if c[0] == "gemm" and c[1][1] == mod_width) == 1
     assert sum(1 for c in fake_osb.calls if c[0] == "gemm" and c[1][1] in (6 * C, 3 * C) and c[1][0] == 2) == 2 * nd + ns
@@ -240,8 +168,8 @@ def test_mmdit_adapter_on_every_linear_vs_oracle_on_merged_weights(fake_osb, tmp
 def test_unload_restores_outputs_and_launches(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora, unload_lora
 
-    plain, m = _rand_model(False, True), _rand_model(False, True)
-    inp = _inputs()
+    plain, m = mmdit_model(False, True), mmdit_model(False, True)
+    inp = mmdit_inputs()
     with torch.no_grad():
         fake_osb.reset()
         want = plain(**inp)
@@ -292,13 +220,13 @@ def test_grouped_modulation_adds_each_layer_update_into_its_slice(fake_osb, tmp_
     serves every adapted layer, and each layer's update is one small GEMM added into its own slice (no block-diagonal B)."""
     from opensora.utils.lora import load_lora
 
-    m = _rand_model()
-    inp = _inputs(B=1)
+    m = mmdit_model()
+    inp = mmdit_inputs(B=1)
     load_lora(m, str(write_adapter(tmp_path, m, targets=r".*(img_mod|modulation)\.lin", r=8, rel=0.5)))
     with torch.no_grad():
         fake_osb.reset()
         m(**inp)
-    C, nd, ns = CFG["hidden_size"], CFG["depth"], CFG["depth_single_blocks"]
+    C, nd, ns = MMDIT_CFG["hidden_size"], MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
     rows1 = [c[1] for c in fake_osb.calls if c[0] == "gemm" and c[1][0] == 1]
     assert sum(1 for c in rows1 if c[1] == (2 * nd * 6 + ns * 3) * C) == 1
     assert sum(1 for c in rows1 if c[1] == (nd + ns) * 8 and c[2] == C) == 1                       # the shared down GEMM
@@ -321,9 +249,9 @@ def _lora_sp_worker(rank, world, port, adapter_dirs, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for (fused, liger, (B, Lt, thw)), d in zip(SP_CASES, adapter_dirs):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             load_lora(m, d)
-            inp = _inputs(B, Lt, thw)
+            inp = mmdit_inputs(B, Lt, thw)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)
@@ -347,7 +275,7 @@ def test_mmdit_ulysses_with_adapter_world2(tmp_path):
 
     dirs = []
     for i, (fused, liger, _) in enumerate(SP_CASES):
-        dirs.append(str(write_adapter(tmp_path / f"a{i}", _rand_model(fused, liger), seed=i)))
+        dirs.append(str(write_adapter(tmp_path / f"a{i}", mmdit_model(fused, liger), seed=i)))
     port = 29500 + (os.getpid() + 17) % 2000
     mgr = mp.Manager()
     ret = mgr.dict()

@@ -149,20 +149,20 @@ def test_mmdit_with_adapter_vs_fp32_oracle_on_merged_weights(tmp_path):
         pytest.skip("no CUDA device")
     from oracle import mmdit_oracle as M
     from opensora.utils.lora import load_lora, unload_lora
-    from tests.test_lora_cpu import merged_state, write_adapter
-    from tests.test_mmdit_gpu import CFG, _ids, _rand_model
+    from tests.adapters import merged_state, write_adapter
+    from tests.models import MMDIT_CFG, mmdit_ids, mmdit_model
 
     results = {}
     for fused, liger in ((True, False), (False, True)):
-        m = _rand_model(fused, liger)
+        m = mmdit_model(fused, liger, device="cuda")
         B, Lt, (T, H, W) = 2, 40, (3, 6, 8)
         g = torch.Generator().manual_seed(3)
         rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-        txt_ids, img_ids = _ids(B, Lt, T, H, W)
+        txt_ids, img_ids = mmdit_ids(B, Lt, T, H, W)
         inp = dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids,
                    timesteps=torch.tensor([0.3, 0.8]), y_vec=rb(B, 96), cond=rb(B, T * H * W, 68),
                    guidance=torch.tensor([4.0, 7.5]))
-        cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
+        cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
         finp = {k: (v.float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
         dinp = {k: v.cuda() for k, v in inp.items()}
 

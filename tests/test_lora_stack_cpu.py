@@ -13,57 +13,9 @@ from tests import mmdit_fp8_lora_ref as LR
 from tests import mmdit_fp8_proj_ref as PR
 from tests import mmdit_fp8_ref as MR
 from tests import fp8_ref as R
-from tests.test_dora_cpu import write_dora_adapter
-from tests.test_lora_cpu import _inputs, _rand_model, linear_names, write_adapter
-from tests.test_mmdit_gpu import CFG
+from tests.adapters import load_stack, stack_registry, stacked_state, write_stack
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
-
-
-def write_stack(tmp_path, model, kinds, targets=None, **kw):
-    """One adapter directory per entry of `kinds` ("lora" / "dora"), all written from the plain `model` with their own
-    seeds; returns the paths."""
-    targets = linear_names(model) if targets is None else targets
-    paths = []
-    for i, kind in enumerate(kinds):
-        path = tmp_path / f"{kind}{i}"
-        args = dict(dict(r=8 + 4 * i, alpha=16, rel=0.1, seed=20 + i, targets=targets), **kw)
-        if kind == "dora":
-            write_dora_adapter(path, model, mag_seed=30 + i, **args)
-        else:
-            write_adapter(path, model, **args)
-        paths.append(str(path))
-    return paths
-
-
-def load_stack(model, paths, names, weights=None):
-    from opensora.utils.lora import load_lora, set_adapters
-
-    for p, n in zip(paths, names):
-        load_lora(model, p, adapter_name=n)
-    return set_adapters(model, names, weights)
-
-
-def stacked_state(model, names, weights):
-    """fp32 state dict of the plain model with the adapters `names` (in that order, with `weights`) merged by peft's
-    recursion, read from each layer's own lora_A / lora_B / scaling / magnitude tensors."""
-    from opensora.utils.lora import is_wrapped
-
-    W = {k.replace(".base_layer.", "."): v.float() for k, v in model.state_dict().items() if ".lora_" not in k}
-    with torch.no_grad():
-        for name, m in model.named_modules():
-            if not is_wrapped(m):
-                continue
-            W0 = m.weight.float()
-            w = W0
-            for n, wt in zip(names, weights):
-                if n not in m.lora_A:
-                    continue
-                upd = m.scaling[n] * wt * (m.lora_B[n].weight.float() @ m.lora_A[n].weight.float())
-                w = w + upd
-                if m.use_dora[n]:
-                    w = (m.lora_magnitude_vector[n].weight.float() / (W0 + upd).norm(dim=1))[:, None] * w
-            W[f"{name}.weight"] = w
-    return W
 
 
 def _oracle(W32, cfg, inp):
@@ -100,10 +52,10 @@ def test_stack_on_every_linear_vs_oracle_on_merged_weights(fake_osb, tmp_path, f
     """tests/test_lora_cpu.py's inputs and bars.  "dora_dora_lora" is "lora_dora_dora" reversed (the same three adapter
     directories, their weights reversed with them): each order matches its own oracle and is far from the other's."""
     kinds, weights = STACKS[stack]
-    m = _rand_model(fused, liger)
-    inp = _inputs()
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
-    paths = write_stack(tmp_path, _rand_model(fused, liger), ("lora", "dora", "dora") if "dora" in stack else kinds,
+    m = mmdit_model(fused, liger)
+    inp = mmdit_inputs()
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
+    paths = write_stack(tmp_path, mmdit_model(fused, liger), ("lora", "dora", "dora") if "dora" in stack else kinds,
                         rel=0.3 if "dora" in stack else 0.1)
     names = ["a", "b", "c"][:len(paths)]
     if stack == "dora_dora_lora":
@@ -138,12 +90,12 @@ def test_reductions_are_bit_identical_with_the_same_launches(fake_osb, tmp_path,
     `set_adapters([])` those of the plain model, `unload_lora("b")` those of loading only a."""
     from opensora.utils.lora import load_lora, set_adapters, unload_lora
 
-    inp = _inputs()
-    pa, pb = write_stack(tmp_path, _rand_model(fused, liger), ("lora", "dora"))
-    only_a = load_lora(_rand_model(fused, liger), pa)
+    inp = mmdit_inputs()
+    pa, pb = write_stack(tmp_path, mmdit_model(fused, liger), ("lora", "dora"))
+    only_a = load_lora(mmdit_model(fused, liger), pa)
     want_a = _run(fake_osb, only_a, inp)
-    want_plain = _run(fake_osb, _rand_model(fused, liger), inp)
-    m = _rand_model(fused, liger)
+    want_plain = _run(fake_osb, mmdit_model(fused, liger), inp)
+    m = mmdit_model(fused, liger)
     load_lora(m, pa)
     load_lora(m, pb, adapter_name="b")
     both = _run(fake_osb, m, inp)
@@ -166,9 +118,9 @@ def _equal_runs(got, want):
 def test_unload_by_name_restores_linears_left_without_adapters(fake_osb, tmp_path):
     from opensora.utils.lora import LoraLinear, active_adapters, load_lora, unload_lora
 
-    m = _rand_model()
-    pa, pb = write_stack(tmp_path, _rand_model(), ("lora", "lora"), targets=["qkv", "linear1"])
-    pc, = write_stack(tmp_path / "c", _rand_model(), ("dora",), targets=["qkv", "img_in"])
+    m = mmdit_model()
+    pa, pb = write_stack(tmp_path, mmdit_model(), ("lora", "lora"), targets=["qkv", "linear1"])
+    pc, = write_stack(tmp_path / "c", mmdit_model(), ("dora",), targets=["qkv", "img_in"])
     load_lora(m, pa, adapter_name="a")
     load_lora(m, pc, adapter_name="c")
     load_lora(m, pb, adapter_name="b")
@@ -188,16 +140,16 @@ def test_unload_by_name_restores_linears_left_without_adapters(fake_osb, tmp_pat
 def test_stack_adds_no_launch_over_one_adapter(fake_osb, tmp_path, kinds):
     """The same Linears with one adapter (of the stack's last kind, so that DoRA's modulation rule is the same) and with
     the stack: the same launch list, only the rank widths of the down GEMMs and updates differ (K = sum of the ranks)."""
-    m1, m2 = _rand_model(False, True), _rand_model(False, True)
-    inp = _inputs()
-    paths = write_stack(tmp_path, _rand_model(False, True), kinds)
+    m1, m2 = mmdit_model(False, True), mmdit_model(False, True)
+    inp = mmdit_inputs()
+    paths = write_stack(tmp_path, mmdit_model(False, True), kinds)
     load_stack(m1, paths[-1:], ["x"])
     load_stack(m2, paths, ["a", "b", "c"][:len(paths)])
     _, one, n1 = _run(fake_osb, m1, inp)
     _, stack, n2 = _run(fake_osb, m2, inp)
     assert [c[0] for c in stack] == [c[0] for c in one] and n1 == n2 == len(one)
     ranks = sum(-(-(8 + 4 * i) // 8) * 8 for i in range(len(kinds)))
-    C = CFG["hidden_size"]
+    C = MMDIT_CFG["hidden_size"]
     # the first double block's image q|k|v down GEMM: [B * Li, C] x [R, C]
     downs = [c for c in stack if c[0] == "gemm" and c[1][2] == C and c[1][1] == ranks]
     assert downs, "no down GEMM with K = sum of the ranks"
@@ -292,63 +244,36 @@ def test_weights_scale_inside_the_dora_norm(fake_osb, tmp_path):
     from opensora.models.mmdit.layers import linear_parts
     from opensora.utils.lora import load_lora, set_adapters
 
-    p, = write_stack(tmp_path, _rand_model(), ("dora",), targets=["img_in", "linear2"])
-    a, b = _rand_model(), _rand_model()
+    p, = write_stack(tmp_path, mmdit_model(), ("dora",), targets=["img_in", "linear2"])
+    a, b = mmdit_model(), mmdit_model()
     load_lora(a, p, scale=0.5)
     load_lora(b, p)
     set_adapters(b, ["default"], [0.5])
     for la, lb in ((a.img_in, b.img_in), (a.single_blocks[0].linear2, b.single_blocks[0].linear2)):
         pa, pb = linear_parts(la)[2], linear_parts(lb)[2]
         assert all(torch.equal(x, y) for x, y in zip(pa, pb))
-    inp = _inputs(B=1)
+    inp = mmdit_inputs(B=1)
     assert torch.equal(_forward(a, inp), _forward(b, inp))
 
 
 # ---- FP8 ---------------------------------------------------------------------------------------------------------------
-def _stack_registry(model):
-    """tests/mmdit_fp8_lora_ref.py's registry for stacks: per adapted Linear the unrolled form of the recursion,
-    A_cat = the A_k one after another, bf16(c_k s_k B_k) side by side and G, c_k = 1 / the product of the g_j of the DoRA
-    adapters before k, G = the product of all of them."""
-    from opensora.utils.lora import adapters_of, is_wrapped
-
-    rows, ads = {}, []
-    with torch.no_grad():
-        for _, m in model.named_modules():
-            stack = adapters_of(m) if is_wrapped(m) else []
-            if not stack:
-                continue
-            W = m.weight.float()
-            G = torch.ones(W.shape[0], device=W.device)
-            As, Bs = [], []
-            for ad in stack:
-                upd = ad.scaling * (ad.B.float() @ ad.A.float())
-                As.append(ad.A.float())
-                Bs.append(((ad.scaling / G)[:, None] * ad.B.float()).to(torch.bfloat16).float())
-                if ad.magnitude is not None:
-                    G = G * ad.magnitude.float() / (W + upd).norm(dim=1)
-            ads.append((torch.cat(As), torch.cat(Bs, 1), G))
-            for i, k in enumerate(LR._row_keys(m.weight)):
-                rows[k] = (len(ads) - 1, i)
-    return rows, ads
-
-
 @pytest.mark.parametrize("fused,liger,proj", [(True, False, True), (False, True, False)])
 def test_fp8_lora_stack_follows_the_emulation(fake_osb, tmp_path, fused, liger, proj):
     """tests/test_mmdit_fp8_lora_cpu.py's inputs and bar: a LoRA, DoRA, LoRA stack on every FP8 Linear, against the
     fp32 oracle on the recursively merged weights; yardstick: the FP8 emulation with the stack."""
-    m = _rand_model(fused, liger)
-    inp = _inputs()
+    m = mmdit_model(fused, liger)
+    inp = mmdit_inputs()
     m.enable_fp8(projections=proj, lora=True)
     base = _forward(m, inp)
     targets = m.fp8_mlp_linears() + (m.fp8_proj_linears() if proj else [])
     names, weights = ["a", "b", "c"], (1.0, 0.8, 1.25)
-    load_stack(m, write_stack(tmp_path, _rand_model(fused, liger), ("lora", "dora", "lora"), targets=targets, rel=0.3),
+    load_stack(m, write_stack(tmp_path, mmdit_model(fused, liger), ("lora", "dora", "lora"), targets=targets, rel=0.3),
                names, weights)
     fake_osb.reset()
     out = _forward(m, inp)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
     ref = _oracle(stacked_state(m, names, weights), cfg, inp)
-    rows, ads = _stack_registry(m)
+    rows, ads = stack_registry(m)
     saved = MR._lin
     MR._lin = LR._lin_with(rows, ads, saved)
     try:
@@ -369,11 +294,11 @@ def test_fp8_lora_stack_follows_the_emulation(fake_osb, tmp_path, fused, liger, 
 
 def test_stacked_a_cat_quantizes_each_adapter_row_alone(fake_osb, tmp_path):
     """The e4m3 A_cat of a stack is the per-row quantization of each adapter's A, rank-padded, one after another."""
-    m = _rand_model(True, False)
+    m = mmdit_model(True, False)
     m.enable_fp8(lora=True)
-    load_stack(m, write_stack(tmp_path, _rand_model(True, False), ("lora", "dora"),
+    load_stack(m, write_stack(tmp_path, mmdit_model(True, False), ("lora", "dora"),
                               targets=["double_blocks.0.img_mlp.0"]), ["a", "b"])
-    _forward(m, _inputs(B=1))
+    _forward(m, mmdit_inputs(B=1))
     (A, q, s), = [v for v in m._fp8_state._la.values()]
     lin = m.double_blocks[0].img_mlp[0]
     want = torch.zeros(8 + 16, A.shape[1])
@@ -386,9 +311,9 @@ def test_stacked_a_cat_quantizes_each_adapter_row_alone(fake_osb, tmp_path):
 def test_refusals(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora, set_adapters, unload_lora
 
-    m = _rand_model()
-    pa, = write_stack(tmp_path / "a", _rand_model(), ("lora",), targets=["qkv"])
-    pb, = write_stack(tmp_path / "b", _rand_model(), ("dora",), targets=["qkv", "double_blocks.0.img_mlp.0"])
+    m = mmdit_model()
+    pa, = write_stack(tmp_path / "a", mmdit_model(), ("lora",), targets=["qkv"])
+    pb, = write_stack(tmp_path / "b", mmdit_model(), ("dora",), targets=["qkv", "double_blocks.0.img_mlp.0"])
     load_lora(m, pa, adapter_name="a")
     with pytest.raises(ValueError, match="already carries a LoRA adapter named 'a'"):
         load_lora(m, pb, adapter_name="a")
@@ -406,13 +331,13 @@ def test_refusals(fake_osb, tmp_path):
     m.enable_fp8(projections=False)
     with pytest.raises(ValueError, match="FP8 MLPs, which take no LoRA"):
         set_adapters(m, ["a", "b"])
-    n = _rand_model()
+    n = mmdit_model()
     n.enable_fp8(projections=True)
     with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
         load_lora(n, pa, adapter_name="a")
     n.enable_fp8(projections=True, lora=True)
     load_stack(n, [pa, pb], ["a", "b"])
-    assert torch.isfinite(_forward(n, _inputs(B=1)).float()).all()
+    assert torch.isfinite(_forward(n, mmdit_inputs(B=1)).float()).all()
 
 
 # ---- sequence parallelism ----------------------------------------------------------------------------------------------
@@ -433,9 +358,9 @@ def _sp_worker(rank, world, port, paths, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for (fused, liger, (B, Lt, thw)), ps in zip(SP_CASES, paths):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             load_stack(m, ps, ["a", "b", "c"], (1.0, 0.8, 1.25))
-            inp = _inputs(B, Lt, thw)
+            inp = mmdit_inputs(B, Lt, thw)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)
@@ -454,7 +379,7 @@ def test_mmdit_ulysses_with_a_stack_world2(tmp_path):
     bit (the stand-in accumulating in fp64)."""
     import torch.multiprocessing as mp
 
-    paths = [write_stack(tmp_path / f"c{i}", _rand_model(fused, liger), ("lora", "dora", "lora"))
+    paths = [write_stack(tmp_path / f"c{i}", mmdit_model(fused, liger), ("lora", "dora", "lora"))
              for i, (fused, liger, _) in enumerate(SP_CASES)]
     port = 29500 + (os.getpid() + 53) % 2000
     ret = mp.Manager().dict()
@@ -470,14 +395,14 @@ def test_prepare_models_stacks_a_list_of_adapters(fake_osb, tmp_path):
     from opensora.utils.lora import active_adapters
     from tests import sampling_toys as T
 
-    pa, pb = write_stack(tmp_path, _rand_model(), ("lora", "dora"))
-    inp = _inputs(B=1)
-    want = load_stack(_rand_model(), [pa, pb], ["default", "adapter_1"], (1.0, 0.7))
-    cfg = dict(model=_rand_model(), ae=T.ToyAE(causal=True), t5=nn.Identity(), clip=nn.Identity(),
+    pa, pb = write_stack(tmp_path, mmdit_model(), ("lora", "dora"))
+    inp = mmdit_inputs(B=1)
+    want = load_stack(mmdit_model(), [pa, pb], ["default", "adapter_1"], (1.0, 0.7))
+    cfg = dict(model=mmdit_model(), ae=T.ToyAE(causal=True), t5=nn.Identity(), clip=nn.Identity(),
                pretrained_lora_path=[pa, (pb, 0.7)])
     m = S.prepare_models(cfg, "cpu", torch.bfloat16)[0]
     assert active_adapters(m) == ["default", "adapter_1"]
     assert m.img_in.adapter_weight == {"default": 1.0, "adapter_1": 0.7}
     assert torch.equal(_forward(m, inp), _forward(want, inp))
-    one = S.prepare_models(dict(cfg, model=_rand_model(), pretrained_lora_path=pa), "cpu", torch.bfloat16)[0]
+    one = S.prepare_models(dict(cfg, model=mmdit_model(), pretrained_lora_path=pa), "cpu", torch.bfloat16)[0]
     assert active_adapters(one) == ["default"]

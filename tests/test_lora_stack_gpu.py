@@ -8,7 +8,8 @@ import torch
 from tests import mmdit_fp8_lora_ref as LR
 from tests import mmdit_fp8_proj_ref as PR
 from tests import mmdit_fp8_ref as MR
-from tests.test_lora_stack_cpu import _stack_registry, load_stack, stacked_state, write_stack
+from tests.adapters import load_stack, stack_registry, stacked_state, write_stack
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -35,13 +36,9 @@ def _oracle(W32, cfg, inp):
 
 
 def _small(fused, liger):
-    from tests.test_lora_cpu import _rand_model
-    from tests.test_mmdit_fp8_gpu import _inputs
-    from tests.test_mmdit_gpu import CFG
-
-    m = _rand_model(fused, liger).cuda()
-    inp = {k: v.cuda() for k, v in _inputs(2, 40, (3, 6, 8)).items()}
-    return m, dict(CFG, fused_qkv=fused, use_liger_rope=liger), inp
+    m = mmdit_model(fused, liger).cuda()
+    inp = {k: v.cuda() for k, v in mmdit_inputs(2, 40, (3, 6, 8), guidance=[4.0, 7.5]).items()}
+    return m, dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger), inp
 
 
 @pytest.mark.parametrize("fused,liger", [(True, False), (False, True)])
@@ -74,7 +71,7 @@ def test_small_mmdit_fp8_stack_against_the_oracle(tmp_path, fused, liger, attn):
     with torch.no_grad():
         out = m(**inp)
     ref = _oracle(stacked_state(m, NAMES, WEIGHTS), cfg, inp)
-    rows, ads = _stack_registry(m)
+    rows, ads = stack_registry(m)
     saved = MR._lin
     MR._lin = LR._lin_with(rows, ads, saved)
     try:

@@ -12,29 +12,12 @@ from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_ref as MR
-from tests.test_host_mmdit_cpu import _rand_model
-from tests.test_lora_cpu import _inputs, write_adapter
-from tests.test_mmdit_gpu import CFG
+from tests.adapters import write_adapter
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E4M3 = torch.float8_e4m3fn
-
-
-def _operands(B, L, H, seed=0, split=None, liger=True):
-    g = torch.Generator().manual_seed(seed)
-    C = H * 128
-    qkv = (torch.randn(B * L, 3 * C, generator=g) * 2).to(torch.bfloat16)
-    qkv[3, 2 * C:2 * C + 5] = 40.0                      # a v column with one large entry
-    qkv[:, 2 * C + 7] = 0.0                             # an all-zero v column: scale 1, codes 0
-    w = [(1 + 0.3 * torch.randn(128, generator=g)).to(torch.bfloat16) for _ in range(4)]
-    ang = torch.randn(L, 64, generator=g)
-    kw = dict(num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H,
-              head_dim=128, q_norm_w=w[0], k_norm_w=w[1], rope_cos=torch.cos(ang), rope_sin=torch.sin(ang),
-              rope_half=liger, q_norm_w2=None, k_norm_w2=None, norm_split=0)
-    if split is not None:
-        kw.update(q_norm_w2=w[2], k_norm_w2=w[3], norm_split=split)
-    return qkv, kw
 
 
 # The S accumulator of a wgmma m64nNk32 holds, in thread (lane % 4 = t), the columns 8 j + 2 t + e of its rows; the FP8
@@ -59,7 +42,7 @@ def test_vt8_permutation_is_the_accumulator_order():
 @pytest.mark.parametrize("liger,split", [(True, 50), (False, None)])
 def test_stand_in_matches_the_contract(fake_osb, liger, split):
     B, L, H = 2, 200, 2
-    qkv, kw = _operands(B, L, H, split=split, liger=liger)
+    qkv, kw = AR.operands_cpu(B, L, H, split=split, liger=liger)
     C = H * 128
     ws = fake_osb.attn_fp8_workspace(B, L, H, "cpu")
     out = torch.zeros(B * L, C, dtype=torch.bfloat16)
@@ -93,7 +76,7 @@ def test_stand_in_matches_the_contract(fake_osb, liger, split):
 
 
 def test_stand_in_refusals(fake_osb):
-    qkv, kw = _operands(1, 64, 2)
+    qkv, kw = AR.operands_cpu(1, 64, 2)
     q, k, v = qkv[:, :256], qkv[:, 256:512], qkv[:, 512:]
     out = torch.empty(64, 256, dtype=torch.bfloat16)
     ws = fake_osb.attn_fp8_workspace(1, 64, 2, "cpu")
@@ -111,7 +94,7 @@ def _case(model, inp, mlps=False):
 
     from oracle import mmdit_oracle as M
 
-    cfg = dict(CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
+    cfg = dict(MMDIT_CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
     with torch.no_grad():
         out = model(**inp)
     W32 = {k: v.float() for k, v in model.state_dict().items()}
@@ -131,7 +114,7 @@ def _case(model, inp, mlps=False):
 def test_host_mmdit_fp8_attention_follows_the_emulation(fake_osb, fused, liger, mlps):
     """C = 256 (2 heads of 128), 2 double + 2 single blocks, FP8 attention (and FP8 MLPs) on the stand-in, against the
     fp32 oracle.  Yardstick: the emulation reference measured in the same test."""
-    m = _rand_model(fused, liger)
+    m = mmdit_model(fused, liger)
     if mlps and fused:   # the two modes compose in either order
         m.enable_fp8_attention()
         m.enable_fp8()
@@ -140,20 +123,20 @@ def test_host_mmdit_fp8_attention_follows_the_emulation(fake_osb, fused, liger, 
         m.enable_fp8_attention()
     else:
         m.enable_fp8_attention()
-    out, emu, floor, ref = _case(m, _inputs(), mlps)
+    out, emu, floor, ref = _case(m, mmdit_inputs(), mlps)
     r_out, r_emu, r_bf = rel_l2(out, ref), rel_l2(emu, ref), rel_l2(floor, ref)
     print(f"[mmdit fp8 attn host] fused={fused} liger={liger} mlps={mlps}: product {r_out:.3e}, FP8 emulation "
           f"{r_emu:.3e}, bf16 oracle {r_bf:.3e} (rel-L2 against the fp32 oracle)")
     assert r_out < 1.1 * r_emu, (r_out, r_emu, r_bf)
     names = [c[0] for c in fake_osb.calls]
-    nd, ns = CFG["depth"], CFG["depth_single_blocks"]
+    nd, ns = MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
     assert names.count("attn_fp8") == nd + ns and "attn_short" not in names
     assert (names.count("gemm_fp8_blocks") > 0) == mlps
 
 
 def test_disable_fp8_attention_restores_the_bf16_bits(fake_osb):
-    m, plain = _rand_model(False, True), _rand_model(False, True)
-    inp = _inputs(B=1)
+    m, plain = mmdit_model(False, True), mmdit_model(False, True)
+    inp = mmdit_inputs(B=1)
     with torch.no_grad():
         want = plain(**inp)
         plain_calls = list(fake_osb.calls)
@@ -171,9 +154,9 @@ def test_disable_fp8_attention_restores_the_bf16_bits(fake_osb):
 def test_lora_adapter_applies_with_fp8_attention(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora
 
-    m = _rand_model(True)
+    m = mmdit_model(True)
     m.enable_fp8_attention()
-    inp = _inputs(B=1)
+    inp = mmdit_inputs(B=1)
     with torch.no_grad():
         base = m(**inp)
         load_lora(m, write_adapter(str(tmp_path / "a"), m, targets=["double_blocks.0.img_attn.qkv",
@@ -188,7 +171,7 @@ def test_lora_adapter_applies_with_fp8_attention(fake_osb, tmp_path):
 def test_fp8_attention_refuses_other_head_sizes():
     from opensora.models.mmdit.model import MMDiTConfig, MMDiTModel
 
-    cfg = dict(CFG, hidden_size=256, num_heads=4, axes_dim=[16, 24, 24], depth=1, depth_single_blocks=1)
+    cfg = dict(MMDIT_CFG, hidden_size=256, num_heads=4, axes_dim=[16, 24, 24], depth=1, depth_single_blocks=1)
     with torch.device("meta"):
         m = MMDiTModel(MMDiTConfig(from_pretrained=None, cache_dir=None, **cfg))
     with pytest.raises(ValueError, match="head size of 128"):
@@ -210,9 +193,9 @@ def _sp_worker(rank, world, port, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for fused, liger in ((True, False), (False, True)):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             m.enable_fp8_attention()
-            inp = _inputs(B=2)
+            inp = mmdit_inputs(B=2)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)

@@ -7,8 +7,7 @@ import torch
 from tests import fake_osb200 as F_
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_ref as MR
-from tests.test_mmdit_fp8_gpu import _inputs, _wide_model
-from tests.test_mmdit_gpu import CFG, _rand_model
+from tests.models import MMDIT_CFG, MMDIT_WIDE, mmdit_inputs, mmdit_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -18,20 +17,6 @@ pytestmark = pytest.mark.gpu
 def _cuda():
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
-
-
-def _operands(B, L, H, liger, split, seed=0, wscale=0.3, wmean=1.0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    C = H * 128
-    qkv = (torch.randn(B * L, 3 * C, device="cuda", generator=g) * 2).to(torch.bfloat16)
-    w = [(wmean + wscale * torch.randn(128, device="cuda", generator=g)).to(torch.bfloat16) for _ in range(4)]
-    ang = torch.rand(L, 64, device="cuda", generator=g) * 6.28
-    kw = dict(num_seqs=B, seqs_per_batch=1, q_strides=(L, 0, 1), k_strides=(L, 0, 1), Lq=L, Lk=L, num_heads=H,
-              head_dim=128, q_norm_w=w[0], k_norm_w=w[1], rope_cos=torch.cos(ang), rope_sin=torch.sin(ang),
-              rope_half=liger, q_norm_w2=None, k_norm_w2=None, norm_split=0)
-    if split is not None:
-        kw.update(q_norm_w2=w[2], k_norm_w2=w[3], norm_split=split)
-    return qkv, kw
 
 
 def _run(qkv, kw):
@@ -48,7 +33,7 @@ def _run(qkv, kw):
 
 @pytest.mark.parametrize("B,L,H,liger,split", [(1, 77, 4, True, 20), (2, 1000, 8, False, 300), (3, 2560, 6, True, 256)])
 def test_prep_matches_the_stand_in(B, L, H, liger, split):
-    qkv, kw = _operands(B, L, H, liger, split)
+    qkv, kw = AR.operands_cuda(B, L, H, liger, split)
     ws, _ = _run(qkv, kw)
     C = H * 128
     skip = ("seqs_per_batch", "Lq", "Lk", "num_heads", "head_dim")
@@ -101,7 +86,7 @@ def _check_kernel(qkv, kw, heads=6, bar=None):
 @pytest.mark.parametrize("B,L,H,liger,split", [(1, 1, 2, True, None), (3, 77, 4, False, 20), (2, 1000, 8, True, 300),
                                                (1, 2560, 24, False, 256), (3, 8828, 24, True, 512)])
 def test_kernel_against_fp32_on_the_workspace_operands(B, L, H, liger, split):
-    _check_kernel(*_operands(B, L, H, liger, split))
+    _check_kernel(*AR.operands_cuda(B, L, H, liger, split))
 
 
 def test_rows_whose_probabilities_underflow_stay_finite():
@@ -109,12 +94,12 @@ def test_rows_whose_probabilities_underflow_stay_finite():
     must stay finite.  The bar is looser than the emulation ratio here: the emulation sums q8 k8 in fp32, while the FP8
     tensor core sums the 128 products with fewer mantissa bits, and at |S| ~ 10^4 that difference moves scores by whole
     log2 units (measured: kernel 1.5e-2, P-emulation 2.3e-4 on an H100)."""
-    qkv, kw = _operands(2, 700, 2, True, 100, wscale=10.0, wmean=40.0)
+    qkv, kw = AR.operands_cuda(2, 700, 2, True, 100, wscale=10.0, wmean=40.0)
     _check_kernel(qkv, kw, bar=0.05)
 
 
 def test_a_second_call_gives_the_same_bits():
-    qkv, kw = _operands(2, 300, 4, True, 50)
+    qkv, kw = AR.operands_cuda(2, 300, 4, True, 50)
     _, a = _run(qkv, kw)
     ws, b = _run(qkv, kw)
     import osb200
@@ -128,7 +113,7 @@ def test_a_second_call_gives_the_same_bits():
 def test_refusals():
     import osb200
 
-    qkv, kw = _operands(1, 64, 2, True, None)
+    qkv, kw = AR.operands_cuda(1, 64, 2, True, None)
     q, k, v = qkv[:, :256], qkv[:, 256:512], qkv[:, 512:]
     out = torch.empty(64, 256, dtype=torch.bfloat16, device="cuda")
     ws = osb200.attn_fp8_workspace(1, 64, 2, "cuda")
@@ -209,15 +194,16 @@ def _check_model(m, cfg, inp, tag, mlps):
 
 @pytest.mark.parametrize("fused,liger,mlps", [(True, False, False), (False, True, False), (False, True, True)])
 def test_small_mmdit_fp8_attention_against_the_oracle(fused, liger, mlps):
-    m = _rand_model(fused, liger)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
-    inp = {k: v.cuda() for k, v in _inputs(2, 40, (3, 6, 8)).items()}
+    m = mmdit_model(fused, liger, device="cuda")
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(2, 40, (3, 6, 8), guidance=[4.0, 7.5]).items()}
     _check_model(m, cfg, inp, f"C=256 fused_qkv={fused} liger={liger}", mlps)
 
 
 @pytest.mark.parametrize("mlps", [False, True])
 def test_full_width_mmdit_fp8_attention_against_the_oracle(mlps):
     """C = 3072 (24 x 128 heads), 2 + 2 blocks, 1 x (256 text + 2304 image) tokens."""
-    m, cfg = _wide_model()
-    inp = {k: v.cuda() for k, v in _inputs(1, 256, (1, 48, 48)).items()}
+    m = mmdit_model(False, True, device="cuda", **MMDIT_WIDE)
+    cfg = dict(MMDIT_CFG, **MMDIT_WIDE, fused_qkv=False, use_liger_rope=True)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(1, 256, (1, 48, 48)).items()}
     _check_model(m, cfg, inp, "C=3072 2+2 blocks L=2560", mlps)

@@ -12,9 +12,8 @@ import torch.nn.functional as F
 from tests import fake_osb200 as F_
 from tests import fp8_ref as R
 from tests import mmdit_fp8_ref as MR
-from tests.test_host_mmdit_cpu import _rand_model
-from tests.test_lora_cpu import _inputs, write_adapter
-from tests.test_mmdit_gpu import CFG
+from tests.adapters import write_adapter
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -97,7 +96,7 @@ def _fp8_case(model, inp):
     """(product with FP8, emulation reference in bf16, bf16 oracle, fp32 oracle) outputs for one model and input."""
     from oracle import mmdit_oracle as M
 
-    cfg = dict(CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
+    cfg = dict(MMDIT_CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
     with torch.no_grad():
         out = model(**inp)
     W32 = {k: v.float() for k, v in model.state_dict().items()}
@@ -116,16 +115,16 @@ def _fp8_case(model, inp):
 def test_host_mmdit_fp8_follows_the_emulation(fake_osb, fused, liger):
     """C = 256 (2 heads), 2 double + 2 single blocks, FP8 MLPs on the stand-in, against the fp32 oracle.  Yardstick: the
     FP8-emulation reference (the oracle in bf16 with its MLPs at the FP8 rounding points), measured in the same test."""
-    m = _rand_model(fused, liger)
+    m = mmdit_model(fused, liger)
     m.enable_fp8()
-    inp = _inputs()
+    inp = mmdit_inputs()
     out, emu, floor, ref = _fp8_case(m, inp)
     r_out, r_emu, r_bf = rel_l2(out, ref), rel_l2(emu, ref), rel_l2(floor, ref)
     print(f"[mmdit fp8 host] fused={fused} liger={liger}: product {r_out:.3e}, FP8 emulation {r_emu:.3e}, "
           f"bf16 oracle {r_bf:.3e} (rel-L2 against the fp32 oracle)")
     assert r_out < 1.1 * r_emu and r_emu > r_bf, (r_out, r_emu, r_bf)
     names = [c[0] for c in fake_osb.calls]
-    nd, ns = CFG["depth"], CFG["depth_single_blocks"]
+    nd, ns = MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
     assert names.count("ln_modulate_fp8") == 2 * nd + ns
     assert names.count("gemm_fp8_blocks") == 2 * (2 * nd + ns)
     # the attention output of every single block, and (first forward on the CPU) the 2 weights of every MLP
@@ -144,8 +143,8 @@ def test_host_mmdit_fp8_follows_the_emulation(fake_osb, fused, liger):
 
 
 def test_disable_fp8_restores_the_bf16_bits(fake_osb):
-    m, plain = _rand_model(False, True), _rand_model(False, True)
-    inp = _inputs(B=1)
+    m, plain = mmdit_model(False, True), mmdit_model(False, True)
+    inp = mmdit_inputs(B=1)
     with torch.no_grad():
         want = plain(**inp)
         m.enable_fp8()
@@ -165,7 +164,7 @@ def test_fp8_refuses_sizes_beyond_the_kernels():
 
     for hidden, heads, ratio, match in ((192, 2, 4.0, "multiples of 128"), (256, 2, 3.25, "multiples of 128"),
                                         (4224, 33, 2.0, "<= 4096")):
-        cfg = dict(CFG, hidden_size=hidden, num_heads=heads, mlp_ratio=ratio, depth=1, depth_single_blocks=1,
+        cfg = dict(MMDIT_CFG, hidden_size=hidden, num_heads=heads, mlp_ratio=ratio, depth=1, depth_single_blocks=1,
                    axes_dim=[hidden // heads - 112, 56, 56])
         with torch.device("meta"):
             m = MMDiTModel(MMDiTConfig(from_pretrained=None, cache_dir=None, **cfg))
@@ -180,7 +179,7 @@ def test_fp8_and_mlp_adapters_refuse_each_other(fake_osb, tmp_path, fused):
     model both refuse it.  Adapters on other Linears keep working with FP8 on."""
     from opensora.utils.lora import load_lora, unload_lora
 
-    m = _rand_model(fused)
+    m = mmdit_model(fused)
     mlp_names = m.fp8_mlp_linears()
     single_mlp = "single_blocks.0." + ("linear1" if fused else "v_mlp")
     assert "double_blocks.0.img_mlp.0" in mlp_names and "single_blocks.1.linear2" in mlp_names and single_mlp in mlp_names
@@ -207,7 +206,7 @@ def test_fp8_and_mlp_adapters_refuse_each_other(fake_osb, tmp_path, fused):
     load_lora(m, write_adapter(str(tmp_path / "proj"), m, targets=["double_blocks.0.img_attn.proj"]))
     m.enable_fp8()
     with torch.no_grad():
-        out = m(**_inputs(B=1))
+        out = m(**mmdit_inputs(B=1))
     assert torch.isfinite(out.float()).all()
 
 
@@ -225,9 +224,9 @@ def _sp_worker(rank, world, port, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for fused, liger in ((True, False), (False, True)):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             m.enable_fp8()
-            inp = _inputs(B=2)
+            inp = mmdit_inputs(B=2)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)

@@ -9,7 +9,7 @@ import torch.nn.functional as F
 
 from tests import fake_osb200 as F_
 from tests import mmdit_fp8_ref as MR
-from tests.test_mmdit_gpu import CFG, _ids, _rand_model
+from tests.models import MMDIT_CFG, MMDIT_WIDE, mmdit_inputs, mmdit_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -139,33 +139,6 @@ def test_quant_blocks_fp8_matches_the_stand_in(rows, K, block, ld):
     assert torch.equal(q.cpu().view(torch.uint8), rq.view(torch.uint8))
 
 
-def _inputs(B, Lt, thw, ctx=128, seed=3):
-    T, H, W = thw
-    g = torch.Generator().manual_seed(seed)
-    rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-    txt_ids, img_ids = _ids(B, Lt, T, H, W)
-    return dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, ctx), txt_ids=txt_ids,
-                timesteps=torch.tensor([0.3, 0.8][:B]), y_vec=rb(B, 96), cond=rb(B, T * H * W, 68),
-                guidance=torch.tensor([4.0, 7.5][:B]))
-
-
-def _wide_model():
-    """C = 3072, 24 x 128 heads, 2 double + 2 single blocks (the shipped layout: split QKV, rotate-half RoPE)."""
-    from opensora.registry import MODELS, build_module
-
-    torch.manual_seed(7)
-    cfg = dict(CFG, hidden_size=3072, num_heads=24, depth=2, depth_single_blocks=2, fused_qkv=False, use_liger_rope=True)
-    m = build_module(dict(type="flux", **cfg), MODELS, device_map="cpu", torch_dtype=torch.float32)
-    g = torch.Generator().manual_seed(11)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if n.endswith("scale"):
-                p.copy_(1 + 0.2 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1 or "cond_in" in n:
-                p.copy_(0.05 * torch.randn(p.shape, generator=g))
-    return m.cuda().to(torch.bfloat16), cfg
-
-
 def _check_model(m, cfg, inp, tag):
     from oracle import mmdit_oracle as M
 
@@ -226,14 +199,15 @@ def _check_model(m, cfg, inp, tag):
 
 @pytest.mark.parametrize("fused,liger", [(True, False), (False, True)])
 def test_small_mmdit_fp8_against_the_oracle(fused, liger):
-    m = _rand_model(fused, liger)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
-    inp = {k: v.cuda() for k, v in _inputs(2, 40, (3, 6, 8)).items()}
+    m = mmdit_model(fused, liger, device="cuda")
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(2, 40, (3, 6, 8), guidance=[4.0, 7.5]).items()}
     _check_model(m, cfg, inp, f"C=256 fused_qkv={fused} liger={liger}")
 
 
 def test_full_width_mmdit_fp8_against_the_oracle():
     """C = 3072 (24 x 128 heads), 2 + 2 blocks, 1 x (256 text + 2304 image) tokens."""
-    m, cfg = _wide_model()
-    inp = {k: v.cuda() for k, v in _inputs(1, 256, (1, 48, 48)).items()}
+    m = mmdit_model(False, True, device="cuda", **MMDIT_WIDE)
+    cfg = dict(MMDIT_CFG, **MMDIT_WIDE, fused_qkv=False, use_liger_rope=True)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(1, 256, (1, 48, 48)).items()}
     _check_model(m, cfg, inp, "C=3072 2+2 blocks L=2560")

@@ -15,9 +15,8 @@ from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_lora_ref as LR
 from tests import mmdit_fp8_proj_ref as PR
 from tests import mmdit_fp8_ref as MR
-from tests.test_dora_cpu import merged_state_dora, write_dora_adapter
-from tests.test_lora_cpu import _inputs, _rand_model, write_adapter
-from tests.test_mmdit_gpu import CFG
+from tests.adapters import merged_state_dora, write_dora_adapter, write_adapter
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
 
 E4M3 = torch.float8_e4m3fn
@@ -67,7 +66,7 @@ def _case(model, inp, proj, attn):
     """(product, emulation reference, fp32 oracle on the merged weights g (W + s B A))."""
     from oracle import mmdit_oracle as M
 
-    cfg = dict(CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
+    cfg = dict(MMDIT_CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
     with torch.no_grad():
         out = model(**inp)
     W32 = merged_state_dora(model)
@@ -88,8 +87,8 @@ def _case(model, inp, proj, attn):
 def test_host_mmdit_fp8_lora_follows_the_emulation(fake_osb, tmp_path, fused, liger, proj, attn, dora):
     """C = 256, 2 double + 2 single blocks, an adapter (update 30% of |W|) on every FP8 Linear, against the fp32 oracle on
     the merged weights.  Yardstick: the FP8-emulation reference with the adapters, measured in the same test."""
-    m = _rand_model(fused, liger)
-    inp = _inputs()
+    m = mmdit_model(fused, liger)
+    inp = mmdit_inputs()
     with torch.no_grad():
         m.enable_fp8(projections=proj)
         base = m(**inp)
@@ -105,7 +104,7 @@ def test_host_mmdit_fp8_lora_follows_the_emulation(fake_osb, tmp_path, fused, li
     assert r_out < 1.1 * r_emu, (r_out, r_emu)
     assert rel_l2(out, base.float()) > 2 * r_out, "the adapter must move the output well beyond the error"
     names = [c[0] for c in fake_osb.calls]
-    nd, ns, B = CFG["depth"], CFG["depth_single_blocks"], inp["img"].shape[0]
+    nd, ns, B = MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"], inp["img"].shape[0]
     # without FP8 projections the q|k|v rows of linear1 / v_mlp (an MLP Linear) run on the bf16 LoRA GEMM
     assert names.count("gemm_lora") == (0 if proj else ns)
     if proj:   # per double block: 2 x B qkv, 2 x B proj, 2 x 2 MLP; per single block: qkv, mlp, linear2
@@ -131,9 +130,9 @@ def _forward(m, inp):
 def test_call_order_unload_and_disable(fake_osb, tmp_path):
     from opensora.utils.lora import unload_lora
 
-    inp = _inputs(B=1)
-    a, b = _rand_model(True, False), _rand_model(True, False)
-    plain = _rand_model(True, False)
+    inp = mmdit_inputs(B=1)
+    a, b = mmdit_model(True, False), mmdit_model(True, False)
+    plain = mmdit_model(True, False)
     path = _adapter(tmp_path, a, _block_targets(a), True)
     load_lora(a, path)
     a.enable_fp8(projections=True, lora=True)
@@ -147,15 +146,15 @@ def test_call_order_unload_and_disable(fake_osb, tmp_path):
     fake_osb.reset()
     assert torch.equal(_forward(a, inp), want) and "gemm_fp8_lora" not in [c[0] for c in fake_osb.calls]
     b.disable_fp8()
-    bf = _rand_model(True, False)
+    bf = mmdit_model(True, False)
     load_lora(bf, path)
     assert torch.equal(_forward(b, inp), _forward(bf, inp))   # back on the bf16 LoRA path
 
 
 @pytest.mark.parametrize("proj", [False, True])
 def test_lora_keyword_without_adapter_gives_the_fp8_bits(fake_osb, proj):
-    inp = _inputs(B=1)
-    a, b = _rand_model(False, True), _rand_model(False, True)
+    inp = mmdit_inputs(B=1)
+    a, b = mmdit_model(False, True), mmdit_model(False, True)
     a.enable_fp8(projections=proj)
     b.enable_fp8(projections=proj, lora=True)
     want = _forward(a, inp)
@@ -169,8 +168,8 @@ def test_cached_a_cat_follows_the_adapter_state(fake_osb, tmp_path):
     model's with the same adapter state."""
     from opensora.utils.lora import unload_lora
 
-    inp = _inputs(B=1)
-    m = _rand_model(True, False)
+    inp = mmdit_inputs(B=1)
+    m = mmdit_model(True, False)
     m.enable_fp8(projections=True, lora=True)
     load_lora(m, _adapter(tmp_path, m, _block_targets(m), True))
     first = _forward(m, inp)
@@ -180,7 +179,7 @@ def test_cached_a_cat_follows_the_adapter_state(fake_osb, tmp_path):
         blk.img_attn.qkv.lora_B["default"].weight.mul_(-1)
         m.single_blocks[1].linear2.lora_magnitude_vector["default"].weight.mul_(1.5)
     edited = _forward(m, inp)
-    fresh = _rand_model(True, False)
+    fresh = mmdit_model(True, False)
     fresh.enable_fp8(projections=True, lora=True)
     sd = {k: v.clone() for k, v in m.state_dict().items()}
     load_lora(fresh, _adapter(tmp_path, fresh, _block_targets(fresh), True, name="b"))
@@ -188,33 +187,33 @@ def test_cached_a_cat_follows_the_adapter_state(fake_osb, tmp_path):
     assert not torch.equal(edited, first) and torch.equal(edited, _forward(fresh, inp))
     unload_lora(m)
     load_lora(m, _adapter(tmp_path, m, _block_targets(m), False, name="c", seed=4))
-    other = _rand_model(True, False)
+    other = mmdit_model(True, False)
     other.enable_fp8(projections=True, lora=True)
     load_lora(other, str(tmp_path / "c"))
     assert torch.equal(_forward(m, inp), _forward(other, inp))
 
 
 def test_default_enable_fp8_still_refuses(fake_osb, tmp_path):
-    m = _rand_model(True, False)
+    m = mmdit_model(True, False)
     load_lora(m, _adapter(tmp_path, m, ["double_blocks.0.img_mlp.0"], False))
     with pytest.raises(ValueError, match="FP8 MLPs cannot run LoRA / DoRA adapters"):
         m.enable_fp8()
-    n = _rand_model(True, False)
+    n = mmdit_model(True, False)
     n.enable_fp8(projections=True)
     with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
         load_lora(n, _adapter(tmp_path, n, ["double_blocks.0.img_attn.proj"], False, name="b"))
     n.enable_fp8(projections=True, lora=True)
     load_lora(n, str(tmp_path / "b"))
-    assert torch.isfinite(_forward(n, _inputs(B=1)).float()).all()
+    assert torch.isfinite(_forward(n, mmdit_inputs(B=1)).float()).all()
 
 
 def test_down_projection_reads_the_fp8_codes(fake_osb, tmp_path):
     """U = bf16(qdq(x) qdq_rows(A_cat)^T): the down GEMM of fc1 reads the LN+modulate codes and an A_cat quantized per
     row, whatever its rank padding."""
-    m = _rand_model(True, False)
+    m = mmdit_model(True, False)
     m.enable_fp8(lora=True)
     load_lora(m, _adapter(tmp_path, m, ["double_blocks.0.img_mlp.0"], False, r=12))
-    _forward(m, _inputs(B=1))
+    _forward(m, mmdit_inputs(B=1))
     fp8 = m._fp8_state
     (A, q, s), = [v for k, v in fp8._la.items()]
     assert A.shape[0] == 16 and q.dtype == E4M3                              # rank 12 padded to 16
@@ -235,12 +234,12 @@ def _sp_worker(rank, world, port, adapter_dir, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for fused, liger, proj, attn in ((True, False, True, True), (False, True, False, False)):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             m.enable_fp8(projections=proj, lora=True)
             if attn:
                 m.enable_fp8_attention()
             load_lora(m, adapter_dir[fused])
-            inp = _inputs(B=2)
+            inp = mmdit_inputs(B=2)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)
@@ -260,7 +259,7 @@ def test_mmdit_fp8_lora_ulysses_world2(tmp_path):
 
     dirs = {}
     for fused in (True, False):
-        m = _rand_model(fused, False)
+        m = mmdit_model(fused, False)
         targets = _block_targets(m) if fused else _mlp_targets(m)
         dirs[fused] = _adapter(tmp_path, m, targets, not fused, name=f"a{int(fused)}")
     port = 29500 + (os.getpid() + 91) % 2000

@@ -11,9 +11,8 @@ from tests import fake_osb200 as F_
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_lora_ref as LR
 from tests import mmdit_fp8_proj_ref as PR
-from tests.test_dora_cpu import merged_state_dora, write_dora_adapter
-from tests.test_lora_cpu import write_adapter
-from tests.test_mmdit_fp8_gpu import _inputs, _wide_model
+from tests.adapters import merged_state_dora, write_adapter, write_dora_adapter
+from tests.models import MMDIT_CFG, MMDIT_WIDE, mmdit_inputs, mmdit_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -207,12 +206,9 @@ def _adapted_case(m, cfg, inp, tmp_path, dora, attn):
 
 @pytest.mark.parametrize("fused,liger,dora,attn", [(True, False, False, False), (False, True, True, True)])
 def test_small_mmdit_fp8_lora_against_the_oracle(tmp_path, fused, liger, dora, attn):
-    from tests.test_lora_cpu import _rand_model
-    from tests.test_mmdit_gpu import CFG
-
-    m = _rand_model(fused, liger).cuda().to(torch.bfloat16)
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
-    inp = {k: v.cuda() for k, v in _inputs(2, 40, (3, 6, 8)).items()}
+    m = mmdit_model(fused, liger).cuda().to(torch.bfloat16)
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(2, 40, (3, 6, 8), guidance=[4.0, 7.5]).items()}
     out, emu, ref = _adapted_case(m, cfg, inp, tmp_path, dora, attn)
     r, _ = report(f"MMDiT C=256 FP8 + {'DoRA' if dora else 'LoRA'} fused={fused} liger={liger} attn={attn}", out, ref)
     r_emu = rel_l2(emu, ref)
@@ -226,8 +222,9 @@ def test_small_mmdit_fp8_lora_against_the_oracle(tmp_path, fused, liger, dora, a
 def test_full_width_mmdit_fp8_lora_against_the_oracle(tmp_path):
     """C = 3072 (24 x 128 heads), 2 + 2 blocks, 1 x (256 text + 2304 image) tokens, DoRA r = 64 on every block Linear,
     FP8 projections and attention."""
-    m, cfg = _wide_model()
-    inp = {k: v.cuda() for k, v in _inputs(1, 256, (1, 48, 48)).items()}
+    m = mmdit_model(False, True, device="cuda", **MMDIT_WIDE)
+    cfg = dict(MMDIT_CFG, **MMDIT_WIDE, fused_qkv=False, use_liger_rope=True)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(1, 256, (1, 48, 48)).items()}
     out, emu, ref = _adapted_case(m, cfg, inp, tmp_path, True, True)
     r, _ = report("MMDiT C=3072 2+2 blocks L=2560 FP8 + DoRA r=64", out, ref)
     r_emu = rel_l2(emu, ref)

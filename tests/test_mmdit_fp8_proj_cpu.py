@@ -13,10 +13,8 @@ import torch
 from tests import fake_osb200 as F_
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_proj_ref as PR
-from tests.test_host_mmdit_cpu import _rand_model
-from tests.test_lora_cpu import _inputs, write_adapter
-from tests.test_mmdit_fp8_attn_cpu import _operands
-from tests.test_mmdit_gpu import CFG
+from tests.adapters import write_adapter
+from tests.models import MMDIT_CFG, mmdit_inputs, mmdit_model
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,7 +25,7 @@ def test_stand_in_block_output_follows_the_block_rule(fake_osb):
     """Codes and scales land in column slices of wider buffers; each (row, head) block is the block rule applied to the
     fp32 attention value, which the bf16 output of `attn_fp8` rounds."""
     B, L, H = 2, 200, 2
-    qkv, kw = _operands(B, L, H, split=50)
+    qkv, kw = AR.operands_cpu(B, L, H, split=50)
     C = H * 128
     q, k, v = qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:]
     ws = fake_osb.attn_fp8_workspace(B, L, H, "cpu")
@@ -56,7 +54,7 @@ def _case(model, inp, attn):
     """(product, emulation reference in bf16, bf16 oracle, fp32 oracle) outputs for one model and input."""
     from oracle import mmdit_oracle as M
 
-    cfg = dict(CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
+    cfg = dict(MMDIT_CFG, fused_qkv=model.config.fused_qkv, use_liger_rope=model.config.use_liger_rope)
     with torch.no_grad():
         out = model(**inp)
     W32 = {k: v.float() for k, v in model.state_dict().items()}
@@ -81,7 +79,7 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(fake_osb, fused, liger,
     fp32 oracle.  Yardstick: the emulation reference measured in the same test.  With as many text as image tokens
     (thw = (1, 4, 6)) both streams of a double block get workspaces of one shape: neither may overwrite the other's
     LN+modulate codes before its q|k|v GEMMs have read them."""
-    m = _rand_model(fused, liger)
+    m = mmdit_model(fused, liger)
     if attn and fused:   # the switches compose in either order
         m.enable_fp8_attention()
         m.enable_fp8(projections=True)
@@ -89,7 +87,7 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(fake_osb, fused, liger,
         m.enable_fp8(projections=True)
         if attn:
             m.enable_fp8_attention()
-    inp = _inputs(thw=thw)
+    inp = mmdit_inputs(thw=thw)
     with torch.no_grad():
         m(**inp)             # weights are quantized at the first forward of a CPU model
     fake_osb.reset()
@@ -100,7 +98,7 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(fake_osb, fused, liger,
     assert r_out < 1.1 * r_emu, (r_out, r_emu, r_bf)
     calls = list(fake_osb.calls)
     names = [c[0] for c in calls]
-    nd, ns = CFG["depth"], CFG["depth_single_blocks"]
+    nd, ns = MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
     assert names.count("ln_modulate") == 1                     # the final layer only: no bf16 LN pass in any block
     assert names.count("ln_modulate_fp8") == 4 * nd + ns       # mod1 + mod2 per stream, one per single block
     assert "attn_short" not in names if attn else "attn_fp8" not in names
@@ -112,8 +110,8 @@ def test_host_mmdit_fp8_projections_follow_the_emulation(fake_osb, fused, liger,
 
 
 def test_enable_fp8_without_keyword_keeps_the_mlp_path(fake_osb):
-    m = _rand_model(True, False)
-    inp = _inputs(B=1)
+    m = mmdit_model(True, False)
+    inp = mmdit_inputs(B=1)
     m.enable_fp8()
     with torch.no_grad():
         m(**inp)
@@ -129,7 +127,7 @@ def test_enable_fp8_without_keyword_keeps_the_mlp_path(fake_osb):
         fake_osb.reset()
         again = m(**inp)
     names = [c[0] for c in mlp_calls]
-    nd, ns = CFG["depth"], CFG["depth_single_blocks"]
+    nd, ns = MMDIT_CFG["depth"], MMDIT_CFG["depth_single_blocks"]
     assert names.count("ln_modulate") == 2 * nd + ns + 1 and names.count("quant_blocks_fp8") == ns
     assert "attn_fp8_blocks" not in names
     assert torch.equal(again, mlp) and fake_osb.calls == mlp_calls
@@ -137,8 +135,8 @@ def test_enable_fp8_without_keyword_keeps_the_mlp_path(fake_osb):
 
 
 def test_disable_fp8_restores_the_bf16_bits(fake_osb):
-    m, plain = _rand_model(False, True), _rand_model(False, True)
-    inp = _inputs(B=1)
+    m, plain = mmdit_model(False, True), mmdit_model(False, True)
+    inp = mmdit_inputs(B=1)
     with torch.no_grad():
         want = plain(**inp)
         plain_calls = list(fake_osb.calls)
@@ -155,19 +153,19 @@ def test_disable_fp8_restores_the_bf16_bits(fake_osb):
 
 
 def test_fp8_proj_linears_lists_the_projections():
-    m = _rand_model(False, False)
+    m = mmdit_model(False, False)
     names = m.fp8_proj_linears()
     assert "double_blocks.0.img_attn.q_proj" in names and "double_blocks.1.txt_attn.proj" in names
     assert "single_blocks.0.k_proj" in names and "single_blocks.1.v_mlp" in names
-    assert len(names) == CFG["depth"] * 2 * 4 + CFG["depth_single_blocks"] * 3
-    assert _rand_model(True, False).fp8_proj_linears()[:2] == ["double_blocks.0.img_attn.qkv",
+    assert len(names) == MMDIT_CFG["depth"] * 2 * 4 + MMDIT_CFG["depth_single_blocks"] * 3
+    assert mmdit_model(True, False).fp8_proj_linears()[:2] == ["double_blocks.0.img_attn.qkv",
                                                                 "double_blocks.0.img_attn.proj"]
 
 
 def test_adapter_refusals(fake_osb, tmp_path):
     from opensora.utils.lora import load_lora, unload_lora
 
-    m = _rand_model(True)
+    m = mmdit_model(True)
     load_lora(m, write_adapter(str(tmp_path / "a"), m, targets=["double_blocks.0.txt_attn.proj"]))
     with pytest.raises(ValueError, match="FP8 projections cannot run LoRA / DoRA adapters"):
         m.enable_fp8(projections=True)
@@ -181,7 +179,7 @@ def test_adapter_refusals(fake_osb, tmp_path):
     with pytest.raises(ValueError, match="FP8 projections, which take no LoRA"):
         load_lora(m, write_adapter(str(tmp_path / "c"), m, targets=["double_blocks.1.img_attn.qkv"]))
     load_lora(m, write_adapter(str(tmp_path / "d"), m, targets=["double_blocks.0.img_mod.lin", "final_layer.linear"]))
-    inp = _inputs(B=1)
+    inp = mmdit_inputs(B=1)
     fake_osb.reset()
     with torch.no_grad():
         out = m(**inp)
@@ -202,11 +200,11 @@ def _sp_worker(rank, world, port, ret):
         fake_osb200.ACC_DTYPE = torch.float64   # row-local GEMMs on a row subset: no M-dependent summation-order noise
         res = []
         for fused, liger, attn in ((True, False, True), (False, True, False)):
-            m = _rand_model(fused, liger)
+            m = mmdit_model(fused, liger)
             m.enable_fp8(projections=True)
             if attn:
                 m.enable_fp8_attention()
-            inp = _inputs(B=2)
+            inp = mmdit_inputs(B=2)
             with torch.no_grad():
                 single = m(**inp)
                 m.enable_sequence_parallel(dist.group.WORLD)

@@ -8,8 +8,7 @@ import torch
 
 from tests import mmdit_fp8_attn_ref as AR
 from tests import mmdit_fp8_proj_ref as PR
-from tests.test_mmdit_fp8_attn_gpu import _operands
-from tests.test_mmdit_fp8_gpu import _inputs, _wide_model
+from tests.models import MMDIT_CFG, MMDIT_WIDE, mmdit_inputs, mmdit_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -28,7 +27,7 @@ def test_block_output_mode(L):
 
     B, H = 3, 24
     C = H * 128
-    qkv, kw = _operands(B, L, H, True, min(256, L // 2))
+    qkv, kw = AR.operands_cuda(B, L, H, True, min(256, L // 2))
     q, k, v = qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:]
     ws = osb200.attn_fp8_workspace(B, L, H, "cuda")
     bf = torch.zeros(B * L, C, dtype=torch.bfloat16, device="cuda")
@@ -109,8 +108,9 @@ def _growth_and_error(m, cfg, inp, attn):
 @pytest.mark.parametrize("attn", [False, True])
 def test_full_width_mmdit_fp8_projections_against_the_oracle(attn):
     """C = 3072 (24 x 128 heads), 2 + 2 blocks, 1 x (256 text + 2304 image) tokens, every block Linear on FP8."""
-    m, cfg = _wide_model()
-    inp = {k: v.cuda() for k, v in _inputs(1, 256, (1, 48, 48)).items()}
+    m = mmdit_model(False, True, device="cuda", **MMDIT_WIDE)
+    cfg = dict(MMDIT_CFG, **MMDIT_WIDE, fused_qkv=False, use_liger_rope=True)
+    inp = {k: v.cuda() for k, v in mmdit_inputs(1, 256, (1, 48, 48)).items()}
     with torch.no_grad():
         plain = m(**inp).clone()
     out, ref, emu, per_block = _growth_and_error(m, cfg, inp, attn)

@@ -4,37 +4,10 @@ which tests/test_oracle_cpu.py pins to fixtures produced by executing the refere
 import pytest
 import torch
 
+from tests.models import MMDIT_CFG, mmdit_ids, mmdit_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
-CFG = dict(in_channels=64, vec_in_dim=96, context_in_dim=128, hidden_size=256, mlp_ratio=4.0, num_heads=2, depth=2,
-           depth_single_blocks=2, axes_dim=[16, 56, 56], theta=10000, qkv_bias=True, guidance_embed=True, cond_embed=True)
-
-
-def _ids(B, Lt, T, H, W):
-    img = torch.zeros(T, H, W, 3)
-    img[..., 0] += torch.arange(T)[:, None, None]
-    img[..., 1] += torch.arange(H)[None, :, None]
-    img[..., 2] += torch.arange(W)[None, None, :]
-    return torch.zeros(B, Lt, 3), img.reshape(1, T * H * W, 3).repeat(B, 1, 1)
-
-
-def _rand_model(fused, liger=False):
-    from opensora.registry import MODELS, build_module
-
-    torch.manual_seed(7)
-    m = build_module(dict(type="flux", fused_qkv=fused, use_liger_rope=liger, **CFG), MODELS, device_map="cpu",
-                     torch_dtype=torch.float32)
-    g = torch.Generator().manual_seed(11)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if n.endswith("scale"):
-                p.copy_(1 + 0.2 * torch.randn(p.shape, generator=g))
-            elif p.dim() == 1:
-                p.copy_(0.05 * torch.randn(p.shape, generator=g))
-            elif "cond_in" in n:
-                p.copy_(0.05 * torch.randn(p.shape, generator=g))
-    return m.cuda().to(torch.bfloat16)
 
 
 @pytest.mark.parametrize("fused,liger,thw", [(True, False, (3, 6, 8)), (False, False, (3, 6, 8)), (False, True, (3, 6, 8)),
@@ -46,18 +19,18 @@ def test_mmdit_model_vs_pinned_oracle(fused, liger, thw):
         pytest.skip("no CUDA device")
     from oracle import mmdit_oracle as M
 
-    m = _rand_model(fused, liger)
+    m = mmdit_model(fused, liger, device="cuda")
     B, Lt = 2, 40
     T, H, W = thw
     g = torch.Generator().manual_seed(3)
     rb = lambda *s: torch.randn(*s, generator=g).to(torch.bfloat16)  # noqa: E731
-    txt_ids, img_ids = _ids(B, Lt, T, H, W)
+    txt_ids, img_ids = mmdit_ids(B, Lt, T, H, W)
     inp = dict(img=rb(B, T * H * W, 64), img_ids=img_ids, txt=rb(B, Lt, 128), txt_ids=txt_ids,
                timesteps=torch.tensor([0.3, 0.8]), y_vec=rb(B, 96), cond=rb(B, T * H * W, 68), guidance=torch.tensor([4.0, 7.5]))
     with torch.no_grad():
         out = m(**{k: v.cuda() for k, v in inp.items()})
     W32 = {k: v.float() for k, v in m.state_dict().items()}
-    cfg = dict(CFG, fused_qkv=fused, use_liger_rope=liger)
+    cfg = dict(MMDIT_CFG, fused_qkv=fused, use_liger_rope=liger)
     finp = {k: (v.float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
     ref = M.model_forward(W32, cfg, finp["img"], finp["img_ids"], finp["txt"], finp["txt_ids"], finp["timesteps"],
                           finp["y_vec"], cond=finp["cond"], guidance=finp["guidance"])
@@ -79,7 +52,7 @@ def test_processor_hook_is_the_plugin_point():
         pytest.skip("no CUDA device")
     from opensora.models.mmdit.layers import DoubleStreamBlockProcessor
 
-    m = _rand_model(True)
+    m = mmdit_model(True, device="cuda")
     calls = []
 
     class Spy(DoubleStreamBlockProcessor):
@@ -90,7 +63,7 @@ def test_processor_hook_is_the_plugin_point():
     for b in m.double_blocks:
         assert isinstance(b.get_processor(), DoubleStreamBlockProcessor)
         b.set_processor(Spy())
-    txt_ids, img_ids = _ids(1, 8, 1, 4, 4)
+    txt_ids, img_ids = mmdit_ids(1, 8, 1, 4, 4)
     with torch.no_grad():
         out = m(img=torch.randn(1, 16, 64).cuda(), img_ids=img_ids.cuda(), txt=torch.randn(1, 8, 128).cuda(), txt_ids=txt_ids.cuda(),
                 timesteps=torch.tensor([0.5]).cuda(), y_vec=torch.randn(1, 96).cuda(), cond=torch.randn(1, 16, 68).cuda(),

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from tests import rf_conditioning_ref as R
+from tests.models import stdit3_pair
 from tests.util import rel_l2
 
 
@@ -192,19 +193,13 @@ def test_sampler_all_ones_mask_matches_t2v(fake_osb):
     assert torch.equal(a, b)
 
 
-def _pair(seed=1234):
-    from tests.smoke_impl import build_pair
-
-    return build_pair("xs", device="cpu", seed=seed)
-
-
 def test_rflow_conditioned_sampler_drives_the_model(fake_osb):
     """RFLOW.sample(frame_mask=...) around the REAL host-side STDiT3 against the oracle loop around the fp32 oracle model,
     both fed the same per-step noise: 4 steps, frame masks [0, 0.5, 1, 1] and [1, 0, 0.5, 1]."""
     from oracle import stdit3_oracle as OS
     from opensora.schedulers import RFLOW
 
-    prod, oracle, cfg = _pair()
+    prod, oracle, cfg = stdit3_pair("xs", device="cpu")
     B, steps = 2, 4
     inp = OS.synthetic_inputs(cfg, B=B, T=4, H=8, W=8, lens=[cfg.model_max_length, 11])
     inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v) for k, v in inp.items()}

@@ -4,6 +4,8 @@ the oracle loop; XL/2 at the benchmark latent)."""
 import pytest
 import torch
 
+from tests.models import stdit3_inputs, stdit3_pair
+from tests.sampling_toys import toy_model
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -93,8 +95,8 @@ def test_all_ones_mask_sampler_is_the_t2v_loop():
         sch = RFLOW(num_sampling_steps=7, cfg_scale=6.0, use_timestep_transform=transform)
         extra = dict(height=torch.full((2,), 360.0, device="cuda"), width=torch.full((2,), 640.0, device="cuda"),
                      num_frames=torch.full((2,), 51, device="cuda"))
-        a = sch.sample(_toy_model, z, y, y, additional_args=extra)
-        b = sch.sample(_toy_model, z, y, y, additional_args=extra, frame_mask=torch.ones(2, 6, device="cuda"))
+        a = sch.sample(toy_model, z, y, y, additional_args=extra)
+        b = sch.sample(toy_model, z, y, y, additional_args=extra, frame_mask=torch.ones(2, 6, device="cuda"))
         assert torch.equal(a, b), transform
 
 
@@ -124,12 +126,6 @@ def test_masked_step_graph_replay_reads_the_schedule():
         assert torch.equal(out, eager)
 
 
-def _toy_model(x, timestep, y, mask=None, x_mask=None, **kw):
-    v = torch.tanh(0.8 * x.float() + y.float().mean(dim=(1, 2, 3))[:, None, None, None, None])
-    v = v * (0.5 + timestep.float()[:, None, None, None, None] / 1000.0)
-    return torch.cat((v, 0.1 * x.float()), dim=1)
-
-
 def test_conditioned_loop_never_synchronises():
     _need_cuda()
     from opensora.schedulers import RFLOW
@@ -140,11 +136,11 @@ def test_conditioned_loop_never_synchronises():
     y = torch.randn(B, 1, 5, 8, device="cuda", generator=g)
     fm = torch.tensor([[0.0, 0.5, 1.0, 1.0, 0.3, 1.0], [1.0, 1.0, 0.0, 0.7, 1.0, 1.0]], device="cuda")
     sch = RFLOW(num_sampling_steps=5, cfg_scale=6.0)
-    sch.sample(_toy_model, z, y, y, frame_mask=fm, generator=g)                   # warm up (module loads, caching allocator)
+    sch.sample(toy_model, z, y, y, frame_mask=fm, generator=g)                   # warm up (module loads, caching allocator)
     torch.cuda.synchronize()
     torch.cuda.set_sync_debug_mode("error")
     try:
-        out = sch.sample(_toy_model, z, y, y, frame_mask=fm, generator=g)
+        out = sch.sample(toy_model, z, y, y, frame_mask=fm, generator=g)
     finally:
         torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()
@@ -153,14 +149,11 @@ def test_conditioned_loop_never_synchronises():
 
 def _i2v(cfg_name, B, T, H, W, steps, seed=11):
     """Strategy "0" (the first latent frame is the reference) through apply_mask_strategy and RFLOW.sample."""
-    from oracle import stdit3_oracle as O
     from opensora.schedulers import RFLOW
     from opensora.utils.inference_utils import apply_mask_strategy
-    from tests.smoke_impl import build_pair
 
-    prod, oracle, cfg = build_pair(cfg_name)
-    inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=[cfg.model_max_length] + [17] * (B - 1))
-    inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
+    prod, oracle, cfg = stdit3_pair(cfg_name)
+    inp = stdit3_inputs(cfg, B, T, H, W, lens=[cfg.model_max_length] + [17] * (B - 1), device="cuda")
     refs = [[torch.randn(cfg.in_channels, 2, H, W, generator=torch.Generator().manual_seed(seed + b)).cuda()] for b in range(B)]
     z = inp["x"].to(torch.bfloat16)
     fm = apply_mask_strategy(z, refs, ["0"] * B, loop_i=0)

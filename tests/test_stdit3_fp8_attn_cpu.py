@@ -13,7 +13,8 @@ import torch.multiprocessing as mp
 
 from tests import fake_osb200 as F_
 from tests import fp8_ref as R
-from tests.mmdit_fp8_attn_ref import attention_from_operands
+from tests import stdit3_fp8_attn_ref as A
+from tests.models import stdit3_inputs, stdit3_pair
 from tests.util import rel_l2
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,18 +29,6 @@ def _tiles(osb, rows, tmap, kinds, H, D, seed, spread=True):
         x[:, 3] = 0.0
     t.dense.copy_(x.to(torch.bfloat16))
     return t
-
-
-def _dequantized(t8, kind, rows, is_v):
-    """fp64 [rows, H, D] values of one kind read back from the e4m3 tiles through the tile map."""
-    ti, r = F_.tile_index(t8.map, rows, t8.codes.device)
-    codes = t8.codes[kind].double()
-    if is_v:
-        codes = F_.v_in_key_order(t8.codes[kind]).double()
-        x = codes[:, ti, r, : t8.head_dim] * t8.scales[kind][:, ti, : t8.head_dim].double()
-    else:
-        x = codes[:, ti, r, : t8.head_dim] * t8.scales[kind][:, ti, r, None].double()
-    return x.transpose(0, 1)
 
 
 @pytest.mark.parametrize("L,D", [(300, 72), (16, 64)])
@@ -62,30 +51,7 @@ def test_conversion_follows_the_contract(fake_osb, L, D):
     amax = torch.zeros(ntiles, H, D).scatter_reduce(0, ti[:, None, None].expand_as(x), x.abs(), "amax")
     sv = torch.where(amax > 0, amax / 448.0, torch.ones_like(amax))
     assert torch.equal(t8.scales[2][..., :D].permute(1, 0, 2), sv) and torch.all(t8.scales[2][..., D:] == 1.0)
-    assert torch.equal(_dequantized(t8, 2, rows, True), (R.e4m3_round(x / sv[ti]) * sv[ti].double()))
-
-
-def _reference(t8, kv8, q_rows, kv_rows, qseq, kseq, kpos, num_seqs, Lk, kv_lens, q_kind, k_kind, v_kind):
-    """(exact fp32 softmax, the P-emulation) on the dequantized e4m3 operands, per output token row [rows, H, D]."""
-    q = _dequantized(t8, q_kind, q_rows, False).float()
-    k = _dequantized(kv8, k_kind, kv_rows, False).float()
-    v = _dequantized(kv8, v_kind, kv_rows, True).float()
-    H, D = t8.heads, t8.head_dim
-    exact = torch.zeros(q_rows, H, D, device=q.device)
-    emu = torch.zeros(q_rows, H, D, device=q.device)
-    for s_ in range(num_seqs):
-        rq = (qseq == s_).nonzero().flatten()
-        rk = (kseq == s_).nonzero().flatten()
-        rk = rk[kpos[rk].argsort()]
-        n = Lk if kv_lens is None else min(int(kv_lens[s_]), Lk)
-        if n <= 0:
-            continue
-        rk = rk[:n]
-        qq, kk, vv = q[rq].transpose(0, 1), k[rk].transpose(0, 1), v[rk].transpose(0, 1)
-        sc = qq @ kk.transpose(-1, -2) * D ** -0.5
-        exact[rq] = (torch.softmax(sc.double(), -1).float() @ vv).transpose(0, 1)
-        emu[rq] = attention_from_operands(qq, kk, vv, D ** -0.5).transpose(0, 1)
-    return exact, emu
+    assert torch.equal(A.dequantized(t8, 2, rows, True), (R.e4m3_round(x / sv[ti]) * sv[ti].double()))
 
 
 CASES = {
@@ -124,7 +90,7 @@ def test_attention_follows_dequantized_softmax(fake_osb, name):
     fake_osb.attn_tiles_fp8(q8, kv8, out, **kw)
     qseq, _ = fake_osb._seq_pos(q8.map, rows, "cpu")
     kseq, kpos = fake_osb._seq_pos(kv8.map, kv_rows, "cpu")
-    exact, emu = _reference(q8, kv8, rows, kv_rows, qseq, kseq, kpos, nseq, Lk, kv_lens, kw.get("q_kind", 0),
+    exact, emu = A.tiles_reference(q8, kv8, rows, kv_rows, qseq, kseq, kpos, nseq, Lk, kv_lens, kw.get("q_kind", 0),
                             kw.get("k_kind", 1), kw.get("v_kind", 2))
     if out_map is not None:   # row (seq, pos) of the tiles' stream lives at the frame-major row of `out`
         so, po = fake_osb._seq_pos(out_map, rows, "cpu")
@@ -141,36 +107,19 @@ def test_attention_follows_dequantized_softmax(fake_osb, name):
         assert not got[qseq == 2].any()
 
 
-def _inputs(cfg, B, T, H, W, lens=None):
-    from oracle import stdit3_oracle as O
-
-    inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=lens)
-    return {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v) for k, v in inp.items()}
-
-
-def _pair(which):
-    if which == "xs72":   # STDiT3-XS/2 as shipped: 4 heads of 72
-        from tests.smoke_impl import build_pair
-
-        return build_pair("xs", device="cpu")
-    return R.build_pair("xs", device="cpu")   # hidden 256: 4 heads of 64, FP8 MLPs possible
-
-
 @pytest.mark.parametrize("which,mlps", [("xs72", False), ("xs64", False), ("xs64", True)])
 def test_host_stdit3_fp8_attention_follows_the_emulation(fake_osb, which, mlps):
     """The product with FP8 attention (and FP8 MLPs) on the stand-in, against the fp32 oracle: at most 1.1x further away
     than the emulation reference (the bf16 oracle with its attentions, and MLPs, at the FP8 rounding points), plain and
     with an x_mask and ragged text."""
-    from tests import stdit3_fp8_attn_ref as A
-
-    prod, oracle, cfg = _pair(which)
+    prod, oracle, cfg = stdit3_pair("xs" if which == "xs72" else which, device="cpu")
     prod.enable_fp8_attention()
     if mlps:
         prod.enable_fp8()
-    inp = _inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 9])
+    inp = stdit3_inputs(cfg, 2, 4, 8, 8, lens=[cfg.model_max_length, 9])
     xm = torch.ones(2, 4, dtype=torch.bool)
     xm[1, 1:3] = False
-    ob = _pair(which)[1].to(torch.bfloat16)
+    ob = stdit3_pair("xs" if which == "xs72" else which, device="cpu")[1].to(torch.bfloat16)
     for kw in ({}, {"x_mask": xm}):
         fake_osb.reset()
         with torch.no_grad():
@@ -195,8 +144,8 @@ def test_host_stdit3_fp8_attention_follows_the_emulation(fake_osb, which, mlps):
 
 
 def test_disable_fp8_attention_restores_the_bf16_path(fake_osb):
-    prod, _, cfg = _pair("xs72")
-    inp = _inputs(cfg, 1, 4, 8, 8)
+    prod, _, cfg = stdit3_pair("xs", device="cpu")
+    inp = stdit3_inputs(cfg, 1, 4, 8, 8)
     with torch.no_grad():
         fake_osb.reset()
         before = prod(**inp)
@@ -223,8 +172,8 @@ def test_head_layout_refusals(fake_osb):
     with pytest.raises(ValueError, match="head sizes 72 and 64"):
         m.enable_fp8_attention()                    # 2 heads of 128
     assert m._fp8_attn is False
-    _, _, cfg = _pair("xs72")
-    inp = _inputs(cfg, 1, 2, 4, 4)
+    _, _, cfg = stdit3_pair("xs", device="cpu")
+    inp = stdit3_inputs(cfg, 1, 2, 4, 4)
     # head tiles need an even head count (3 heads of 72, with and without FP8 attention) and a head size they are built
     # for (4 heads of 96): the forward refuses both before its first launch
     for heads, hidden, fp8 in ((3, 216, False), (3, 216, True), (4, 384, False)):
@@ -248,11 +197,11 @@ def _sp_worker(rank, world, port, ret):
 
         sys.modules["osb200"] = fake_osb200
         torch.manual_seed(0)
-        prod, _, cfg = _pair("xs72")
+        prod, _, cfg = stdit3_pair("xs", device="cpu")
         prod.enable_fp8_attention()
         # 16 x 16 latent: S = 64 (spatial sequences packed in pairs), T = 4 (temporal sequences packed 32 per tile): each
         # rank's S / 2 = 32 columns fill whole temporal tiles, so both runs group the same sequences into one v scale
-        inp = _inputs(cfg, 2, 4, 16, 16, lens=[cfg.model_max_length, 9])
+        inp = stdit3_inputs(cfg, 2, 4, 16, 16, lens=[cfg.model_max_length, 9])
         xm = torch.ones(2, 4, dtype=torch.bool)
         xm[1, 2:] = False
         with torch.no_grad():

@@ -10,7 +10,8 @@ import torch
 
 from tests import fake_osb200 as F_
 from tests import fp8_ref as R
-from tests.test_stdit3_fp8_attn_cpu import _reference
+from tests import stdit3_fp8_attn_ref as A
+from tests.models import stdit3_inputs, stdit3_pair
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -129,7 +130,7 @@ def test_attention_against_dequantized_softmax(name):
     lq, lkv = logical(q8), logical(kv8)
     qseq, _ = F_._seq_pos(q8.map, rows, "cuda")
     kseq, kpos = F_._seq_pos(kv8.map, kv_rows, "cuda")
-    exact, emu = _reference(lq, lkv, rows, kv_rows, qseq, kseq, kpos, kw["num_seqs"], Lk,
+    exact, emu = A.tiles_reference(lq, lkv, rows, kv_rows, qseq, kseq, kpos, kw["num_seqs"], Lk,
                             None if kv_lens is None else kv_lens.cpu(), kw.get("q_kind", 0), kw.get("k_kind", 1),
                             kw.get("v_kind", 2))
     got = out.float().view(rows, H, D)
@@ -169,24 +170,15 @@ def test_output_scatter_is_the_unscattered_output():
         assert torch.equal(bufs[p][dst[sel]].view(torch.int16), plain[src[sel]].view(torch.int16))
 
 
-def _inputs(cfg, B, T, H, W, lens=None):
-    from oracle import stdit3_oracle as O
-
-    inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=lens)
-    return {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
-
-
 @pytest.mark.parametrize("mlps", [False, True])
 def test_xl_fp8_attention_at_the_benchmark_shape(mlps):
     """STDiT3-XL/2, full depth, 1x4x64x32x32, FP8 attention (and FP8 MLPs), against the fp32 oracle: at most 1.1x the
     error of the emulation reference, and the residual stream never jumps by more than 3x between consecutive blocks."""
-    from tests import stdit3_fp8_attn_ref as A
-
-    prod, oracle, cfg = R.build_pair("xl")
+    prod, oracle, cfg = stdit3_pair("xl")
     prod.enable_fp8_attention()
     if mlps:
         prod.enable_fp8()
-    inp = _inputs(cfg, 1, 64, 32, 32, lens=[260])
+    inp = stdit3_inputs(cfg, 1, 64, 32, 32, lens=[260], device="cuda")
     oracle = oracle.cuda()
     ref_x, got_x = [], []
     hooks = [b.register_forward_hook(lambda m, a, out: ref_x.append(out.detach().float()))
@@ -231,11 +223,9 @@ def test_xl_fp8_attention_at_the_benchmark_shape(mlps):
 def test_graph_replay_and_disable():
     """STDiT3-XS/2 (4 heads of 72) with an x_mask and ragged text: the captured step replays to the eager bits, and
     disable_fp8_attention() gives the bits of a model that never enabled it."""
-    from tests.smoke_impl import build_pair
-
-    prod, oracle, cfg = build_pair("xs")
-    plain = build_pair("xs")[0]
-    inp = _inputs(cfg, 2, 8, 16, 16, lens=[300, 21])
+    prod, oracle, cfg = stdit3_pair("xs")
+    plain = stdit3_pair("xs")[0]
+    inp = stdit3_inputs(cfg, 2, 8, 16, 16, lens=[300, 21], device="cuda")
     xm = torch.ones(2, 8, dtype=torch.bool, device="cuda")
     xm[1, :3] = False
     with torch.no_grad():

@@ -10,6 +10,7 @@ than 1.1x, and must stay below an absolute
 import pytest
 import torch
 
+from tests.models import stdit3_pair
 from tests.util import rel_l2, report
 
 pytestmark = pytest.mark.gpu
@@ -17,9 +18,8 @@ pytestmark = pytest.mark.gpu
 
 def _run(cfg_name, B, T, H, W, x_mask=None, lens=None):
     from oracle import stdit3_oracle as O
-    from tests.smoke_impl import build_pair
 
-    prod, oracle, cfg = build_pair(cfg_name)
+    prod, oracle, cfg = stdit3_pair(cfg_name)
     inp = O.synthetic_inputs(cfg, B=B, T=T, H=H, W=W, lens=lens)
     inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
     if x_mask is not None:
@@ -101,9 +101,8 @@ def test_xl_parity_at_the_benchmark_shape():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     from oracle import stdit3_oracle as O
-    from tests.smoke_impl import build_pair
 
-    prod, oracle, cfg = build_pair("xl")
+    prod, oracle, cfg = stdit3_pair("xl")
     inp = O.synthetic_inputs(cfg, B=1, T=64, H=32, W=32, lens=[260])
     inp = {k: (v.to(torch.bfloat16).float() if v.is_floating_point() else v).cuda() for k, v in inp.items()}
     oracle = oracle.cuda()

@@ -5,7 +5,7 @@ pipeline (T5 -> STDiT3-XS/2 -> RFLOW).  Each case prints its error, floor and ra
 import pytest
 import torch
 
-from tests.test_text_encoder_gpu import _encoder_parity
+from tests.text_gpu_common import encoder_parity
 from tests.util import rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -31,7 +31,7 @@ def test_masked_golden_case_on_device(tmp_path):
                      torch_dtype=torch.bfloat16)
     ids, mask = ids.cuda(), mask.cuda()
     torch.backends.cuda.matmul.allow_tf32 = False
-    _encoder_parity("T5 tiny masked 3x300", emb.encode(ids, mask), t5_encode_masked(wb, tf.T5_TINY, ids, mask),
+    encoder_parity("T5 tiny masked 3x300", emb.encode(ids, mask), t5_encode_masked(wb, tf.T5_TINY, ids, mask),
                     t5_encode_masked(wb, tf.T5_TINY, ids, mask, torch.bfloat16), 5e-2)
 
 
@@ -56,7 +56,7 @@ def test_full_t5_xxl_masked_vs_oracle(tmp_path):
     fp32 = t5_encode_masked(w, cfg, ids, mask)
     bf16 = t5_encode_masked(w, cfg, ids, mask, torch.bfloat16)
     # random 24-layer T5 weights grow the residual stream: the bf16 floor itself is about 0.11 here
-    _encoder_parity("T5-XXL masked 4x300", out, fp32, bf16, 0.15)
+    encoder_parity("T5-XXL masked 4x300", out, fp32, bf16, 0.15)
     bar = 1.1 * rel_l2(bf16.float(), fp32)
     for b, n in enumerate(lens[:2]):   # the short prompts' real tokens: without the mask they attend ~300 pads
         drop = rel_l2(unmasked[b, :n].float(), out[b, :n].float())

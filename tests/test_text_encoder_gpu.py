@@ -10,6 +10,8 @@ import numpy as np
 import pytest
 import torch
 
+from tests.text_gpu_common import encoder_parity
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -204,13 +206,6 @@ def test_text_epilogues(block_n, N, epi):
 
 
 # ---- whole encoders -------------------------------------------------------------------------------------------------
-def _encoder_parity(name, out, fp32, bf16, cap):
-    err = float((out.float() - fp32).norm() / fp32.norm())
-    floor = float((bf16.float() - fp32).norm() / fp32.norm())
-    print(f"{name}: rel-L2 error {err:.3e}, bf16 floor {floor:.3e}, ratio {err / floor:.3f}")
-    assert err <= 1.1 * floor and err < cap, (name, err, floor)
-
-
 def test_golden_config_encoders_vs_oracle(tmp_path):
     _osb()
     from oracle import text_oracle as O
@@ -223,14 +218,14 @@ def test_golden_config_encoders_vs_oracle(tmp_path):
     emb = HFEmbedder(tf.write_checkpoint(str(tmp_path / "t5"), tf.T5_TINY, wb), max_length=512, device_map="cuda",
                      torch_dtype=torch.bfloat16, tokenizer=tf.t5_tokenizer())
     ids = torch.from_numpy(g["t5_ids"]).cuda()
-    _encoder_parity("T5 tiny", emb.encode(ids), O.t5_encode(wb, tf.T5_TINY, ids), O.t5_encode(wb, tf.T5_TINY, ids, torch.bfloat16), 5e-2)
+    encoder_parity("T5 tiny", emb.encode(ids), O.t5_encode(wb, tf.T5_TINY, ids), O.t5_encode(wb, tf.T5_TINY, ids, torch.bfloat16), 5e-2)
     for tag in ("legacy", "eos"):
         cfg = json.loads(str(g[f"clip_{tag}_cfg"]))
         wc = {k_: v.bfloat16().float() for k_, v in tf.clip_weights(cfg, tf.SEED_CLIP).items()}
         emb = HFEmbedder(tf.write_checkpoint(str(tmp_path / "openai" / tag), cfg, wc), max_length=77, device_map="cuda",
                          torch_dtype=torch.bfloat16)
         ids = torch.from_numpy(g[f"clip_{tag}_ids"]).cuda()
-        _encoder_parity(f"CLIP tiny {tag}", emb.encode(ids), O.clip_encode(wc, cfg, ids),
+        encoder_parity(f"CLIP tiny {tag}", emb.encode(ids), O.clip_encode(wc, cfg, ids),
                         O.clip_encode(wc, cfg, ids, torch.bfloat16), 5e-2)
 
 
@@ -249,7 +244,7 @@ def test_full_t5_xxl_vs_oracle(tmp_path):
     out = emb.encode(ids)
     torch.backends.cuda.matmul.allow_tf32 = False
     # random 24-layer T5 weights grow the residual stream: the bf16 floor itself is about 0.11 here
-    _encoder_parity("T5-XXL 2x512", out, O.t5_encode(w, cfg, ids), O.t5_encode(w, cfg, ids, torch.bfloat16), 0.15)
+    encoder_parity("T5-XXL 2x512", out, O.t5_encode(w, cfg, ids), O.t5_encode(w, cfg, ids, torch.bfloat16), 0.15)
 
 
 def test_full_clip_l_vs_oracle_and_graph_replay(tmp_path):
@@ -268,7 +263,7 @@ def test_full_clip_l_vs_oracle_and_graph_replay(tmp_path):
     ids[0, 21:] = ids[1, 51:] = cfg["vocab_size"] - 1
     out = emb.encode(ids)
     torch.backends.cuda.matmul.allow_tf32 = False
-    _encoder_parity("CLIP-L 2x77", out, O.clip_encode(w, cfg, ids), O.clip_encode(w, cfg, ids, torch.bfloat16), 5e-2)
+    encoder_parity("CLIP-L 2x77", out, O.clip_encode(w, cfg, ids), O.clip_encode(w, cfg, ids, torch.bfloat16), 5e-2)
     # graph replay of the same encode equals the eager call, bit for bit
     static = ids.clone()
     s = torch.cuda.Stream()

@@ -6,7 +6,6 @@ from osb200's per-launch profile; the card name and power limit read in the same
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 
@@ -15,18 +14,12 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "open-sora_b200")]
 
+from tests.timing import card, window_ms  # noqa: E402
+
 
 def _time(fn, iters):
-    for _ in range(2):
-        fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
+    window_ms(fn, 2)   # warm-up
+    return window_ms(fn, iters)
 
 
 def main():
@@ -40,9 +33,7 @@ def main():
 
     osb200.init()
     torch.set_grad_enabled(False)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    res = {"gpu": q[0] if q else "unknown"}
+    res = {"gpu": ", ".join(card())}
     with tempfile.TemporaryDirectory() as tmp:
         for tag, cfg, is_clip, L in (("t5_xxl", tf.T5_XXL, False, 512), ("clip_l", tf.CLIP_L, True, 77)):
             shapes = _clip_shapes(cfg) if is_clip else _t5_shapes(cfg)

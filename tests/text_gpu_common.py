@@ -60,3 +60,10 @@ def build(tmp_dir: str, cfg: dict, weights: dict, is_clip: bool, max_length: int
                                       tokenizer=tokenizer)
     finally:
         conditioner.load_checkpoint = real
+
+
+def encoder_parity(name, out, fp32, bf16, cap):
+    err = float((out.float() - fp32).norm() / fp32.norm())
+    floor = float((bf16.float() - fp32).norm() / fp32.norm())
+    print(f"{name}: rel-L2 error {err:.3e}, bf16 floor {floor:.3e}, ratio {err / floor:.3f}")
+    assert err <= 1.1 * floor and err < cap, (name, err, floor)

@@ -11,12 +11,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "open-sora_b200"))
+
+from tests.timing import card, window_ms  # noqa: E402
 
 D = 512
 
@@ -41,12 +42,6 @@ def parse(argv=None):
     return a
 
 
-def card():
-    q = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], text=True)
-    name, power, clock = [v.strip() for v in q.splitlines()[0].split(",")]
-    return {"name": name, "power_limit": power, "max_sm_clock": clock}
-
-
 def sdpa_loop(q, k, v, T, hw):
     import torch
 
@@ -55,18 +50,6 @@ def sdpa_loop(q, k, v, T, hw):
         o[:, :, f * hw:(f + 1) * hw] = torch.nn.functional.scaled_dot_product_attention(
             q[:, :, f * hw:(f + 1) * hw], k[:, :, :(f + 1) * hw], v[:, :, :(f + 1) * hw])
     return o
-
-
-def timed(fn, reps):
-    import torch
-
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(reps):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / reps
 
 
 def bench_shape(T, h, w, windows):
@@ -86,12 +69,12 @@ def bench_shape(T, h, w, windows):
         outs[name] = fn().reshape(T * hw, D).clone()
         torch.cuda.synchronize()
         peak[name] = (torch.cuda.max_memory_allocated() - base) / 2**20
-    one = {n: timed(fn, 1) for n, fn in paths.items()}
+    one = {n: window_ms(fn, 1) for n, fn in paths.items()}
     reps = {n: max(1, int(300.0 / max(ms, 1e-3))) for n, ms in one.items()}     # ~0.3 s windows
     ms = {n: [] for n in paths}
     for _ in range(windows):                            # alternated windows
         for n, fn in paths.items():
-            ms[n].append(timed(fn, reps[n]))
+            ms[n].append(window_ms(fn, reps[n]))
     fl = attention_flop(T, hw)
     res = {"latent": [T, h, w], "tokens": T * hw, "tflop": fl / 1e12,
            "rel_l2_between_paths": float((outs["osb_attn_frames"].double() - outs["sdpa_loop"].double()).norm() / outs["sdpa_loop"].double().norm())}
@@ -124,14 +107,11 @@ def bench_model(T, H, W):
                 del out
                 torch.cuda.synchronize()
                 torch.cuda.reset_peak_memory_stats()
-                times = []
-                for _ in range(2):
-                    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    s.record()
-                    out = fn()
-                    e.record()
-                    torch.cuda.synchronize()
-                    times.append(s.elapsed_time(e))
+                # two timed calls of one pass each; the pass's output is kept for the comparison below, and the first
+                # call's output stays allocated while the second runs, so the peak covers both
+                last = {}
+                times = [window_ms(lambda: last.update(out=fn()), 1) for _ in range(2)]
+                out = last.pop("out")
                 tag = f"{leg}_{'native' if native else 'sdpa'}"
                 res[tag] = {"ms": times, "peak_gib": torch.cuda.max_memory_allocated() / 2**30}
                 if native:
@@ -149,7 +129,12 @@ def main(argv=None):
 
     if not torch.cuda.is_available():
         raise SystemExit("vae_attn_bench: needs a CUDA device (H100); there is no CPU path for a timing")
-    res = {"card": card(), "torch": torch.__version__, "shapes": [], "model": None}
+    name, q = card()
+    if q == "unknown":
+        raise SystemExit("vae_attn_bench: nvidia-smi gave no power limit and clock; a timing is not reported without them")
+    power, clock = q.split(", ")
+    res = {"card": {"name": name, "power_limit": power, "max_sm_clock": clock}, "torch": torch.__version__, "shapes": [],
+           "model": None}
     for T, h, w in a.shapes:
         res["shapes"].append(bench_shape(T, h, w, a.windows))
         print(json.dumps(res["shapes"][-1]), flush=True)
